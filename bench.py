@@ -1,11 +1,12 @@
 #!/usr/bin/env python
-"""bench.py — the BASELINE.json configs on B200, one JSON line (contract: DESIGN.md §Measurement).
+"""bench.py — the BASELINE.json configs on H100, one JSON line (contract: DESIGN.md §Measurement).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload all|vitl14|knn|ivf|e2e|plumbing]
+                  [--dump-outputs DIR]
 
 Workloads (BASELINE.json `configs`):
   plumbing configs[0] ViT-B/32 clip_inference on 100 synthetic images + captions through the reference's own reader /
-                      runner / writer (baseline/_ref, unmodified) around the CUDA ClipMapper     -> samples/s
+                      runner / writer (oracle/_ref, unmodified) around the CUDA ClipMapper     -> samples/s
   vitl14  configs[1]  ViT-L/14 image+text inference, synthetic 224^2, batch 1024 per GPU   -> pairs/s
   knn     configs[2]  brute-force cosine kNN, 100M x 768 fp16 rows per GPU, 1000 queries, top-40 -> queries/s
   ivf     configs[3]  IVF-Flat (nlist 65536, nprobe 16/64), rows range-sharded over the ranks, one all-gather -> queries/s
@@ -20,6 +21,9 @@ max over ranks); `e2e` = the same metric through the host-buffer API (H2D/D2H in
 `cpu_baseline` = the oracle port on the host cores on a bounded sample (rank 0, N=1 only);
 `parity_checked` = results of the timed configuration verified after the timed region (oracle as the checker).
 `--impl reference`: the CPU oracle port of the same workload on the host cores (bounded sample per step).
+`--steps K` is the number of timed steps of every workload.  `--dump-outputs DIR`: after the timed steps, what the last
+timed step of each workload returned to its caller is written as DIR/<workload>_<name>.npy (float32 or float64; inputs
+are seeded, so two builds can be compared output for output).
 """
 import argparse
 import json
@@ -33,7 +37,9 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-FALLBACK_PEAKS = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}
+# NVIDIA's H100 SXM data sheet (700 W card, dense BF16); MEASURED_PEAKS.json replaces them where present.  No
+# sustained BF16 rate has been measured on H100: without that file the "sustained" peak is the data-sheet figure.
+FALLBACK_PEAKS = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}
 # The reference's published ViT-L/14 numbers (BASELINE.md section 1): samples/s by GPU count, A100.
 PUBLISHED_VITL14 = {1: 312.0, 8: 2500.0}
 TOL = 2e-6   # |fp32 sum - exact| of unit vectors, d <= 1024 (tests/test_knn_gpu.py)
@@ -46,19 +52,8 @@ def load_peaks():
         d["_source"] = "measured"
         return d
     d = dict(FALLBACK_PEAKS)
-    d["_source"] = "fallback"
+    d["_source"] = "H100 data sheet (no sustained rate measured):"
     return d
-
-
-def load_traffic(key):
-    """Per-launch DRAM bytes of a kernel from the committed ncu summary of this round (profiles/r02_traffic.json)."""
-    p = os.path.join(ROOT, "profiles", "r02_traffic.json")
-    if not os.path.exists(p):
-        return None, None
-    t = json.load(open(p)).get(key)
-    if not t:
-        return None, None
-    return t.get("bytes_per_launch"), t.get("source")
 
 
 def physical_cores():
@@ -81,6 +76,30 @@ def tower_gemm_flops(t, tokens):
 
 def tower_attn_flops(t, T):
     return t.layers * 4 * T * T * t.width
+
+
+DUMP_ARRAY_BYTES = 5 << 20   # per array: at most 12 arrays (every workload) stay under 64 MB in all
+
+
+def dump(ctx, workload, arrays):
+    """--dump-outputs: what one timed step returned, as float32 (float64 kept) .npy files.  An array larger than
+    DUMP_ARRAY_BYTES is reduced to a fixed seeded sample of its rows, whose indices go to <name>_rows.npy."""
+    import numpy as np
+
+    if not ctx.args.dump_outputs or ctx.rank != 0:
+        return
+    os.makedirs(ctx.args.dump_outputs, exist_ok=True)
+    for name, a in arrays.items():
+        if hasattr(a, "detach"):
+            a = a.detach().cpu().numpy()
+        a = np.asarray(a)
+        a = a if a.dtype == np.float64 else a.astype(np.float32)
+        if a.nbytes > DUMP_ARRAY_BYTES:
+            keep = max(1, DUMP_ARRAY_BYTES // max(1, a[0].nbytes))
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], size=keep, replace=False))
+            a = a[rows]
+            np.save(os.path.join(ctx.args.dump_outputs, "%s_%s_rows.npy" % (workload, name)), rows.astype(np.float64))
+        np.save(os.path.join(ctx.args.dump_outputs, "%s_%s.npy" % (workload, name)), a)
 
 
 def arch_flops(arch):
@@ -290,9 +309,11 @@ def wl_vitl14(ctx):
     tok_host = synth_tokens(torch, B, arch, g).pin_memory()
     px_dev, tok_dev = px_host.to(ctx.dev), tok_host.to(ctx.dev)
 
+    last = {}
+
     def step_device():
-        model.embed_image_device(px_dev)
-        model.embed_text_device(tok_dev)
+        last["image_embeddings"] = model.embed_image_device(px_dev)
+        last["text_embeddings"] = model.embed_text_device(tok_dev)
 
     for _ in range(W):
         step_device()
@@ -300,6 +321,7 @@ def wl_vitl14(ctx):
     launches0 = m.launch_count()
     ms_per_step = ctx.timed(step_device, K)                  # the timed region: no per-kernel events inside
     launches = m.launch_count() - launches0
+    dump(ctx, "vitl14", last)
     # per-kernel-class device time: a second pass of the same K steps with CUDA events around every kernel
     model.set_profiling(True)
     for _ in range(K):
@@ -353,7 +375,6 @@ def wl_vitl14(ctx):
     gemm_flops = (fl["image_gemm"] + fl["text_gemm"]) * B
     achieved = gemm_flops / (gemm_ms / 1e3) / 1e12
     peak = ctx.peaks.get("bf16_tflops_sustained", FALLBACK_PEAKS["bf16_tflops_sustained"])
-    traffic, traffic_src = load_traffic("gemm_bf16_tcgen05_pair_kernel")
     out = {
         "metric": "ViT-L/14 embeds/s (image+text pairs/s)", "value": value, "unit": "pairs/s", "n_gpus": ctx.world,
         "steps": K, "warmup": W, "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak",
@@ -370,8 +391,8 @@ def wl_vitl14(ctx):
                 "api": "B200Clip.embed_image/embed_text (what ClipMapper.__call__ runs), pinned host tensors"},
         "gpu_launches": int(launches),
         "roofline": {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-                     "traffic": traffic, "traffic_source": traffic_src,
-                     "kernel": "gemm_bf16_tcgen05_pair_kernel (cta_group::2; the few small GEMMs use the single-CTA variant)",
+                     "traffic": None,
+                     "kernel": "gemm_bf16_wgmma_kernel (128x128 tiles, two consumer warpgroups, TMA ring)",
                      "launches_per_step": gemm_launches, "peak_source": "%s bf16_tflops_sustained" % ctx.peaks["_source"],
                      "flops_per_step": gemm_flops, "gemm_ms_per_step": gemm_ms,
                      "timing": "CUDA events around every GEMM launch in a second pass of the same %d steps" % K},
@@ -451,13 +472,19 @@ def wl_knn(ctx):
     sh = m.ShardedIndex(idx, device=ctx.dev)
     q = synth_rows(nq, d, m.SynthSpec(seed=4321), dtype="float32", device=ctx.local)
     q1 = q[:1].contiguous()
-    Wk, Kk = max(1, min(args.warmup, 2)), max(1, args.knn_steps)
+    Wk, Kk = max(1, min(args.warmup, 2)), max(1, args.steps)
     for _ in range(Wk):
         sh.search_device(q, k)
     sampler = ctx.sampler()
     launches0 = m.launch_count()
-    ms = ctx.timed(lambda: sh.search_device(q, k), Kk)
+    last = {}
+
+    def step():
+        last["D"], last["I"] = sh.search_device(q, k)
+
+    ms = ctx.timed(step, Kk)
     launches = m.launch_count() - launches0
+    dump(ctx, "knn", {"D": last["D"], "I": last["I"].double()})
     s_ms, s_n = idx.last_scan_ms()
     fallbacks = idx.last_hi_only_fallbacks()
     # serving shape: one query at a time (clip_back.py:362 issues nq=1)
@@ -516,7 +543,6 @@ def wl_knn(ctx):
     ach1 = bytes_per_launch / (s1_ms / max(s1_n, 1) / 1e3) / 1e9
     flops = 2.0 * rows * d * nq
     ach_tc = flops / (s_ms / 1e3) / 1e12 if s_ms > 0 else 0.0
-    traffic, traffic_src = load_traffic("flat_scan_staged_kernel")
     out = {
         "metric": "brute-force kNN queries/s (%d x %d fp16 rows per GPU, %d queries, top-%d)" % (rows, d, nq, k),
         "value": nq / (ms / 1e3), "unit": "queries/s", "n_gpus": ctx.world, "steps": Kk, "warmup": Wk, "ms_per_step": ms,
@@ -532,12 +558,12 @@ def wl_knn(ctx):
         "gpu_launches": int(launches),
         "roofline": {"bound": "tensor", "achieved": ach_tc, "peak": peak_tc, "unit": "TFLOP/s", "frac": ach_tc / peak_tc,
                      "traffic": None,
-                     "kernel": "scan_mma_kernel (tcgen05 cta_group::2; hi-only pass incl. its two sampling passes; re-score/verify/select outside)",
+                     "kernel": "scan_mma_kernel (wgmma m64n256k16; hi-only pass incl. its two sampling passes; re-score/verify/select outside)",
                      "flops_per_step": flops, "scan_ms_per_step": s_ms, "scan_launches_per_step": s_n,
                      "peak_source": "%s bf16_tflops_sustained" % ctx.peaks["_source"],
                      "whole_search_tflops": flops / (ms / 1e3) / 1e12},
         "roofline_nq1": {"bound": "hbm", "achieved": ach1, "peak": peak_hbm, "unit": "GB/s", "frac": ach1 / peak_hbm,
-                         "traffic": traffic, "traffic_source": traffic_src,
+                         "traffic": None,
                          "kernel": "flat_scan_staged_kernel<1,3> (nq=1 serving shape, cp.async.bulk ring)",
                          "bytes_per_launch": bytes_per_launch, "peak_source": "%s hbm_gbs" % ctx.peaks["_source"]},
         "parity_checked": parity["checked"], "parity": parity,
@@ -667,14 +693,20 @@ def wl_ivf(ctx, d=768):
     sampler = ctx.sampler()
     per = {}
     launches = 0
-    Kk = max(2, args.knn_steps)
+    Kk = max(1, args.steps)
     for nprobe in (16, 64):
         idx.nprobe = nprobe
         for _ in range(2):
             sh.search_device(q, k)
         l0 = m.launch_count()
-        ms = ctx.timed(lambda: sh.search_device(q, k), Kk)
+        last = {}
+
+        def step():
+            last["D"], last["I"] = sh.search_device(q, k)
+
+        ms = ctx.timed(step, Kk)
         launches += m.launch_count() - l0
+        dump(ctx, "ivf", {"nprobe%d_D" % nprobe: last["D"], "nprobe%d_I" % nprobe: last["I"].double()})
         s_ms, s_n = idx.last_scan_ms()
         for _ in range(3):
             sh.search_device(q1, k)
@@ -720,7 +752,7 @@ def wl_ivf(ctx, d=768):
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f16 rows, f32 query, f32 accumulate",
         "data": "synthetic (clustered: 65536 generating centroids, rows = normalise(3 c + noise))",
         "config": {"workload": "IVF-Flat cosine kNN, nlist %d, nprobe 16 (and 64), %d x %d fp16 rows per GPU, %d GPUs range-sharded "
-                               "(%d rows in total; 1B x 768 fp16 = 1.5 TB does not fit 8 x 180 GB), one all-gather of per-shard top-%d, "
+                               "(%d rows in total; 1B x 768 fp16 = 1.5 TB does not fit 8 x 80 GB), one all-gather of per-shard top-%d, "
                                "%d queries (BASELINE configs[3])" % (nlist, rows, d, ctx.world, rows * ctx.world, k, nq),
                    "l2": "each query scans its own lists (%.2f MB at nprobe 16); %d queries touch %.1f GB > L2"
                          % (p16["bytes_per_query"] / 1e6, nq, p16["bytes_per_query"] * nq / 1e9),
@@ -787,13 +819,21 @@ def wl_e2e(ctx):
     launches = m.launch_count() - l0
     lat_ms = np.array(lat) * 1e3
     # device-resident throughput: batches of 64 queries, embed + search, results stay on the device
+    last = {}
+
     def step_dev():
+        Ds, Is = [], []
         for s in range(0, nreq - 63, 64):
             qv = model.embed_text_device(toks_dev[s:s + 64], dtype=torch.float32)
-            sh.search_device(qv, k)
+            Dq, Iq = sh.search_device(qv, k)
+            Ds.append(Dq)
+            Is.append(Iq)
+        last["D"], last["I"] = Ds, Is
     step_dev()
     nb = len(range(0, nreq - 63, 64)) * 64
-    ms_dev = ctx.timed(step_dev, 3)
+    Ke = max(1, args.steps)
+    ms_dev = ctx.timed(step_dev, Ke)
+    dump(ctx, "e2e", {"D": torch.cat(last["D"]), "I": torch.cat(last["I"]).double()})
     # closed loop through the micro-batching front: `conc` client threads, each waits for its answer before the next
     conc = 64
     mb = m.MicroBatcher(model, sh if ctx.world == 1 else idx, max_batch=64, max_wait_ms=0.3, k=k)
@@ -863,7 +903,7 @@ def wl_e2e(ctx):
     p50 = float(np.percentile(lat_ms, 50))
     out = {
         "metric": "clip_back query path queries/s (ViT-H/14 text -> embed -> IVF-Flat kNN over %d x %d rows per GPU -> ids)" % (rows, d),
-        "value": nb / (ms_dev / 1e3), "unit": "queries/s", "n_gpus": ctx.world, "steps": 3, "warmup": 1,
+        "value": nb / (ms_dev / 1e3), "unit": "queries/s", "n_gpus": ctx.world, "steps": Ke, "warmup": 1,
         "ms_per_step": ms_dev, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "baseline_note": "README.md:433-435: reference averages 18.6 ms text embed + 26.7 ms knn on its CPU/A100 setup",
         "dtype": "bf16 text tower (fp32 accumulate), f16 rows / f32 query search", "data": "synthetic",
@@ -932,13 +972,13 @@ def cpu_baseline_e2e(ctx, arch, d, k, nprobe, rows_gpu, nlist_gpu, nquery=8):
                       % (nquery, cores, n_s, nlist_s, per_list)}
 
 
-# ---- the B200 arm ---------------------------------------------------------------------------------------------
+# ---- the CUDA arm ----------------------------------------------------------------------------------------------
 # ---- configs[0]: the clip_inference plumbing (reference reader -> runner -> mapper -> writer) -------------------
-REF_INFERENCE = os.path.join(ROOT, "baseline", "_ref", "clip_retrieval", "clip_inference")
+REF_INFERENCE = os.path.join(ROOT, "oracle", "_ref", "clip_retrieval", "clip_inference")
 
 
 def ref_inference_module(name):
-    """reader.py / runner.py / writer.py of the UNMODIFIED reference install under baseline/_ref, loaded by file path
+    """reader.py / runner.py / writer.py of the UNMODIFIED reference install under oracle/_ref, loaded by file path
     (the package's __init__ imports flask/faiss/all_clip, which are not installable offline; these three files only
     need torch, PIL, fsspec and pyarrow)."""
     import importlib.util
@@ -1039,10 +1079,10 @@ def wl_plumbing(ctx):
     base = {"metric": "ViT-B/32 clip_inference samples/s (image + caption files -> fp16 .npy shards)", "unit": "samples/s",
             "n_gpus": ctx.world, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
             "config": {"workload": "ViT-B/32 clip_inference on %d synthetic images + captions per GPU through the reference's own FilesReader / "
-                                   "Runner / NumpyWriter (baseline/_ref, unmodified), batch %d, %d output partitions (BASELINE configs[0])"
+                                   "Runner / NumpyWriter (oracle/_ref, unmodified), batch %d, %d output partitions (BASELINE configs[0])"
                                    % (n, bs, parts)}}
     if not os.path.isdir(REF_INFERENCE):
-        base.update({"unavailable": "baseline/_ref (the reference install, made by __graft_entry__.build() where /root/reference exists) "
+        base.update({"unavailable": "oracle/_ref (the reference install, made by __graft_entry__.build() where the reference checkout exists) "
                                     "is not in this tree", "parity_checked": None})
         return base
     tmp = tempfile.mkdtemp(prefix="b200clip_plumbing_%d_" % ctx.rank)
@@ -1060,7 +1100,7 @@ def wl_plumbing(ctx):
             mapper.enable_image, mapper.enable_text = img, txt
             return mapper(batch)
 
-        steps, times, inside = max(1, min(ctx.args.steps, 3)), [], []
+        steps, times, inside = max(1, ctx.args.steps), [], []
         launches0 = None
         for it in range(1 + steps):                                      # one warm-up job, then `steps` timed jobs
             out = os.path.join(tmp, "gpu_%d" % it)
@@ -1076,6 +1116,8 @@ def wl_plumbing(ctx):
                 inside.append(sec)
         launches = (m.launch_count() - launches0) // steps
         t_job = statistics.median(times)
+        img_last, txt_last = read_plumbing_output(os.path.join(tmp, "gpu_%d" % steps))
+        dump(ctx, "plumbing", {"image_embeddings": np.concatenate(img_last), "text_embeddings": np.concatenate(txt_last)})
         img_g, txt_g = read_plumbing_output(os.path.join(tmp, "gpu_1"))
         ok_layout = (len(img_g) == parts and len(txt_g) == parts
                      and all(a.dtype == np.float16 and a.shape == (n // parts, arch.embed_dim) for a in img_g + txt_g))
@@ -1161,18 +1203,15 @@ def run_reference(args):
     if rank != 0:
         return
     world = int(os.environ.get("WORLD_SIZE", "1"))
-    K, W = max(1, min(args.steps, 3)), 1
+    K, W = max(1, args.steps), 1
     cores = physical_cores()
     n = max(2, min(args.cpu_sample, 64))
     vals, secs = [], []
-    t_all = time.perf_counter()
     cpu_embed_sample("ViT-L/14", min(4, n), cores, budget_s=20.0)            # warm-up step
     for _ in range(K):
         v, done, dt = cpu_embed_sample("ViT-L/14", n, cores, budget_s=60.0)
         vals.append(v)
         secs.append(dt)
-        if time.perf_counter() - t_all > 200:
-            break
     value = statistics.median(vals)
     cb = {"value": value, "unit": "pairs/s", "cores": cores, "kind": "port",
           "sample": "median of %d steps of %d image+text pairs (chunks of 16), fp32 oracle/clip_ref.py, torch %d threads (physical cores); "
@@ -1228,12 +1267,13 @@ def main():
     ap.add_argument("--no-ivf", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-plumbing", action="store_true")
-    ap.add_argument("--knn-rows", type=int, default=100_000_000)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR")
+    # index sizes for one 80 GB H100: 40M x 768 fp16 = 61 GB (flat, IVF); 25M x 1024 fp16 = 51 GB next to ViT-H/14 (e2e)
+    ap.add_argument("--knn-rows", type=int, default=40_000_000)
     ap.add_argument("--knn-nq", type=int, default=1000)
-    ap.add_argument("--knn-steps", type=int, default=2)
-    ap.add_argument("--ivf-rows", type=int, default=100_000_000)
+    ap.add_argument("--ivf-rows", type=int, default=40_000_000)
     ap.add_argument("--ivf-nlist", type=int, default=65536)
-    ap.add_argument("--e2e-rows", type=int, default=75_000_000)
+    ap.add_argument("--e2e-rows", type=int, default=25_000_000)
     ap.add_argument("--e2e-queries", type=int, default=256)
     args = ap.parse_args()
     if args.impl == "reference":

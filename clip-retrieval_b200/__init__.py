@@ -1,4 +1,4 @@
-"""b200clip — B200-native (sm_100a) hot path for rom1504/clip-retrieval.
+"""b200clip — H100-native (sm_90a) hot path for rom1504/clip-retrieval.
 
 Two paths, each behind the reference's own Python seam (SURVEY.md §8b):
   * search: `B200FlatIndex` / `B200IVFFlatIndex` — the FAISS index object of

@@ -115,10 +115,6 @@ PROTOTYPES = {
     "b200_clip_set_profiling": (_i, [_vp, _i]),
     "b200_layernorm_bf16_device": (_i, [_vp, _vp, _vp, _vp, _i64, _i, _i, _vp]),
     "b200_attention_bf16_device": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
-    "b200_attention_tc_bf16_device": (_i, [_vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp]),
-    "b200_gemm_set_pair_mode": (_i, [_i]),
-    "b200_gemm_set_tma_store": (_i, [_i]),
-    "b200_attention_set_variant": (_i, [_i]),
     "b200_gemm_bf16_device": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "b200_index_last_hi_only_fallbacks": (_i, [_vp]),
     "b200_kmeans_train_f16": (_i, [_vp, _i64, _i, _i, _i, C.c_uint64, _i, _vp, _vp, _i]),

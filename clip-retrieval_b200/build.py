@@ -1,8 +1,7 @@
-"""Build the b200clip shared library (sm_100a only) in-tree with nvcc.
+"""Build the b200clip shared library (sm_90a only: H100) in-tree with nvcc.
 
 `python clip-retrieval_b200/build.py` or `__graft_entry__.build()`.  Objects land in
-clip-retrieval_b200/build/, the library in clip-retrieval_b200/lib/libb200clip.so (git-ignored,
-but it travels to the GPU box with the gpurun snapshot).
+clip-retrieval_b200/build/, the library in clip-retrieval_b200/lib/libb200clip.so (both git-ignored).
 """
 import os
 import shutil
@@ -16,12 +15,12 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "lib", "libb200clip.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "-Xcompiler", "-Wall",
     "--expt-relaxed-constexpr",
-] + os.environ.get("B200_NVCC_EXTRA", "").split()   # e.g. -DB200_TIMING_EXPERIMENTS for tools/gemm_exp.sh, tools/scan_exp.sh
+]
 
 
 def _nvcc():
@@ -41,7 +40,7 @@ def _deps_mtime():
 
 
 def build(verbose=False, force=False):
-    """Compile every csrc/*.cu for sm_100a and link the C-ABI library.  Returns its path."""
+    """Compile every csrc/*.cu for sm_90a and link the C-ABI library.  Returns its path."""
     os.makedirs(OBJ, exist_ok=True)
     os.makedirs(os.path.dirname(LIB), exist_ok=True)
     nvcc = _nvcc()
@@ -72,7 +71,7 @@ def build(verbose=False, force=False):
                 if verbose and log:
                     print(log)
     if jobs or not os.path.exists(LIB) or any(os.path.getmtime(o) > os.path.getmtime(LIB) for o in objs):
-        cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

@@ -3,7 +3,7 @@
 // fused with the L2-normalise + cast that follows each call in the reference.
 //
 // Data layout in HBM: weights packed once as bf16 [N, K] row-major (the layout both open_clip's
-// state_dict and the tcgen05 B operand use), LayerNorm affine / biases / positional tables fp32;
+// state_dict and the wgmma B operand use), LayerNorm affine / biases / positional tables fp32;
 // activations bf16 [B*T, width] row-major, one buffer per role (x residual stream, h LN output,
 // qkv, a attention output, f MLP hidden), sized for max_batch at create time so every TMA
 // descriptor is built once.
@@ -19,15 +19,13 @@
 #include <cstdlib>
 
 namespace b200 {
-int attention_tc2_r02i(const CUtensorMap& tmBig, const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int heads, int w,
-                       int causal, int sms, cudaStream_t st);
 
 struct Linear {
   __nv_bfloat16* w = nullptr;  // [N, K]
   float* b = nullptr;          // [N] or null (folded LayerNorm: d[n] = sum_k beta[k] W[n,k] + b[n])
   float* lnc = nullptr;        // folded LayerNorm: c[n] = sum_k W'[n,k], W' = bf16(W * gamma)  (gemm.cuh)
   int N = 0, K = 0;
-  CUtensorMap tm256, tm128, tm64, tm32;   // weight boxes of BN rows x 64 columns for every tile width
+  CUtensorMap tm128, tm64, tm32;   // weight boxes of BN rows x 64 columns for every tile width
 };
 
 struct Layer {
@@ -41,15 +39,9 @@ struct Tower {
   // activations
   __nv_bfloat16 *x = nullptr, *h = nullptr, *qkv = nullptr, *a = nullptr, *f = nullptr;
   CUtensorMap tm_h, tm_a, tm_f, tm_x;
-  CUtensorMap ts_x, ts_qkv, ts_f;   // store / residual maps (boxes of 32 rows x 64 columns) over x, qkv, f
+  CUtensorMap tm_qkv;          // qkv in boxes of 64 rows x 64 columns: Q / K tiles of the wgmma attention
+  bool wgmma_attn = false;
   float2* stats = nullptr;     // folded LayerNorm: (mean, M2) per 64-column slot of every row of x
-  // tcgen05 attention (head dim 64, T <= 320): V^T buffer + maps over qkv / V^T
-  bool use_tc_attn = false;
-  int Tp = 0;
-  __nv_bfloat16* vt = nullptr;
-  CUtensorMap tm_qk, tm_vt;
-  CUtensorMap tm_qkv3;   // per-sample 3-D map over qkv [max_batch, T, 3w] (attention_tc3.cu)
-  float* kmax = nullptr; // [max_batch * heads] max key norm per (sample, head): the softmax bound of attention_tc3.cu
   float *lnf_g = nullptr, *lnf_b = nullptr;  // ln_post / ln_final
   __nv_bfloat16* proj = nullptr;             // [width, D]
 };
@@ -63,7 +55,7 @@ enum { CLS_GEMM = 0, CLS_ATTN = 1, CLS_LN = 2, CLS_OTHER = 3,
 
 struct b200_clip {
   b200_clip_config cfg;
-  int device = 0, sms = 148;
+  int device = 0, sms = 132;
   bool loaded = false;
   b200::Tower vis, txt;
   // vision front end
@@ -72,7 +64,6 @@ struct b200_clip {
   __nv_bfloat16* cols = nullptr;  // [max_batch*g*g, Kp]
   CUtensorMap tm_cols;
   __nv_bfloat16* vpos = nullptr;  // positional_embedding bf16 [T, w] (residual operand of the patch GEMM)
-  CUtensorMap ts_vpos;            // its residual map (boxes of 32 rows x 64 columns)
   float* cls_pos0 = nullptr;      // class_embedding + positional_embedding[0]
   float *lnpre_g = nullptr, *lnpre_b = nullptr;
   // text front end
@@ -101,12 +92,7 @@ struct b200_clip {
   void* g_out = nullptr;
   bool use_graphs = true;      // B200_GRAPHS=0 disables (A/B, debugging)
   cudaStream_t cap_stream = nullptr;
-  cudaStream_t s_side = nullptr;             // side stream of the attention's leftover-row kernel (fork / join per layer)
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  bool fuse_ln = false;        // LayerNorm folded into the qkv / fc GEMMs (B200_FUSE_LN=1): correct, but measured slower than the LN kernel it removes (DESIGN.md)
-  int attn_gen = 2;            // 3: attention_tc3.cu (single score pass); 2: attention_tc2.cu (B200_ATTN_GEN; default 2 until verified)
-  bool attn_pipelined = true;  // two query tiles in flight (attention_tc2.cu) where the shape allows
-  bool attn_v_direct = true;   // P.V reads V from the qkv buffer as an MN-major operand (no V^T copy)
+  bool fuse_ln = false;        // LayerNorm folded into the qkv / fc GEMMs (B200_FUSE_LN=1)
   struct Span { int cls; cudaEvent_t a, b; };
   std::vector<Span> spans;
   int span_used = 0;
@@ -133,7 +119,6 @@ static int make_linear(b200_clip* m, Linear* l, int N, int K, bool bias) {
     B200_TRY(dev_alloc(m, &l->b, (size_t)N));
     B200_CUDA(cudaMemset(l->b, 0, (size_t)N * 4));
   }
-  B200_TRY(make_tmap_2d(&l->tm256, l->w, 1, N, K, K, 256, GEMM_BK));
   B200_TRY(make_tmap_2d(&l->tm128, l->w, 1, N, K, K, 128, GEMM_BK));
   B200_TRY(make_tmap_2d(&l->tm64, l->w, 1, N, K, K, 64, GEMM_BK));
   B200_TRY(make_tmap_2d(&l->tm32, l->w, 1, N, K, K, 32, GEMM_BK));
@@ -159,34 +144,20 @@ static int make_tower(b200_clip* m, Tower* t, const b200_tower_config& c, int T,
   B200_TRY(dev_alloc(m, &t->x, rows * w));
   B200_TRY(dev_alloc(m, &t->h, rows * w));
   B200_TRY(dev_alloc(m, &t->qkv, rows * 3 * w));
-  // rows past the current batch are read (then multiplied by P = 0) by the attention's 128-row V boxes: keep them finite
-  B200_CUDA(cudaMemset(t->qkv, 0, rows * 3 * w * 2));
   B200_TRY(dev_alloc(m, &t->a, rows * w));
   B200_TRY(dev_alloc(m, &t->f, rows * c.mlp));
   B200_TRY(make_tmap_2d(&t->tm_h, t->h, 1, rows, w, w, GEMM_BM, GEMM_BK));
   B200_TRY(make_tmap_2d(&t->tm_a, t->a, 1, rows, w, w, GEMM_BM, GEMM_BK));
   B200_TRY(make_tmap_2d(&t->tm_f, t->f, 1, rows, c.mlp, c.mlp, GEMM_BM, GEMM_BK));
   B200_TRY(make_tmap_2d(&t->tm_x, t->x, 1, rows, w, w, GEMM_BM, GEMM_BK));
-  B200_TRY(make_tmap_2d(&t->ts_x, t->x, 1, rows, w, w, 32, 64));
-  B200_TRY(make_tmap_2d(&t->ts_qkv, t->qkv, 1, rows, 3 * (size_t)w, 3 * (size_t)w, 32, 64));
-  B200_TRY(make_tmap_2d(&t->ts_f, t->f, 1, rows, c.mlp, c.mlp, 32, 64));
+  t->wgmma_attn = attention_wgmma_supported(T, c.heads, w);
+  if (t->wgmma_attn) B200_TRY(make_tmap_2d(&t->tm_qkv, t->qkv, 1, rows, 3 * (size_t)w, 3 * (size_t)w, 64, 64));
   if (m->fuse_ln && w % 64 == 0 && w <= 64 * LN_MAX_SLOTS) {
     B200_TRY(dev_alloc(m, &t->stats, rows * (size_t)(w / 64)));
     for (auto& L : t->L) {
       B200_TRY(dev_alloc(m, &L.qkv.lnc, (size_t)3 * w));
       B200_TRY(dev_alloc(m, &L.fc.lnc, (size_t)c.mlp));
     }
-  }
-  t->use_tc_attn = attention_tc_supported(T, c.heads, w);
-  if (t->use_tc_attn) {
-    t->Tp = (T + 7) / 8 * 8;
-    const size_t vt_rows = (size_t)m->cfg.max_batch * c.heads * 64;
-    B200_TRY(dev_alloc(m, &t->vt, vt_rows * t->Tp));
-    B200_CUDA(cudaMemset(t->vt, 0, vt_rows * t->Tp * 2));  // key padding stays zero (0 * garbage would be NaN)
-    B200_TRY(make_tmap_2d(&t->tm_qk, t->qkv, 1, rows, 3 * (size_t)w, 3 * (size_t)w, 128, 64));
-    B200_TRY(make_tmap_2d(&t->tm_vt, t->vt, 1, vt_rows, t->Tp, t->Tp, 64, 64));
-    B200_TRY(make_tmap_3d(&t->tm_qkv3, t->qkv, 1, (uint64_t)m->cfg.max_batch, (uint64_t)T, 3 * (uint64_t)w, 3 * (uint64_t)w, 128));
-    B200_TRY(dev_alloc(m, &t->kmax, (size_t)m->cfg.max_batch * c.heads));
   }
   return B200_OK;
 }
@@ -212,15 +183,15 @@ struct SpanGuard {
 };
 
 static int run_linear(b200_clip* m, const CUtensorMap& tmA, const Linear& l, int M, GemmEpilogue ep, cudaStream_t st,
-                      int kind = CLS_GEMM, const CUtensorMap* tmC = nullptr, const CUtensorMap* tmR = nullptr) {
+                      int kind = CLS_GEMM) {
   SpanGuard sg(m, kind, st);
   int bn = gemm_pick_bn(M, l.N, m->sms);
   // row statistics are written per 64-column slot by ONE thread: the narrow tiles split a slot over two warps
   if (ep.stats_out != nullptr && bn < 128) bn = 128;
   ep.bias = l.b;
   m->last_launches++;
-  const CUtensorMap& tmB = bn == 256 ? l.tm256 : (bn == 64 ? l.tm64 : (bn == 32 ? l.tm32 : l.tm128));   // pair mode: tm128
-  return gemm_bf16_launch(tmA, tmB, bn, M, l.N, l.K, ep, m->sms, st, tmC, tmR);
+  const CUtensorMap& tmB = bn == 64 ? l.tm64 : (bn == 32 ? l.tm32 : l.tm128);
+  return gemm_bf16_launch(tmA, tmB, bn, M, l.N, l.K, ep, st);
 }
 
 static int run_blocks(b200_clip* m, Tower& t, int B, int causal, cudaStream_t st) {
@@ -239,30 +210,21 @@ static int run_blocks(b200_clip* m, Tower& t, int B, int causal, cudaStream_t st
       B200_TRY(layernorm_rows(t.x, w, t.h, w, L.ln1_g, L.ln1_b, M, w, st)); }
     GemmEpilogue e1; e1.out = t.qkv; e1.out_ld = 3 * w;
     if (fused) { e1.ln_stats = t.stats; e1.ln_c = L.qkv.lnc; e1.ln_w = w; }
-    if (t.use_tc_attn && !m->attn_v_direct) {
-      e1.vt = t.vt; e1.vt_col0 = 2 * w; e1.vt_T = t.T; e1.vt_Tp = t.Tp; e1.vt_hd = 64; e1.vt_heads = t.heads;
-    }
-    B200_TRY(run_linear(m, fused ? t.tm_x : t.tm_h, L.qkv, M, e1, st, CLS_G_QKV, &t.ts_qkv));
+    B200_TRY(run_linear(m, fused ? t.tm_x : t.tm_h, L.qkv, M, e1, st, CLS_G_QKV));
     { SpanGuard sg(m, CLS_ATTN, st); m->last_launches++;
-      if (t.use_tc_attn && m->attn_gen == 3 && attention_tc3_supported(t.T, t.heads, w))
-        B200_TRY(attention_tc3(t.tm_qkv3, t.qkv, t.a, t.kmax, B, t.T, t.heads, w, causal, m->sms, st, m->s_side, m->ev_fork, m->ev_join));
-      else if (t.use_tc_attn && m->attn_pipelined && attention_tc2_supported(t.T, t.heads, w)) {
-        if (m->attn_gen == 4) { B200_TRY(attention_tc2_r02i(t.tm_qk, t.qkv, t.a, B, t.T, t.heads, w, causal, m->sms, st)); }
-        else { B200_TRY(attention_tc2(t.tm_qk, t.qkv, t.a, B, t.T, t.heads, w, causal, m->sms, st, m->s_side, m->ev_fork, m->ev_join)); }
-      }
-      else if (t.use_tc_attn) B200_TRY(attention_tc(t.tm_qk, t.tm_vt, t.a, B, t.T, t.heads, w, causal, m->attn_v_direct ? 1 : 0, m->sms, st));
+      if (t.wgmma_attn) B200_TRY(attention_wgmma(t.tm_qkv, t.qkv, t.a, B, t.T, t.heads, w, causal, st));
       else B200_TRY(attention(t.qkv, t.a, B, t.T, t.heads, w, causal, st)); }
     GemmEpilogue e2; e2.out = t.x; e2.out_ld = w; e2.residual = t.x; e2.res_ld = w;
     if (fused) e2.stats_out = t.stats;
-    B200_TRY(run_linear(m, t.tm_a, L.out, M, e2, st, CLS_G_OUT, &t.ts_x, &t.ts_x));
+    B200_TRY(run_linear(m, t.tm_a, L.out, M, e2, st, CLS_G_OUT));
     if (!fused) { SpanGuard sg(m, CLS_LN, st); m->last_launches++;
       B200_TRY(layernorm_rows(t.x, w, t.h, w, L.ln2_g, L.ln2_b, M, w, st)); }
     GemmEpilogue e3; e3.out = t.f; e3.out_ld = t.mlp; e3.act = act;
     if (fused) { e3.ln_stats = t.stats; e3.ln_c = L.fc.lnc; e3.ln_w = w; }
-    B200_TRY(run_linear(m, fused ? t.tm_x : t.tm_h, L.fc, M, e3, st, CLS_G_FC, &t.ts_f));
+    B200_TRY(run_linear(m, fused ? t.tm_x : t.tm_h, L.fc, M, e3, st, CLS_G_FC));
     GemmEpilogue e4; e4.out = t.x; e4.out_ld = w; e4.residual = t.x; e4.res_ld = w;
     if (fused) e4.stats_out = t.stats;
-    B200_TRY(run_linear(m, t.tm_f, L.proj, M, e4, st, CLS_G_PROJ, &t.ts_x, &t.ts_x));
+    B200_TRY(run_linear(m, t.tm_f, L.proj, M, e4, st, CLS_G_PROJ));
   }
   return B200_OK;
 }
@@ -277,7 +239,7 @@ static int encode_image_chunk(b200_clip* m, const float* d_px, int B, void* d_ou
   // patch embedding: x[b*T + 1 + p, :] = cols[b*g*g + p, :] · conv^T + positional_embedding[1 + p]
   GemmEpilogue ep; ep.out = t.x; ep.out_ld = w; ep.out_group = g * g;
   ep.residual = m->vpos; ep.res_ld = w; ep.res_row_mod = g * g; ep.res_row_off = 1;
-  B200_TRY(run_linear(m, m->tm_cols, m->conv, B * g * g, ep, st, CLS_GEMM, &t.ts_x, &m->ts_vpos));
+  B200_TRY(run_linear(m, m->tm_cols, m->conv, B * g * g, ep, st, CLS_GEMM));
   { SpanGuard sg(m, CLS_LN, st); m->last_launches++;
     B200_TRY(layernorm_rows(t.x, w, t.x, w, m->lnpre_g, m->lnpre_b, (int64_t)B * T, w, st)); }
   B200_TRY(run_blocks(m, t, B, 0, st));
@@ -436,10 +398,8 @@ int b200_clip_create(const b200_clip_config* cfg, int device, b200_clip** out) {
   m->cfg = *cfg;
   m->device = device;
   m->sms = sm_count(device);
-  if (const char* g = getenv("B200_ATTN_GEN")) m->attn_gen = atoi(g);
-  // LayerNorm folded into the qkv / fc GEMMs stays opt-in: at throughput batch sizes the epilogue is the pair GEMM's
-  // bottleneck and the fold costs more than the LN kernel it removes (profiles/r02d_model_ab.txt); at serving batch
-  // sizes the row statistics need >= 128-column tiles, which undoes the narrow-tile weight streaming.
+  // LayerNorm folded into the qkv / fc GEMMs stays opt-in: it adds per-row statistics work to the GEMM epilogue, and at
+  // serving batch sizes the row statistics need >= 128-column tiles, which undoes the narrow-tile weight streaming.
   if (const char* g = getenv("B200_FUSE_LN")) m->fuse_ln = atoi(g) != 0;
   if (const char* g = getenv("B200_GRAPHS")) m->use_graphs = atoi(g) != 0;
   m->grid = cfg->image_size / cfg->patch;
@@ -456,7 +416,6 @@ int b200_clip_create(const b200_clip_config* cfg, int device, b200_clip** out) {
     B200_CUDA(cudaMemset(m->cols, 0, prow * m->Kp * 2));
     B200_TRY(make_tmap_2d(&m->tm_cols, m->cols, 1, prow, m->Kp, m->Kp, GEMM_BM, GEMM_BK));
     B200_TRY(dev_alloc(m, &m->vpos, (size_t)T * cfg->vision.width));
-    B200_TRY(make_tmap_2d(&m->ts_vpos, m->vpos, 1, (uint64_t)T, (uint64_t)cfg->vision.width, (uint64_t)cfg->vision.width, 32, 64));
     B200_TRY(dev_alloc(m, &m->cls_pos0, (size_t)cfg->vision.width));
     B200_TRY(dev_alloc(m, &m->lnpre_g, (size_t)cfg->vision.width));
     B200_TRY(dev_alloc(m, &m->lnpre_b, (size_t)cfg->vision.width));
@@ -470,9 +429,6 @@ int b200_clip_create(const b200_clip_config* cfg, int device, b200_clip** out) {
     m->allocs.push_back(m->stage_in);
     B200_CUDA(cudaMalloc(&m->stage_out, (size_t)cfg->max_batch * cfg->embed_dim * 4));
     m->allocs.push_back(m->stage_out);
-    B200_CUDA(cudaStreamCreateWithFlags(&m->s_side, cudaStreamNonBlocking));
-    B200_CUDA(cudaEventCreateWithFlags(&m->ev_fork, cudaEventDisableTiming));
-    B200_CUDA(cudaEventCreateWithFlags(&m->ev_join, cudaEventDisableTiming));
     const int gb = std::min(GRAPH_MAX_B, cfg->max_batch);
     B200_CUDA(cudaMalloc(&m->g_in, std::max((size_t)gb * 3 * cfg->image_size * cfg->image_size * 4, (size_t)gb * cfg->context_length * 8)));
     m->allocs.push_back(m->g_in);
@@ -498,9 +454,6 @@ int b200_clip_destroy(b200_clip* m) {
   if (m->act_ev) cudaEventDestroy(m->act_ev);
   for (auto& kv : m->graphs) if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
   if (m->cap_stream) cudaStreamDestroy(m->cap_stream);
-  if (m->s_side) cudaStreamDestroy(m->s_side);
-  if (m->ev_fork) cudaEventDestroy(m->ev_fork);
-  if (m->ev_join) cudaEventDestroy(m->ev_join);
   if (m->s_copy) {
     cudaStreamDestroy(m->s_copy); cudaStreamDestroy(m->s_comp);
     for (int i = 0; i < 4; i++) { cudaEventDestroy(m->ev_in[i]); cudaEventDestroy(m->ev_done[i]); }
@@ -710,66 +663,13 @@ int b200_attention_bf16_device(const void* d_qkv, void* d_out, int B, int T, int
                                void* stream) {
   B200_CHECK(d_qkv && d_out && B >= 0 && T >= 1, B200_ERR_INVALID, "attention: bad argument");
   DeviceGuard g(device);
+  if (B > 0 && attention_wgmma_supported(T, heads, w)) {
+    CUtensorMap tm;
+    B200_TRY(make_tmap_2d(&tm, d_qkv, 1, (uint64_t)B * T, 3 * (uint64_t)w, 3 * (uint64_t)w, 64, 64));
+    return attention_wgmma(tm, (const __nv_bfloat16*)d_qkv, (__nv_bfloat16*)d_out, B, T, heads, w, causal, (cudaStream_t)stream);
+  }
   return attention((const __nv_bfloat16*)d_qkv, (__nv_bfloat16*)d_out, B, T, heads, w, causal, (cudaStream_t)stream);
 }
-
-int b200_attention_tc_bf16_device(const void* d_qkv, const void* d_vt, int Tp, void* d_out, int B, int T, int heads, int w,
-                                  int causal, int device, void* stream) {
-  B200_CHECK(d_qkv && d_out && B >= 0 && T >= 1 && (d_vt == nullptr || (Tp >= T && Tp % 8 == 0)) && (Tp >= 0 || d_vt == nullptr), B200_ERR_INVALID,
-             "attention_tc: bad argument");
-  DeviceGuard g(device);
-  CUtensorMap tq, tv;
-  B200_TRY(make_tmap_2d(&tq, d_qkv, 1, (uint64_t)B * T, 3 * (uint64_t)w, 3 * (uint64_t)w, 128, 64));
-  if (d_vt) B200_TRY(make_tmap_2d(&tv, d_vt, 1, (uint64_t)B * heads * 64, (uint64_t)Tp, (uint64_t)Tp, 64, 64));
-  else tv = tq;
-  // Tp == -2: third generation (attention_tc3.cu), per-sample 3-D tensor map
-  if (Tp == -2) {
-    CUtensorMap t3;
-    B200_TRY(make_tmap_3d(&t3, d_qkv, 1, (uint64_t)B, (uint64_t)T, 3 * (uint64_t)w, 3 * (uint64_t)w, 128));
-    // stand-alone test / timing entry: a grow-only scratch per device, kept for the life of the process
-    static std::mutex smu;
-    static float* scratch[64] = {};
-    static size_t scratch_n[64] = {};
-    std::lock_guard<std::mutex> lock(smu);
-    const size_t need = (size_t)std::max(1, B * heads);
-    if (scratch_n[device & 63] < need) {
-      if (scratch[device & 63]) { cudaDeviceSynchronize(); cudaFree(scratch[device & 63]); }
-      scratch[device & 63] = nullptr;
-      B200_CUDA(cudaMalloc((void**)&scratch[device & 63], need * 4));
-      scratch_n[device & 63] = need;
-    }
-    return attention_tc3(t3, (const __nv_bfloat16*)d_qkv, (__nv_bfloat16*)d_out, scratch[device & 63], B, T, heads, w, causal,
-                         sm_count(device), (cudaStream_t)stream);
-  }
-  // Tp == -3: attention_tc2 with the leftover rows (T mod 128 in 1..4) on a second stream, as the model runs it
-  if (Tp == -3) {
-    static std::mutex smu;
-    static cudaStream_t side[64] = {};
-    static cudaEvent_t ev[64][2] = {};
-    std::lock_guard<std::mutex> lock(smu);
-    const int d = device & 63;
-    if (!side[d]) {
-      B200_CUDA(cudaStreamCreateWithFlags(&side[d], cudaStreamNonBlocking));
-      B200_CUDA(cudaEventCreateWithFlags(&ev[d][0], cudaEventDisableTiming));
-      B200_CUDA(cudaEventCreateWithFlags(&ev[d][1], cudaEventDisableTiming));
-    }
-    return attention_tc2(tq, (const __nv_bfloat16*)d_qkv, (__nv_bfloat16*)d_out, B, T, heads, w, causal, sm_count(device),
-                         (cudaStream_t)stream, side[d], ev[d][0], ev[d][1], 1);
-  }
-  // Tp == -4: the round-2 session-i build of attention_tc2 (A/B reference for one measurement session)
-  if (Tp == -4)
-    return attention_tc2_r02i(tq, (const __nv_bfloat16*)d_qkv, (__nv_bfloat16*)d_out, B, T, heads, w, causal, sm_count(device),
-                              (cudaStream_t)stream);
-  // Tp < 0: the two-tiles-in-flight kernel (attention_tc2.cu), every row on the tensor cores
-  if (Tp < 0)
-    return attention_tc2(tq, (const __nv_bfloat16*)d_qkv, (__nv_bfloat16*)d_out, B, T, heads, w, causal, sm_count(device),
-                         (cudaStream_t)stream);
-  // d_vt == NULL: V is read from the qkv buffer (MN-major operand); else from the V^T buffer
-  return attention_tc(tq, tv, (__nv_bfloat16*)d_out, B, T, heads, w, causal, d_vt == nullptr ? 1 : 0, sm_count(device),
-                      (cudaStream_t)stream);
-}
-
-int b200_attention_set_variant(int variant) { return attention_tc2_set_variant(variant); }
 
 int b200_clip_set_profiling(b200_clip* m, int on) {
   B200_CHECK(m, B200_ERR_INVALID, "set_profiling: null handle");

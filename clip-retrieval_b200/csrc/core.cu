@@ -18,10 +18,10 @@ int sm_count(int device) {
   static int cached[64];
   static std::once_flag once;
   std::call_once(once, [] { for (int& c : cached) c = 0; });
-  if (device < 0 || device >= 64) return 148;
+  if (device < 0 || device >= 64) return 132;
   if (cached[device] == 0) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || n <= 0) n = 132;
     cached[device] = n;
   }
   return cached[device];
@@ -30,5 +30,5 @@ int sm_count(int device) {
 }  // namespace b200
 
 extern "C" const char* b200_last_error(void) { return b200::g_err; }
-extern "C" const char* b200_version(void) { return "b200clip 0.1 (sm_100a)"; }
+extern "C" const char* b200_version(void) { return "b200clip 0.1 (sm_90a)"; }
 extern "C" int64_t b200_launch_count(void) { return (int64_t)b200::g_launches.load(); }

@@ -203,7 +203,7 @@ int layernorm_rows(const __nv_bfloat16* in, int64_t in_ld, __nv_bfloat16* out, i
   B200_CHECK(w % 8 == 0 && w <= LN_MAXC * 256, B200_ERR_UNSUPPORTED, "layernorm: width %d (need %%8, <= 2048)", w);
   if (rows == 0) return B200_OK;
   // persistent: enough blocks to fill the chip, each warp strides over rows
-  const unsigned grid = (unsigned)std::min<int64_t>((rows + 7) / 8, (int64_t)148 * 6);
+  const unsigned grid = (unsigned)std::min<int64_t>((rows + 7) / 8, (int64_t)132 * 6);
   switch ((w / 8 + 31) / 32) {
     case 1: layernorm_kernel<1><<<grid, 256, 0, st>>>(in, in_ld, out, out_ld, gamma, beta, rows, w); break;
     case 2: layernorm_kernel<2><<<grid, 256, 0, st>>>(in, in_ld, out, out_ld, gamma, beta, rows, w); break;
@@ -306,8 +306,8 @@ pool_proj_kernel(const __nv_bfloat16* __restrict__ x, int T, int w, const int* _
     else reinterpret_cast<float*>(out)[(size_t)b * D + j] = v;
   }
 }
-// One block per sample leaves the projection to a w-long dependent loop per thread: 0.76 ms at batch 1 (a single SM,
-// clip_back.py:226-246's shape) and still 0.72 ms per call at batch 1024 (profiles/r02n_launch_shares.txt).  Here a
+// One block per sample leaves the projection to a w-long dependent loop per thread on a single SM at batch 1
+// (clip_back.py:226-246's shape).  Here a
 // block owns 64 output columns of one sample: the pooled row is normalised redundantly per block (w values), the projection is split over
 // 64 columns x 4 quarters of the reduction dimension, raw features go to `feat` and a second tiny kernel normalises.
 __global__ void __launch_bounds__(256)

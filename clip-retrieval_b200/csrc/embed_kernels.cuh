@@ -19,34 +19,14 @@ int layernorm_rows(const __nv_bfloat16* in, int64_t in_ld, __nv_bfloat16* out, i
                    const float* beta, int64_t rows, int w, cudaStream_t st);
 // (mean, M2) per 64-column slot of every row of x [rows, w] (w % 64 == 0): seeds GemmEpilogue::ln_stats.
 int row_stats(const __nv_bfloat16* x, int64_t rows, int w, float2* stats, cudaStream_t st);
-// K4: multi-head attention over the fused qkv buffer [B*T, 3w] -> out [B*T, w]; causal for text.
+// K4: multi-head attention over the fused qkv buffer [B*T, 3w] -> out [B*T, w]; causal for text.  mma.sync kernel
+// (attention.cu) for the head dimensions the wgmma kernel does not take (80, 96, 128).
 int attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int heads, int w, int causal, cudaStream_t st);
-// K4 on tcgen05 (attention_tc.cu): head dim 64, T <= 320.  tmQK: qkv buffer [rows, 3w] box 128x64;
-// tmVt: V^T buffer [B*heads*64, Tp] box 64x64 (written by the QKV GEMM epilogue, GemmEpilogue::vt).
-bool attention_tc_supported(int T, int heads, int w);
-int attention_tc(const CUtensorMap& tmQK, const CUtensorMap& tmVt, __nv_bfloat16* out, int B, int T, int heads, int w,
-                 int causal, int v_direct, int sms, cudaStream_t st);
-// Two-tiles-in-flight variant (attention_tc2.cu): head dim 64, T <= 264; V read from the qkv buffer.
-bool attention_tc2_supported(int T, int heads, int w);
-// side / ev_fork / ev_join + tail_mode 1 (or -1 and B200_ATTN_TAIL_KERNEL=1): when T leaves 1..4 query rows after the last
-// full 128-row tile (T = 257), those rows run as attention_tail_rows on `side`, concurrently with the tensor-core kernel,
-// instead of a padded tile.  Measured slower (profiles/r02j_attention_tail_ab.txt): off by default.
-int attention_tc2(const CUtensorMap& tmBig, const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int heads, int w,
-                  int causal, int sms, cudaStream_t st, cudaStream_t side = nullptr, cudaEvent_t ev_fork = nullptr,
-                  cudaEvent_t ev_join = nullptr, int tail_mode = -1);
-int attention_tc2_set_variant(int v);   // returns the previous variant; v < 0 only reads it
-// Query rows row0 .. row0 + nrows - 1 of every (sample, head) on the FMA pipe: one warp per row, exact two-pass softmax,
-// K and V from the qkv buffer (attention_tc3.cu).
-int attention_tail_rows(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int heads, int w, int causal, int row0,
-                        int nrows, cudaStream_t st);
-// Third generation (attention_tc3.cu): one pass over the scores (Cauchy-Schwarz bound instead of the row maximum),
-// leftover query rows (T mod 128 <= 8) on the FMA pipe, per-sample 3-D tensor map tm3 over qkv [B, T, 3w], box 128x64.
-bool attention_tc3_supported(int T, int heads, int w);
-// side / ev_fork / ev_join (optional): the leftover query rows (T mod 128 <= 4) run as a small kernel on `side`
-// concurrently with the tensor-core kernel; without them they run on `st` before it.
-int attention_tc3(const CUtensorMap& tm3, const __nv_bfloat16* qkv, __nv_bfloat16* out, float* kmax_scratch /*[B*heads]*/,
-                  int B, int T, int heads, int w, int causal, int sms, cudaStream_t st, cudaStream_t side = nullptr,
-                  cudaEvent_t ev_fork = nullptr, cudaEvent_t ev_join = nullptr);
+// K4 on wgmma (attention_wgmma.cu) for head dim 64, T <= 320: tmQKV is a map over the qkv buffer [rows, 3w] with
+// boxes of 64 rows x 64 columns (128B swizzle), rows >= B*T of it are never used unmasked.
+bool attention_wgmma_supported(int T, int heads, int w);
+int attention_wgmma(const CUtensorMap& tmQKV, const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int heads, int w,
+                    int causal, cudaStream_t st);
 // K8/K10/K11: pooled row (x[b*T + pool_index(b)]) -> LN -> @ proj [w, D] -> optional L2 normalise
 // -> fp16 or fp32.  pool_idx == nullptr pools token 0 (vision); else row pool_idx[b] (text EOT).
 int pool_ln_proj_norm(const __nv_bfloat16* x, int T, int w, const int* pool_idx, const float* gamma, const float* beta,

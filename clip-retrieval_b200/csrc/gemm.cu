@@ -1,6 +1,5 @@
-// Host side of the tcgen05 GEMM: tensor-map construction, launch, and the stand-alone C-ABI entry.
+// Host side of the wgmma GEMM: tensor-map construction, launch, and the stand-alone C-ABI entry.
 #include "gemm.cuh"
-#include "gemm2.cuh"
 #include <mutex>
 #include <cstdlib>
 #include <algorithm>
@@ -45,79 +44,22 @@ int make_tmap_2d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t row
   return B200_OK;
 }
 
-// 3-D tensor [n2, n1, n0] (16-bit elements, innermost n0 contiguous, row pitch ld_elems, sample pitch n1 * ld_elems),
-// boxes of 1 x box_rows x 64 elements with the 128-byte swizzle; rows >= n1 of a box are zero-filled.
-int make_tmap_3d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t n2, uint64_t n1, uint64_t n0, uint64_t ld_elems,
-                 uint32_t box_rows) {
-  encode_tiled_fn enc = get_encode();
-  B200_CHECK(enc != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
-  B200_CHECK(((uintptr_t)ptr & 15) == 0 && (ld_elems * 2) % 16 == 0, B200_ERR_INVALID,
-             "tensor map: base and row pitch must be 16-byte aligned (ptr=%p ld=%llu)", ptr, (unsigned long long)ld_elems);
-  B200_CHECK(box_rows >= 1 && box_rows <= 256 && n0 >= 64, B200_ERR_INVALID, "tensor map: bad 3-D box");
-  cuuint64_t dims[3] = {n0, n1, n2};
-  cuuint64_t strides[2] = {ld_elems * 2, n1 * ld_elems * 2};
-  cuuint32_t box[3] = {64, box_rows, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(out, dtype_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3,
-                   const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled (3-D) failed with %d", (int)r);
-  return B200_OK;
-}
-
-static bool g_pair_enabled = true;
-void gemm_set_pair_mode(bool on) { g_pair_enabled = on; }
-// pair kernel: results through shared memory + TMA stores (B200_GEMM_TMA_STORE=0/1; default in gemm_tma_store_default)
-static bool gemm_tma_store_default() {
-  const char* e = getenv("B200_GEMM_TMA_STORE");
-  return e ? atoi(e) != 0 : true;    // verified on B200: bit-identical to the register path, +20 % on the K=1024 shapes (profiles/r02d)
-}
-static bool g_tma_store = gemm_tma_store_default();
-void gemm_set_tma_store(bool on) { g_tma_store = on; }
-
-// Column-block choice; GEMM_MODE_PAIR (= 512) selects the CTA-pair kernel (256x256 tiles over two
-// SMs, B operand through the 128-row tensor map) for problems that fill the chip with such tiles.
 int gemm_pick_bn(int M, int N, int sms) {
-  const long pair_tiles = (long)((M + 255) / 256) * ((N + 255) / 256);
-  if (g_pair_enabled && pair_tiles >= 2 * (long)(sms / 2) && N >= 256) return GEMM_MODE_PAIR;
   const long mb = (M + GEMM_BM - 1) / GEMM_BM;
   const long tiles128 = mb * ((N + 127) / 128);
   if (tiles128 < sms && N >= 64) {
-    // serving shapes (a few row blocks): the GEMM is a weight read; spread it over as many SMs as there are tiles
     const long tiles64 = mb * ((N + 63) / 64);
     return tiles64 < sms ? 32 : 64;
   }
-  if (N % 256 != 0 && N % 128 == 0) return 128;
-  const long tiles256 = mb * ((N + 255) / 256);
-  if (tiles256 < sms && N > 128) return 128;  // small problems: more, narrower tiles
-  return 256;
+  return 128;
 }
-
-// TMA-store pair kernel with the epilogue flavour fixed at compile time (epi_pack8): activation | residual << 2
-typedef void (*pair_kernel_fn)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, int, int, int, GemmEpilogue);
-static pair_kernel_fn pair_spec_kernel(int spec) {
-  switch (spec) {
-    case 0: return gemm_bf16_tcgen05_pair_kernel<true, 0>;
-    case 1: return gemm_bf16_tcgen05_pair_kernel<true, 1>;
-    case 2: return gemm_bf16_tcgen05_pair_kernel<true, 2>;
-    case 4: return gemm_bf16_tcgen05_pair_kernel<true, 4>;
-    case 5: return gemm_bf16_tcgen05_pair_kernel<true, 5>;
-    case 6: return gemm_bf16_tcgen05_pair_kernel<true, 6>;
-    default: return nullptr;
-  }
-}
-static bool gemm_pair_spec_default() {
-  const char* e = getenv("B200_GEMM_SPEC");
-  return e ? atoi(e) != 0 : true;
-}
-static bool g_pair_spec = gemm_pair_spec_default();   // B200_GEMM_SPEC=0: the generic run-time epilogue (A/B, parity)
 
 template <int BN, int SPEC>
 static int launch_bn_spec(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, const GemmEpilogue& ep,
-                          int sms, cudaStream_t st) {
+                          cudaStream_t st) {
   using Cfg = GemmCfg<BN>;
   static std::atomic<unsigned long long> configured{0};  // bit per device: the attribute is per context
-  auto kern = gemm_bf16_tcgen05_kernel<BN, SPEC>;
+  auto kern = gemm_bf16_wgmma_kernel<BN, SPEC>;
   int dev = 0;
   B200_CUDA(cudaGetDevice(&dev));
   if (!(configured.load() >> (dev & 63) & 1ull)) {
@@ -125,35 +67,34 @@ static int launch_bn_spec(const CUtensorMap& tmA, const CUtensorMap& tmB, int M,
     configured.fetch_or(1ull << (dev & 63));
   }
   const long tiles = (long)((M + GEMM_BM - 1) / GEMM_BM) * ((N + BN - 1) / BN);
-  const int grid = (int)(tiles < sms ? tiles : sms);
-  kern<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(tmA, tmB, M, N, K, ep);
+  kern<<<(unsigned)tiles, GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(tmA, tmB, M, N, K, ep);
   B200_LAUNCH_OK();
   return B200_OK;
 }
 
-// single-CTA kernels: the epilogue flavour (activation | residual << 2) fixed at compile time unless the LayerNorm fold,
-// the row statistics or the transposed-V output are in use
+// the epilogue flavour (activation | residual << 2) fixed at compile time unless the LayerNorm fold or the row
+// statistics are in use
 template <int BN>
 static int launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, const GemmEpilogue& ep,
-                     int sms, cudaStream_t st) {
-  const bool plain = g_pair_spec && ep.ln_stats == nullptr && ep.stats_out == nullptr && ep.ln_c == nullptr && ep.vt == nullptr &&
+                     cudaStream_t st) {
+  const bool plain = ep.ln_stats == nullptr && ep.stats_out == nullptr && ep.ln_c == nullptr &&
                      ep.act >= 0 && ep.act <= 2;
   if (plain) {
     switch ((ep.act & 3) | (ep.residual ? 4 : 0)) {
-      case 0: return launch_bn_spec<BN, 0>(tmA, tmB, M, N, K, ep, sms, st);
-      case 1: return launch_bn_spec<BN, 1>(tmA, tmB, M, N, K, ep, sms, st);
-      case 2: return launch_bn_spec<BN, 2>(tmA, tmB, M, N, K, ep, sms, st);
-      case 4: return launch_bn_spec<BN, 4>(tmA, tmB, M, N, K, ep, sms, st);
-      case 5: return launch_bn_spec<BN, 5>(tmA, tmB, M, N, K, ep, sms, st);
-      case 6: return launch_bn_spec<BN, 6>(tmA, tmB, M, N, K, ep, sms, st);
+      case 0: return launch_bn_spec<BN, 0>(tmA, tmB, M, N, K, ep, st);
+      case 1: return launch_bn_spec<BN, 1>(tmA, tmB, M, N, K, ep, st);
+      case 2: return launch_bn_spec<BN, 2>(tmA, tmB, M, N, K, ep, st);
+      case 4: return launch_bn_spec<BN, 4>(tmA, tmB, M, N, K, ep, st);
+      case 5: return launch_bn_spec<BN, 5>(tmA, tmB, M, N, K, ep, st);
+      case 6: return launch_bn_spec<BN, 6>(tmA, tmB, M, N, K, ep, st);
       default: break;
     }
   }
-  return launch_bn_spec<BN, -1>(tmA, tmB, M, N, K, ep, sms, st);
+  return launch_bn_spec<BN, -1>(tmA, tmB, M, N, K, ep, st);
 }
 
 int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int M, int N, int K,
-                     const GemmEpilogue& ep, int sms, cudaStream_t st, const CUtensorMap* tmC, const CUtensorMap* tmR) {
+                     const GemmEpilogue& ep, cudaStream_t st) {
   B200_CHECK(M >= 1 && N >= 8 && K >= 8 && N % 8 == 0 && K % 8 == 0, B200_ERR_INVALID,
              "gemm: need M>=1 and N, K multiples of 8 (M=%d N=%d K=%d)", M, N, K);
   B200_CHECK(ep.out != nullptr && ep.out_ld % 8 == 0 && ((uintptr_t)ep.out & 15) == 0, B200_ERR_INVALID,
@@ -165,43 +106,9 @@ int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int
   B200_CHECK(ep.ln_stats == nullptr || (ep.ln_c != nullptr && ep.ln_w > 0 && ep.ln_w % 64 == 0), B200_ERR_INVALID,
              "gemm: folded LayerNorm needs c and a row width that is a multiple of 64 (ln_w=%d)", ep.ln_w);
   B200_CHECK(ep.ln_stats == nullptr || ep.ln_w <= 64 * LN_MAX_SLOTS, B200_ERR_UNSUPPORTED, "gemm: folded LayerNorm supports rows of at most %d columns", 64 * LN_MAX_SLOTS);
-  if (bn == GEMM_MODE_PAIR) {
-    static std::atomic<unsigned long long> configured{0};
-    int dev = 0;
-    B200_CUDA(cudaGetDevice(&dev));
-    if (!(configured.load() >> (dev & 63) & 1ull)) {
-      B200_CUDA(cudaFuncSetAttribute(gemm_bf16_tcgen05_pair_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     G2Cfg<false>::SMEM_BYTES));
-      B200_CUDA(cudaFuncSetAttribute(gemm_bf16_tcgen05_pair_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     G2Cfg<true>::SMEM_BYTES));
-      for (int spec = 0; spec < 8; spec++)
-        if (pair_spec_kernel(spec)) B200_CUDA(cudaFuncSetAttribute(pair_spec_kernel(spec), cudaFuncAttributeMaxDynamicSharedMemorySize, G2Cfg<true>::SMEM_BYTES));
-      configured.fetch_or(1ull << (dev & 63));
-    }
-    const long tiles = (long)((M + G2_BM - 1) / G2_BM) * ((N + G2_BN - 1) / G2_BN);
-    const int pairs = (int)std::min<long>(tiles, sms / 2);
-    // results through shared memory + TMA stores when the caller provides the output (and residual) tensor maps
-    const bool tma_st = g_tma_store && tmC != nullptr && ep.vt == nullptr && (ep.residual == nullptr || tmR != nullptr);
-    if (tma_st) {
-      GemmEpilogue e2 = ep;
-      e2.tma_store = 1;
-      // the epilogue flavour fixed at compile time whenever the LayerNorm fold / row statistics are off (always, by default)
-      const int spec = (ep.act & 3) | (ep.residual ? 4 : 0);
-      pair_kernel_fn kern = gemm_bf16_tcgen05_pair_kernel<true>;
-      if (g_pair_spec && ep.ln_stats == nullptr && ep.stats_out == nullptr && ep.ln_c == nullptr && ep.act >= 0 && ep.act <= 2 &&
-          pair_spec_kernel(spec) != nullptr)
-        kern = pair_spec_kernel(spec);
-      kern<<<2 * pairs, GEMM_THREADS, G2Cfg<true>::SMEM_BYTES, st>>>(tmA, tmB, *tmC, ep.residual ? *tmR : *tmC, M, N, K, e2);
-    } else {
-      gemm_bf16_tcgen05_pair_kernel<false><<<2 * pairs, GEMM_THREADS, G2Cfg<false>::SMEM_BYTES, st>>>(tmA, tmB, tmA, tmA, M, N, K, ep);
-    }
-    B200_LAUNCH_OK();
-    return B200_OK;
-  }
-  if (bn == 256) return launch_bn<256>(tmA, tmB, M, N, K, ep, sms, st);
-  if (bn == 128) return launch_bn<128>(tmA, tmB, M, N, K, ep, sms, st);
-  if (bn == 64) return launch_bn<64>(tmA, tmB, M, N, K, ep, sms, st);
-  if (bn == 32) return launch_bn<32>(tmA, tmB, M, N, K, ep, sms, st);
+  if (bn == 128) return launch_bn<128>(tmA, tmB, M, N, K, ep, st);
+  if (bn == 64) return launch_bn<64>(tmA, tmB, M, N, K, ep, st);
+  if (bn == 32) return launch_bn<32>(tmA, tmB, M, N, K, ep, st);
   set_error("gemm: unsupported column block %d", bn);
   return B200_ERR_INVALID;
 }
@@ -219,80 +126,13 @@ extern "C" int b200_gemm_bf16_device(const void* d_A, const void* d_W, const flo
   const int bn = gemm_pick_bn(M, N, sms);
   CUtensorMap tmA, tmB;
   B200_TRY(make_tmap_2d(&tmA, d_A, 1, (uint64_t)M, (uint64_t)K, (uint64_t)K, GEMM_BM, GEMM_BK));
-  // Timing experiments (library built with -DB200_TIMING_EXPERIMENTS only; ignored otherwise).
-  // B200_GEMM_HALFB=1 (timing experiment, wrong numbers): each CTA of a pair loads only 64 of its 128 B rows,
-  // i.e. the operand traffic a 2-pair cluster with a multicast B tile would have (48 instead of 64 B/clk/SM).
-#ifdef B200_TIMING_EXPERIMENTS
-  static const bool half_b = getenv("B200_GEMM_HALFB") != nullptr;
-#else
-  static const bool half_b = false;
-#endif
-  const bool exp_half = half_b && bn == GEMM_MODE_PAIR;
-  B200_TRY(make_tmap_2d(&tmB, d_W, 1, (uint64_t)N, (uint64_t)K, (uint64_t)K,
-                        bn == GEMM_MODE_PAIR ? (exp_half ? 64u : 128u) : (uint32_t)bn, GEMM_BK));
+  B200_TRY(make_tmap_2d(&tmB, d_W, 1, (uint64_t)N, (uint64_t)K, (uint64_t)K, (uint32_t)bn, GEMM_BK));
   GemmEpilogue ep;
-  if (exp_half) ep.exp_b_bytes = 64 * GEMM_BK * 2;
-#ifdef B200_TIMING_EXPERIMENTS
-  static const bool no_ldtm = getenv("B200_GEMM_NOLDTM") != nullptr;   // timing experiment: epilogue without tcgen05.ld
-#else
-  static const bool no_ldtm = false;
-#endif
-  if (no_ldtm && bn == GEMM_MODE_PAIR) ep.exp_skip_tmem = 1;
-#ifdef B200_TIMING_EXPERIMENTS
-  static const bool no_store = getenv("B200_GEMM_NOSTORE") != nullptr;   // timing experiment: epilogue without global stores
-  if (no_store) ep.exp_skip_store = 1;
-#endif
   ep.bias = d_bias;
   ep.residual = (const __nv_bfloat16*)d_residual;
   ep.res_ld = N;
   ep.out = (__nv_bfloat16*)d_C;
   ep.out_ld = N;
   ep.act = act;
-  // B200_GEMM_DEBUG=1: print where the MMA issuer of the pair kernel waits (bring-up aid; syncs the stream)
-  static const bool dbg_on = getenv("B200_GEMM_DEBUG") != nullptr;
-  if (dbg_on && bn == GEMM_MODE_PAIR) {
-    unsigned long long* d = nullptr;
-    B200_CUDA(cudaMalloc((void**)&d, 64));
-    B200_CUDA(cudaMemsetAsync(d, 0, 64, (cudaStream_t)stream));
-    ep.dbg = d;
-    CUtensorMap dC, dR;
-    const bool maps = N >= 64;
-    if (maps) {
-      B200_TRY(make_tmap_2d(&dC, d_C, 1, (uint64_t)M, (uint64_t)N, (uint64_t)N, 32, 64));
-      if (d_residual) B200_TRY(make_tmap_2d(&dR, d_residual, 1, (uint64_t)M, (uint64_t)N, (uint64_t)N, 32, 64));
-    }
-    int rc = gemm_bf16_launch(tmA, tmB, bn, M, N, K, ep, sms, (cudaStream_t)stream, maps ? &dC : nullptr,
-                              maps && d_residual ? &dR : nullptr);
-    unsigned long long h[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    B200_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-    B200_CUDA(cudaMemcpy(h, d, 64, cudaMemcpyDeviceToHost));
-    cudaFree(d);
-    const double pairs = sms / 2;
-    const double tiles_per_pair = ((M + 255) / 256) * (double)((N + 255) / 256) / pairs;
-    fprintf(stderr, "[gemm dbg] M=%d N=%d K=%d act=%d res=%d: issuer cycles/pair %.0f (%.0f per tile), wait operands %.1f%%, wait accumulator %.1f%%, producer wait-for-slot %.1f%%"
-                    " | epilogue warp 0 of the leader, cycles per tile: before the accumulator wait %.0f, waiting for the accumulator %.0f, accumulator -> TMEM released %.0f, released -> end of tile %.0f\n",
-            M, N, K, act, d_residual != nullptr, h[2] / pairs, h[2] / pairs / tiles_per_pair, 100.0 * h[0] / (double)h[2], 100.0 * h[1] / (double)h[2],
-            100.0 * h[3] / (double)h[2], h[4] / pairs / tiles_per_pair, h[5] / pairs / tiles_per_pair, h[6] / pairs / tiles_per_pair,
-            h[7] / pairs / tiles_per_pair);
-    return rc;
-  }
-  CUtensorMap tmC, tmR;
-  const bool st_maps = bn == GEMM_MODE_PAIR && N >= 64;
-  if (st_maps) {
-    B200_TRY(make_tmap_2d(&tmC, d_C, 1, (uint64_t)M, (uint64_t)N, (uint64_t)N, 32, 64));
-    if (d_residual) B200_TRY(make_tmap_2d(&tmR, d_residual, 1, (uint64_t)M, (uint64_t)N, (uint64_t)N, 32, 64));
-  }
-  return gemm_bf16_launch(tmA, tmB, bn, M, N, K, ep, sms, (cudaStream_t)stream, st_maps ? &tmC : nullptr,
-                          (st_maps && d_residual) ? &tmR : nullptr);
-}
-
-extern "C" int b200_gemm_set_tma_store(int on) {
-  b200::gemm_set_tma_store(on != 0);
-  b200::g_pair_spec = on != 2;   // 2: TMA stores with the generic run-time epilogue (parity / A/B against the specialised ones)
-  return B200_OK;
-}
-
-extern "C" int b200_gemm_set_pair_mode(int on) {
-  b200::gemm_set_pair_mode(on != 0);
-  return B200_OK;
+  return gemm_bf16_launch(tmA, tmB, bn, M, N, K, ep, (cudaStream_t)stream);
 }

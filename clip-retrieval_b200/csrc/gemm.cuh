@@ -1,17 +1,17 @@
-// tcgen05 GEMM core of the embed path (SURVEY.md §2.2 K1, K3, K5, K6, K7):
+// wgmma GEMM core of the embed path (SURVEY.md §2.2 K1, K3, K5, K6, K7):
 //   C[M,N] = epilogue(A[M,K] · W[N,K]^T)     A, W bf16 row-major (both "K-major"), fp32 accumulate.
 //
-// Persistent, warp-specialised, one CTA per SM:
+// One 128 x BN output tile per CTA, warp-specialised, two CTAs per SM:
 //   warp 8      TMA producer: cp.async.bulk.tensor 128x64 (A) and BNx64 (W) boxes, 128B swizzle,
-//               into a 4..6-stage shared-memory ring guarded by full/empty mbarriers;
-//   warp 9      allocates the 512 TMEM columns and issues tcgen05.mma (128 x BN x 16 per instruction,
-//               4 per stage); tcgen05.commit releases ring slots and publishes finished accumulators;
-//   warps 0..7  epilogue, two warps per TMEM lane quarter splitting the tile's columns: tcgen05.ld of
-//               the fp32 accumulator (each thread owns one output row), + bias, activation,
+//               into a 3..4-stage shared-memory ring guarded by full/empty mbarriers;
+//   warps 0..7  two consumer warpgroups, each issuing wgmma m64nBNk16 over its 64 rows of the tile
+//               (fp32 accumulator in registers); a ring slot is released once the wgmma group that
+//               read it has completed.  After the k-loop the accumulators go through shared memory
+//               (the drained ring) so that the epilogue sees one row per thread: + bias, activation,
 //               + residual, bf16 pack, 16-byte global stores.
-// Two accumulator stages (2 x BN columns of TMEM) let the epilogue of tile i overlap the main loop
-// of tile i+1.  Tiles are walked in groups of 16 row-blocks x all column-blocks so the activation
-// rows of a group stay in L2 while the weights (a few MB) are re-read from L2, not HBM.
+// Two CTAs per SM let the epilogue of one tile overlap the k-loop of the other.  Tiles are numbered
+// in groups of 16 row-blocks x all column-blocks so the activation rows of a group stay in L2 while
+// the weights (a few MB) are re-read from L2, not HBM.
 // Roofline: tensor pipe; 2*M*N*K flops per launch.
 #pragma once
 #include "common.cuh"
@@ -21,17 +21,12 @@ namespace b200 {
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;
-constexpr int GEMM_UMMA_K = 16;
-constexpr int GEMM_THREADS = 320;  // warps 0..7 epilogue (two per SM sub-partition), warp 8 TMA, warp 9 MMA
+constexpr int GEMM_MMA_K = 16;
+constexpr int GEMM_THREADS = 288;  // warps 0..7: two consumer warpgroups (64 rows each), warp 8: TMA producer
 constexpr int GEMM_GROUP_M = 16;
-// Warp roles.  The two single-thread roles sit on the HIGHEST warp ids: the sub-partition arbiter
-// favours higher warp ids, and an MMA issuer starved by busy epilogue warps shows up as tensor-pipe
-// bubbles (80% tensor-active at K=1024 vs 95% at K=4096 in profiles/r01c).
-constexpr int GEMM_WARP_TMA = 8;   // warps 0..7: epilogue
-constexpr int GEMM_WARP_MMA = 9;
+constexpr int GEMM_WARP_TMA = 8;
 
 enum { ACT_NONE = 0, ACT_QUICK_GELU = 1, ACT_GELU = 2 };
-constexpr int GEMM_MODE_PAIR = 512;  // gemm_pick_bn result selecting the cta_group::2 kernel (gemm2.cuh)
 
 struct GemmEpilogue {
   const float* bias = nullptr;              // [N] fp32 or null
@@ -43,7 +38,6 @@ struct GemmEpilogue {
   int64_t out_ld = 0;
   int out_group = 0;                        // > 0: out row = (row / g) * (g + 1) + 1 + row % g  (cls slot)
   int act = ACT_NONE;
-  int tma_store = 0;                        // pair kernel: results leave through shared memory and TMA stores (gemm2.cuh)
   // LayerNorm folded into this GEMM (K5/K6 of SURVEY §2.2 without a separate normalisation pass): A is the RAW
   // residual stream x and the weights carry gamma (W'[n,k] = W[n,k] * gamma[k]), so
   //   LN(x) W^T + b = rstd * (x W'^T - mean * c) + d,   c[n] = sum_k W'[n,k],  d[n] = sum_k beta[k] W[n,k] + b[n].
@@ -55,28 +49,16 @@ struct GemmEpilogue {
   // Row statistics of what this epilogue stores (bf16-rounded), one (mean, M2) record per 64 output columns:
   // stats_out[row * (N / 64) + slot].  Set on the GEMMs that write the residual stream.
   float2* stats_out = nullptr;
-  // Optional transposed store of the V third of a QKV projection (columns >= vt_col0): element
-  // (row = b*T + t, col = vt_col0 + h*hd + dd) goes to vt[((b*heads + h)*hd + dd) * vt_Tp + t], i.e. V^T
-  // per (sample, head) with keys contiguous — the K-major B operand of the P.V MMA (attention_tc.cu).
-  unsigned long long* dbg = nullptr;   // optional (8 counters): [4..7] epilogue warp 0 per-tile phases; [0] cycles the MMA issuer waited for operands, [1] for a free
-                                       // accumulator, [2] total issuer cycles, [3] producer waits for a free slot (pair kernel)
-  int exp_b_bytes = 0;                 // timing experiment only (B200_GEMM_HALFB): bytes of B each CTA really loads per stage
-  int exp_skip_tmem = 0;               // timing experiment only (B200_GEMM_NOLDTM): the epilogue does not read the accumulator
-  int exp_skip_store = 0;              // timing experiment only (B200_GEMM_NOSTORE): results are computed but not stored
-  __nv_bfloat16* vt = nullptr;
-  int vt_col0 = 0, vt_T = 1, vt_Tp = 0, vt_hd = 64, vt_heads = 1;
 };
 
 // Per-row constants of the epilogue, computed once per tile.
 struct EpiRow {
   __nv_bfloat16* out_ptr;
   const __nv_bfloat16* res_ptr;
-  __nv_bfloat16* vt_ptr;   // vt + (b*heads*hd) * Tp + t   (add (h*hd + dd) * Tp)
   float ln_a, ln_b;        // folded LayerNorm: value = acc * ln_a + (ln_b * c[col] + d[col]);  (1, 0) when off
 };
 // (mean, rstd) of a row from its 64-column slot records (Chan's combination of equal-sized groups).  Every record
-// load is issued before the first is used: a loop that consumed them one by one paid the L2 latency `slots` times
-// per tile and made the LN-folded GEMMs epilogue-bound (qkv 39.8 -> 61.0 ms, fc 52.2 -> 92.9 ms, profiles/r02a).
+// load is issued before the first is used: consuming them one by one pays the L2 latency `slots` times per row.
 constexpr int LN_MAX_SLOTS = 24;   // row width <= 1536
 __device__ __forceinline__ void ln_row_coeffs(const float2* __restrict__ rec, int slots, int w, float& a, float& b) {
   float2 v[LN_MAX_SLOTS];
@@ -104,29 +86,25 @@ __device__ __forceinline__ EpiRow epi_row(const GemmEpilogue& ep, int row, int n
   if (ep.res_row_mod > 0) res_row = ep.res_row_off + row % ep.res_row_mod;
   r.out_ptr = ep.out + out_row * ep.out_ld + n0;
   r.res_ptr = ep.residual ? ep.residual + res_row * ep.res_ld + n0 : nullptr;
-  r.vt_ptr = nullptr;
   r.ln_a = 1.0f;
   r.ln_b = 0.0f;
-  if (ep.vt) {
-    const int b = row / ep.vt_T, t = row - b * ep.vt_T;
-    r.vt_ptr = ep.vt + (int64_t)b * ep.vt_heads * ep.vt_hd * ep.vt_Tp + t;
-  }
   return r;
 }
 
 template <int BN>
 struct GemmCfg {
-  // ring depth: the narrow tiles are latency-bound (a CTA's k-loop advances one k-block per TMA round trip divided
-  // by the stages in flight: 278 ns per k-block with 6 stages at BN = 32, profiles/r02b_serve_launches.csv), and
-  // their stages are small — so they get the deepest rings that fit
-  static constexpr int STAGES = BN == 256 ? 4 : (BN == 128 ? 6 : (BN == 64 ? 8 : 10));
+  static_assert(BN == 32 || BN == 64 || BN == 128, "tile widths: 32, 64, 128");
+  // narrow tiles (BN = 64 / 32) exist for the serving shapes: with M <= 128 rows a GEMM has N / BN tiles in total, and
+  // the weight read (the whole cost at batch 1) is spread over that many SMs.  The ring stays under ~100 KB so that two
+  // CTAs share an SM.
+  static constexpr int STAGES = BN == 128 ? 3 : 4;
   static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;
   static constexpr int B_BYTES = BN * GEMM_BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * BN * 4 + 256 + 1024;  // ring + bias + LN c + barriers + align slack
-  static constexpr int TMEM_COLS = 2 * BN;                                         // 512, 256, 128 or 64 (power of two >= 32)
-  // narrow tiles (BN = 64 / 32) exist for the serving shapes: with M <= 128 rows a GEMM has N / BN tiles in total, and
-  // the weight read (the whole cost at batch 1) is spread over that many SMs — 6 SMs at BN = 128 for N = 768
+  static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
+  static constexpr int STG_LD = BN + 4;   // fp32 staging row pitch (floats): conflict-free 16-byte row reads
+  static_assert(GEMM_BM * STG_LD * 4 <= RING_BYTES, "the accumulator staging tile reuses the ring");
+  static constexpr int SMEM_BYTES = RING_BYTES + 2 * BN * 4 + 256 + 1024;  // ring + bias + LN c + barriers + align slack
 };
 
 __device__ __forceinline__ void gemm_tile_coords(int tile, int mb, int nb, int& m_blk, int& n_blk) {
@@ -161,11 +139,13 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
 }
 
 // bias + activation + residual + bf16 store of 8 consecutive columns (col = offset inside the tile)
-// `rr` = the residual's 8 values, prefetched before the accumulator wait (its HBM latency would
-// otherwise sit in the middle of the epilogue: 57% of the stall samples in profiles/r01c).
+// `rr` = the residual's 8 values, loaded before the accumulator is read so that their HBM latency does not sit in
+// the middle of the epilogue.
 // s_bias = bias (or the folded LayerNorm's d), s_c = the folded LayerNorm's c (read only when ep.ln_stats is set).
 // st_k / st_s / st_q: running shifted sums of the stored values for the row statistics (ep.stats_out).
-// SPEC: see epi_pack8 below (-1 = every feature decided at run time; 0..7 = activation | residual << 2 at compile time).
+// SPEC: -1 = every feature decided at run time; 0..7 = activation | residual << 2 fixed at compile time (no LayerNorm
+// fold, no row statistics): the generic flavour carries a run-time activation switch around an inlined
+// erff for every element plus the fold / statistics paths.
 template <int SPEC>
 __device__ __forceinline__ void epi_store8(const GemmEpilogue& ep, const EpiRow& er, const uint32_t* r8,
                                            const float* s_bias, const float* s_c, int col, int n0, const uint4& rr,
@@ -186,26 +166,15 @@ __device__ __forceinline__ void epi_store8(const GemmEpilogue& ep, const EpiRow&
   if (has_res) {
     const float2 a = unpack_bf16x2(rr.x), b = unpack_bf16x2(rr.y), cc = unpack_bf16x2(rr.z), dd = unpack_bf16x2(rr.w);
     // __fadd_rn: never contracted with the activation's last multiply into an FMA — every epilogue flavour (run-time or
-    // compile-time, pair or single CTA) rounds the same way and stays bit-identical to the others
+    // compile-time) rounds the same way and stays bit-identical to the others
     v[0] = __fadd_rn(v[0], a.x); v[1] = __fadd_rn(v[1], a.y); v[2] = __fadd_rn(v[2], b.x); v[3] = __fadd_rn(v[3], b.y);
     v[4] = __fadd_rn(v[4], cc.x); v[5] = __fadd_rn(v[5], cc.y); v[6] = __fadd_rn(v[6], dd.x); v[7] = __fadd_rn(v[7], dd.y);
-  }
-  if (SPEC < 0 && er.vt_ptr != nullptr && n0 + col >= ep.vt_col0) {
-    __nv_bfloat16* p = er.vt_ptr + (int64_t)(n0 + col - ep.vt_col0) * ep.vt_Tp;
-#pragma unroll
-    for (int j = 0; j < 8; j++) p[(int64_t)j * ep.vt_Tp] = __float2bfloat16_rn(v[j]);
-    return;
   }
   uint4 o;
   o.x = pack_bf16x2(v[0], v[1]);
   o.y = pack_bf16x2(v[2], v[3]);
   o.z = pack_bf16x2(v[4], v[5]);
   o.w = pack_bf16x2(v[6], v[7]);
-#ifdef B200_TIMING_EXPERIMENTS
-  if (ep.exp_skip_store) {
-    if (o.x == 0x7fc07fc1u && o.w == 0x12345678u) *reinterpret_cast<uint4*>(er.out_ptr + col) = o;   // never true: keeps the math alive
-  } else
-#endif
   *reinterpret_cast<uint4*>(er.out_ptr + col) = o;
   if (use_stats) {
     // statistics of the values as stored (bf16), shifted by the slot's first value to keep the sums small
@@ -217,53 +186,6 @@ __device__ __forceinline__ void epi_store8(const GemmEpilogue& ep, const EpiRow&
       st_q = fmaf(e[j], e[j], st_q);
     }
   }
-}
-
-// The eight finished values of columns col..col+7 of this thread's row (bias / folded LayerNorm, activation, residual
-// given as 8 packed bf16 in `rr`), packed to bf16; optional row-statistics accumulation as in epi_store8.
-// SPEC >= 0 fixes the epilogue flavour at compile time (bits 0-1 activation, bit 2 residual; no LayerNorm fold, no row
-// statistics): the generic flavour (SPEC = -1) carries a run-time activation switch — two or three branches around
-// an inlined erff for EVERY element — plus the fold / statistics paths, 12 300 SASS instructions in the pair kernel, and
-// its epilogue took ~11 000 cycles per 128x256 tile against 8 192 for the MMAs of a K = 1024 tile (B200_GEMM_DEBUG,
-// profiles/r02o_gemm_epilogue_phases.txt): the K = 1024 GEMMs were bound by instruction fetch and branches.
-template <int SPEC>
-__device__ __forceinline__ uint4 epi_pack8(const GemmEpilogue& ep, const EpiRow& er, const uint32_t* r8, const float* s_bias,
-                                           const float* s_c, int col, bool has_res, const uint4& rr, float st_k, float& st_s,
-                                           float& st_q) {
-  const int act = SPEC >= 0 ? (SPEC & 3) : ep.act;
-  const bool use_ln = SPEC < 0 && ep.ln_stats != nullptr;
-  const bool use_stats = SPEC < 0 && ep.stats_out != nullptr;
-  float v[8];
-  if (use_ln) {
-#pragma unroll
-    for (int j = 0; j < 8; j++)
-      v[j] = act_apply(fmaf(__uint_as_float(r8[j]), er.ln_a, fmaf(er.ln_b, s_c[col + j], s_bias[col + j])), act);
-  } else {
-#pragma unroll
-    for (int j = 0; j < 8; j++) v[j] = act_apply(__uint_as_float(r8[j]) + s_bias[col + j], act);
-  }
-  if (has_res) {
-    const float2 a = unpack_bf16x2(rr.x), b = unpack_bf16x2(rr.y), cc = unpack_bf16x2(rr.z), dd = unpack_bf16x2(rr.w);
-    // __fadd_rn: never contracted with the activation's last multiply into an FMA — every epilogue flavour (run-time or
-    // compile-time, pair or single CTA) rounds the same way and stays bit-identical to the others
-    v[0] = __fadd_rn(v[0], a.x); v[1] = __fadd_rn(v[1], a.y); v[2] = __fadd_rn(v[2], b.x); v[3] = __fadd_rn(v[3], b.y);
-    v[4] = __fadd_rn(v[4], cc.x); v[5] = __fadd_rn(v[5], cc.y); v[6] = __fadd_rn(v[6], dd.x); v[7] = __fadd_rn(v[7], dd.y);
-  }
-  uint4 o;
-  o.x = pack_bf16x2(v[0], v[1]);
-  o.y = pack_bf16x2(v[2], v[3]);
-  o.z = pack_bf16x2(v[4], v[5]);
-  o.w = pack_bf16x2(v[6], v[7]);
-  if (use_stats) {
-    const float2 f0 = unpack_bf16x2(o.x), f1 = unpack_bf16x2(o.y), f2 = unpack_bf16x2(o.z), f3 = unpack_bf16x2(o.w);
-    const float e[8] = {f0.x - st_k, f0.y - st_k, f1.x - st_k, f1.y - st_k, f2.x - st_k, f2.y - st_k, f3.x - st_k, f3.y - st_k};
-#pragma unroll
-    for (int j = 0; j < 8; j++) {
-      st_s += e[j];
-      st_q = fmaf(e[j], e[j], st_q);
-    }
-  }
-  return o;
 }
 
 // One 32-column chunk `c` of the tile for this thread's row: the four 8-column groups, and (stats_out) the
@@ -297,9 +219,9 @@ __device__ __forceinline__ void epi_chunk(const GemmEpilogue& ep, const EpiRow& 
 }
 
 template <int BN, int SPEC = -1>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N,
-                         int K, GemmEpilogue ep) {
+__global__ void __launch_bounds__(GEMM_THREADS, 2)
+gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N,
+                       int K, GemmEpilogue ep) {
   using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
@@ -307,181 +229,126 @@ gemm_bf16_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_c
   uint8_t* base = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
   uint8_t* sA = base;
   uint8_t* sB = base + STAGES * Cfg::A_BYTES;
-  float* s_bias = reinterpret_cast<float*>(base + STAGES * Cfg::STAGE_BYTES);
+  float* s_bias = reinterpret_cast<float*>(base + Cfg::RING_BYTES);
   float* s_c = s_bias + BN;
   uint64_t* full = reinterpret_cast<uint64_t*>(s_c + BN);
   uint64_t* empty = full + STAGES;
-  uint64_t* tfull = empty + STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(tempty + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int mb = (M + GEMM_BM - 1) / GEMM_BM, nb = (N + BN - 1) / BN, kb = (K + GEMM_BK - 1) / GEMM_BK;
-  const int tiles = mb * nb;
+  int m_blk, n_blk;
+  gemm_tile_coords(blockIdx.x, mb, nb, m_blk, n_blk);
+  const int n0 = n_blk * BN;
 
-  if (warp == GEMM_WARP_TMA && lane == 0) {
-    ptx::prefetch_tensormap(&tmA);
-    ptx::prefetch_tensormap(&tmB);
-  }
-  if (warp == GEMM_WARP_MMA) {
-    if (lane == 0) {
-      for (int s = 0; s < STAGES; s++) {
-        ptx::mbar_init(&full[s], 1);
-        ptx::mbar_init(&empty[s], 1);
-      }
-      for (int a = 0; a < 2; a++) {
-        ptx::mbar_init(&tfull[a], 1);
-        ptx::mbar_init(&tempty[a], 8);  // one arrive per epilogue warp
-      }
-      ptx::fence_barrier_init();
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; s++) {
+      ptx::mbar_init(&full[s], 1);
+      ptx::mbar_init(&empty[s], 8);  // one arrive per consumer warp
     }
-    __syncwarp();
-    ptx::tmem_alloc(s_tmem, Cfg::TMEM_COLS);
-    ptx::tmem_relinquish();
+    ptx::fence_barrier_init();
   }
-  ptx::tc_fence_before();
+  for (int j = threadIdx.x; j < BN; j += GEMM_THREADS) {
+    s_bias[j] = (ep.bias != nullptr && n0 + j < N) ? ep.bias[n0 + j] : 0.0f;
+    if (SPEC < 0) s_c[j] = (ep.ln_c != nullptr && n0 + j < N) ? ep.ln_c[n0 + j] : 0.0f;
+  }
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *s_tmem;
 
   if (warp == GEMM_WARP_TMA) {
     // ---------------- TMA producer ----------------
     if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-        int m_blk, n_blk;
-        gemm_tile_coords(tile, mb, nb, m_blk, n_blk);
-        for (int kbi = 0; kbi < kb; kbi++) {
-          ptx::mbar_wait(&empty[stage], phase ^ 1);
-          ptx::mbar_arrive_expect_tx(&full[stage], Cfg::STAGE_BYTES);
-          ptx::tma_load_2d(sA + stage * Cfg::A_BYTES, &tmA, &full[stage], kbi * GEMM_BK, m_blk * GEMM_BM);
-          ptx::tma_load_2d(sB + stage * Cfg::B_BYTES, &tmB, &full[stage], kbi * GEMM_BK, n_blk * BN);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
+      ptx::prefetch_tensormap(&tmA);
+      ptx::prefetch_tensormap(&tmB);
+      for (int kbi = 0; kbi < kb; kbi++) {
+        const int stage = kbi % STAGES;
+        if (kbi >= STAGES) ptx::mbar_wait(&empty[stage], ((kbi / STAGES) - 1) & 1);
+        ptx::mbar_arrive_expect_tx(&full[stage], Cfg::STAGE_BYTES);
+        ptx::tma_load_2d(sA + stage * Cfg::A_BYTES, &tmA, &full[stage], kbi * GEMM_BK, m_blk * GEMM_BM);
+        ptx::tma_load_2d(sB + stage * Cfg::B_BYTES, &tmB, &full[stage], kbi * GEMM_BK, n0);
       }
     }
-    __syncwarp();
-  } else if (warp == GEMM_WARP_MMA) {
-    // ---------------- MMA issuer ----------------
-    if (lane == 0) {
-      constexpr uint32_t idesc = ptx::umma_idesc_f16(GEMM_BM, BN, true);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-        ptx::mbar_wait(&tempty[acc], acc_phase ^ 1);
-        ptx::tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * BN;
-        for (int kbi = 0; kbi < kb; kbi++) {
-          ptx::mbar_wait(&full[stage], phase);
-          ptx::tc_fence_after();
-          const uint64_t da = ptx::umma_desc_k_sw128(ptx::smem_u32(sA + stage * Cfg::A_BYTES));
-          const uint64_t db = ptx::umma_desc_k_sw128(ptx::smem_u32(sB + stage * Cfg::B_BYTES));
-#pragma unroll
-          for (int k = 0; k < GEMM_BK / GEMM_UMMA_K; k++) {
-            // advance 16 elements (32 bytes) along K inside the 128-byte swizzled row
-            ptx::umma_f16(tmem_d, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (kbi | k) != 0 ? 1u : 0u);
-          }
-          ptx::umma_commit(&empty[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        ptx::umma_commit(&tfull[acc]);
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
-    __syncwarp();
-  } else {
-    // ---------------- epilogue (warps 0..7) ----------------
-    const int q = warp & 3;                 // TMEM lane quarter this warp may read
-    const int et = warp * 32 + lane;  // 0..255 (epilogue warps are warps 0..7)
-    const int half = warp >> 2;        // which half of the tile columns this warp drains
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-      int m_blk, n_blk;
-      gemm_tile_coords(tile, mb, nb, m_blk, n_blk);
-      const int n0 = n_blk * BN;
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-#pragma unroll
-      for (int j = et; j < BN; j += 256) {
-        s_bias[j] = (ep.bias != nullptr && n0 + j < N) ? ep.bias[n0 + j] : 0.0f;
-        if (SPEC < 0) s_c[j] = (ep.ln_c != nullptr && n0 + j < N) ? ep.ln_c[n0 + j] : 0.0f;
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-
-      const int row = m_blk * GEMM_BM + q * 32 + lane;
-      const bool row_ok = row < M;
-      EpiRow er = epi_row(ep, row, n0);
-      if (SPEC < 0 && ep.ln_stats != nullptr && row_ok) ln_row_coeffs(ep.ln_stats + (int64_t)row * (ep.ln_w >> 6), ep.ln_w >> 6, ep.ln_w, er.ln_a, er.ln_b);
-      float st_k = 0.f, st_s = 0.f, st_q = 0.f;
-      constexpr int CPW = BN >= 64 ? BN / 64 : 1;   // 32-column chunks per epilogue warp
-      if (half * CPW * 32 >= BN) {
-        // BN = 32: the second warp of each lane quarter has no columns; it only takes part in the hand-shake
-        ptx::mbar_wait(&tfull[acc], acc_phase);
-        ptx::tc_fence_after();
-        ptx::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&tempty[acc]);
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-        continue;
-      }
-      uint4 res[CPW][4];
-#pragma unroll
-      for (int ci = 0; ci < CPW; ci++) {
-#pragma unroll
-        for (int g = 0; g < 4; g++) {
-          const int col = (half * CPW + ci) * 32 + g * 8;
-          const bool want = SPEC >= 0 ? ((SPEC >> 2) & 1) != 0 : er.res_ptr != nullptr;
-          res[ci][g] = (row_ok && want && n0 + col < N)
-                           ? *reinterpret_cast<const uint4*>(er.res_ptr + col) : make_uint4(0u, 0u, 0u, 0u);
-        }
-      }
-
-      ptx::mbar_wait(&tfull[acc], acc_phase);
-      ptx::tc_fence_after();
-
-#pragma unroll
-      for (int ci = 0; ci < CPW; ci++) {
-        const int c = half * CPW + ci;
-        uint32_t r[32];
-        ptx::tmem_ld_32x32b_x32(tmem_base + acc * BN + c * 32 + ((uint32_t)(q * 32) << 16), r);
-        ptx::tmem_ld_wait();
-        if (ci == CPW - 1) {
-          // accumulator fully drained into registers: hand the TMEM stage back to the MMA warp
-          ptx::tc_fence_before();
-          __syncwarp();
-          if (lane == 0) ptx::mbar_arrive(&tempty[acc]);
-        }
-        if (row_ok) epi_chunk<SPEC>(ep, er, r, s_bias, s_c, c, n0, N, row, res[ci], st_k, st_s, st_q);
-      }
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
+    return;
   }
 
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == GEMM_WARP_MMA) ptx::tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+  // ---------------- consumers (warps 0..7): wgmma main loop ----------------
+  const int wg = warp >> 2;   // rows wg*64 .. wg*64+63 of the tile
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; i++) acc[i] = 0.f;
+  for (int kbi = 0; kbi < kb; kbi++) {
+    const int stage = kbi % STAGES;
+    ptx::mbar_wait(&full[stage], (kbi / STAGES) & 1);
+    ptx::wgmma_fence();
+    const uint64_t da = ptx::wgmma_desc_k_sw128(ptx::smem_u32(sA + stage * Cfg::A_BYTES + wg * 64 * 128));
+    const uint64_t db = ptx::wgmma_desc_k_sw128(ptx::smem_u32(sB + stage * Cfg::B_BYTES));
+#pragma unroll
+    for (int k = 0; k < GEMM_BK / GEMM_MMA_K; k++)
+      ptx::wgmma_bf16<BN>(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kbi | k) != 0 ? 1u : 0u);
+    ptx::wgmma_commit();
+    // the group of the previous k-block has completed: its ring slot may be refilled
+    ptx::wgmma_wait<1>();
+    if (kbi > 0 && lane == 0) ptx::mbar_arrive(&empty[(kbi - 1) % STAGES]);
+  }
+  ptx::wgmma_wait<0>();
+  ptx::fence_regs(acc);
+
+  // ---------------- epilogue ----------------
+  // every load has landed and every wgmma has read its operands: the ring becomes the fp32 staging tile
+  float* stg = reinterpret_cast<float*>(base);
+  ptx::fence_proxy_async();
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  {
+    const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < BN / 8; j++) {
+      *reinterpret_cast<float2*>(stg + r * Cfg::STG_LD + 8 * j + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(stg + (r + 8) * Cfg::STG_LD + 8 * j + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
+  }
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+
+  const int q = warp & 3;            // 32-row quarter of the tile
+  const int half = warp >> 2;        // which half of the tile columns this warp drains
+  const int lrow = q * 32 + lane;
+  const int row = m_blk * GEMM_BM + lrow;
+  const bool row_ok = row < M;
+  constexpr int CPW = BN >= 64 ? BN / 64 : 1;   // 32-column chunks per epilogue warp
+  if (!row_ok || half * CPW * 32 >= BN) return;  // BN = 32: the second warp of each quarter has no columns
+  EpiRow er = epi_row(ep, row, n0);
+  if (SPEC < 0 && ep.ln_stats != nullptr) ln_row_coeffs(ep.ln_stats + (int64_t)row * (ep.ln_w >> 6), ep.ln_w >> 6, ep.ln_w, er.ln_a, er.ln_b);
+  float st_k = 0.f, st_s = 0.f, st_q = 0.f;
+  uint4 res[CPW][4];
+#pragma unroll
+  for (int ci = 0; ci < CPW; ci++) {
+#pragma unroll
+    for (int g = 0; g < 4; g++) {
+      const int col = (half * CPW + ci) * 32 + g * 8;
+      const bool want = SPEC >= 0 ? ((SPEC >> 2) & 1) != 0 : er.res_ptr != nullptr;
+      res[ci][g] = (want && n0 + col < N) ? *reinterpret_cast<const uint4*>(er.res_ptr + col) : make_uint4(0u, 0u, 0u, 0u);
+    }
+  }
+#pragma unroll
+  for (int ci = 0; ci < CPW; ci++) {
+    const int c = half * CPW + ci;
+    uint32_t r[32];
+    const float4* src4 = reinterpret_cast<const float4*>(stg + lrow * Cfg::STG_LD + c * 32);
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+      const float4 v = src4[i];
+      r[4 * i] = __float_as_uint(v.x); r[4 * i + 1] = __float_as_uint(v.y);
+      r[4 * i + 2] = __float_as_uint(v.z); r[4 * i + 3] = __float_as_uint(v.w);
+    }
+    epi_chunk<SPEC>(ep, er, r, s_bias, s_c, c, n0, N, row, res[ci], st_k, st_s, st_q);
+  }
 }
 
 // host side (gemm.cu)
 int make_tmap_2d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t rows, uint64_t cols, uint64_t ld_elems,
                  uint32_t box_rows, uint32_t box_cols);
-int make_tmap_3d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t n2, uint64_t n1, uint64_t n0, uint64_t ld_elems,
-                 uint32_t box_rows);
-// tmC / tmR (optional): maps over the output / residual matrices with boxes of 32 rows x 64 columns; when given, the
-// pair kernel stores through shared memory + TMA (and prefetches the residual tile the same way).
+// tmB must have boxes of bn rows x 64 columns.
 int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int M, int N, int K,
-                     const GemmEpilogue& ep, int sms, cudaStream_t st, const CUtensorMap* tmC = nullptr,
-                     const CUtensorMap* tmR = nullptr);
-// Pick the column-block width for a GEMM with N output columns (256, or 128 when N % 256 != 0 or the
-// grid would be under-filled).
+                     const GemmEpilogue& ep, cudaStream_t st);
+// Pick the column-block width for a GEMM with N output columns (128, or 64 / 32 when the grid would be
+// under-filled).
 int gemm_pick_bn(int M, int N, int sms);
-void gemm_set_pair_mode(bool on);
-void gemm_set_tma_store(bool on);
 
 }  // namespace b200

@@ -8,14 +8,14 @@
 struct b200_index {
   int d = 0;
   int device = 0;
-  int sms = 148;
+  int sms = 132;
   int64_t ntotal = 0;
   int64_t capacity = 0;     // rows allocated in `rows`
   bool reserved = false;
   __half* rows = nullptr;   // flat: insertion order.  IVF: list order after finalize.
   int64_t id_base = 0;
   bool use_staged = true;   // FMA scan through the cp.async.bulk shared-memory ring (knn_scan.cu)
-  bool use_mma = true;      // batched queries go through the tcgen05 scan (knn_mma.cu)
+  bool use_mma = true;      // batched queries go through the wgmma scan (knn_mma.cu)
   bool use_hi_only = true;  // > 128 queries: approximate hi-only pass + exact re-score + proof (knn_mma.cu)
   int last_hi_only_fallbacks = 0;   // queries of the last batched search whose proof failed (re-run split)
   const __half* norm_rows[2] = {nullptr, nullptr};   // cache of max_row ||x||^2 per scanned table

@@ -4,28 +4,27 @@
 //
 //   S[row, q] = sum_j X[row, j] * Q[q, j]          X fp16 rows (HBM), Q fp32 queries
 //
-// tcgen05 kind::f16 needs fp16 operands, and rounding the query to fp16 (2^-11 relative) would swap
+// wgmma with fp16 operands needs the query in fp16, and rounding it (2^-11 relative) would swap
 // near-tied neighbours, so each fp32 query is split into two fp16 rows: hi = fp16(q) and
 // lo = fp16((q - hi) * 2^11); the products with fp16 rows are exact in fp32, the two partial sums
-// are accumulated in separate TMEM columns and recombined as s = s_hi + s_lo * 2^-11 in the
+// are accumulated in separate accumulator columns and recombined as s = s_hi + s_lo * 2^-11 in the
 // epilogue (22 significant bits of the query: below the fp32 accumulation noise already accepted
 // for the FMA kernel).
 //
-// Structure = the pair GEMM core (gemm2.cuh): warp 0 TMA producer (X box 128x64, half of the Q' box
-// per CTA, 128B swizzle, 6-stage ring), warp 1 MMA issuer (cta_group::2, 256x256x16, two TMEM
-// accumulator stages), warps 2..9 epilogue (two per TMEM lane quarter, alternate 32-column chunks).
-// A CTA pair owns whole 256-row tiles (tile = pair + i*npairs) and walks all query groups of a
-// tile back to back, so the X tile is re-read from L2, not HBM.  Epilogue: thread = row; a score
-// that reaches the query's current threshold is appended to the (CTA, query) candidate buffer
-// (atomic counter in shared memory, buffer in global/L2); buffers are compacted to their k best by
-// the epilogue warps between tiles, which raises the threshold.  A final select merges the CTAs.
-// Thresholds are warmed up by two sampling passes (one row tile per CTA pair, then every 32nd row
+// Structure = the GEMM core (gemm.cuh): warp 4 TMA producer (X box 64x64, Q' box 256x64, 128B
+// swizzle, 5-stage ring), warps 0..3 one consumer warpgroup issuing wgmma m64n256k16 over the 64
+// rows of the tile with the accumulator in registers (128 fp32 per thread: with five warps per CTA no
+// SM sub-partition holds more than two of them, which leaves room for it).  A CTA owns whole 64-row tiles
+// (tile = cta + i*ctas) and walks all query groups of a tile back to back, so the X tile is re-read
+// from L2, not HBM.  Epilogue, in the accumulator's own register layout: a score that reaches the
+// query's current threshold is appended to the (CTA, query) candidate buffer (atomic counter in
+// shared memory, buffer in global/L2); buffers are compacted to their k best by the consumer warps
+// between groups, which raises the threshold.  A final select merges the CTAs.
+// Thresholds are warmed up by two sampling passes (one row tile per CTA, then every 32nd row
 // tile: the k-th best score of a subset is a valid lower bound for the full set), so the full pass
 // almost never takes the append path.
 // Roofline: tensor pipe (4*N*d*nq flops with the split) for large nq, HBM (N*d*2 bytes per 128
-// queries) below ~64 queries per pass.  ncu (profiles/r01f_final_summary.txt): one 128-query group
-// over 20M x 768 rows takes 4.64 ms with the tensor pipe 98 % active AND 30.7 GB read from DRAM
-// (6.6 TB/s) — both roofs at once; every further group costs the same tensor time again.
+// queries) below ~64 queries per pass; every further 128-query group costs the same tensor time again.
 //
 // Above 128 queries the split is therefore the cost, and the kernel has a second mode (HILO =
 // false): only the hi halves are multiplied (256 queries per group, half the flops), which yields
@@ -47,16 +46,18 @@ namespace b200 {
 int launch_topk_select(const unsigned long long* in, int64_t in_stride_q, int64_t M, int k, int C,
                        unsigned long long* out, int64_t out_stride_q, int slices, int nq, cudaStream_t st);
 
-constexpr int MS_BM = 128;       // rows per tile
+constexpr int MS_BM = 64;        // rows per tile
 constexpr int MS_QG = 128;       // queries per group (256 MMA columns: hi | lo)
 constexpr int MS_BN = 256;
 constexpr int MS_BK = 64;
-constexpr int MS_STAGES = 6;
+constexpr int MS_STAGES = 5;
 constexpr int MS_CAP = 512;      // candidate buffer entries per (CTA, query)
 constexpr int MS_KMAX = 128;     // k supported by this path
-constexpr int MS_THREADS = 320;   // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue (two per TMEM lane quarter)
+constexpr int MS_THREADS = 160;   // warps 0..3: the consumer warpgroup, warp 4: TMA producer
+constexpr int MS_WARP_TMA = 4;
+constexpr int MS_CONSUMERS = 128;
 constexpr int MS_A_BYTES = MS_BM * MS_BK * 2;
-constexpr int MS_B_BYTES = (MS_BN / 2) * MS_BK * 2;  // each CTA of the pair stages half of the Q' tile
+constexpr int MS_B_BYTES = MS_BN * MS_BK * 2;
 constexpr int MS_STAGE_BYTES = MS_A_BYTES + MS_B_BYTES;
 
 // fp32 queries -> fp16 [groups*256, d].  Split mode: row g*256 + c (c < 128) = hi of query
@@ -242,12 +243,11 @@ __device__ __forceinline__ float compact_buffer(unsigned long long* buf, int cou
 }
 
 template <bool HILO>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(MS_THREADS, 1)
+__global__ void __launch_bounds__(MS_THREADS, 1)
 scan_mma_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmQ, int64_t n, int d,
                 int nq, int groups, int k, unsigned long long* __restrict__ cand /* [grid][groups*128][CAP] */,
                 unsigned long long* __restrict__ dense /* [nq][grid][k] */, int tile_stride,
-                const float* __restrict__ thr_init /* [nq] lower bounds on the k-th best score, or null */,
-                int exp_mode /* timing experiments: 1 = read TMEM but skip the tests, 2 = read one chunk, test all */) {
+                const float* __restrict__ thr_init /* [nq] lower bounds on the k-th best score, or null */) {
   constexpr int QG = HILO ? MS_QG : MS_BN;   // queries per group: 128 (hi | lo columns) or 256 (hi only)
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = ptx::smem_u32(smem_raw);
@@ -258,223 +258,130 @@ scan_mma_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
   int* s_cnt = reinterpret_cast<int*>(s_thr + groups * QG);                    // [groups*QG]
   uint64_t* full = reinterpret_cast<uint64_t*>(s_cnt + groups * QG);
   uint64_t* empty = full + MS_STAGES;
-  uint64_t* tfull = empty + MS_STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(tempty + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // CTA pair (cta_group::2): a pair owns 256-row tiles, each CTA stages its own 128 rows of X and half
-  // of the 256 Q' rows (CTA 0 the hi parts, CTA 1 the lo parts); the epilogue is per CTA (its rows).
-  const uint32_t rank = ptx::cluster_ctarank();
-  const bool leader = rank == 0;
-  const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-  const int64_t row_tiles = (n + 2 * MS_BM - 1) / (2 * MS_BM);
+  const int64_t row_tiles = (n + MS_BM - 1) / MS_BM;
   const int kb = (d + MS_BK - 1) / MS_BK;
 
   for (int i = threadIdx.x; i < groups * QG; i += blockDim.x) {
     s_thr[i] = (thr_init != nullptr && i < nq) ? thr_init[i] : -INFINITY;
     s_cnt[i] = 0;
   }
-  if (warp == 0 && lane == 0) {
-    ptx::prefetch_tensormap(&tmX);
-    ptx::prefetch_tensormap(&tmQ);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < MS_STAGES; s++) {
-        ptx::mbar_init(&full[s], 1);
-        ptx::mbar_init(&empty[s], 1);
-      }
-      for (int a = 0; a < 2; a++) {
-        ptx::mbar_init(&tfull[a], 1);
-        ptx::mbar_init(&tempty[a], 16);   // 8 epilogue warps x 2 CTAs
-      }
-      ptx::fence_barrier_init();
+  if (threadIdx.x == 0) {
+    for (int st = 0; st < MS_STAGES; st++) {
+      ptx::mbar_init(&full[st], 1);
+      ptx::mbar_init(&empty[st], 4);   // one arrive per consumer warp
     }
-    __syncwarp();
-    ptx::tmem_alloc_pair(s_tmem, 512);
-    ptx::tmem_relinquish_pair();
+    ptx::fence_barrier_init();
   }
   __syncthreads();
-  ptx::tc_fence_before();
-  ptx::cluster_sync_all();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *s_tmem;
 
-  if (warp == 0) {
+  if (warp == MS_WARP_TMA) {
     if (lane == 0) {
+      ptx::prefetch_tensormap(&tmX);
+      ptx::prefetch_tensormap(&tmQ);
       int stage = 0;
       uint32_t phase = 0;
-      for (int64_t rt = (int64_t)pair * tile_stride; rt < row_tiles; rt += (int64_t)npairs * tile_stride) {
+      for (int64_t rt = (int64_t)blockIdx.x * tile_stride; rt < row_tiles; rt += (int64_t)gridDim.x * tile_stride) {
         for (int g = 0; g < groups; g++) {
           for (int kbi = 0; kbi < kb; kbi++) {
             ptx::mbar_wait(&empty[stage], phase ^ 1);
-            ptx::tma_load_2d_pair(sA + stage * MS_A_BYTES, &tmX, &full[stage], kbi * MS_BK,
-                                  (int32_t)(rt * 2 * MS_BM + rank * MS_BM));
-            ptx::tma_load_2d_pair(sB + stage * MS_B_BYTES, &tmQ, &full[stage], kbi * MS_BK,
-                                  g * MS_BN + (int)rank * (MS_BN / 2));
-            if (leader) ptx::mbar_arrive_expect_tx(&full[stage], 2 * MS_STAGE_BYTES);
+            ptx::mbar_arrive_expect_tx(&full[stage], MS_STAGE_BYTES);
+            ptx::tma_load_2d(sA + stage * MS_A_BYTES, &tmX, &full[stage], kbi * MS_BK, (int32_t)(rt * MS_BM));
+            ptx::tma_load_2d(sB + stage * MS_B_BYTES, &tmQ, &full[stage], kbi * MS_BK, g * MS_BN);
             if (++stage == MS_STAGES) { stage = 0; phase ^= 1; }
           }
         }
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (leader && lane == 0) {
-      constexpr uint32_t idesc = ptx::umma_idesc_f16(2 * MS_BM, MS_BN, false);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int64_t rt = (int64_t)pair * tile_stride; rt < row_tiles; rt += (int64_t)npairs * tile_stride) {
-        for (int g = 0; g < groups; g++) {
-          ptx::mbar_wait(&tempty[acc], acc_phase ^ 1);
-          ptx::tc_fence_after();
-          const uint32_t tmem_d = tmem_base + acc * MS_BN;
-          for (int kbi = 0; kbi < kb; kbi++) {
-            ptx::mbar_wait(&full[stage], phase);
-            ptx::tc_fence_after();
-            const uint64_t da = ptx::umma_desc_k_sw128(ptx::smem_u32(sA + stage * MS_A_BYTES));
-            const uint64_t db = ptx::umma_desc_k_sw128(ptx::smem_u32(sB + stage * MS_B_BYTES));
-#pragma unroll
-            for (int kk = 0; kk < MS_BK / 16; kk++)
-              ptx::umma_f16_pair(tmem_d, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), idesc, (kbi | kk) != 0 ? 1u : 0u);
-            ptx::umma_commit_pair(&empty[stage], 3);
-            if (++stage == MS_STAGES) { stage = 0; phase ^= 1; }
-          }
-          ptx::umma_commit_pair(&tfull[acc], 3);
-          acc ^= 1;
-          if (acc == 0) acc_phase ^= 1;
-        }
-      }
-    }
-    __syncwarp();
-  } else {
-    // ---------------- epilogue: thresholded append + compaction ----------------
-    const int q4 = warp & 3;          // TMEM lane quarter this warp may read (warp id % 4)
-    const int ew = warp - 2;          // 0..7
-    const int half = ew >> 2;         // the two warps of a quarter take alternate 32-column chunks
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    unsigned long long* my_cand = cand + (int64_t)blockIdx.x * groups * QG * MS_CAP;
-    const uint32_t tempty0_remote = ptx::mapa_u32(ptx::smem_u32(&tempty[0]), 0);
-    for (int64_t rt = (int64_t)pair * tile_stride; rt < row_tiles; rt += (int64_t)npairs * tile_stride) {
-      const int64_t row = rt * 2 * MS_BM + rank * MS_BM + q4 * 32 + lane;
-      const bool row_ok = row < n;
-      for (int g = 0; g < groups; g++) {
-        ptx::mbar_wait(&tfull[acc], acc_phase);
-        ptx::tc_fence_after();
-        const uint32_t tbase = tmem_base + acc * MS_BN + ((uint32_t)(q4 * 32) << 16);
-        const int gq = min(QG, nq - g * QG);   // live queries of this group
-        const int nchunks = (gq + 31) / 32;
-        const int my_last = nchunks - 1 - ((nchunks - 1 - half) & 1);   // last chunk index of this warp (< half: none)
-        if (my_last < half) {   // nothing to read in this accumulator: release it right away
-          ptx::tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            if (leader) ptx::mbar_arrive(&tempty[acc]);
-            else ptx::mbar_arrive_cluster(tempty0_remote + (uint32_t)acc * 8u);
-          }
-        }
-#pragma unroll 1
-        for (int c = half; c < nchunks; c += 2) {
-          uint32_t hi[32], lo[HILO ? 32 : 1];
-#ifdef B200_TIMING_EXPERIMENTS
-          if (exp_mode != 2 || c == half)
-#endif
-          {
-            ptx::tmem_ld_32x32b_x32(tbase + c * 32, hi);
-            if constexpr (HILO) ptx::tmem_ld_32x32b_x32(tbase + MS_QG + c * 32, lo);
-            ptx::tmem_ld_wait();
-          }
-          if (c == my_last) {
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-              if (leader) ptx::mbar_arrive(&tempty[acc]);
-              else ptx::mbar_arrive_cluster(tempty0_remote + (uint32_t)acc * 8u);
-            }
-          }
-#ifdef B200_TIMING_EXPERIMENTS
-          if (row_ok && exp_mode != 1) {
-#else
-          if (row_ok) {
-#endif
-            // branch-free common case: recombine, compare against the 32 thresholds (vector loads from
-            // shared memory), collect the rare hits in a bit mask; only then take the append path.
-            const int qbase = g * QG + c * 32;
-            const float4* thr4 = reinterpret_cast<const float4*>(s_thr + qbase);
-            uint32_t mask = 0;
-#pragma unroll
-            for (int j4 = 0; j4 < 8; j4++) {
-              const float4 t = thr4[j4];
-              const float th[4] = {t.x, t.y, t.z, t.w};
-#pragma unroll
-              for (int e = 0; e < 4; e++) {
-                const int j = j4 * 4 + e;
-                float s = __uint_as_float(hi[j]);
-                if constexpr (HILO) {
-                  s = fmaf(__uint_as_float(lo[j]), 1.0f / 2048.0f, s);
-                  hi[j] = __float_as_uint(s);
-                }
-                mask |= (s >= th[e]) ? (1u << j) : 0u;
-              }
-            }
-            const int live = nq - qbase;  // queries of this chunk that exist
-            if (live < 32) mask &= (1u << (live > 0 ? live : 0)) - 1u;
-            if (mask) {
-#pragma unroll
-              for (int j = 0; j < 32; j++) {
-                if (mask & (1u << j)) {
-                  const int q = qbase + j;
-                  const int pos = atomicAdd(&s_cnt[q], 1);
-                  if (pos < MS_CAP) my_cand[(int64_t)q * MS_CAP + pos] = make_key(__uint_as_float(hi[j]), (uint32_t)row);
-                }
-              }
-            }
-          }
-        }
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-        // compaction of this group's buffers that could overflow during the next tile
-        __threadfence_block();
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        // each warp owns 32 queries of the group; one lane-parallel look at their counters (the common case
-        // — nothing close to overflowing — costs one shared load and a ballot instead of 32 dependent loads)
-        for (int qb = ew * 32; qb < gq; qb += 256) {
-          const int ql = qb + lane;
-          const int my_cnt = ql < gq ? s_cnt[g * QG + ql] : 0;
-          unsigned need = __ballot_sync(FULL, my_cnt > MS_CAP - MS_BM);
-          while (need) {
-            const int b = __ffs(need) - 1;
-            need &= need - 1;
-            const int q = g * QG + qb + b;
-            const int cnt = __shfl_sync(FULL, my_cnt, b);
-            const float thr = compact_buffer(my_cand + (int64_t)q * MS_CAP, min(cnt, MS_CAP), k, lane);
-            if (lane == 0) {
-              s_cnt[q] = min(cnt, k);
-              if (thr > s_thr[q]) s_thr[q] = thr;
-            }
-          }
-        }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-      }
-    }
-    // final pass: every (CTA, query) buffer reduced to its k best and written densely for the merge
-    for (int q = ew; q < nq; q += 8) {
-      unsigned long long* buf = my_cand + (int64_t)q * MS_CAP;
-      const int cnt = s_cnt[q];
-      if (cnt > k) compact_buffer(buf, min(cnt, MS_CAP), k, lane);
-      const int have = min(cnt, k);   // slots past `have` were never written: emit the empty key
-      unsigned long long* o = dense + ((int64_t)q * gridDim.x + blockIdx.x) * k;
-      for (int j = lane; j < k; j += 32) o[j] = j < have ? buf[j] : 0ull;
-    }
+    return;
   }
 
-  ptx::tc_fence_before();
-  ptx::cluster_sync_all();
-  if (warp == 1) ptx::tmem_dealloc_pair(tmem_base, 512);
+  // ---------------- consumers: wgmma, thresholded append, compaction ----------------
+  int stage = 0;
+  uint32_t phase = 0;
+  unsigned long long* my_cand = cand + (int64_t)blockIdx.x * groups * QG * MS_CAP;
+  float acc[MS_BN / 2];
+  for (int64_t rt = (int64_t)blockIdx.x * tile_stride; rt < row_tiles; rt += (int64_t)gridDim.x * tile_stride) {
+    // accumulator rows of this thread: r0 and r0 + 8
+    const int64_t r0 = rt * MS_BM + warp * 16 + (lane >> 2);
+    for (int g = 0; g < groups; g++) {
+      int prev = -1;
+      for (int kbi = 0; kbi < kb; kbi++) {
+        ptx::mbar_wait(&full[stage], phase);
+        ptx::wgmma_fence();
+        const uint64_t da = ptx::wgmma_desc_k_sw128(ptx::smem_u32(sA + stage * MS_A_BYTES));
+        const uint64_t db = ptx::wgmma_desc_k_sw128(ptx::smem_u32(sB + stage * MS_B_BYTES));
+#pragma unroll
+        for (int kk = 0; kk < MS_BK / 16; kk++)
+          ptx::wgmma_m64n256k16_f16(acc, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), (kbi | kk) != 0 ? 1u : 0u);
+        ptx::wgmma_commit();
+        // the group of the previous k-block has completed: its ring slot may be refilled
+        ptx::wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == MS_STAGES) { stage = 0; phase ^= 1; }
+      }
+      ptx::wgmma_wait<0>();
+      ptx::fence_regs(acc);
+      if (lane == 0) ptx::mbar_arrive(&empty[prev]);
+
+      // register i of this thread: row r0 + 8 * ((i / 2) % 2), column 8 * (i / 4) + 2 * (lane % 4) + i % 2; in split
+      // mode column c < 128 holds the hi product of query c and column c + 128 its lo product.
+#pragma unroll
+      for (int j = 0; j < QG / 8; j++) {
+#pragma unroll
+        for (int e = 0; e < 2; e++) {
+          const int col = 8 * j + 2 * (lane & 3) + e;
+          const int q = g * QG + col;
+          if (q >= nq) continue;
+          const float th = s_thr[q];
+#pragma unroll
+          for (int h = 0; h < 2; h++) {
+            float sc = acc[4 * j + 2 * h + e];
+            if constexpr (HILO) sc = fmaf(acc[4 * (j + MS_QG / 8) + 2 * h + e], 1.0f / 2048.0f, sc);
+            const int64_t row = r0 + 8 * h;
+            if (sc >= th && row < n) {
+              const int pos = atomicAdd(&s_cnt[q], 1);
+              if (pos < MS_CAP) my_cand[(int64_t)q * MS_CAP + pos] = make_key(sc, (uint32_t)row);
+            }
+          }
+        }
+      }
+      // compaction of this group's buffers that could overflow during the next tile
+      const int gq = min(QG, nq - g * QG);   // live queries of this group
+      __threadfence_block();
+      asm volatile("bar.sync 1, %0;" ::"n"(MS_CONSUMERS) : "memory");
+      // each warp owns 32 queries of the group; one lane-parallel look at their counters (the common case
+      // — nothing close to overflowing — costs one shared load and a ballot instead of 32 dependent loads)
+      for (int qb = warp * 32; qb < gq; qb += MS_CONSUMERS) {
+        const int ql = qb + lane;
+        const int my_cnt = ql < gq ? s_cnt[g * QG + ql] : 0;
+        unsigned need = __ballot_sync(FULL, my_cnt > MS_CAP - MS_BM);
+        while (need) {
+          const int b = __ffs(need) - 1;
+          need &= need - 1;
+          const int q = g * QG + qb + b;
+          const int cnt = __shfl_sync(FULL, my_cnt, b);
+          const float thr = compact_buffer(my_cand + (int64_t)q * MS_CAP, min(cnt, MS_CAP), k, lane);
+          if (lane == 0) {
+            s_cnt[q] = min(cnt, k);
+            if (thr > s_thr[q]) s_thr[q] = thr;
+          }
+        }
+      }
+      asm volatile("bar.sync 1, %0;" ::"n"(MS_CONSUMERS) : "memory");
+    }
+  }
+  // final pass: every (CTA, query) buffer reduced to its k best and written densely for the merge
+  for (int q = warp; q < nq; q += MS_CONSUMERS / 32) {
+    unsigned long long* buf = my_cand + (int64_t)q * MS_CAP;
+    const int cnt = s_cnt[q];
+    if (cnt > k) compact_buffer(buf, min(cnt, MS_CAP), k, lane);
+    const int have = min(cnt, k);   // slots past `have` were never written: emit the empty key
+    unsigned long long* o = dense + ((int64_t)q * gridDim.x + blockIdx.x) * k;
+    for (int j = lane; j < k; j += 32) o[j] = j < have ? buf[j] : 0ull;
+  }
 }
 
 int make_tmap_2d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t rows, uint64_t cols, uint64_t ld_elems,
@@ -486,7 +393,7 @@ static int scan_mma_passes(b200_index* idx, const __half* rows, int64_t n, const
                            unsigned long long* d_keys_out, cudaStream_t st) {
   constexpr int QG = HILO ? MS_QG : MS_BN;
   const int d = idx->d;
-  const int grid = idx->sms & ~1;  // CTA pairs
+  const int grid = idx->sms;
   const int QMAX = 1024;  // queries per launch (thresholds/counters live in shared memory)
   for (int q0 = 0; q0 < nq; q0 += QMAX) {
     const int nqb = std::min(QMAX, nq - q0);
@@ -507,7 +414,7 @@ static int scan_mma_passes(b200_index* idx, const __half* rows, int64_t n, const
     }
     CUtensorMap tmX, tmQ;
     B200_TRY(make_tmap_2d(&tmX, rows, 0, (uint64_t)n, (uint64_t)d, (uint64_t)d, MS_BM, MS_BK));
-    B200_TRY(make_tmap_2d(&tmQ, Qp, 0, (uint64_t)groups * MS_BN, (uint64_t)d, (uint64_t)d, MS_BN / 2, MS_BK));
+    B200_TRY(make_tmap_2d(&tmQ, Qp, 0, (uint64_t)groups * MS_BN, (uint64_t)d, (uint64_t)d, MS_BN, MS_BK));
     const size_t smem = (size_t)MS_STAGES * MS_STAGE_BYTES + (size_t)groups * QG * 8 + 256 + 1024;
     B200_CUDA(cudaFuncSetAttribute(scan_mma_kernel<HILO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     if ((int)idx->ev.size() < idx->ev_used + 2) {
@@ -518,31 +425,26 @@ static int scan_mma_passes(b200_index* idx, const __half* rows, int64_t n, const
       idx->ev.push_back(b);
     }
     // sampling passes first (strided row tiles), each seeding the next pass's thresholds
-    const int64_t row_tiles = (n + 2 * MS_BM - 1) / (2 * MS_BM);
+    const int64_t row_tiles = (n + MS_BM - 1) / MS_BM;
     const int64_t M = (int64_t)grid * k;
     int C = 2048;
     while (C < 2 * k) C <<= 1;
     unsigned long long* keys_q = d_keys_out + (size_t)q0 * k;
     // Pass schedule.  The first pass starts from -inf thresholds, where EVERY score is appended and the
-    // buffers are compacted every third tile (ncu: 2.55 ms for 3 % of the tiles at 4 % tensor-active), so it
-    // is kept to one tile per CTA pair (a sample of npairs*256 rows, no compaction before the final one);
-    // its k-th best scores seed a 1/32 pass, whose k-th best scores seed the full pass.
-    const int64_t npairs = grid / 2;
+    // buffers are compacted every third tile, so it is kept to one tile per CTA (a sample of ctas*64 rows, no
+    // compaction before the final one); its k-th best scores seed a 1/32 pass, whose k-th best scores seed the
+    // full pass.
+    const int64_t ctas = grid;
     int strides[3], npass = 0;
-    if (row_tiles >= 8 * npairs) strides[npass++] = (int)std::min<int64_t>(row_tiles / npairs, 1 << 30);
-    if (npass == 1 && strides[0] > 64 && row_tiles / 32 >= 2 * npairs) strides[npass++] = 32;
+    if (row_tiles >= 8 * ctas) strides[npass++] = (int)std::min<int64_t>(row_tiles / ctas, 1 << 30);
+    if (npass == 1 && strides[0] > 64 && row_tiles / 32 >= 2 * ctas) strides[npass++] = 32;
     strides[npass++] = 1;
     bool have_thr = false;
     B200_CUDA(cudaEventRecord(idx->ev[idx->ev_used], st));
     for (int pi = 0; pi < npass; pi++) {
       const int stride = strides[pi];
-#ifdef B200_TIMING_EXPERIMENTS
-      static const int exp_mode = getenv("B200_SCAN_EXP") ? atoi(getenv("B200_SCAN_EXP")) : 0;
-#else
-      const int exp_mode = 0;
-#endif
       scan_mma_kernel<HILO><<<grid, MS_THREADS, smem, st>>>(tmX, tmQ, n, d, nqb, groups, k, cand, dense, stride,
-                                                            have_thr ? thr : nullptr, exp_mode);
+                                                            have_thr ? thr : nullptr);
       B200_LAUNCH_OK();
       idx->last_scan_launches++;
       if (stride == 1) B200_CUDA(cudaEventRecord(idx->ev[idx->ev_used + 1], st));

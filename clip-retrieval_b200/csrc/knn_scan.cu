@@ -486,7 +486,7 @@ int scan_topk_keys(b200_index* idx, const __half* rows, int64_t n, const float* 
   const int64_t total_warps = (int64_t)p.grid * p.warps_out;
   const int64_t M1 = total_warps * k;
   // level 1: one sort round per block (a block sorts one C-entry chunk of the candidates) — the select of a single
-  // query is latency, not throughput: 5 blocks x 5 dependent sort rounds took 98 us at nq = 1 (profiles/r02a)
+  // query is latency, not throughput: dependent sort rounds per block are what it costs
   int slices = (int)std::min<int64_t>(256, std::max<int64_t>(1, (M1 + p.C - 1) / p.C));
   const int C2 = std::min(p.C, std::max(next_pow2(2 * k), next_pow2(slices * k)));   // level 2 buffer: slices * k keys
   const int QB = 64;  // queries per batch (bounds the scratch)

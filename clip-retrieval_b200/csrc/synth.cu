@@ -90,7 +90,7 @@ int synth_rows_indirect_f16(__half* out, const uint32_t* src_rows, int64_t n, in
                             const b200_synth_spec* spec, cudaStream_t st) {
   if (n == 0) return B200_OK;
   int64_t blocks = (n + 7) / 8;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   synth_rows_indirect_kernel<<<(unsigned)blocks, 256, 0, st>>>(out, src_rows, n, d, row0, *spec);
   B200_LAUNCH_OK();
   return B200_OK;
@@ -104,7 +104,7 @@ int synth_rows(OutT* d_out, int64_t n, int d, int64_t row0, const b200_synth_spe
   if (n == 0) return B200_OK;
   const int threads = 256;
   int64_t blocks = (n + 7) / 8;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   synth_rows_kernel<OutT><<<(unsigned)blocks, threads, 0, st>>>(d_out, n, d, row0, *spec);
   B200_LAUNCH_OK();
   return B200_OK;

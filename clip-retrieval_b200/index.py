@@ -227,8 +227,8 @@ class _IndexBase:
         return out[0].cpu().numpy()
 
     def set_tensor_scan(self, on):
-        """Batched queries use the tcgen05 scan by default; False forces the FMA scan.  An int is passed
-        through as the C ABI's bit flags (1 tcgen05 scan, 4 no bulk-copy ring, 8 split mode only)."""
+        """Batched queries use the wgmma scan by default; False forces the FMA scan.  An int is passed
+        through as the C ABI's bit flags (1 wgmma scan, 4 no bulk-copy ring, 8 split mode only)."""
         flags = (1 if on else 0) if isinstance(on, bool) else int(on)
         check(lib.b200_index_set_tensor_scan(self._h, flags), "set_tensor_scan")
 
@@ -429,7 +429,7 @@ class _IdMapped:
 
 
 def index_from_faiss(info, device=0):
-    """B200 index from the arrays faiss_io.read_faiss_index returns."""
+    """Index from the arrays faiss_io.read_faiss_index returns."""
     d, ids = info["d"], info["ids"]
     if info["kind"] == "flat":
         index = B200FlatIndex(d, device=device)

@@ -222,7 +222,7 @@ def convert_hf_state_dict(sd, arch):
 
 
 class B200Clip:
-    """CLIP towers on one B200.  `encode_image` / `encode_text` follow the reference model's
+    """CLIP towers on one GPU.  `encode_image` / `encode_text` follow the reference model's
     contract (CUDA tensors in, fp32 feature tensor out); `embed_*` fuse the normalise + cast of
     mapper.py:58-59,66-67 into the last kernel and are what `ClipMapper` calls."""
 

@@ -1,5 +1,5 @@
 /*
- * b200clip.h — C ABI of the B200-native hot path for rom1504/clip-retrieval.
+ * b200clip.h — C ABI of the CUDA-native hot path (H100, sm_90a) for rom1504/clip-retrieval.
  *
  * The reference (pure Python) has no FFI of its own; its hot-path seams are duck-typed Python
  * objects (SURVEY.md §8b).  Each entry point below names the reference call it replaces.
@@ -35,7 +35,7 @@ typedef enum b200_status {
 } b200_status;
 
 const char* b200_last_error(void);
-/* Library version string and the SM architecture it was compiled for ("sm_100a"). */
+/* Library version string and the SM architecture it was compiled for ("sm_90a"). */
 const char* b200_version(void);
 /* Number of kernel launches this library has issued in this process (all handles, all streams).
  * bench.py reads it before/after the timed region to report `gpu_launches`. */
@@ -103,9 +103,9 @@ int b200_index_set_id_base(b200_index* idx, int64_t id_base);
  * (clip_back.py:357-361,368-369). */
 int b200_index_set_nprobe(b200_index* idx, int nprobe);
 int b200_index_get_nprobe(const b200_index* idx);
-/* Batched queries (nq > 4, k <= 128) go through the tcgen05 scan by default; 0 forces the FMA scan
- * (kept for A/B measurements and parity tests between the paths).  Bit flags: 1 = tcgen05 scan on,
- * 4 = FMA scan without the bulk-copy ring, 8 = tcgen05 scan always in hi/lo split mode (no
+/* Batched queries (nq > 4, k <= 128) go through the wgmma scan by default; 0 forces the FMA scan
+ * (kept for A/B measurements and parity tests between the paths).  Bit flags: 1 = wgmma scan on,
+ * 4 = FMA scan without the bulk-copy ring, 8 = wgmma scan always in hi/lo split mode (no
  * approximate hi-only pass + exact re-score for nq > 128). */
 int b200_index_set_tensor_scan(b200_index* idx, int on);
 /* Queries of the last batched search whose exactness proof failed in hi-only mode and were re-run
@@ -224,25 +224,11 @@ int b200_clip_last_timing(b200_clip* m, float* ms_by_class /*[8]: gemm, attentio
 /* Enable per-class event timing (event records between kernels; off by default); resets the sums. */
 int b200_clip_set_profiling(b200_clip* m, int on);
 
-/* Stand-alone GEMM entry used by the tests and the roofline bench of the tcgen05 core:
+/* Stand-alone GEMM entry used by the tests of the wgmma core:
  * C[M,N] (bf16) = act(A[M,K] (bf16, row-major) · W[N,K]^T (bf16, row-major) + bias[N] (fp32|NULL))
  *               (+ residual[M,N] bf16 | NULL).  act: 0 none, 1 quick_gelu, 2 gelu(erf). */
 int b200_gemm_bf16_device(const void* d_A, const void* d_W, const float* d_bias, const void* d_residual,
                           void* d_C, int M, int N, int K, int act, int device, void* stream);
-
-/* Large GEMMs run on CTA pairs (tcgen05 cta_group::2, 256x256 tiles) by default; 0 forces the
- * single-CTA 128x256 kernel for every shape (A/B measurements, parity between the two kernels). */
-int b200_gemm_set_pair_mode(int on);
-/* CTA-pair kernel only: 1 (default) = results (and the residual operand) travel through shared memory and TMA tensor
- * stores / loads, epilogue flavour (activation, residual) fixed at compile time; 2 = the same with every epilogue
- * feature decided at run time; 0 = per-thread 16-byte global stores / loads (A/B, parity tests: all three are
- * bit-identical). */
-int b200_gemm_set_tma_store(int on);
-/* attention_tc2 (head dim 64, T <= 264) softmax-loop variant, for A/B measurements and parity between the variants:
- * bit 0 = tcgen05.ld of the next 32-column chunk in flight while the current one is processed, bit 1 = unmasked loop
- * copies for chunks no lane masks, bit 2 / bit 3 = P.V issued per 64 / 128 keys as the softmax writes them (else once per
- * tile).  Returns the previous variant; a negative argument only reads it. */
-int b200_attention_set_variant(int variant);
 
 /* Stand-alone entries of the two other embed kernels, for their parity tests:
  * LayerNorm (eps 1e-5) over rows of `w` bf16 values; multi-head attention over a fused qkv buffer
@@ -251,15 +237,6 @@ int b200_layernorm_bf16_device(const void* d_in, void* d_out, const float* d_gam
                                int64_t rows, int w, int device, void* stream);
 int b200_attention_bf16_device(const void* d_qkv, void* d_out, int B, int T, int heads, int w, int causal,
                                int device, void* stream);
-/* tcgen05 attention (head dim 64, T <= 320): the Q and K thirds are read from d_qkv, V^T from d_vt
- * ([B*heads*64, Tp] bf16, keys contiguous, columns >= T zero) — the layout the QKV GEMM epilogue writes.
- * d_vt == NULL selects the kernels that read V from d_qkv (MN-major operand); Tp then names the generation under test:
- *   0  attention_tc (one tile in flight)      -1  attention_tc2 (production; variant: b200_attention_set_variant)
- *  -2  attention_tc3                          -3  attention_tc2 + leftover-row kernel on a second stream
- *  -4  the frozen session-i build of attention_tc2 (same-process A/B reference, profiles/r02o_*). */
-int b200_attention_tc_bf16_device(const void* d_qkv, const void* d_vt, int Tp, void* d_out, int B, int T, int heads,
-                                  int w, int causal, int device, void* stream);
-
 /* ---- image transform in front of the embed path (SURVEY §8(f) row 1) ----------------------------
  * Replaces `preprocess(PIL.Image)` as the reference calls it per image on the host
  * (clip_retrieval/clip_inference/reader.py:98-106,158-165; the object `load_clip` returns,

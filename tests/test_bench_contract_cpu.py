@@ -32,7 +32,7 @@ def test_reference_arm_other_ranks_exit_quietly():
 
 def test_plumbing_helpers_drive_the_reference_runner(tmp_path):
     """configs[0] helpers of bench.py on the CPU: the synthetic tokenizer ends every caption with the largest id (the
-    text tower pools at argmax), and a ClipMapper-contract callable driven by the reference's own Runner (baseline/_ref)
+    text tower pools at argmax), and a ClipMapper-contract callable driven by the reference's own Runner (oracle/_ref)
     produces the writer's shard layout in the sampler's order."""
     import numpy as np
     import pytest
@@ -45,7 +45,7 @@ def test_plumbing_helpers_drive_the_reference_runner(tmp_path):
     assert tok.shape == (3, 77) and tok.dtype == torch.int64
     assert all(int(row.argmax()) == int((row != 0).sum()) - 1 and int(row.max()) == 49407 and int(row[0]) == 49406 for row in tok)
     if not os.path.isdir(bench.REF_INFERENCE):
-        pytest.skip("baseline/_ref (reference install) not in this tree")
+        pytest.skip("oracle/_ref (reference install) not in this tree")
     from clip_retrieval_b200.model import make_preprocess
 
     n, parts, bs, d = 10, 2, 4, 16

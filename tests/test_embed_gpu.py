@@ -119,35 +119,6 @@ def test_vit_l14_matches_oracle():
     assert ci.max() <= COS_TOL and ct.max() <= COS_TOL, (ci, ct)
 
 
-@pytest.mark.timeout(120)
-@pytest.mark.parametrize("B,T,heads,causal", [(3, 257, 4, 0), (2, 77, 3, 1), (2, 200, 2, 1), (1, 264, 2, 0), (2, 16, 2, 0)])
-def test_tcgen05_attention_variants_are_bit_identical(B, T, heads, causal):
-    """The softmax-loop variants of attention_tc2 (pipelined tcgen05.ld, unmasked loop copies, block-wise P.V issue)
-    reorder loads and hand-shakes, not arithmetic: every variant must reproduce variant 0 bit for bit."""
-    import torch
-    from clip_retrieval_b200._lib import lib, check
-
-    w = heads * 64
-    g = torch.Generator(device="cuda").manual_seed(T * 7 + heads)
-    qkv = torch.randn(B * T, 3 * w, device="cuda", generator=g).bfloat16()
-    old = lib.b200_attention_set_variant(-1)
-    try:
-        outs = []
-        for v in range(16):
-            lib.b200_attention_set_variant(v)
-            out = torch.full((B * T, w), float("nan"), device="cuda", dtype=torch.bfloat16)
-            for _ in range(2):   # twice: the second launch starts from the barrier phases the first one left
-                check(lib.b200_attention_tc_bf16_device(qkv.data_ptr(), None, -1, out.data_ptr(), B, T, heads, w, causal, 0,
-                                                        torch.cuda.current_stream().cuda_stream), "attention_tc2")
-            torch.cuda.synchronize()
-            assert not torch.isnan(out.float()).any(), "variant %d" % v
-            outs.append(out)
-        for v in range(1, 16):
-            assert torch.equal(outs[0], outs[v]), "variant %d differs from variant 0" % v
-    finally:
-        lib.b200_attention_set_variant(old)
-
-
 @pytest.mark.timeout(300)
 def test_mapper_drop_in_contract():
     """The reference's own mapper test pins shape[0] and dtype float16 (tests/test_clip_inference/
@@ -197,8 +168,9 @@ def test_zero_feature_row_is_nan_like_reference():
 @pytest.mark.parametrize("B,T,heads,causal", [(2, 257, 16, 0), (3, 77, 8, 1), (2, 50, 12, 0), (1, 1, 2, 0), (5, 128, 4, 1),
                                               (1, 320, 2, 0), (40, 257, 16, 0), (3, 260, 2, 0), (2, 256, 2, 1), (7, 129, 3, 0), (2, 258, 3, 1)])
 def test_tcgen05_attention_matches_fp32_reference(B, T, heads, causal):
-    """tcgen05 attention (TMA K / V^T tiles, scores and output in TMEM, P through swizzled shared
-    memory) against a plain fp32 PyTorch softmax(QK^T)V of the same bf16 inputs."""
+    """The shapes that pinned the Blackwell tensor-core attention, now on the attention kernel the model runs on H100:
+    head dimension 64 at sequence lengths around its 16-row query blocks and 32-key blocks (T = 1, 128, 129, 256..260,
+    320) and at the ViT-L/14 batch shape, against a plain fp32 PyTorch softmax(QK^T)V of the same bf16 inputs."""
     import torch
     from clip_retrieval_b200._lib import lib, check
 
@@ -206,18 +178,9 @@ def test_tcgen05_attention_matches_fp32_reference(B, T, heads, causal):
     w = heads * hd
     g = torch.Generator(device="cuda").manual_seed(B * 1000 + T + w)
     qkv = torch.randn(B * T, 3 * w, device="cuda", generator=g).bfloat16()
-    Tp = (T + 7) // 8 * 8
-    v = qkv[:, 2 * w:].view(B, T, heads, hd)
-    vt = torch.zeros(B, heads, hd, Tp, device="cuda", dtype=torch.bfloat16)
-    vt[..., :T] = v.permute(0, 2, 3, 1)
     out = torch.full((B * T, w), float("nan"), device="cuda", dtype=torch.bfloat16)
-    check(lib.b200_attention_tc_bf16_device(qkv.data_ptr(), vt.data_ptr(), Tp, out.data_ptr(), B, T, heads, w, causal, 0,
-                                            torch.cuda.current_stream().cuda_stream), "attention_tc")
-    # second variant: no V^T copy, V read from the qkv buffer as an MN-major tensor-core operand
-    out2 = torch.full((B * T, w), float("nan"), device="cuda", dtype=torch.bfloat16)
-    check(lib.b200_attention_tc_bf16_device(qkv.data_ptr(), None, 0, out2.data_ptr(), B, T, heads, w, causal, 0,
-                                            torch.cuda.current_stream().cuda_stream), "attention_tc")
-    assert torch.equal(out, out2), "V^T and MN-major V paths disagree: max diff %g" % (out.float() - out2.float()).abs().nan_to_num(1e9).max().item()
+    check(lib.b200_attention_bf16_device(qkv.data_ptr(), out.data_ptr(), B, T, heads, w, causal, 0,
+                                         torch.cuda.current_stream().cuda_stream), "attention")
     q, k, vv = qkv.float().view(B, T, 3, heads, hd).permute(2, 0, 3, 1, 4)
     s = (q @ k.transpose(-1, -2)) * hd ** -0.5
     if causal:
@@ -226,29 +189,6 @@ def test_tcgen05_attention_matches_fp32_reference(B, T, heads, causal):
     err = (out.float() - ref).abs()
     assert not torch.isnan(out.float()).any()
     assert bool((err <= ref.abs() * 2 ** -7 + 2e-2).all()), "max err %g" % err.max().item()
-    if T <= 264:
-        # third variant: two query tiles in flight, keys past 256 on the FMA pipe (attention_tc2.cu)
-        out3 = torch.full((B * T, w), float("nan"), device="cuda", dtype=torch.bfloat16)
-        check(lib.b200_attention_tc_bf16_device(qkv.data_ptr(), None, -1, out3.data_ptr(), B, T, heads, w, causal, 0,
-                                                torch.cuda.current_stream().cuda_stream), "attention_tc2")
-        err3 = (out3.float() - ref).abs()
-        assert not torch.isnan(out3.float()).any()
-        assert bool((err3 <= ref.abs() * 2 ** -7 + 2e-2).all()), "tc2 max err %g" % err3.max().item()
-        # the same kernel with the leftover rows (T mod 128 in 1..4) in attention_tail_rows on a second stream
-        out3b = torch.full((B * T, w), float("nan"), device="cuda", dtype=torch.bfloat16)
-        check(lib.b200_attention_tc_bf16_device(qkv.data_ptr(), None, -3, out3b.data_ptr(), B, T, heads, w, causal, 0,
-                                                torch.cuda.current_stream().cuda_stream), "attention_tc2+tail")
-        torch.cuda.synchronize()
-        err3b = (out3b.float() - ref).abs()
-        assert not torch.isnan(out3b.float()).any()
-        assert bool((err3b <= ref.abs() * 2 ** -7 + 2e-2).all()), "tc2+tail max err %g" % err3b.max().item()
-        # fourth variant (production): one score pass against a Cauchy-Schwarz bound, leftover rows on the FMA pipe
-        out4 = torch.full((B * T, w), float("nan"), device="cuda", dtype=torch.bfloat16)
-        check(lib.b200_attention_tc_bf16_device(qkv.data_ptr(), None, -2, out4.data_ptr(), B, T, heads, w, causal, 0,
-                                                torch.cuda.current_stream().cuda_stream), "attention_tc3")
-        err4 = (out4.float() - ref).abs()
-        assert not torch.isnan(out4.float()).any()
-        assert bool((err4 <= ref.abs() * 2 ** -7 + 2e-2).all()), "tc3 max err %g" % err4.max().item()
 
 
 @pytest.mark.timeout(120)
@@ -269,23 +209,46 @@ def test_tcgen05_attention_second_key_block_dominates():
     out = torch.full((B * T, w), float("nan"), device="cuda", dtype=torch.bfloat16)
     q, k, vv = qkv.float().view(B, T, 3, heads, hd).permute(2, 0, 3, 1, 4)
     ref = (torch.softmax((q @ k.transpose(-1, -2)) * hd ** -0.5, -1) @ vv).transpose(1, 2).reshape(B * T, w)
-    for gen in (-1, -3, -2):
-        out = torch.full((B * T, w), float("nan"), device="cuda", dtype=torch.bfloat16)
-        check(lib.b200_attention_tc_bf16_device(qkv.data_ptr(), None, gen, out.data_ptr(), B, T, heads, w, 0, 0,
-                                                torch.cuda.current_stream().cuda_stream), "attention_tc%d" % (1 - gen))
-        err = (out.float() - ref).abs()
-        assert not torch.isnan(out.float()).any()
-        assert bool((err <= ref.abs() * 2 ** -7 + 2e-2).all()), "gen %d max err %g" % (gen, err.max().item())
+    check(lib.b200_attention_bf16_device(qkv.data_ptr(), out.data_ptr(), B, T, heads, w, 0, 0,
+                                         torch.cuda.current_stream().cuda_stream), "attention")
+    err = (out.float() - ref).abs()
+    assert not torch.isnan(out.float()).any()
+    assert bool((err <= ref.abs() * 2 ** -7 + 2e-2).all()), "max err %g" % err.max().item()
+
+
+@pytest.mark.timeout(120)
+@pytest.mark.parametrize("B,T,heads,causal", [(3, 257, 4, 0), (2, 77, 3, 1), (2, 200, 2, 1), (1, 264, 2, 0), (2, 16, 2, 0)])
+def test_tcgen05_attention_variants_are_bit_identical(B, T, heads, causal):
+    """Work decomposition changes loads and scheduling, not arithmetic: a sample's attention output must not depend on
+    the batch it runs in or on repeated launches (one (head, sample) per block; the query-block split per warp
+    depends on T only).  Every sample alone, twice, must reproduce the batched result bit for bit."""
+    import torch
+    from clip_retrieval_b200._lib import lib, check
+
+    w = heads * 64
+    g = torch.Generator(device="cuda").manual_seed(T * 7 + heads)
+    qkv = torch.randn(B * T, 3 * w, device="cuda", generator=g).bfloat16()
+    st = torch.cuda.current_stream().cuda_stream
+    full = torch.full((B * T, w), float("nan"), device="cuda", dtype=torch.bfloat16)
+    check(lib.b200_attention_bf16_device(qkv.data_ptr(), full.data_ptr(), B, T, heads, w, causal, 0, st), "attention")
+    torch.cuda.synchronize()
+    assert not torch.isnan(full.float()).any()
+    for b in range(B):
+        for _ in range(2):
+            one = torch.full((T, w), float("nan"), device="cuda", dtype=torch.bfloat16)
+            src = qkv[b * T:(b + 1) * T].contiguous()
+            check(lib.b200_attention_bf16_device(src.data_ptr(), one.data_ptr(), 1, T, heads, w, causal, 0, st), "attention")
+            torch.cuda.synchronize()
+            assert torch.equal(one, full[b * T:(b + 1) * T]), "sample %d differs from its batched result" % b
 
 
 @pytest.mark.timeout(120)
 @pytest.mark.parametrize("T,causal", [(257, 0), (77, 1), (200, 0)])
 def test_tcgen05_attention_single_pass_bound_and_fallback(T, causal):
-    """attention_tc3 subtracts a Cauchy-Schwarz bound |q| * max|k| instead of the row maximum.  (a) Keys with a huge
-    norm that are nearly orthogonal to every query push the bound far above the true maximum: the kernel must detect
-    the slack and repeat the pass with exact maxima.  (b) Large aligned scores (true maximum near the bound, scores
-    spread over > 100 log2 units) must neither overflow nor lose the small terms that still matter.  (c) A sample
-    whose neighbour in the batch holds non-finite activations must not be contaminated (per-sample tensor maps)."""
+    """Inputs that broke a bound-based softmax, on the attention kernel the model runs on H100 (online softmax with the
+    running row maximum).  (a) Keys with a huge norm that are nearly orthogonal to every query.  (b) Large aligned
+    scores (spread over > 100 log2 units) must neither overflow nor lose the small terms that still matter.  (c) A
+    sample whose neighbour in the batch holds non-finite activations must not be contaminated."""
     import torch
     from clip_retrieval_b200._lib import lib, check
 
@@ -307,8 +270,8 @@ def test_tcgen05_attention_single_pass_bound_and_fallback(T, causal):
     poisoned = qkv.clone()
     poisoned.view(B, T, 3, heads, hd)[2] = float("inf")
     out = torch.full((B * T, w), float("nan"), device="cuda", dtype=torch.bfloat16)
-    check(lib.b200_attention_tc_bf16_device(poisoned.data_ptr(), None, -2, out.data_ptr(), B, T, heads, w, causal, 0,
-                                            torch.cuda.current_stream().cuda_stream), "attention_tc3")
+    check(lib.b200_attention_bf16_device(poisoned.data_ptr(), out.data_ptr(), B, T, heads, w, causal, 0,
+                                         torch.cuda.current_stream().cuda_stream), "attention")
     q, k, vv = ref_in.float().view(B, T, 3, heads, hd).permute(2, 0, 3, 1, 4)
     s = (q @ k.transpose(-1, -2)) * hd ** -0.5
     if causal:

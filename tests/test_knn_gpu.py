@@ -202,7 +202,7 @@ def test_full_size_properties_sharded_idempotent(b200):
 @pytest.mark.parametrize("nq,k,n,d", [(5, 40, 4096, 768), (64, 40, 60000, 768), (130, 128, 50021, 768), (300, 1, 33000, 512),
                                       (1000, 40, 150000, 768), (17, 40, 20000, 1024)])
 def test_tensor_scan_matches_oracle_and_fma_scan(b200, nq, k, n, d):
-    """The tcgen05 batch scan (fp32 query split into fp16 hi/lo) against the float64 ranking and
+    """The wgmma batch scan (fp32 query split into fp16 hi/lo) against the float64 ranking and
     against the FMA scan of the same index."""
     X = synth_ref.rows_f16(n, d)
     Q = _queries(nq, d)
@@ -223,7 +223,7 @@ def test_tensor_scan_matches_oracle_and_fma_scan(b200, nq, k, n, d):
 @pytest.mark.parametrize("nq,k,n,d", [(129, 40, 50021, 768), (300, 40, 200000, 768), (1000, 10, 150000, 512),
                                       (257, 64, 33000, 1024)])
 def test_hi_only_scan_is_exact(b200, nq, k, n, d):
-    """More than 128 queries: approximate hi-only tcgen05 pass + exact re-score + per-query proof
+    """More than 128 queries: approximate hi-only wgmma pass + exact re-score + per-query proof
     (knn_mma.cu).  Must equal the float64 ranking and the split-mode scan of the same index."""
     X = synth_ref.rows_f16(n, d)
     Q = _queries(nq, d)

@@ -115,123 +115,93 @@ def test_postfilter_oracle_known_answers():
     np.testing.assert_array_equal(R.get_violent_items(P, E), [0, 2, 3])
 
 
-REF_BACK = "/root/reference/clip_retrieval/clip_back.py"
+# What the original clip_back.py / mapper.py return on the seeded inputs below (KnnService and ClipMapper methods
+# extracted with ast and executed unmodified): tests/golden/make_reference_golden.py.
+REF_CALLS = os.path.join(os.path.dirname(__file__), "golden", "reference_calls.json")
 
 
-@pytest.mark.skipif(not os.path.exists(REF_BACK), reason="reference checkout not present (GPU box)")
+def _ref_calls():
+    import json
+
+    with open(REF_CALLS) as fh:
+        return json.load(fh)
+
+
 def test_postfilter_oracle_matches_reference_functions():
     """Pins oracle/postfilter_ref.py on the reference's OWN code: `KnnService.connected_components` and
-    `get_violent_items` (clip_back.py:270-288,321-324) are dependency-free methods, so their source is
-    extracted from the reference file with `ast` and executed here (clip_back itself cannot be imported:
-    flask / faiss are absent) and compared with the restatement on random graphs."""
-    import ast
-    import textwrap
-    from collections import defaultdict
+    `get_violent_items` (clip_back.py:270-288,321-324), run on 20 random graphs and one prompt set; their results
+    are stored in the golden file and compared with the restatement."""
+    import sys
+
     from oracle import postfilter_ref as R
 
-    src = open(REF_BACK).read()
-    tree = ast.parse(src)
-    cls = next(n for n in tree.body if isinstance(n, ast.ClassDef) and n.name == "KnnService")
-    fns = {}
-    for node in cls.body:
-        if isinstance(node, ast.FunctionDef) and node.name in ("connected_components", "get_violent_items"):
-            ns = {"np": np}
-            exec(textwrap.dedent(ast.get_source_segment(src, node)), ns)   # the reference's code, unmodified
-            fns[node.name] = ns[node.name]
-    assert set(fns) == {"connected_components", "get_violent_items"}
-    rng = np.random.default_rng(0)
-    for trial in range(20):
-        k = int(rng.integers(2, 60))
-        A = rng.random((k, k)) < 0.05
-        A = A | A.T | np.eye(k, dtype=bool)
-        neigh = defaultdict(list)
-        for i in range(k):
-            for j in np.nonzero(A[i])[0]:
-                neigh[int(i)].append(int(j))
-        ref_groups = fns["connected_components"](None, neigh)
+    sys.path.insert(0, os.path.join(os.path.dirname(__file__), "golden"))
+    import make_reference_golden as G
+
+    gold = _ref_calls()
+    graphs, E, P = G.postfilter_inputs()
+    assert len(gold["connected_components"]) == len(graphs)
+    for A, ref_groups in zip(graphs, gold["connected_components"]):
         ref_drop = sorted(e for g in ref_groups for e in g[1:])
         assert R.get_non_uniques(None, adjacency=A) == ref_drop
-        assert sorted(map(sorted, R.connected_components(neigh))) == sorted(map(sorted, ref_groups))
-    E = rng.standard_normal((200, 64)).astype(np.float32)
-    P = rng.standard_normal((3, 64)).astype(np.float32)
-    np.testing.assert_array_equal(R.get_violent_items(P, E), fns["get_violent_items"](None, P, E))
+        assert sorted(map(sorted, R.connected_components(G.neighbours(A)))) == ref_groups
+    np.testing.assert_array_equal(R.get_violent_items(P, E), gold["get_violent_items"])
 
 
-REF_MAPPER = "/root/reference/clip_retrieval/clip_inference/mapper.py"
-
-
-@pytest.mark.skipif(not os.path.exists(REF_MAPPER), reason="reference checkout not present (GPU box)")
 def test_mapper_glue_matches_reference_call():
-    """The reference's own `ClipMapper.__call__` (mapper.py:49-78) — extracted with `ast`, executed unmodified
-    with the oracle's encoders standing in for `model.encode_image/encode_text` (all_clip is not installable)
-    — must return exactly what oracle.clip_ref.mapper_image / mapper_text return: this pins the normalise +
-    fp16-cast glue and the five-key output contract on the reference's code, bit for bit."""
-    import ast
-    import textwrap
-    import types
+    """The reference's own `ClipMapper.__call__` (mapper.py:49-78) on fixed seeded features standing in for
+    `model.encode_image/encode_text`: the oracle's glue (normalise + fp16 cast, oracle.clip_ref.mapper_image /
+    mapper_text with the same features) must return exactly what it returned, and the five-key output contract."""
+    import sys
+
     import torch
 
-    src = open(REF_MAPPER).read()
-    tree = ast.parse(src)
-    cls = next(n for n in tree.body if isinstance(n, ast.ClassDef) and n.name == "ClipMapper")
-    call = next(n for n in cls.body if isinstance(n, ast.FunctionDef) and n.name == "__call__")
-    ns = {"torch": torch, "np": np}
-    exec(textwrap.dedent(ast.get_source_segment(src, call)), ns)
-    cfg = clip_ref.CONFIGS["tiny"]
-    sd = clip_ref.make_state_dict(cfg, seed=0)
-    px = clip_ref.synth_images(5, cfg, seed=1)
-    tk = clip_ref.synth_tokens(5, cfg, seed=1)
-    me = types.SimpleNamespace(enable_image=True, enable_text=True, enable_metadata=True, use_mclip=False, device="cpu",
-                               model_img=lambda x: clip_ref.encode_image(sd, cfg, x),
-                               model_txt=lambda x: clip_ref.encode_text(sd, cfg, x))
-    item = {"image_tensor": px, "text_tokens": tk, "image_filename": list("abcde"), "text": list("vwxyz"), "metadata": list("12345")}
-    out = ns["__call__"](me, item)
-    assert list(out) == ["image_embs", "text_embs", "image_filename", "text", "metadata"]
-    assert out["image_embs"].dtype == np.float16 and out["text_embs"].dtype == np.float16
-    assert np.array_equal(out["image_embs"], clip_ref.mapper_image(sd, cfg, px))
-    assert np.array_equal(out["text_embs"], clip_ref.mapper_text(sd, cfg, tk))
-    assert out["image_filename"] == list("abcde") and out["text"] == list("vwxyz") and out["metadata"] == list("12345")
+    sys.path.insert(0, os.path.join(os.path.dirname(__file__), "golden"))
+    import make_reference_golden as G
+
+    gold = _ref_calls()["mapper_call"]
+    fi, ft = G.mapper_features()
+    old_i, old_t = clip_ref.encode_image, clip_ref.encode_text
+    try:
+        clip_ref.encode_image = lambda sd, cfg, x: fi.clone()
+        clip_ref.encode_text = lambda sd, cfg, x: ft.clone()
+        got_i = clip_ref.mapper_image(None, None, torch.zeros(5, 3, 4, 4))
+        got_t = clip_ref.mapper_text(None, None, torch.zeros(5, 77, dtype=torch.int64))
+    finally:
+        clip_ref.encode_image, clip_ref.encode_text = old_i, old_t
+    assert gold["keys"] == ["image_embs", "text_embs", "image_filename", "text", "metadata"]
+    assert gold["dtype"] == "float16" and got_i.dtype == np.float16 and got_t.dtype == np.float16
+    assert np.array_equal(got_i, np.asarray(gold["image_embs"], dtype=np.float32).astype(np.float16))
+    assert np.array_equal(got_t, np.asarray(gold["text_embs"], dtype=np.float32).astype(np.float16))
+    assert gold["image_filename"] == list("abcde") and gold["text"] == list("vwxyz") and gold["metadata"] == list("12345")
 
 
-@pytest.mark.skipif(not os.path.exists(REF_BACK), reason="reference checkout not present (GPU box)")
 def test_index_contract_through_reference_knn_search():
-    """The reference's own `KnnService.knn_search` + `post_filter` + `normalized` (clip_back.py:194-197,313-399),
-    extracted with `ast` and executed unmodified, driven by an index object with the oracle's
-    `search_and_reconstruct` (the contract B200FlatIndex is tested against on the GPU): -1 padding when
-    k > ntotal is truncated, distances stay descending, and dedup runs on the reconstructed rows."""
-    import ast
-    import contextlib
-    import textwrap
-    import types
+    """The reference's own `KnnService.knn_search` + `post_filter` + `normalized` (clip_back.py:194-197,313-399) driven
+    by an index with the oracle's `search_and_reconstruct` (the contract B200FlatIndex is tested against on the GPU):
+    its results, stored in the golden file, must be what the oracle's search and dedup give — -1 padding when
+    k > ntotal is truncated, distances stay descending, and dedup drops the later hit of an exact duplicate."""
+    import sys
+
     from oracle import postfilter_ref as R
 
-    src = open(REF_BACK).read()
-    tree = ast.parse(src)
-    cls = next(n for n in tree.body if isinstance(n, ast.ClassDef) and n.name == "KnnService")
-    timer = types.SimpleNamespace(time=lambda: contextlib.nullcontext())
-    ns = {"np": np, "KNN_INDEX_TIME": timer, "DEDUP_TIME": timer, "SAFETY_TIME": timer}
-    norm = next(n for n in tree.body if isinstance(n, ast.FunctionDef) and n.name == "normalized")
-    exec(ast.get_source_segment(src, norm), ns)
-    for node in cls.body:
-        if isinstance(node, ast.FunctionDef) and node.name in ("knn_search", "post_filter", "connected_components_dedup"):
-            exec(textwrap.dedent(ast.get_source_segment(src, node)), ns)
+    sys.path.insert(0, os.path.join(os.path.dirname(__file__), "golden"))
+    import make_reference_golden as G
 
-    d, n = 64, 30
-    X = synth_ref.rows_f16(n, d)
-    X[7] = X[3]                                     # an exact duplicate pair: dedup must drop the later hit
-    index = types.SimpleNamespace(search_and_reconstruct=lambda q, k: knn_ref.flat_search_and_reconstruct(X, q, k))
-    svc = types.SimpleNamespace(get_non_uniques=lambda emb, threshold=0.94: R.get_non_uniques(emb, threshold))
-    svc.connected_components_dedup = lambda emb: ns["connected_components_dedup"](svc, emb)
-    svc.post_filter = lambda *a: ns["post_filter"](svc, *a)
-    res = types.SimpleNamespace(image_index=index, text_index=index, metadata_is_ordered_by_ivf=False, safety_model=None,
-                                violence_detector=None)
+    gold = _ref_calls()
+    X = G.index_contract_rows()
     q = X[3:4].astype(np.float32)
-    dist, ind = ns["knn_search"](svc, q, "image", 40, res, False, False, False)     # k=40 > ntotal=30 -> -1 tail
-    D, I = knn_ref.flat_search(X, q, 40)
-    assert (I[0, 30:] == -1).all() and len(ind) == 30 and [int(i) for i in ind] == I[0, :30].tolist()
-    assert np.all(np.diff(np.array(dist)) <= 0) and set(int(i) for i in ind[:2]) == {3, 7}
-    dist2, ind2 = ns["knn_search"](svc, q, "image", 40, res, True, False, False)    # with dedup
-    assert len(ind2) == 29 and int(ind2[0]) == 3 and 7 not in [int(i) for i in ind2]
+    D, I, Rr = knn_ref.flat_search_and_reconstruct(X, q, 40)
+    live = I[0] >= 0
+    assert (I[0, 30:] == -1).all() and int(live.sum()) == 30
+    ind, dist = gold["knn_search"]["ind"], gold["knn_search"]["dist"]
+    assert ind == I[0, live].tolist()
+    np.testing.assert_allclose(dist, D[0, live], rtol=0, atol=1e-6)
+    assert np.all(np.diff(np.array(dist)) <= 0) and set(ind[:2]) == {3, 7}
+    drop = set(R.get_non_uniques(Rr[0, live], 0.94))
+    kept = [int(i) for j, i in enumerate(I[0, live]) if j not in drop]
+    ind2 = gold["knn_search_dedup"]["ind"]
+    assert ind2 == kept and len(ind2) == 29 and ind2[0] == 3 and 7 not in ind2
 
 
 def test_ivf_c_restatement_matches_numpy_oracle():

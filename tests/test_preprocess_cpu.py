@@ -1,10 +1,8 @@
 """Pins the preprocess oracle (oracle/preprocess_ref.py): against Pillow + torchvision running here,
-against the committed golden derived from the reference's test_tensors fixtures, and — when
-/root/reference is present (build container) — against those fixtures directly."""
-import glob
+against the committed golden derived from the reference's test_tensors fixtures, and against all seven of those
+fixtures (their JPEGs under golden/ref_images, the sha256 of the reference's tensors in golden/reference_calls.json)."""
 import hashlib
 import os
-import pickle
 
 import numpy as np
 import pytest
@@ -12,7 +10,8 @@ import pytest
 from oracle import preprocess_ref as P
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden", "preprocess_ref.npz")
-REF = "/root/reference/tests/test_clip_inference"
+REF_IMAGES = os.path.join(os.path.dirname(__file__), "golden", "ref_images")
+REF_CALLS = os.path.join(os.path.dirname(__file__), "golden", "reference_calls.json")
 
 
 def _torchvision_transform(n_px):
@@ -54,17 +53,17 @@ def test_oracle_matches_committed_reference_golden():
     assert n == 4
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout not present (GPU box)")
 def test_oracle_matches_reference_fixtures():
+    import json
+
     from PIL import Image
+    with open(REF_CALLS) as fh:
+        want = json.load(fh)["preprocess_fixture_sha256"]
     seen = 0
-    for f in sorted(glob.glob(REF + "/test_tensors/*.pkl")):
-        with open(f, "rb") as fh:
-            o = pickle.load(fh)
-        for name, t in zip(o["image_filename"], o["image_tensor"]):
-            px = np.asarray(Image.open(f"{REF}/test_images/{name}.jpg").convert("RGB"))
-            assert np.array_equal(P.preprocess(px), t.numpy()), name
-            seen += 1
+    for name, digest in sorted(want.items()):
+        px = np.asarray(Image.open(os.path.join(REF_IMAGES, name + ".jpg")).convert("RGB"))
+        assert hashlib.sha256(P.preprocess(px).astype(np.float32).tobytes()).hexdigest() == digest, name
+        seen += 1
     assert seen == 7
 
 

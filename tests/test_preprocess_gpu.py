@@ -99,7 +99,7 @@ def test_gpu_jpeg_decode_feeds_the_transform():
         want = gold[n]
         assert got.shape == want.shape and got.dtype == np.uint8
         diff = np.abs(got.astype(np.int32) - want.astype(np.int32))
-        # measured on B200 / nvJPEG 12.4: 4:4:4 and grey < 1 level on average; 4:2:0 1.5 (chroma upsampling), 99 % within 6
+        # nvJPEG and Pillow upsample chroma differently (4:2:0): bounds on the mean and 99th percentile, not bit-exactness
         assert diff.mean() <= 2.5 and np.percentile(diff, 99) <= 10, (n, diff.mean(), np.percentile(diff, 99), diff.max())
     # the batch path: decode + transform on the device, plus one non-JPEG blob that must fall back to the host decode
     import io

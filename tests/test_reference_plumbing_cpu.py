@@ -1,6 +1,6 @@
 """BASELINE.json configs[0] — "ViT-B/32 clip_inference on 100 synthetic 224^2 images + captions, CPU ref
-(plumbing)" — run through the REFERENCE'S OWN reader, runner and writer (importable by file path in the
-build container: reader.py / runner.py / writer.py only need torch, PIL, fsspec, pyarrow) with the
+(plumbing)" — run through the REFERENCE'S OWN reader, runner and writer (importable by file path from the
+install under oracle/_ref: reader.py / runner.py / writer.py only need torch, PIL, fsspec, pyarrow) with the
 reference's own `ClipMapper.__call__` (extracted with ast; its `all_clip` model is replaced by the oracle's
 ViT-B/32 encoders, seeded weights).  What it pins, on the reference's code:
   * the `preprocess` object `clip_retrieval_b200.load_clip` returns drops into `FilesReader`;
@@ -18,8 +18,10 @@ import numpy as np
 import pytest
 import torch
 
-REF = "/root/reference/clip_retrieval/clip_inference"
-pytestmark = pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout not present (GPU box)")
+# the unmodified reference package, installed by __graft_entry__.build() (oracle/Makefile, target `ref`)
+REF = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "clip_retrieval",
+                   "clip_inference")
+pytestmark = pytest.mark.skipif(not os.path.isdir(REF), reason="oracle/_ref (reference install) not in this tree")
 
 
 def _ref_module(name):

@@ -1,5 +1,5 @@
 """BASELINE.json configs[0] on the GPU: the reference's OWN FilesReader, Runner and NumpyWriter — the unmodified
-install under baseline/_ref, which travels to the GPU box (/root/reference does not) — around the CUDA `ClipMapper`
+install under oracle/_ref, made by build() where the reference checkout exists — around the CUDA `ClipMapper`
 (clip_retrieval/clip_inference/runner.py:27-62 calls `mapper(batch)` and hands the dict to `writer`; worker.py:52-117
 builds exactly these objects).  The written shards are compared row for row with the fp32 oracle mapper applied to
 the same files in the partition order `runner.Sampler` defines, and loaded back through `load_index`."""
@@ -12,7 +12,7 @@ import bench
 from oracle import clip_ref
 
 pytestmark = [pytest.mark.gpu,
-              pytest.mark.skipif(not os.path.isdir(bench.REF_INFERENCE), reason="baseline/_ref (reference install) not in this tree")]
+              pytest.mark.skipif(not os.path.isdir(bench.REF_INFERENCE), reason="oracle/_ref (reference install) not in this tree")]
 
 
 @pytest.mark.timeout(600)

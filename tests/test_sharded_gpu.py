@@ -123,7 +123,7 @@ def test_single_process_sharded_search_c_abi(use_nccl):
         D2, I2 = sh.search(Q, k)
         assert np.array_equal(I, I2) and np.array_equal(D, D2)
     if not use_nccl:
-        assert sh.peer_mode, "B200 boxes map every peer over NVSwitch"
+        assert sh.peer_mode, "NVSwitch boxes map every peer"
 
 
 def _nccl_worker(rank, world, port, out_dir):
