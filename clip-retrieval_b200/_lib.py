@@ -65,7 +65,24 @@ class TensorViewC(C.Structure):
     ]
 
 
-_vp, _i, _i64, _fp = C.c_void_p, C.c_int, C.c_int64, C.POINTER(C.c_float)
+class GemmEpilogueC(C.Structure):
+    _fields_ = [
+        ("bias", C.c_void_p),
+        ("residual", C.c_void_p),
+        ("res_ld", C.c_int64),
+        ("res_row_mod", C.c_int32),
+        ("res_row_off", C.c_int32),
+        ("out_ld", C.c_int64),
+        ("out_group", C.c_int32),
+        ("act", C.c_int32),
+        ("ln_stats", C.c_void_p),
+        ("ln_c", C.c_void_p),
+        ("ln_w", C.c_int32),
+        ("stats_out", C.c_void_p),
+    ]
+
+
+_vp, _i, _i64, _fp =C.c_void_p, C.c_int, C.c_int64, C.POINTER(C.c_float)
 
 # name -> (restype, argtypes).  Kept in one table so tests can check every symbol of the header.
 PROTOTYPES = {
@@ -116,6 +133,8 @@ PROTOTYPES = {
     "b200_layernorm_bf16_device": (_i, [_vp, _vp, _vp, _vp, _i64, _i, _i, _vp]),
     "b200_attention_bf16_device": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "b200_gemm_bf16_device": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "b200_gemm_bf16_ex_device": (_i, [_vp, _vp, _vp, _i, _i, _i, C.POINTER(GemmEpilogueC), _i, _i, _i, _vp]),
+    "b200_row_stats_bf16_device": (_i, [_vp, _i64, _i, _vp, _i, _vp]),
     "b200_index_last_hi_only_fallbacks": (_i, [_vp]),
     "b200_kmeans_train_f16": (_i, [_vp, _i64, _i, _i, _i, C.c_uint64, _i, _vp, _vp, _i]),
     "b200_dedup_device": (_i, [_vp, _i, _i, C.c_float, _vp, _vp, _vp, C.c_size_t, _i, _vp]),

@@ -659,6 +659,11 @@ int b200_layernorm_bf16_device(const void* d_in, void* d_out, const float* d_gam
   return layernorm_rows((const __nv_bfloat16*)d_in, w, (__nv_bfloat16*)d_out, w, d_gamma, d_beta, rows, w,
                         (cudaStream_t)stream);
 }
+int b200_row_stats_bf16_device(const void* d_x, int64_t rows, int w, void* d_stats, int device, void* stream) {
+  B200_CHECK(d_x && d_stats && rows >= 0 && w > 0, B200_ERR_INVALID, "row_stats: bad argument");
+  DeviceGuard g(device);
+  return row_stats((const __nv_bfloat16*)d_x, rows, w, (float2*)d_stats, (cudaStream_t)stream);
+}
 int b200_attention_bf16_device(const void* d_qkv, void* d_out, int B, int T, int heads, int w, int causal, int device,
                                void* stream) {
   B200_CHECK(d_qkv && d_out && B >= 0 && T >= 1, B200_ERR_INVALID, "attention: bad argument");

@@ -76,8 +76,8 @@ static int launch_bn_spec(const CUtensorMap& tmA, const CUtensorMap& tmB, int M,
 // statistics are in use
 template <int BN>
 static int launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, const GemmEpilogue& ep,
-                     cudaStream_t st) {
-  const bool plain = ep.ln_stats == nullptr && ep.stats_out == nullptr && ep.ln_c == nullptr &&
+                     cudaStream_t st, bool generic) {
+  const bool plain = !generic && ep.ln_stats == nullptr && ep.stats_out == nullptr && ep.ln_c == nullptr &&
                      ep.act >= 0 && ep.act <= 2;
   if (plain) {
     switch ((ep.act & 3) | (ep.residual ? 4 : 0)) {
@@ -94,7 +94,7 @@ static int launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int 
 }
 
 int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int M, int N, int K,
-                     const GemmEpilogue& ep, cudaStream_t st) {
+                     const GemmEpilogue& ep, cudaStream_t st, bool generic) {
   B200_CHECK(M >= 1 && N >= 8 && K >= 8 && N % 8 == 0 && K % 8 == 0, B200_ERR_INVALID,
              "gemm: need M>=1 and N, K multiples of 8 (M=%d N=%d K=%d)", M, N, K);
   B200_CHECK(ep.out != nullptr && ep.out_ld % 8 == 0 && ((uintptr_t)ep.out & 15) == 0, B200_ERR_INVALID,
@@ -106,9 +106,9 @@ int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int
   B200_CHECK(ep.ln_stats == nullptr || (ep.ln_c != nullptr && ep.ln_w > 0 && ep.ln_w % 64 == 0), B200_ERR_INVALID,
              "gemm: folded LayerNorm needs c and a row width that is a multiple of 64 (ln_w=%d)", ep.ln_w);
   B200_CHECK(ep.ln_stats == nullptr || ep.ln_w <= 64 * LN_MAX_SLOTS, B200_ERR_UNSUPPORTED, "gemm: folded LayerNorm supports rows of at most %d columns", 64 * LN_MAX_SLOTS);
-  if (bn == 128) return launch_bn<128>(tmA, tmB, M, N, K, ep, st);
-  if (bn == 64) return launch_bn<64>(tmA, tmB, M, N, K, ep, st);
-  if (bn == 32) return launch_bn<32>(tmA, tmB, M, N, K, ep, st);
+  if (bn == 128) return launch_bn<128>(tmA, tmB, M, N, K, ep, st, generic);
+  if (bn == 64) return launch_bn<64>(tmA, tmB, M, N, K, ep, st, generic);
+  if (bn == 32) return launch_bn<32>(tmA, tmB, M, N, K, ep, st, generic);
   set_error("gemm: unsupported column block %d", bn);
   return B200_ERR_INVALID;
 }
@@ -117,16 +117,26 @@ int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int
 
 using namespace b200;
 
-extern "C" int b200_gemm_bf16_device(const void* d_A, const void* d_W, const float* d_bias, const void* d_residual,
-                                     void* d_C, int M, int N, int K, int act, int device, void* stream) {
-  B200_CHECK(d_A && d_W && d_C, B200_ERR_INVALID, "gemm: null operand");
-  B200_CHECK(act >= 0 && act <= 2, B200_ERR_INVALID, "gemm: act=%d", act);
+// The stand-alone entries: A [M, K] and W [N, K] contiguous, everything else as the epilogue says.  bn = 0 takes
+// gemm_pick_bn's width (raised to 128 when row statistics are written, as the model does).
+static int gemm_entry(const void* d_A, const void* d_W, int M, int N, int K, GemmEpilogue ep, int bn, bool generic,
+                      int device, void* stream) {
+  B200_CHECK(d_A && d_W && ep.out, B200_ERR_INVALID, "gemm: null operand");
+  B200_CHECK(ep.act >= 0 && ep.act <= 2, B200_ERR_INVALID, "gemm: act=%d", ep.act);
+  B200_CHECK(bn == 0 || bn == 32 || bn == 64 || bn == 128, B200_ERR_INVALID, "gemm: unsupported column block %d", bn);
   DeviceGuard g(device);
-  const int sms = sm_count(device);
-  const int bn = gemm_pick_bn(M, N, sms);
+  if (bn == 0) {
+    bn = gemm_pick_bn(M, N, sm_count(device));
+    if (ep.stats_out != nullptr && bn < 128) bn = 128;
+  }
   CUtensorMap tmA, tmB;
   B200_TRY(make_tmap_2d(&tmA, d_A, 1, (uint64_t)M, (uint64_t)K, (uint64_t)K, GEMM_BM, GEMM_BK));
   B200_TRY(make_tmap_2d(&tmB, d_W, 1, (uint64_t)N, (uint64_t)K, (uint64_t)K, (uint32_t)bn, GEMM_BK));
+  return gemm_bf16_launch(tmA, tmB, bn, M, N, K, ep, (cudaStream_t)stream, generic);
+}
+
+extern "C" int b200_gemm_bf16_device(const void* d_A, const void* d_W, const float* d_bias, const void* d_residual,
+                                     void* d_C, int M, int N, int K, int act, int device, void* stream) {
   GemmEpilogue ep;
   ep.bias = d_bias;
   ep.residual = (const __nv_bfloat16*)d_residual;
@@ -134,5 +144,25 @@ extern "C" int b200_gemm_bf16_device(const void* d_A, const void* d_W, const flo
   ep.out = (__nv_bfloat16*)d_C;
   ep.out_ld = N;
   ep.act = act;
-  return gemm_bf16_launch(tmA, tmB, bn, M, N, K, ep, (cudaStream_t)stream);
+  return gemm_entry(d_A, d_W, M, N, K, ep, 0, false, device, stream);
+}
+
+extern "C" int b200_gemm_bf16_ex_device(const void* d_A, const void* d_W, void* d_C, int M, int N, int K,
+                                        const b200_gemm_epilogue* e, int bn, int force_generic, int device, void* stream) {
+  B200_CHECK(e != nullptr, B200_ERR_INVALID, "gemm: null epilogue");
+  GemmEpilogue ep;
+  ep.bias = e->bias;
+  ep.residual = (const __nv_bfloat16*)e->residual;
+  ep.res_ld = e->res_ld > 0 ? e->res_ld : N;
+  ep.res_row_mod = e->res_row_mod;
+  ep.res_row_off = e->res_row_off;
+  ep.out = (__nv_bfloat16*)d_C;
+  ep.out_ld = e->out_ld > 0 ? e->out_ld : N;
+  ep.out_group = e->out_group;
+  ep.act = e->act;
+  ep.ln_stats = (const float2*)e->ln_stats;
+  ep.ln_c = e->ln_c;
+  ep.ln_w = e->ln_w;
+  ep.stats_out = (float2*)e->stats_out;
+  return gemm_entry(d_A, d_W, M, N, K, ep, bn, force_generic != 0, device, stream);
 }

@@ -344,9 +344,10 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 // host side (gemm.cu)
 int make_tmap_2d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t rows, uint64_t cols, uint64_t ld_elems,
                  uint32_t box_rows, uint32_t box_cols);
-// tmB must have boxes of bn rows x 64 columns.
+// tmB must have boxes of bn rows x 64 columns.  generic = true launches the run-time epilogue flavour (SPEC = -1)
+// even where a compile-time flavour applies (the tests check that both store the same bits).
 int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int M, int N, int K,
-                     const GemmEpilogue& ep, cudaStream_t st);
+                     const GemmEpilogue& ep, cudaStream_t st, bool generic = false);
 // Pick the column-block width for a GEMM with N output columns (128, or 64 / 32 when the grid would be
 // under-filled).
 int gemm_pick_bn(int M, int N, int sms);

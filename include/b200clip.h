@@ -230,6 +230,37 @@ int b200_clip_set_profiling(b200_clip* m, int on);
 int b200_gemm_bf16_device(const void* d_A, const void* d_W, const float* d_bias, const void* d_residual,
                           void* d_C, int M, int N, int K, int act, int device, void* stream);
 
+/* The same GEMM with the whole epilogue the model uses (what b200_gemm_bf16_device is a special case of), for the
+ * kernel-level tests of every tile width and epilogue flavour.  Row r of the product goes to output row
+ *   r                                                  (out_group == 0)
+ *   (r / out_group) * (out_group + 1) + 1 + r % out_group  (out_group > 0: one cls row skipped per group)
+ * and reads residual row r, or res_row_off + r % res_row_mod when res_row_mod > 0.  ld 0 means N.
+ * Folded LayerNorm (ln_stats != NULL): A is the raw row x, W carries gamma (W' = W * gamma), bias = d, and the
+ * result is rstd * (x W'^T - mean * ln_c) + d, with mean / rstd (eps 1e-5) combined from ln_w / 64 (mean, M2)
+ * float2 records per row.  stats_out != NULL: one (mean, M2) float2 record per 64 stored columns of every row
+ * (needs N % 64 == 0 and 128-wide column blocks).
+ * bn: 0 = the width the library picks (128 whenever stats_out is set), else 32, 64 or 128.
+ * force_generic != 0: the epilogue flavour that decides every feature at run time, even where a compile-time
+ * flavour exists; both store the same bits. */
+typedef struct b200_gemm_epilogue {
+  const float* bias;        /* [N] fp32 or NULL */
+  const void* residual;     /* bf16, added after the activation, or NULL; may equal the output (in-place update) */
+  int64_t res_ld;
+  int32_t res_row_mod, res_row_off;
+  int64_t out_ld;
+  int32_t out_group;
+  int32_t act;              /* 0 none, 1 quick_gelu, 2 gelu(erf) */
+  const void* ln_stats;     /* float2 [M, ln_w / 64] or NULL */
+  const float* ln_c;        /* [N] */
+  int32_t ln_w;
+  void* stats_out;          /* float2 [M, N / 64] or NULL */
+} b200_gemm_epilogue;
+int b200_gemm_bf16_ex_device(const void* d_A, const void* d_W, void* d_C, int M, int N, int K,
+                             const b200_gemm_epilogue* ep, int bn, int force_generic, int device, void* stream);
+/* The (mean, M2) records of the folded LayerNorm for rows of w bf16 values (w % 64 == 0): d_stats float2
+ * [rows, w / 64], record s of a row = mean and sum of squared deviations of its columns 64 s .. 64 s + 63. */
+int b200_row_stats_bf16_device(const void* d_x, int64_t rows, int w, void* d_stats, int device, void* stream);
+
 /* Stand-alone entries of the two other embed kernels, for their parity tests:
  * LayerNorm (eps 1e-5) over rows of `w` bf16 values; multi-head attention over a fused qkv buffer
  * [B*T, 3w] (q | k | v, heads of w/heads columns) -> [B*T, w], causal != 0 adds the text mask. */

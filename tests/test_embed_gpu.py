@@ -49,6 +49,58 @@ def test_layernorm_matches_fp32_reference():
         assert bool((err <= ref.abs() * 2 ** -7 + 1e-2).all()), "rows=%d w=%d max err %g" % (rows, w, err.max().item())
 
 
+def attention_ref64(qkv, B, T, heads, hd, causal):
+    """float64 softmax(Q K^T hd^-0.5 [+ causal mask]) V of the bf16 qkv buffer, its per-element error bound, and P.
+
+    Bound: |out - ref| <= 2^-8 |ref| + (2^-8 + 2 ds + 2^-18) * sum_t P_t |v_t|.
+    - 2^-8 |ref|: the bf16 store.
+    - 2^-8 * sum_t P_t |v_t|: both kernels round P to bf16 (relative 2^-8) before P.V, and normalise by the fp32 sum
+      of the unrounded P.
+    - ds: the fp32 error of a score, (hd / 16 + 2) * 2^-22 * max_t |q| . |k_t| * hd^-0.5 (see test_gemm_gpu.py); a
+      score off by ds moves P_t by at most a factor exp(2 ds).
+    - 2^-18: exp2f, the fp32 P.V sums and the final division.
+    A key dropped or wrongly admitted moves the output by P_t |v_t|, which this bound only sees when P_t is large:
+    the one-hot probes below check every key of the tile edges exactly."""
+    import torch
+
+    q, k, v = qkv.double().view(B, T, 3, heads, hd).permute(2, 0, 3, 1, 4)
+    sc = hd ** -0.5
+    s = (q @ k.transpose(-1, -2)) * sc
+    mag = (q.abs() @ k.abs().transpose(-1, -2)) * sc
+    if causal:
+        mask = torch.ones(T, T, dtype=torch.bool, device=qkv.device).triu_(1)
+        s = s.masked_fill(mask, float("-inf"))
+        mag = mag.masked_fill(mask, 0.0)
+    P = torch.softmax(s, -1)
+    ds = (hd // 16 + 2) * 2.0 ** -22 * mag.amax(-1, keepdim=True)
+    ref = P @ v
+    spread = P @ v.abs()
+    bound = 2.0 ** -8 * ref.abs() + (2.0 ** -8 + 2 * ds + 2.0 ** -18) * spread
+    flat = lambda t: t.transpose(1, 2).reshape(B * T, heads * hd)   # noqa: E731
+    return flat(ref), flat(bound), P
+
+
+def run_attention(qkv, B, T, heads, w, causal):
+    import torch
+    from clip_retrieval_b200._lib import lib, check
+
+    out = torch.full((B * T, w), float("nan"), device="cuda", dtype=torch.bfloat16)
+    check(lib.b200_attention_bf16_device(qkv.data_ptr(), out.data_ptr(), B, T, heads, w, causal, 0,
+                                         torch.cuda.current_stream().cuda_stream), "attention")
+    torch.cuda.synchronize()
+    return out
+
+
+def assert_attention_close(out, ref, bound, what=""):
+    import torch
+
+    got = out.double()
+    assert not torch.isnan(got).any(), what
+    err = (got - ref).abs()
+    assert bool((err <= bound).all()), "%s: max err / bound %g (max err %g)" % (what, (err / bound).max().item(),
+                                                                                 err.max().item())
+
+
 @pytest.mark.timeout(120)
 @pytest.mark.parametrize("B,T,heads,hd,causal", [
     (2, 50, 12, 64, 0), (3, 77, 8, 64, 1), (2, 257, 16, 64, 0), (1, 257, 16, 80, 0), (2, 1, 2, 64, 0),
@@ -56,23 +108,91 @@ def test_layernorm_matches_fp32_reference():
 ])
 def test_attention_matches_fp32_reference(B, T, heads, hd, causal):
     import torch
-    from clip_retrieval_b200._lib import lib, check
 
     w = heads * hd
     g = torch.Generator(device="cuda").manual_seed(B * 1000 + T + w)
     qkv = torch.randn(B * T, 3 * w, device="cuda", generator=g).bfloat16()
-    out = torch.full((B * T, w), float("nan"), device="cuda", dtype=torch.bfloat16)
-    check(lib.b200_attention_bf16_device(qkv.data_ptr(), out.data_ptr(), B, T, heads, w, causal, 0,
-                                         torch.cuda.current_stream().cuda_stream), "attention")
-    q, k, v = qkv.float().view(B, T, 3, heads, hd).permute(2, 0, 3, 1, 4)
-    s = (q @ k.transpose(-1, -2)) * hd ** -0.5
+    out = run_attention(qkv, B, T, heads, w, causal)
+    ref, bound, _ = attention_ref64(qkv, B, T, heads, hd, causal)
+    assert_attention_close(out, ref, bound)
+
+
+def _attention_shapes():
+    """(T, heads, head dim, causal) of both towers of every architecture the model table names, and head dim 64 on
+    both sides of the wgmma (T <= 320) / mma.sync switch and around the 64-row / 64-key blocks."""
+    import clip_retrieval_b200 as m
+
+    shapes = set()
+    for a in m.ARCHS.values():
+        shapes.add(((a.image_size // a.patch) ** 2 + 1, a.vision.heads, a.vision.width // a.vision.heads, 0))
+        shapes.add((a.context_length, a.text.heads, a.text.width // a.text.heads, 1))
+    for T in (63, 64, 65, 127, 128, 129, 319, 320, 321):
+        for causal in (0, 1):
+            shapes.add((T, 2, 64, causal))
+    return sorted(shapes)
+
+
+@pytest.mark.timeout(120)
+@pytest.mark.parametrize("T,heads,hd,causal", _attention_shapes())
+def test_attention_model_shapes_match_float64(T, heads, hd, causal):
+    """Every model's attention shape at B = 2 (T = 577 of ViT-L/14@336px, head dim 80 of ViT-H/14, its text tower)
+    and the kernel switch-over, against the float64 reference."""
+    import torch
+
+    B, w = 2, heads * hd
+    g = torch.Generator(device="cuda").manual_seed(T * 3 + w + causal)
+    qkv = torch.randn(B * T, 3 * w, device="cuda", generator=g).bfloat16()
+    out = run_attention(qkv, B, T, heads, w, causal)
+    ref, bound, _ = attention_ref64(qkv, B, T, heads, hd, causal)
+    assert_attention_close(out, ref, bound, "T=%d heads=%d hd=%d causal=%d" % (T, heads, hd, causal))
+
+
+PROBE_DIMS = (0, 7, 8, 63)
+
+
+@pytest.mark.timeout(120)
+@pytest.mark.parametrize("causal", [0, 1])
+@pytest.mark.parametrize("T,hd", [(65, 64), (129, 64), (257, 64), (320, 64), (321, 64), (577, 64), (257, 80),
+                                  (77, 64), (130, 128)])
+def test_attention_one_hot_v_probes(T, hd, causal):
+    """V is zero except one 1.0 per (sample, head): key t, dim j.  The output of that (sample, head) in dim j is then
+    P[r, t] alone, and every other output is exactly 0.0: the rows a causal mask hides (r < t), every other dim
+    (this pins the V-transpose swizzle), and the dims of the neighbouring samples' probes (a key of the next sample
+    read through the same tile, or a row of another sample, would show there).  One launch of 5 samples x 9 heads
+    carries each key of {0, 1, 31, 32, 63, 64, 65, T-2, T-1} (those < T) with 5 dims {0, 7, 8, 63, hd-1}; within a
+    head, the 5 samples use 5 different dims."""
+    import torch
+
+    keys = sorted({t for t in (0, 1, 31, 32, 63, 64, 65, T - 2, T - 1) if t < T})
+    dims = sorted(set(PROBE_DIMS + (hd - 1,)) | ({33} if hd - 1 in PROBE_DIMS else set()))
+    B, heads = 5, len(keys)
+    w = heads * hd
+    g = torch.Generator(device="cuda").manual_seed(T + hd + causal)
+    qkv = torch.randn(B * T, 3 * w, device="cuda", generator=g)
+    view = qkv.view(B, T, 3, heads, hd)
+    view[:, :, 2] = 0.0
+    probe = {}
+    for h, t in enumerate(keys):
+        for b in range(B):
+            j = dims[(b + h) % len(dims)]
+            view[b, t, 2, h, j] = 1.0
+            probe[(b, h)] = (t, j)
+    qkv = qkv.bfloat16()
+    out = run_attention(qkv, B, T, heads, w, causal).view(B, T, heads, hd).double()
+    _, _, P = attention_ref64(qkv, B, T, heads, hd, causal)
+    want = torch.zeros(B, T, heads, hd, dtype=torch.float64, device="cuda")
+    for (b, h), (t, j) in probe.items():
+        want[b, :, h, j] = P[b, h, :, t]
+    zero = want == 0
+    assert bool((out[zero] == 0).all()), "%d outputs that must be exactly 0 are not (first: %s)" % (
+        int((out[zero] != 0).sum()), torch.nonzero(zero & (out != 0))[:1].tolist())
+    err = (out[~zero] - want[~zero]).abs()
+    # P rounded to bf16, then the output: two roundings of at most 2^-8 each, plus the fp32 normalisation
+    assert bool((err <= (2.0 ** -7 + 2.0 ** -12) * want[~zero]).all()), \
+        "probe P[r, t]: max rel err %g" % (err / want[~zero]).max().item()
     if causal:
-        s = s + torch.full((T, T), float("-inf"), device="cuda").triu_(1)
-    ref = (torch.softmax(s, -1) @ v).transpose(1, 2).reshape(B * T, w)
-    err = (out.float() - ref).abs()
-    assert not torch.isnan(out.float()).any()
-    # P is rounded to bf16 before P.V and the output to bf16: 2^-7 relative + 2e-2 absolute
-    assert bool((err <= ref.abs() * 2 ** -7 + 2e-2).all()), "max err %g" % err.max().item()
+        for (b, h), (t, j) in probe.items():
+            assert bool((out[b, :t, h, j] == 0).all()) and bool((out[b, t:, h, j] > 0).all()), (b, h, t, j)
 
 
 @pytest.mark.timeout(300)
@@ -168,35 +288,25 @@ def test_zero_feature_row_is_nan_like_reference():
 @pytest.mark.parametrize("B,T,heads,causal", [(2, 257, 16, 0), (3, 77, 8, 1), (2, 50, 12, 0), (1, 1, 2, 0), (5, 128, 4, 1),
                                               (1, 320, 2, 0), (40, 257, 16, 0), (3, 260, 2, 0), (2, 256, 2, 1), (7, 129, 3, 0), (2, 258, 3, 1)])
 def test_tcgen05_attention_matches_fp32_reference(B, T, heads, causal):
-    """The shapes that pinned the Blackwell tensor-core attention, now on the attention kernel the model runs on H100:
-    head dimension 64 at sequence lengths around its 16-row query blocks and 32-key blocks (T = 1, 128, 129, 256..260,
-    320) and at the ViT-L/14 batch shape, against a plain fp32 PyTorch softmax(QK^T)V of the same bf16 inputs."""
+    """Head dimension 64 on the wgmma attention kernel (T <= 320) at sequence lengths around its 64-row query tiles
+    and 64-key blocks (T = 1, 128, 129, 256..260, 320) and at the ViT-L/14 batch shape, against the float64
+    reference of the same bf16 inputs."""
     import torch
-    from clip_retrieval_b200._lib import lib, check
 
     hd = 64
     w = heads * hd
     g = torch.Generator(device="cuda").manual_seed(B * 1000 + T + w)
     qkv = torch.randn(B * T, 3 * w, device="cuda", generator=g).bfloat16()
-    out = torch.full((B * T, w), float("nan"), device="cuda", dtype=torch.bfloat16)
-    check(lib.b200_attention_bf16_device(qkv.data_ptr(), out.data_ptr(), B, T, heads, w, causal, 0,
-                                         torch.cuda.current_stream().cuda_stream), "attention")
-    q, k, vv = qkv.float().view(B, T, 3, heads, hd).permute(2, 0, 3, 1, 4)
-    s = (q @ k.transpose(-1, -2)) * hd ** -0.5
-    if causal:
-        s = s + torch.full((T, T), float("-inf"), device="cuda").triu_(1)
-    ref = (torch.softmax(s, -1) @ vv).transpose(1, 2).reshape(B * T, w)
-    err = (out.float() - ref).abs()
-    assert not torch.isnan(out.float()).any()
-    assert bool((err <= ref.abs() * 2 ** -7 + 2e-2).all()), "max err %g" % err.max().item()
+    out = run_attention(qkv, B, T, heads, w, causal)
+    ref, bound, _ = attention_ref64(qkv, B, T, heads, hd, causal)
+    assert_attention_close(out, ref, bound)
 
 
 @pytest.mark.timeout(120)
 def test_tcgen05_attention_second_key_block_dominates():
-    """Scores whose maximum sits far into the row (keys >= 128 scaled up): a guard for any softmax
-    variant that processes the key columns in blocks with a running reference maximum."""
+    """Scores whose maximum sits far into the row (keys >= 128 scaled up): the online softmax must rescale what it
+    accumulated under the running maximum of the earlier key blocks."""
     import torch
-    from clip_retrieval_b200._lib import lib, check
 
     B, T, heads, hd = 3, 257, 4, 64
     w = heads * hd
@@ -206,22 +316,17 @@ def test_tcgen05_attention_second_key_block_dominates():
     kview[0, 128:, 1] *= 6.0          # sample 0: every row sees much larger scores in the second block
     kview[1, 200:230, 1, 0] *= 6.0    # sample 1, head 0 only
     qkv = qkv.bfloat16()
-    out = torch.full((B * T, w), float("nan"), device="cuda", dtype=torch.bfloat16)
-    q, k, vv = qkv.float().view(B, T, 3, heads, hd).permute(2, 0, 3, 1, 4)
-    ref = (torch.softmax((q @ k.transpose(-1, -2)) * hd ** -0.5, -1) @ vv).transpose(1, 2).reshape(B * T, w)
-    check(lib.b200_attention_bf16_device(qkv.data_ptr(), out.data_ptr(), B, T, heads, w, 0, 0,
-                                         torch.cuda.current_stream().cuda_stream), "attention")
-    err = (out.float() - ref).abs()
-    assert not torch.isnan(out.float()).any()
-    assert bool((err <= ref.abs() * 2 ** -7 + 2e-2).all()), "max err %g" % err.max().item()
+    out = run_attention(qkv, B, T, heads, w, 0)
+    ref, bound, _ = attention_ref64(qkv, B, T, heads, hd, 0)
+    assert_attention_close(out, ref, bound)
 
 
 @pytest.mark.timeout(120)
 @pytest.mark.parametrize("B,T,heads,causal", [(3, 257, 4, 0), (2, 77, 3, 1), (2, 200, 2, 1), (1, 264, 2, 0), (2, 16, 2, 0)])
 def test_tcgen05_attention_variants_are_bit_identical(B, T, heads, causal):
     """Work decomposition changes loads and scheduling, not arithmetic: a sample's attention output must not depend on
-    the batch it runs in or on repeated launches (one (head, sample) per block; the query-block split per warp
-    depends on T only).  Every sample alone, twice, must reproduce the batched result bit for bit."""
+    the batch it runs in or on repeated launches (one (query tile, head, sample) per CTA; keys of the next sample
+    that a tile reads are masked).  Every sample alone, twice, must reproduce the batched result bit for bit."""
     import torch
     from clip_retrieval_b200._lib import lib, check
 
@@ -245,8 +350,8 @@ def test_tcgen05_attention_variants_are_bit_identical(B, T, heads, causal):
 @pytest.mark.timeout(120)
 @pytest.mark.parametrize("T,causal", [(257, 0), (77, 1), (200, 0)])
 def test_tcgen05_attention_single_pass_bound_and_fallback(T, causal):
-    """Inputs that broke a bound-based softmax, on the attention kernel the model runs on H100 (online softmax with the
-    running row maximum).  (a) Keys with a huge norm that are nearly orthogonal to every query.  (b) Large aligned
+    """Inputs that break a softmax built on a precomputed score bound; the kernels run an online softmax with the
+    running row maximum.  (a) Keys with a huge norm that are nearly orthogonal to every query.  (b) Large aligned
     scores (spread over > 100 log2 units) must neither overflow nor lose the small terms that still matter.  (c) A
     sample whose neighbour in the batch holds non-finite activations must not be contaminated."""
     import torch

@@ -200,10 +200,12 @@ def test_full_size_properties_sharded_idempotent(b200):
 
 @pytest.mark.timeout(300)
 @pytest.mark.parametrize("nq,k,n,d", [(5, 40, 4096, 768), (64, 40, 60000, 768), (130, 128, 50021, 768), (300, 1, 33000, 512),
-                                      (1000, 40, 150000, 768), (17, 40, 20000, 1024)])
+                                      (1000, 40, 150000, 768), (17, 40, 20000, 1024),
+                                      (40, 40, 30011, 200), (300, 40, 30011, 1280), (64, 64, 20000, 2048)])
 def test_tensor_scan_matches_oracle_and_fma_scan(b200, nq, k, n, d):
     """The wgmma batch scan (fp32 query split into fp16 hi/lo) against the float64 ranking and
-    against the FMA scan of the same index."""
+    against the FMA scan of the same index.  d = 200 ends inside a 64-column TMA box (zero-filled K tail);
+    d = 1280 and 2048 run past 1024 columns."""
     X = synth_ref.rows_f16(n, d)
     Q = _queries(nq, d)
     idx = b200.B200FlatIndex(d)
@@ -221,7 +223,8 @@ def test_tensor_scan_matches_oracle_and_fma_scan(b200, nq, k, n, d):
 
 @pytest.mark.timeout(300)
 @pytest.mark.parametrize("nq,k,n,d", [(129, 40, 50021, 768), (300, 40, 200000, 768), (1000, 10, 150000, 512),
-                                      (257, 64, 33000, 1024)])
+                                      (257, 64, 33000, 1024), (200, 40, 30011, 200), (257, 40, 30011, 1280),
+                                      (300, 10, 20000, 2048)])
 def test_hi_only_scan_is_exact(b200, nq, k, n, d):
     """More than 128 queries: approximate hi-only wgmma pass + exact re-score + per-query proof
     (knn_mma.cu).  Must equal the float64 ranking and the split-mode scan of the same index."""
