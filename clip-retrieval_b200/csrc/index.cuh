@@ -35,8 +35,7 @@ struct b200_index {
   int64_t npending = 0, pending_cap = 0;
   int64_t max_list = 0;
   std::vector<uint32_t> pending_lists;   // explicit list of every pending row (0xFFFFFFFF: assign by max inner product)
-  uint32_t* id_to_slot = nullptr;         // device [ntotal]: inverse of row_ids, built on the first reconstruct-by-id
-  int64_t id_to_slot_n = -1;
+  uint32_t* id_to_slot = nullptr;         // device [ntotal]: inverse of row_ids, rebuilt whenever the store changes
 
   // scratch
   void* ws[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // 0: scan internals; 1..3: callers; 4,5: hi-only mode

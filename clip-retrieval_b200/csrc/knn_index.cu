@@ -25,16 +25,17 @@ int range_scan(b200_index* idx, const __half* rows, int64_t n, const float* d_q,
                unsigned int cap, unsigned int* d_count, cudaStream_t st);
 int ivf_range_scan(b200_index* idx, const float* d_q, float thresh, unsigned long long* d_out, unsigned int cap,
                    unsigned int* d_count, cudaStream_t st);
-int ivf_id_to_slot(b200_index* idx, const uint32_t** out);
 
 __global__ void f32_to_f16_kernel(const float* __restrict__ in, __half* __restrict__ out, int64_t count) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < count) out[i] = __float2half_rn(in[i]);
 }
 
-// Reconstruct: one warp per (query, rank); slot < 0 or key 0 -> all-ones bits (what FAISS leaves).
+// Reconstruct: one warp per (query, rank); key 0 -> all-ones bits (what FAISS leaves).  Keys hold local ids;
+// `id_to_slot` (IVF) maps them to the list-ordered store, flat indexes store rows in id order.
 __global__ void gather_rows_from_keys_kernel(const __half* __restrict__ rows, int d,
-                                             const unsigned long long* __restrict__ keys, int64_t count,
+                                             const unsigned long long* __restrict__ keys,
+                                             const uint32_t* __restrict__ id_to_slot, int64_t count,
                                              float* __restrict__ out) {
   const int lane = threadIdx.x & 31;
   const int64_t w = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -44,7 +45,9 @@ __global__ void gather_rows_from_keys_kernel(const __half* __restrict__ rows, in
   if (key == 0ull) {
     for (int j = lane; j < d; j += 32) o[j] = __uint_as_float(0xffffffffu);
   } else {
-    const __half* r = rows + (int64_t)key_id(key) * d;
+    uint32_t slot = key_id(key);
+    if (id_to_slot) slot = id_to_slot[slot];
+    const __half* r = rows + (int64_t)slot * d;
     for (int j = lane; j < d; j += 32) o[j] = __half2float(r[j]);
   }
 }
@@ -150,18 +153,17 @@ static int search_device_impl(b200_index* idx, const float* d_q, int nq, int k, 
   void* ws = nullptr;
   B200_TRY(index_ws(idx, 1, (size_t)nq * k * 8, &ws));
   unsigned long long* keys = (unsigned long long*)ws;
-  const uint32_t* slot_to_id = nullptr;
   if (idx->nlist > 0) {
     B200_TRY(ivf_finalize(idx));
-    B200_TRY(ivf_search_keys(idx, d_q, nq, k, keys, st));
-    slot_to_id = idx->row_ids;
+    B200_TRY(ivf_search_keys(idx, d_q, nq, k, keys, st));   // keys carry insertion ids, not slots
   } else {
     B200_TRY(scan_topk_keys(idx, idx->rows, idx->ntotal, d_q, nq, k, keys, st));
   }
-  B200_TRY(decode_keys(keys, (int64_t)nq * k, idx->id_base, slot_to_id, d_D, d_I, st));
+  B200_TRY(decode_keys(keys, (int64_t)nq * k, idx->id_base, nullptr, d_D, d_I, st));
   if (d_R) {
     const int64_t count = (int64_t)nq * k;
-    gather_rows_from_keys_kernel<<<(unsigned)((count + 7) / 8), 256, 0, st>>>(idx->rows, idx->d, keys, count, d_R);
+    gather_rows_from_keys_kernel<<<(unsigned)((count + 7) / 8), 256, 0, st>>>(idx->rows, idx->d, keys,
+                                                                               idx->id_to_slot, count, d_R);
     B200_LAUNCH_OK();
   }
   return B200_OK;
@@ -558,7 +560,7 @@ int b200_index_reconstruct_device(b200_index* idx, const int64_t* d_ids, int64_t
   if (idx->nlist > 0) {
     std::lock_guard<std::mutex> lock(idx->mu);
     B200_TRY(ivf_finalize(idx));
-    B200_TRY(ivf_id_to_slot(idx, &id_to_slot));
+    id_to_slot = idx->id_to_slot;
   }
   gather_rows_from_slots_kernel<<<(unsigned)((n + 7) / 8), 256, 0, (cudaStream_t)stream>>>(
       idx->rows, idx->d, d_ids, idx->id_base, idx->ntotal, id_to_slot, n, d_R);

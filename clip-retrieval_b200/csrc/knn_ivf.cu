@@ -2,11 +2,14 @@
 // reference touches through faiss.extract_index_ivf(index).nprobe (clip_back.py:357-361,368-369).
 //
 // Layout in HBM: rows are stored LIST AFTER LIST (`rows`, fp16 [ntotal, d]) with `list_offsets`
-// [nlist+1] and `row_ids` (slot -> insertion id), so a probed list is one contiguous stream.
+// [nlist+1] and `row_ids` (slot -> insertion id), so a probed list is one contiguous stream; its inverse
+// `id_to_slot` is rebuilt whenever the store changes (finalize, add_synthetic), never during a search.
 // Search = (1) coarse: the flat scan kernel over the centroid matrix with k = nprobe;
 //          (2) list scan: one CTA per (query, probe, segment) streams its slice of the list with the
 //              same warp-per-row 128-bit loads / fp32 FMA / per-warp replace-worst lists as the flat
 //              scan; (3) the chunked bitonic select over the per-warp candidates of each query.
+// List-scan keys carry the insertion id (row_ids[slot]), not the slot, so equal scores come back in
+// ascending id order even when the tied rows sit in different lists (explicit lists of an index file).
 // HBM-bound: bytes per query = nprobe * (N/nlist) * d * 2 (+ nlist * d * 2 for the coarse step).
 #include "index.cuh"
 #include "topk.cuh"
@@ -154,9 +157,9 @@ __global__ void sorted_src_to_ids_kernel(const uint32_t* __restrict__ src, int64
 // ---- list scan ---------------------------------------------------------------------------------------
 template <int CH>
 __global__ void __launch_bounds__(256)
-ivf_scan_kernel(const uint4* __restrict__ X, int cpr, const float* __restrict__ Q, const unsigned long long* __restrict__ probes,
-                int nprobe, int segs, const int64_t* __restrict__ offsets, int k,
-                unsigned long long* __restrict__ out_keys, int64_t out_stride_q) {
+ivf_scan_kernel(const uint4* __restrict__ X, const uint32_t* __restrict__ row_ids, int cpr, const float* __restrict__ Q,
+                const unsigned long long* __restrict__ probes, int nprobe, int segs, const int64_t* __restrict__ offsets,
+                int k, unsigned long long* __restrict__ out_keys, int64_t out_stride_q) {
   extern __shared__ unsigned long long s_keys[];  // [warps][k]
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   const int seg = blockIdx.x % segs;
@@ -218,9 +221,13 @@ ivf_scan_kernel(const uint4* __restrict__ X, int cpr, const float* __restrict__ 
       warp_transpose_reduce<4>(acc, lane);
       const float s = acc[0];
       const int64_t my_r = r0 + (lane >> 3);
-      const unsigned long long key = make_key(s, (uint32_t)my_r);
       const bool live = ((lane & 7) == 0) && my_r < end && (s == s);
-      unsigned pend = __ballot_sync(FULL, live && key > worst);
+      // Only a row scoring at least the worst kept score can enter the list; the insertion id that breaks its
+      // ties is loaded for those rows alone (every row while the list fills, rarely after).
+      const bool reach = live && f32_to_ordered(s) >= (uint32_t)(worst >> 32);
+      unsigned long long key = 0ull;
+      if (reach) key = make_key(s, __ldg(row_ids + my_r));
+      unsigned pend = __ballot_sync(FULL, reach && key > worst);
       while (pend) {
         const int src = __ffs(pend) - 1;
         pend &= pend - 1;
@@ -234,8 +241,8 @@ ivf_scan_kernel(const uint4* __restrict__ X, int cpr, const float* __restrict__ 
   for (int j = lane; j < k; j += 32) o[j] = wkeys[j];
 }
 
-typedef void (*ivf_scan_fn)(const uint4*, int, const float*, const unsigned long long*, int, int, const int64_t*, int,
-                            unsigned long long*, int64_t);
+typedef void (*ivf_scan_fn)(const uint4*, const uint32_t*, int, const float*, const unsigned long long*, int, int,
+                            const int64_t*, int, unsigned long long*, int64_t);
 static ivf_scan_fn pick_ivf_scan(int ch) {
   switch (ch) {
     case 1: return ivf_scan_kernel<1>;
@@ -321,6 +328,19 @@ static int refresh_host_offsets(b200_index* idx) {
   return B200_OK;
 }
 
+// id -> slot: the inverse of row_ids, for reconstruct-by-id and for the rows of search_and_reconstruct.  Built
+// whenever the store changes so that a search (possibly under CUDA-graph capture) never allocates it.
+static int build_id_to_slot(b200_index* idx) {
+  if (idx->id_to_slot) B200_CUDA(cudaFree(idx->id_to_slot));
+  idx->id_to_slot = nullptr;
+  if (idx->ntotal == 0) return B200_OK;
+  B200_CUDA(cudaMalloc((void**)&idx->id_to_slot, (size_t)idx->ntotal * 4));
+  invert_ids_kernel<<<(unsigned)((idx->ntotal + 255) / 256), 256>>>(idx->row_ids, idx->ntotal, idx->id_to_slot);
+  B200_LAUNCH_OK();
+  B200_CUDA(cudaDeviceSynchronize());
+  return B200_OK;
+}
+
 int ivf_finalize(b200_index* idx) {
   if (idx->npending == 0) return B200_OK;
   const int d = idx->d, cpr = d / 8, ch = (cpr + 31) / 32;
@@ -377,7 +397,7 @@ int ivf_finalize(b200_index* idx) {
   idx->row_ids = nids;
   idx->capacity = n;
   idx->ntotal = n;
-  idx->id_to_slot_n = -1;
+  B200_TRY(build_id_to_slot(idx));
   return refresh_host_offsets(idx);
 }
 
@@ -426,6 +446,7 @@ int ivf_add_synthetic(b200_index* idx, int64_t n, int64_t row0, const b200_synth
   B200_CUDA(cudaFree(to_free));
   idx->ntotal = n;
   idx->capacity = n;
+  B200_TRY(build_id_to_slot(idx));
   return refresh_host_offsets(idx);
 }
 
@@ -488,8 +509,8 @@ int ivf_search_keys(b200_index* idx, const float* d_q, int nq, int k, unsigned l
     }
     B200_CUDA(index_record(idx, idx->ev[idx->ev_used], st));
     fn<<<(unsigned)((int64_t)qb * nprobe * segs), threads, smem, st>>>(
-        reinterpret_cast<const uint4*>(idx->rows), cpr, d_q + (size_t)q0 * d, probes + (size_t)q0 * nprobe, nprobe, segs,
-        idx->list_offsets, k, k1, M);
+        reinterpret_cast<const uint4*>(idx->rows), idx->row_ids, cpr, d_q + (size_t)q0 * d, probes + (size_t)q0 * nprobe,
+        nprobe, segs, idx->list_offsets, k, k1, M);
     B200_LAUNCH_OK();
     B200_CUDA(index_record(idx, idx->ev[idx->ev_used + 1], st));
     idx->ev_used += 2;
@@ -500,26 +521,10 @@ int ivf_search_keys(b200_index* idx, const float* d_q, int nq, int k, unsigned l
   return B200_OK;
 }
 
-// id -> slot map for reconstruct-by-id on the list-ordered store (built once per finalize)
-int ivf_id_to_slot(b200_index* idx, const uint32_t** out) {
-  if (idx->id_to_slot_n != idx->ntotal) {
-    if (idx->id_to_slot) B200_CUDA(cudaFree(idx->id_to_slot));
-    idx->id_to_slot = nullptr;
-    if (idx->ntotal > 0) {
-      B200_CUDA(cudaMalloc((void**)&idx->id_to_slot, (size_t)idx->ntotal * 4));
-      invert_ids_kernel<<<(unsigned)((idx->ntotal + 255) / 256), 256>>>(idx->row_ids, idx->ntotal, idx->id_to_slot);
-      B200_LAUNCH_OK();
-      B200_CUDA(cudaDeviceSynchronize());
-    }
-    idx->id_to_slot_n = idx->ntotal;
-  }
-  *out = idx->id_to_slot;
-  return B200_OK;
-}
-
 // ---- range search over the probed lists (index.range_search on an IVF index: clip_filter.py:52) -----------
 // FAISS IndexIVF::range_search visits the nprobe lists of the query and reports every row whose inner product
-// exceeds the threshold.  One CTA per (probe, segment); hits are appended as (score, slot) keys.
+// exceeds the threshold.  One CTA per (probe, segment); hits are appended as (score, slot) keys (decoded to ids
+// through row_ids; the host sorts the hits by id, so no tie order is needed here).
 template <int CH>
 __global__ void __launch_bounds__(256)
 ivf_range_kernel(const uint4* __restrict__ X, int cpr, const float* __restrict__ Q, const unsigned long long* __restrict__ probes,

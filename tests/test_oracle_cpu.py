@@ -99,6 +99,56 @@ def test_ivf_oracle_nprobe_all_equals_flat():
     assert np.array_equal(m[1], If)
 
 
+def test_ivf_check_accepts_the_oracle_and_rejects_wrong_results():
+    """knn_ref.ivf_check (the checker of tests/test_ivf_scale_gpu.py) passes the numpy IVF oracle's own result,
+    skips only queries with a near-tie at the nprobe boundary, and fails each kind of wrong result."""
+    d, nlist, n, k, nprobe = 64, 40, 6000, 25, 3
+    X = synth_ref.rows_f16(n, d, clustered=True, nlist=nlist)
+    C = synth_ref.centroids_f32(nlist, d).astype(np.float16)
+    Q = synth_ref.rows_f32(30, d, seed=9, clustered=True, nlist=nlist)
+    assign = knn_ref.ivf_assign(X, C)
+    D, I, _ = knn_ref.ivf_search(X, assign, C, Q, k, nprobe, id_base=7)
+    ok, msg, checked = knn_ref.ivf_check(D, I, X, assign, C, Q, k, nprobe, id_base=7)
+    assert ok and checked == 30, msg
+    # an exact tie at query 0's nprobe boundary (two equal centroids): a result from either list is not a
+    # failure; the one the float64 ranking does not pick is skipped
+    order = np.argsort(-knn_ref.scores_f64(C, Q[:1])[0], kind="stable")
+    a, b = sorted(order[nprobe - 1:nprobe + 1])
+    Ct = C.copy()
+    Ct[b] = Ct[a]
+    kt = 400   # reaches into every probed list
+    Dt, It, _ = knn_ref.ivf_search(X, assign, Ct, Q, kt, nprobe)
+    ok, msg, checked = knn_ref.ivf_check(Dt, It, X, assign, Ct, Q, kt, nprobe)
+    assert ok and checked == 30, (msg, checked)
+    Ca = Ct.copy()
+    Ca[a] = -Ca[a]
+    Dt[:1], It[:1], _ = knn_ref.ivf_search(X, assign, Ca, Q[:1], kt, nprobe)   # probes list b instead of a
+    ok, msg, checked = knn_ref.ivf_check(Dt, It, X, assign, Ct, Q, kt, nprobe)
+    assert ok and checked == 29, (msg, checked)
+    wrong = []
+    I2 = I.copy(); I2[4, [0, 1]] = I2[4, [1, 0]]; wrong.append((D, I2))                  # order
+    outside = np.nonzero(~np.isin(assign, np.argsort(-knn_ref.scores_f64(C, Q[5:6])[0])[:nprobe]))[0][0]
+    I2 = I.copy(); I2[5, -1] = 7 + outside; wrong.append((D, I2))                        # row of an unprobed list
+    D2 = D.copy(); D2[6, 3] += 1e-5; wrong.append((D2, I))                              # score error
+    D2, I2 = D.copy(), I.copy(); D2[7, -1], I2[7, -1] = knn_ref.NEG, -1; wrong.append((D2, I2))  # short result
+    for Dw, Iw in wrong:
+        ok, msg, _ = knn_ref.ivf_check(Dw, Iw, X, assign, C, Q, k, nprobe, id_base=7)
+        assert not ok
+    # exact ties across lists: ascending id is required, slot order is not enough
+    Xd = np.concatenate([X, X[:1], X[:1]])
+    ad = np.concatenate([assign, [assign[0] - 1 if assign[0] > 0 else 1, assign[0]]])
+    Qd = X[:1].astype(np.float32)
+    Dd, Id, _ = knn_ref.ivf_search(Xd, ad, C, Qd, 3, nlist)
+    assert list(Id[0]) == [0, n, n + 1]
+    assert knn_ref.ivf_check(Dd, Id, Xd, ad, C, Qd, 3, nlist)[0]
+    assert not knn_ref.ivf_check(Dd, Id[:, [1, 0, 2]], Xd, ad, C, Qd, 3, nlist)[0]
+    # probes on empty lists: the result must be all padding
+    ae = np.where(assign == assign[0], (assign[0] + 1) % nlist, assign)
+    De, Ie, _ = knn_ref.ivf_search(X, ae, C, X[:1].astype(np.float32), 5, 1)
+    assert (Ie == -1).all() and knn_ref.ivf_check(De, Ie, X, ae, C, X[:1].astype(np.float32), 5, 1)[0]
+    assert not knn_ref.ivf_check(De, Ie + 1, X, ae, C, X[:1].astype(np.float32), 5, 1)[0]
+
+
 def test_postfilter_oracle_known_answers():
     """oracle/postfilter_ref.py (clip_back.py:270-324 restated): hand-checkable graphs."""
     from oracle import postfilter_ref as R
