@@ -1,13 +1,20 @@
 // K4 (SURVEY.md §2.2) on wgmma for head dimension 64 and T <= 320 (every CLIP tower of the benchmark configs but the
 // ViT-H/14 image tower, whose head dimension is 80): softmax(Q K^T * hd^-0.5 [+ causal mask]) V per (sample, head).
 //
-// One CTA = one warpgroup = 64 query rows of one (sample, head).  TMA brings the Q tile and every 64-key block of K
-// (boxes of 64 rows x 64 columns of the qkv buffer, 128B swizzle) behind one mbarrier; V is read with ordinary loads
-// and written transposed (keys contiguous, same swizzle) so that P.V takes it as a K-major operand, with keys >= T
-// zeroed.  Per key block: S = Q K^T (4 x wgmma m64n64k16, both operands in shared memory), mask, online softmax in
-// fp32 registers, then O += P V (4 x wgmma m64n64k16 with P as the register A operand: the S accumulator fragment,
-// packed to bf16, is exactly the A fragment of the next MMA).  Rows and keys past T of a tile come from the
-// neighbouring sample or the TMA zero fill: their scores are masked and their outputs never stored.
+// One CTA = one (sample, head), two consumer warpgroups.  At the start one thread issues every TMA load of the head:
+// the first Q tile of each warpgroup, then K and V block by block (64 keys x 64 dims each, 128B swizzle, one mbarrier
+// per block so that the first Q K^T waits for K_0 alone), then the second Q tile of each warpgroup.  The map is 3-D over
+// (column, token, sample) and clipped at T, so rows >= T of every box are zeros: the next sample is never read.
+// Warpgroup g takes query tiles g, g + 2, g + 4 (64 rows each) from two Q slots; when the last Q K^T of a tile has
+// completed, the slot is refilled with the tile after next.  K and V are read once per (sample, head) and stay in shared
+// memory for every query tile.
+//
+// Per key block j of a query tile: S = Q K^T (4 x wgmma m64nNk16, both operands in shared memory), online softmax in
+// fp32 registers, then O += P V (wgmma m64n64k16 with P as the register A operand -- the S accumulator fragment packed
+// to bf16 is exactly the A fragment -- and V as the MN-major B operand straight from its TMA tile).  S_{j+1} is issued
+// before the softmax of block j, so the tensor cores work on it while the warpgroup computes exponentials.  Only the
+// last key block of a tile (the end of the sequence, or the causal diagonal) is masked, and it is computed on
+// N = 16 * ceil(keys / 16) columns and as many k16 steps of P V.
 #include "embed_kernels.cuh"
 #include "gemm.cuh"
 #include "ptx.cuh"
@@ -16,142 +23,235 @@
 namespace b200 {
 
 constexpr int ATTW_HD = 64;
-constexpr int ATTW_BQ = 64;                        // query rows per CTA
+constexpr int ATTW_BQ = 64;                        // query rows per tile
 constexpr int ATTW_BK = 64;                        // keys per block
 constexpr int ATTW_MAX_T = 320;
 constexpr int ATTW_MAX_KB = ATTW_MAX_T / ATTW_BK;  // 5
 constexpr int ATTW_TILE = 64 * 128;                // one 64 x 64 bf16 tile, 8 KB
-constexpr int ATTW_SMEM = (1 + 2 * ATTW_MAX_KB) * ATTW_TILE + 64 + 1024;
+constexpr int ATTW_QSLOTS = 4;                     // two Q tiles per consumer warpgroup
+constexpr int ATTW_THREADS = 256;
+// barriers: K blocks, V blocks, Q slots
+constexpr int ATTW_NBAR = 2 * ATTW_MAX_KB + ATTW_QSLOTS;
+constexpr int ATTW_BAR_BYTES = 8 * ATTW_NBAR;
+
+// K and V of every key block plus the Q slots, and 1 KB to align the tiles.  The barriers live in that alignment gap
+// when it is large enough, else after the tiles: at T = 320 this is 115 712 B, so two CTAs share an SM.
+static int attw_smem_bytes(int T) {
+  return (2 * ((T + ATTW_BK - 1) / ATTW_BK) + ATTW_QSLOTS) * ATTW_TILE + 1024;
+}
 
 __device__ __forceinline__ uint32_t attw_pack(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
-__global__ void __launch_bounds__(128)
-attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const __nv_bfloat16* __restrict__ qkv,
-                       __nv_bfloat16* __restrict__ out, int T, int w, float scale_log2e, int causal) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = ptx::smem_u32(smem_raw);
-  uint8_t* base = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
-  uint8_t* sQ = base;
-  uint8_t* sK = base + ATTW_TILE;                          // [kb] tiles: 64 keys x 64 dims
-  uint8_t* sVt = sK + ATTW_MAX_KB * ATTW_TILE;             // [kb] tiles: 64 dims x 64 keys
-  uint64_t* bar = reinterpret_cast<uint64_t*>(sVt + ATTW_MAX_KB * ATTW_TILE);
+// S = Q K^T of one key block on `cols` (16, 32, 48 or 64) columns; accumulator registers past cols / 2 are not written.
+__device__ __forceinline__ void attw_qk(float (&s)[32], uint64_t dq, uint64_t dk, int cols) {
+  ptx::wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < ATTW_HD / 16; k++) {
+    const uint64_t a = dq + (uint64_t)(k * 2), b = dk + (uint64_t)(k * 2);
+    const uint32_t acc = k != 0 ? 1u : 0u;
+    if (cols == 64) ptx::wgmma_m64n64k16_bf16(s, a, b, acc);
+    else if (cols == 48) ptx::wgmma_m64n48k16_bf16(*reinterpret_cast<float(*)[24]>(&s[0]), a, b, acc);
+    else if (cols == 32) ptx::wgmma_m64n32k16_bf16(*reinterpret_cast<float(*)[16]>(&s[0]), a, b, acc);
+    else ptx::wgmma_m64n16k16_bf16(*reinterpret_cast<float(*)[8]>(&s[0]), a, b, acc);
+  }
+  ptx::wgmma_commit();
+}
 
-  const int q0 = blockIdx.x * ATTW_BQ, h = blockIdx.y, b = blockIdx.z;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int kend = causal ? min(T, q0 + ATTW_BQ) : T;      // keys this tile can see
-  const int nkb = (kend + ATTW_BK - 1) / ATTW_BK;
-  const int64_t row0 = (int64_t)b * T;
+struct AttwRow {
+  float m_lo, m_hi, l_lo, l_hi;
+};
+
+// Online softmax of one score block (in place: s becomes P, unnormalised) and the matching rescale of O.
+// accumulator fragment: register i holds row 16*warp + lane/4 + 8*((i/2)%2), column 8*(i/4) + 2*(lane%4) + i%2
+template <bool MASK>
+__device__ __forceinline__ void attw_softmax(float (&s)[32], float (&o)[32], AttwRow& r, int lane, int key0, int kend,
+                                             int r_lo, int causal, float scale_log2e) {
+  float bm_lo = -INFINITY, bm_hi = -INFINITY;
+#pragma unroll
+  for (int i = 0; i < 32; i++) {
+    if (MASK) {
+      const int key = key0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+      const int row = r_lo + 8 * ((i >> 1) & 1);
+      if (key >= kend || (causal && key > row)) s[i] = -INFINITY;
+    }
+    if ((i >> 1) & 1) bm_hi = fmaxf(bm_hi, s[i]);
+    else bm_lo = fmaxf(bm_lo, s[i]);
+  }
+  bm_lo = fmaxf(bm_lo, __shfl_xor_sync(0xffffffffu, bm_lo, 1));
+  bm_lo = fmaxf(bm_lo, __shfl_xor_sync(0xffffffffu, bm_lo, 2));
+  bm_hi = fmaxf(bm_hi, __shfl_xor_sync(0xffffffffu, bm_hi, 1));
+  bm_hi = fmaxf(bm_hi, __shfl_xor_sync(0xffffffffu, bm_hi, 2));
+  const float mn_lo = fmaxf(r.m_lo, bm_lo), mn_hi = fmaxf(r.m_hi, bm_hi);
+  // rows that have seen no live key yet keep m = -inf; avoid (-inf) - (-inf)
+  const float ms_lo = mn_lo == -INFINITY ? 0.f : mn_lo, ms_hi = mn_hi == -INFINITY ? 0.f : mn_hi;
+  const float a_lo = exp2f((r.m_lo - ms_lo) * scale_log2e), a_hi = exp2f((r.m_hi - ms_hi) * scale_log2e);
+  r.m_lo = mn_lo;
+  r.m_hi = mn_hi;
+  r.l_lo *= a_lo;
+  r.l_hi *= a_hi;
+#pragma unroll
+  for (int i = 0; i < 32; i++) {
+    const bool hi = (i >> 1) & 1;
+    o[i] *= hi ? a_hi : a_lo;
+    // (s - m) * scale rounded as written, not fused into one fma: P, and so every embedding, stays bit for bit what
+    // the earlier one-tile-per-CTA kernel computed
+    s[i] = exp2f((s[i] - (hi ? ms_hi : ms_lo)) * scale_log2e);
+    if (hi) r.l_hi += s[i];
+    else r.l_lo += s[i];
+  }
+}
+
+// 4 x 4 transpose of 32-bit words across the lanes of a quad: lane q returns, in b[k], word q of lane k's a[].
+__device__ __forceinline__ void attw_quad_transpose(const uint32_t (&a)[4], uint32_t (&b)[4], int q) {
+#pragma unroll
+  for (int k = 0; k < 4; k++) b[k] = a[k];
+#pragma unroll
+  for (int x = 1; x < 4; x++) {
+    const int p = q ^ x;   // partner lane in the quad: it wants my a[p], I want its a[q]
+    const uint32_t send = p == 0 ? a[0] : p == 1 ? a[1] : p == 2 ? a[2] : a[3];
+    const uint32_t got = __shfl_xor_sync(0xffffffffu, send, x);
+#pragma unroll
+    for (int k = 0; k < 4; k++)
+      if (k == p) b[k] = got;
+  }
+}
+
+__global__ void __launch_bounds__(ATTW_THREADS, 2)
+attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __restrict__ out, int T, int w,
+                       float scale_log2e, int causal) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t pad = (1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u;
+  uint8_t* base = smem_raw + pad;
+  const int nkb = (T + ATTW_BK - 1) / ATTW_BK;      // key blocks of the head; also its query tiles
+  uint8_t* sK = base;                                // [nkb] 64 keys x 64 dims
+  uint8_t* sV = sK + nkb * ATTW_TILE;                // [nkb] 64 keys x 64 dims
+  uint8_t* sQ = sV + nkb * ATTW_TILE;                // [ATTW_QSLOTS]: slots 2g, 2g + 1 belong to warpgroup g
+  uint64_t* bar = reinterpret_cast<uint64_t*>(pad >= (uint32_t)ATTW_BAR_BYTES ? smem_raw : sQ + ATTW_QSLOTS * ATTW_TILE);
+  uint64_t* barK = bar;
+  uint64_t* barV = bar + ATTW_MAX_KB;
+  uint64_t* barQ = bar + 2 * ATTW_MAX_KB;
+
+  const int h = blockIdx.x, b = blockIdx.y;
+  // the warpgroup index through a shuffle: the compiler then knows it is uniform across the warp, and so is every
+  // branch around a wgmma that depends on it (else it serialises the wgmmas)
+  const int wg = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 7, 0);
+  const int tid = threadIdx.x & 127, warp = tid >> 5, lane = tid & 31;
+  const int cq = h * ATTW_HD, ck = w + h * ATTW_HD, cv = 2 * w + h * ATTW_HD;
+  // query tile t: warpgroup t % 2, its (t / 2)-th tile, in slot 2 (t % 2) + (t / 2) % 2, phase (t / 4) % 2
+  auto load_q = [&](int t) {
+    const int slot = 2 * (t & 1) + ((t >> 1) & 1);
+    ptx::mbar_arrive_expect_tx(barQ + slot, ATTW_TILE);
+    ptx::tma_load_3d(sQ + slot * ATTW_TILE, &tmQKV, barQ + slot, cq, t * ATTW_BQ, b);
+  };
 
   if (threadIdx.x == 0) {
     ptx::prefetch_tensormap(&tmQKV);
-    ptx::mbar_init(bar, 1);
+    for (int i = 0; i < ATTW_NBAR; i++) ptx::mbar_init(bar + i, 1);
     ptx::fence_barrier_init();
   }
   __syncthreads();
   if (threadIdx.x == 0) {
-    ptx::mbar_arrive_expect_tx(bar, (uint32_t)(1 + nkb) * ATTW_TILE);
-    ptx::tma_load_2d(sQ, &tmQKV, bar, h * ATTW_HD, (int32_t)(row0 + q0));
-    for (int j = 0; j < nkb; j++) ptx::tma_load_2d(sK + j * ATTW_TILE, &tmQKV, bar, w + h * ATTW_HD, (int32_t)(row0 + j * ATTW_BK));
-  }
-  // V^T: element (dim d, key t) of block t / 64 at row d, 16-byte chunk ((t % 64) / 8) ^ (d % 8), as the 128B swizzle
-  // places it; keys >= T are zero (P is 0 there, and 0 * garbage could be NaN)
-  const __nv_bfloat16* vbase = qkv + row0 * 3 * w + 2 * w + h * ATTW_HD;
-  for (int i = threadIdx.x; i < nkb * ATTW_BK * 8; i += blockDim.x) {
-    const int t = i >> 3, c = i & 7;
-    uint4 v = make_uint4(0u, 0u, 0u, 0u);
-    if (t < T) v = *reinterpret_cast<const uint4*>(vbase + (int64_t)t * 3 * w + c * 8);
-    const __nv_bfloat16* e = reinterpret_cast<const __nv_bfloat16*>(&v);
-    uint8_t* tile = sVt + (t >> 6) * ATTW_TILE;
-    const int tk = t & 63;
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-      const int d = c * 8 + k;
-      *reinterpret_cast<__nv_bfloat16*>(tile + d * 128 + ((((tk >> 3) ^ (d & 7)) << 4) | ((tk & 7) << 1))) = e[k];
+    load_q(0);
+    if (nkb > 1) load_q(1);
+    for (int j = 0; j < nkb; j++) {
+      ptx::mbar_arrive_expect_tx(barK + j, ATTW_TILE);
+      ptx::tma_load_3d(sK + j * ATTW_TILE, &tmQKV, barK + j, ck, j * ATTW_BK, b);
+      ptx::mbar_arrive_expect_tx(barV + j, ATTW_TILE);
+      ptx::tma_load_3d(sV + j * ATTW_TILE, &tmQKV, barV + j, cv, j * ATTW_BK, b);
     }
+    for (int t = 2; t < nkb && t < ATTW_QSLOTS; t++) load_q(t);
   }
-  ptx::fence_proxy_async();   // generic-proxy writes of V^T -> visible to wgmma
-  __syncthreads();
-  ptx::mbar_wait(bar, 0);
 
-  // accumulator fragment: register i holds row 16*warp + lane/4 + 8*((i/2)%2), column 8*(i/4) + 2*(lane%4) + i%2
-  const int r_lo = q0 + 16 * warp + (lane >> 2), r_hi = r_lo + 8;
-  float o[32];
+  __nv_bfloat16* ob = out + (int64_t)b * T * w + h * ATTW_HD;
+  for (int t = wg; t < nkb; t += 2) {
+    const int slot = 2 * wg + ((t >> 1) & 1);
+    const int q0 = t * ATTW_BQ;
+    const int kend = causal ? min(T, q0 + ATTW_BQ) : T;       // keys this tile can see
+    const int nkt = (kend + ATTW_BK - 1) / ATTW_BK;
+    const int last_cols = 16 * ((kend - (nkt - 1) * ATTW_BK + 15) / 16);
+    const int r_lo = q0 + 16 * warp + (lane >> 2);
+    ptx::mbar_wait(barQ + slot, (t >> 2) & 1);
+    const uint64_t dq = ptx::wgmma_desc_k_sw128(ptx::smem_u32(sQ + slot * ATTW_TILE));
+
+    float o[32];
 #pragma unroll
-  for (int i = 0; i < 32; i++) o[i] = 0.f;
-  float m_lo = -INFINITY, m_hi = -INFINITY, l_lo = 0.f, l_hi = 0.f;
-  const uint64_t dq = ptx::wgmma_desc_k_sw128(ptx::smem_u32(sQ));
-
-  for (int j = 0; j < nkb; j++) {
+    for (int i = 0; i < 32; i++) o[i] = 0.f;
+    ptx::fence_regs(o);   // zeroed before S_0 is issued, not in the middle of the wgmma pipeline
+    AttwRow r{-INFINITY, -INFINITY, 0.f, 0.f};
     float s[32];
-    ptx::wgmma_fence();
-    const uint64_t dk = ptx::wgmma_desc_k_sw128(ptx::smem_u32(sK + j * ATTW_TILE));
-#pragma unroll
-    for (int k = 0; k < ATTW_HD / 16; k++) ptx::wgmma_bf16<64>(s, dq + (uint64_t)(k * 2), dk + (uint64_t)(k * 2), k != 0 ? 1u : 0u);
-    ptx::wgmma_commit();
-    ptx::wgmma_wait<0>();
-    ptx::fence_regs(s);
 
-    float bm_lo = -INFINITY, bm_hi = -INFINITY;
+    auto issue_s = [&](int j) {
+      ptx::mbar_wait(barK + j, 0);
+      attw_qk(s, dq, ptx::wgmma_desc_k_sw128(ptx::smem_u32(sK + j * ATTW_TILE)), j == nkt - 1 ? last_cols : 64);
+      ptx::fence_regs(s);
+    };
+    // block j: S_j and P_{j-1} V_{j-1} are in flight.  Once they are done: softmax of block j, then O += P_j V_j and
+    // S_{j+1} = Q K_{j+1}^T go to the tensor cores back to back (S is free once P_j is packed)
+    auto block = [&](int j) {
+      const bool last = j == nkt - 1;
+      ptx::wgmma_wait<0>();
+      ptx::fence_regs(s);
+      ptx::fence_regs(o);
+      if (last) {
+        // the tile's last Q K^T is done: once every warp of the warpgroup is here, the Q slot can be refilled
+        ptx::named_barrier_sync(1 + wg, 128);
+        if (tid == 0 && t + ATTW_QSLOTS < nkb) load_q(t + ATTW_QSLOTS);
+        attw_softmax<true>(s, o, r, lane, j * ATTW_BK, kend, r_lo, causal, scale_log2e);
+      } else {
+        attw_softmax<false>(s, o, r, lane, j * ATTW_BK, kend, r_lo, causal, scale_log2e);
+      }
+      // P as the A operand: k-slice kk covers accumulator column blocks 2kk, 2kk+1
+      uint32_t pa[4][4];
 #pragma unroll
-    for (int i = 0; i < 32; i++) {
-      const int key = j * ATTW_BK + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
-      const int row = ((i >> 1) & 1) ? r_hi : r_lo;
-      if (key >= T || (causal && key > row)) s[i] = -INFINITY;
-      if ((i >> 1) & 1) bm_hi = fmaxf(bm_hi, s[i]);
-      else bm_lo = fmaxf(bm_lo, s[i]);
-    }
-    bm_lo = fmaxf(bm_lo, __shfl_xor_sync(0xffffffffu, bm_lo, 1));
-    bm_lo = fmaxf(bm_lo, __shfl_xor_sync(0xffffffffu, bm_lo, 2));
-    bm_hi = fmaxf(bm_hi, __shfl_xor_sync(0xffffffffu, bm_hi, 1));
-    bm_hi = fmaxf(bm_hi, __shfl_xor_sync(0xffffffffu, bm_hi, 2));
-    const float mn_lo = fmaxf(m_lo, bm_lo), mn_hi = fmaxf(m_hi, bm_hi);
-    // rows that have seen no live key yet keep m = -inf; avoid (-inf) - (-inf)
-    const float ms_lo = mn_lo == -INFINITY ? 0.f : mn_lo, ms_hi = mn_hi == -INFINITY ? 0.f : mn_hi;
-    const float a_lo = exp2f((m_lo - ms_lo) * scale_log2e), a_hi = exp2f((m_hi - ms_hi) * scale_log2e);
-    m_lo = mn_lo;
-    m_hi = mn_hi;
-    l_lo *= a_lo;
-    l_hi *= a_hi;
+      for (int kk = 0; kk < 4; kk++) {
+        pa[kk][0] = attw_pack(s[8 * kk + 0], s[8 * kk + 1]);
+        pa[kk][1] = attw_pack(s[8 * kk + 2], s[8 * kk + 3]);
+        pa[kk][2] = attw_pack(s[8 * kk + 4], s[8 * kk + 5]);
+        pa[kk][3] = attw_pack(s[8 * kk + 6], s[8 * kk + 7]);
+      }
+      const int ksteps = last ? last_cols / 16 : 4;
+      ptx::mbar_wait(barV + j, 0);
+      ptx::wgmma_fence();
+      const uint64_t dv = ptx::wgmma_desc_mn_sw128(ptx::smem_u32(sV + j * ATTW_TILE));
 #pragma unroll
-    for (int i = 0; i < 32; i++) {
-      const bool hi = (i >> 1) & 1;
-      o[i] *= hi ? a_hi : a_lo;
-      s[i] = exp2f((s[i] - (hi ? ms_hi : ms_lo)) * scale_log2e);
-      if (hi) l_hi += s[i];
-      else l_lo += s[i];
-    }
-    // P as the A operand: k-slice kk covers accumulator column blocks 2kk, 2kk+1
-    uint32_t pa[4][4];
-#pragma unroll
-    for (int kk = 0; kk < 4; kk++) {
-      pa[kk][0] = attw_pack(s[8 * kk + 0], s[8 * kk + 1]);
-      pa[kk][1] = attw_pack(s[8 * kk + 2], s[8 * kk + 3]);
-      pa[kk][2] = attw_pack(s[8 * kk + 4], s[8 * kk + 5]);
-      pa[kk][3] = attw_pack(s[8 * kk + 6], s[8 * kk + 7]);
-    }
-    ptx::wgmma_fence();
-    const uint64_t dv = ptx::wgmma_desc_k_sw128(ptx::smem_u32(sVt + j * ATTW_TILE));
-#pragma unroll
-    for (int kk = 0; kk < 4; kk++) ptx::wgmma_m64n64k16_bf16_rs(o, pa[kk], dv + (uint64_t)(kk * 2), 1u);
-    ptx::wgmma_commit();
+      for (int kk = 0; kk < 4; kk++)
+        if (kk < ksteps) ptx::wgmma_m64n64k16_bf16_rs_tb(o, pa[kk], dv + (uint64_t)kk * ptx::WGMMA_DESC_MN_SW128_K16, 1u);
+      ptx::wgmma_commit();
+      ptx::fence_regs(o);
+      if (!last) issue_s(j + 1);
+    };
+
+    issue_s(0);
+#pragma unroll 1
+    for (int j = 0; j < nkt; j++) block(j);
     ptx::wgmma_wait<0>();
     ptx::fence_regs(o);
-  }
 
-  l_lo += __shfl_xor_sync(0xffffffffu, l_lo, 1);
-  l_lo += __shfl_xor_sync(0xffffffffu, l_lo, 2);
-  l_hi += __shfl_xor_sync(0xffffffffu, l_hi, 1);
-  l_hi += __shfl_xor_sync(0xffffffffu, l_hi, 2);
-  const float i_lo = 1.0f / l_lo, i_hi = 1.0f / l_hi;
-  __nv_bfloat16* ob = out + row0 * w + h * ATTW_HD;
+    float l_lo = r.l_lo, l_hi = r.l_hi;
+    l_lo += __shfl_xor_sync(0xffffffffu, l_lo, 1);
+    l_lo += __shfl_xor_sync(0xffffffffu, l_lo, 2);
+    l_hi += __shfl_xor_sync(0xffffffffu, l_hi, 1);
+    l_hi += __shfl_xor_sync(0xffffffffu, l_hi, 2);
+    const float i_lo = 1.0f / l_lo, i_hi = 1.0f / l_hi;
+    // 16-byte stores: the quad of lanes holding a row exchanges words so that lane q owns columns 8q..8q+7 and
+    // 32+8q..32+8q+7 of both its rows
+    const int q = lane & 3;
 #pragma unroll
-  for (int n = 0; n < 8; n++) {
-    const int col = 8 * n + 2 * (lane & 3);
-    if (r_lo < T) *reinterpret_cast<uint32_t*>(ob + (int64_t)r_lo * w + col) = attw_pack(o[4 * n] * i_lo, o[4 * n + 1] * i_lo);
-    if (r_hi < T) *reinterpret_cast<uint32_t*>(ob + (int64_t)r_hi * w + col) = attw_pack(o[4 * n + 2] * i_hi, o[4 * n + 3] * i_hi);
+    for (int half = 0; half < 2; half++) {
+      const int row = r_lo + 8 * half;
+      const float inv = half ? i_hi : i_lo;
+#pragma unroll
+      for (int g = 0; g < 2; g++) {
+        uint32_t a[4], c[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) a[k] = attw_pack(o[4 * (4 * g + k) + 2 * half] * inv, o[4 * (4 * g + k) + 2 * half + 1] * inv);
+        attw_quad_transpose(a, c, q);
+        if (row < T) *reinterpret_cast<uint4*>(ob + (int64_t)row * w + 8 * (4 * g + q)) = make_uint4(c[0], c[1], c[2], c[3]);
+      }
+    }
   }
 }
 
@@ -159,8 +259,8 @@ bool attention_wgmma_supported(int T, int heads, int w) {
   return heads > 0 && w == heads * ATTW_HD && T >= 1 && T <= ATTW_MAX_T;
 }
 
-int attention_wgmma(const CUtensorMap& tmQKV, const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int heads, int w,
-                    int causal, cudaStream_t st) {
+int attention_wgmma(const CUtensorMap& tmQKV, __nv_bfloat16* out, int B, int T, int heads, int w, int causal,
+                    cudaStream_t st) {
   B200_CHECK(attention_wgmma_supported(T, heads, w), B200_ERR_UNSUPPORTED,
              "attention_wgmma: head dim 64 and T <= %d only (T=%d heads=%d w=%d)", ATTW_MAX_T, T, heads, w);
   if (B == 0) return B200_OK;
@@ -168,12 +268,12 @@ int attention_wgmma(const CUtensorMap& tmQKV, const __nv_bfloat16* qkv, __nv_bfl
   int dev = 0;
   B200_CUDA(cudaGetDevice(&dev));
   if (!(configured.load() >> (dev & 63) & 1ull)) {
-    B200_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTW_SMEM));
+    B200_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   attw_smem_bytes(ATTW_MAX_T)));
     configured.fetch_or(1ull << (dev & 63));
   }
   const float scale_log2e = 0.125f * 1.4426950408889634f;   // hd^-0.5 * log2(e)
-  attention_wgmma_kernel<<<dim3((T + ATTW_BQ - 1) / ATTW_BQ, heads, B), 128, ATTW_SMEM, st>>>(tmQKV, qkv, out, T, w,
-                                                                                             scale_log2e, causal);
+  attention_wgmma_kernel<<<dim3(heads, B), ATTW_THREADS, attw_smem_bytes(T), st>>>(tmQKV, out, T, w, scale_log2e, causal);
   B200_LAUNCH_OK();
   return B200_OK;
 }

@@ -39,7 +39,7 @@ struct Tower {
   // activations
   __nv_bfloat16 *x = nullptr, *h = nullptr, *qkv = nullptr, *a = nullptr, *f = nullptr;
   CUtensorMap tm_h, tm_a, tm_f, tm_x;
-  CUtensorMap tm_qkv;          // qkv in boxes of 64 rows x 64 columns: Q / K tiles of the wgmma attention
+  CUtensorMap tm_qkv;          // qkv as [max_batch, T, 3w] in boxes of 64 tokens x 64 columns: Q / K / V tiles of the wgmma attention
   bool wgmma_attn = false;
   float2* stats = nullptr;     // folded LayerNorm: (mean, M2) per 64-column slot of every row of x
   float *lnf_g = nullptr, *lnf_b = nullptr;  // ln_post / ln_final
@@ -151,7 +151,8 @@ static int make_tower(b200_clip* m, Tower* t, const b200_tower_config& c, int T,
   B200_TRY(make_tmap_2d(&t->tm_f, t->f, 1, rows, c.mlp, c.mlp, GEMM_BM, GEMM_BK));
   B200_TRY(make_tmap_2d(&t->tm_x, t->x, 1, rows, w, w, GEMM_BM, GEMM_BK));
   t->wgmma_attn = attention_wgmma_supported(T, c.heads, w);
-  if (t->wgmma_attn) B200_TRY(make_tmap_2d(&t->tm_qkv, t->qkv, 1, rows, 3 * (size_t)w, 3 * (size_t)w, 64, 64));
+  if (t->wgmma_attn)
+    B200_TRY(make_tmap_3d(&t->tm_qkv, t->qkv, 1, m->cfg.max_batch, T, 3 * (size_t)w, 3 * (size_t)w, (size_t)T * 3 * w, 64, 64));
   if (m->fuse_ln && w % 64 == 0 && w <= 64 * LN_MAX_SLOTS) {
     B200_TRY(dev_alloc(m, &t->stats, rows * (size_t)(w / 64)));
     for (auto& L : t->L) {
@@ -212,7 +213,7 @@ static int run_blocks(b200_clip* m, Tower& t, int B, int causal, cudaStream_t st
     if (fused) { e1.ln_stats = t.stats; e1.ln_c = L.qkv.lnc; e1.ln_w = w; }
     B200_TRY(run_linear(m, fused ? t.tm_x : t.tm_h, L.qkv, M, e1, st, CLS_G_QKV));
     { SpanGuard sg(m, CLS_ATTN, st); m->last_launches++;
-      if (t.wgmma_attn) B200_TRY(attention_wgmma(t.tm_qkv, t.qkv, t.a, B, t.T, t.heads, w, causal, st));
+      if (t.wgmma_attn) B200_TRY(attention_wgmma(t.tm_qkv, t.a, B, t.T, t.heads, w, causal, st));
       else B200_TRY(attention(t.qkv, t.a, B, t.T, t.heads, w, causal, st)); }
     GemmEpilogue e2; e2.out = t.x; e2.out_ld = w; e2.residual = t.x; e2.res_ld = w;
     if (fused) e2.stats_out = t.stats;
@@ -670,8 +671,8 @@ int b200_attention_bf16_device(const void* d_qkv, void* d_out, int B, int T, int
   DeviceGuard g(device);
   if (B > 0 && attention_wgmma_supported(T, heads, w)) {
     CUtensorMap tm;
-    B200_TRY(make_tmap_2d(&tm, d_qkv, 1, (uint64_t)B * T, 3 * (uint64_t)w, 3 * (uint64_t)w, 64, 64));
-    return attention_wgmma(tm, (const __nv_bfloat16*)d_qkv, (__nv_bfloat16*)d_out, B, T, heads, w, causal, (cudaStream_t)stream);
+    B200_TRY(make_tmap_3d(&tm, d_qkv, 1, (uint64_t)B, (uint64_t)T, 3 * (uint64_t)w, 3 * (uint64_t)w, (uint64_t)T * 3 * w, 64, 64));
+    return attention_wgmma(tm, (__nv_bfloat16*)d_out, B, T, heads, w, causal, (cudaStream_t)stream);
   }
   return attention((const __nv_bfloat16*)d_qkv, (__nv_bfloat16*)d_out, B, T, heads, w, causal, (cudaStream_t)stream);
 }

@@ -22,11 +22,12 @@ int row_stats(const __nv_bfloat16* x, int64_t rows, int w, float2* stats, cudaSt
 // K4: multi-head attention over the fused qkv buffer [B*T, 3w] -> out [B*T, w]; causal for text.  mma.sync kernel
 // (attention.cu) for the head dimensions the wgmma kernel does not take (80, 96, 128).
 int attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int heads, int w, int causal, cudaStream_t st);
-// K4 on wgmma (attention_wgmma.cu) for head dim 64, T <= 320: tmQKV is a map over the qkv buffer [rows, 3w] with
-// boxes of 64 rows x 64 columns (128B swizzle), rows >= B*T of it are never used unmasked.
+// K4 on wgmma (attention_wgmma.cu) for head dim 64, T <= 320: tmQKV is a 3-D map over the qkv buffer seen as
+// [samples >= B, T, 3w] (make_tmap_3d, row pitch 3w, plane pitch T * 3w) with boxes of 64 tokens x 64 columns (128B
+// swizzle); a box is clipped at token T of its sample, so keys and values past the end read as zeros.
 bool attention_wgmma_supported(int T, int heads, int w);
-int attention_wgmma(const CUtensorMap& tmQKV, const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int heads, int w,
-                    int causal, cudaStream_t st);
+int attention_wgmma(const CUtensorMap& tmQKV, __nv_bfloat16* out, int B, int T, int heads, int w, int causal,
+                    cudaStream_t st);
 // K8/K10/K11: pooled row (x[b*T + pool_index(b)]) -> LN -> @ proj [w, D] -> optional L2 normalise
 // -> fp16 or fp32.  pool_idx == nullptr pools token 0 (vision); else row pool_idx[b] (text EOT).
 int pool_ln_proj_norm(const __nv_bfloat16* x, int T, int w, const int* pool_idx, const float* gamma, const float* beta,

@@ -44,6 +44,28 @@ int make_tmap_2d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t row
   return B200_OK;
 }
 
+// 3-D row-major tensor [planes, rows, cols] (16-bit elements) with row pitch ld_row and plane pitch ld_plane (in
+// elements), tiled in boxes of box_rows x box_cols x 1 plane (box_cols * 2 bytes must be 128: the swizzle span).  A box
+// that runs past `rows` is clipped at the end of its plane: those rows are read as zeros, never from the next plane.
+int make_tmap_3d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t planes, uint64_t rows, uint64_t cols,
+                 uint64_t ld_row, uint64_t ld_plane, uint32_t box_rows, uint32_t box_cols) {
+  encode_tiled_fn enc = get_encode();
+  B200_CHECK(enc != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
+  B200_CHECK(((uintptr_t)ptr & 15) == 0 && (ld_row * 2) % 16 == 0 && (ld_plane * 2) % 16 == 0, B200_ERR_INVALID,
+             "tensor map: base and pitches must be 16-byte aligned (ptr=%p ld_row=%llu ld_plane=%llu)", ptr,
+             (unsigned long long)ld_row, (unsigned long long)ld_plane);
+  B200_CHECK(box_cols * 2 == 128 && box_rows >= 1 && box_rows <= 256, B200_ERR_INVALID, "tensor map: bad box");
+  cuuint64_t dims[3] = {cols, rows, planes};
+  cuuint64_t strides[2] = {ld_row * 2, ld_plane * 2};
+  cuuint32_t box[3] = {box_cols, box_rows, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = enc(out, dtype_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3,
+                   const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled failed with %d", (int)r);
+  return B200_OK;
+}
+
 int gemm_pick_bn(int M, int N, int sms) {
   const long mb = (M + GEMM_BM - 1) / GEMM_BM;
   const long tiles128 = mb * ((N + 127) / 128);

@@ -344,6 +344,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 // host side (gemm.cu)
 int make_tmap_2d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t rows, uint64_t cols, uint64_t ld_elems,
                  uint32_t box_rows, uint32_t box_cols);
+int make_tmap_3d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t planes, uint64_t rows, uint64_t cols,
+                 uint64_t ld_row, uint64_t ld_plane, uint32_t box_rows, uint32_t box_cols);
 // tmB must have boxes of bn rows x 64 columns.  generic = true launches the run-time epilogue flavour (SPEC = -1)
 // even where a compile-time flavour applies (the tests check that both store the same bits).
 int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int M, int N, int K,

@@ -58,6 +58,19 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
+// 3-D tiled load: coordinates are (c0 = innermost element index, c1 = row index, c2 = plane index).  Rows outside the
+// map's extent in c1 are written as zeros.
+__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int32_t c0, int32_t c1,
+                                            int32_t c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
+// Barrier `id` (1..15; 0 is __syncthreads) over `count` threads, e.g. the 128 of one warpgroup.
+__device__ __forceinline__ void named_barrier_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 // ---- wgmma (warpgroup MMA) ---------------------------------------------------------------------------
 // Shared-memory matrix descriptor, K-major operand tile stored as rows of 128 bytes with the 128-byte
 // swizzle (what a TMA box of 64 16-bit elements x R rows with CU_TENSOR_MAP_SWIZZLE_128B writes; the
@@ -70,6 +83,24 @@ __device__ __forceinline__ uint64_t wgmma_desc_k_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
+  return d;
+}
+// Shared-memory matrix descriptor, MN-major B operand of N = 64 columns (the transposed-B form, imm-trans-b = 1):
+// the tile is stored K row by K row, 64 16-bit elements (128 bytes) of N per row, with the 128-byte swizzle (what a TMA
+// box of 64 elements x R rows with CU_TENSOR_MAP_SWIZZLE_128B writes; tile base 1024-byte aligned).  The swizzle atom
+// is 64 N elements x 8 K rows:
+//   bits [0,14)  start address >> 4
+//   bits [16,30) byte offset >> 4 between atoms along N: never used at N = 64, set to the K stride below
+//   bits [32,46) byte offset >> 4 = 1024 B between 8-row groups along K
+//   bits [62,64) layout = 1 (SWIZZLE_128B)
+// One k16 step spans two 8-row groups: advancing 16 elements along K adds 2048 B, i.e. 128, to the descriptor.
+constexpr uint64_t WGMMA_DESC_MN_SW128_K16 = 2048 >> 4;
+__device__ __forceinline__ uint64_t wgmma_desc_mn_sw128(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+  d |= (uint64_t)(1024 >> 4) << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
   d |= (uint64_t)1 << 62;
   return d;
@@ -87,6 +118,22 @@ __device__ __forceinline__ void fence_regs(float (&d)[R]) {
   for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// D[64 x 16] (+)= A[64 x 16] * B[16 x 16]^T, bf16 operands from shared memory (K-major), fp32 accumulate
+__device__ __forceinline__ void wgmma_m64n16k16_bf16(float (&d)[8], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(da), "l"(db), "r"(accumulate));
+}
+// D[64 x 48] (+)= A[64 x 16] * B[48 x 16]^T, bf16 operands from shared memory (K-major), fp32 accumulate
+__device__ __forceinline__ void wgmma_m64n48k16_bf16(float (&d)[24], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "l"(da), "l"(db), "r"(accumulate));
+}
 // D[64 x 32] (+)= A[64 x 16] * B[32 x 16]^T, bf16 operands from shared memory (K-major), fp32 accumulate
 __device__ __forceinline__ void wgmma_m64n32k16_bf16(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
@@ -127,6 +174,15 @@ __device__ __forceinline__ void wgmma_m64n64k16_bf16_rs(float (&d)[32], const ui
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+}
+// The same with B MN-major (imm-trans-b = 1): B[k][n] is read from a tile stored K row by K row with N contiguous
+// (wgmma_desc_mn_sw128), e.g. V as it lies in memory for O += P V.
+__device__ __forceinline__ void wgmma_m64n64k16_bf16_rs_tb(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
 }
