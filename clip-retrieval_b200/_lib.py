@@ -136,6 +136,7 @@ PROTOTYPES = {
     "b200_gemm_bf16_ex_device": (_i, [_vp, _vp, _vp, _i, _i, _i, C.POINTER(GemmEpilogueC), _i, _i, _i, _vp]),
     "b200_row_stats_bf16_device": (_i, [_vp, _i64, _i, _vp, _i, _vp]),
     "b200_index_last_hi_only_fallbacks": (_i, [_vp]),
+    "b200_index_last_scan_plan": (_i, [_vp, _vp]),
     "b200_kmeans_train_f16": (_i, [_vp, _i64, _i, _i, _i, C.c_uint64, _i, _vp, _vp, _i]),
     "b200_dedup_device": (_i, [_vp, _i, _i, C.c_float, _vp, _vp, _vp, C.c_size_t, _i, _vp]),
     "b200_prompt_argmax_device": (_i, [_vp, _i, _i, _vp, _i, _i, _vp, _i, _vp]),

@@ -61,6 +61,9 @@ struct b200_index {
   std::vector<cudaEvent_t> ev;   // pairs
   int ev_used = 0;
   int last_scan_launches = 0;
+  // {kernel, queries per pass, 16-byte chunks per lane, ring stages} of the last eager exhaustive scan;
+  // kernel: 0 register FMA, 1 staged FMA (bulk-copy ring), 2 wgmma split, 3 wgmma hi-only.  -1 before any scan.
+  int last_scan_plan[4] = {-1, -1, -1, -1};
 };
 
 namespace b200 {

@@ -377,6 +377,12 @@ int b200_index_set_tensor_scan(b200_index* idx, int on) {
 
 int b200_index_last_hi_only_fallbacks(const b200_index* idx) { return idx ? idx->last_hi_only_fallbacks : -1; }
 
+int b200_index_last_scan_plan(const b200_index* idx, int32_t* h_plan) {
+  B200_CHECK(idx && h_plan, B200_ERR_INVALID, "last_scan_plan: null argument");
+  for (int i = 0; i < 4; i++) h_plan[i] = idx->last_scan_plan[i];
+  return B200_OK;
+}
+
 int b200_index_ivf_lists(b200_index* idx, int64_t* h_sizes, int64_t* h_ids) {
   B200_CHECK(idx && h_sizes, B200_ERR_INVALID, "ivf_lists: null argument");
   B200_CHECK(idx->nlist > 0, B200_ERR_STATE, "ivf_lists: not an IVF index");

@@ -490,8 +490,12 @@ int scan_topk_keys_mma(b200_index* idx, const __half* rows, int64_t n, const flo
   B200_CHECK(n < (1ll << 31), B200_ERR_UNSUPPORTED, "mma scan: at most 2^31 rows per shard");
   // Up to one split-mode group the scan is HBM-bound already; beyond, halve the tensor work.
   const int kc = 2 * k;
-  if (!idx->use_hi_only || nq <= MS_QG || kc > MS_KMAX || n < 4 * (int64_t)kc)
-    return scan_mma_passes<true>(idx, rows, n, d_q, nq, k, d_keys_out, st);
+  const bool hi_only = idx->use_hi_only && nq > MS_QG && kc <= MS_KMAX && n >= 4 * (int64_t)kc;
+  idx->last_scan_plan[0] = hi_only ? 3 : 2;
+  idx->last_scan_plan[1] = hi_only ? MS_BN : MS_QG;
+  idx->last_scan_plan[2] = (d / 8 + 31) / 32;
+  idx->last_scan_plan[3] = MS_STAGES;
+  if (!hi_only) return scan_mma_passes<true>(idx, rows, n, d_q, nq, k, d_keys_out, st);
 
   float* d_bound = nullptr;
   B200_TRY(row_norm_bound(idx, rows, n, &d_bound, st));

@@ -483,6 +483,10 @@ int scan_topk_keys(b200_index* idx, const __half* rows, int64_t n, const float* 
     return scan_topk_keys_mma(idx, rows, n, d_q, nq, k, d_keys_out, st);
   ScanPlan p;
   B200_TRY(plan_scan(idx, k, nq, &p));
+  idx->last_scan_plan[0] = p.sfn ? 1 : 0;
+  idx->last_scan_plan[1] = p.nqp;
+  idx->last_scan_plan[2] = (d / 8 + 31) / 32;
+  idx->last_scan_plan[3] = p.stages;
   const int64_t total_warps = (int64_t)p.grid * p.warps_out;
   const int64_t M1 = total_warps * k;
   // level 1: one sort round per block (a block sorts one C-entry chunk of the candidates) — the select of a single

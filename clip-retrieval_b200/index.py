@@ -235,6 +235,13 @@ class _IndexBase:
     def last_hi_only_fallbacks(self):
         return int(lib.b200_index_last_hi_only_fallbacks(self._h))
 
+    def last_scan_plan(self):
+        """(kernel, queries per pass, chunks per lane, ring stages) of the last eager exhaustive scan; kernel 0 =
+        register FMA, 1 = FMA through the bulk-copy ring, 2 = wgmma split, 3 = wgmma hi-only (include/b200clip.h)."""
+        plan = np.zeros(4, dtype=np.int32)
+        check(lib.b200_index_last_scan_plan(self._h, plan.ctypes.data), "last_scan_plan")
+        return tuple(int(v) for v in plan)
+
     def last_scan_ms(self):
         ms = C.c_float(0)
         n = C.c_int(0)

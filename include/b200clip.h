@@ -111,6 +111,12 @@ int b200_index_set_tensor_scan(b200_index* idx, int on);
 /* Queries of the last batched search whose exactness proof failed in hi-only mode and were re-run
  * in split mode (0 in the common case; diagnostic). */
 int b200_index_last_hi_only_fallbacks(const b200_index* idx);
+/* Plan of the last exhaustive scan launched eagerly on this handle (flat search, or the coarse step of an
+ * IVF search): h_plan[4] = {kernel, queries per pass, 16-byte chunks per lane = ceil(d / 256), ring stages}.
+ * kernel: 0 register FMA scan, 1 FMA scan through the bulk-copy ring, 2 wgmma split (hi/lo) scan, 3 wgmma
+ * hi-only scan (queries whose proof fails are re-run in split mode).  All -1 before the first scan.  A
+ * replayed CUDA graph runs no host code and leaves it unchanged. */
+int b200_index_last_scan_plan(const b200_index* idx, int32_t* h_plan);
 /* IVF introspection used by ivf_metadata_ordering.get_old_to_new_mapping
  * (ivf_metadata_ordering.py:46-64): sizes[nlist] and, list after list, the ids in list order. */
 int b200_index_ivf_lists(b200_index* idx, int64_t* h_sizes, int64_t* h_ids);
