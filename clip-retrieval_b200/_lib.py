@@ -93,6 +93,10 @@ PROTOTYPES = {
     "b200_synth_rows_f32": (_i, [_vp, _i64, _i, _i64, C.POINTER(SynthSpecC), _vp]),
     "b200_index_create_flat": (_i, [_i, _i, C.POINTER(_vp)]),
     "b200_index_create_ivfflat": (_i, [_i, _i, _vp, _i, C.POINTER(_vp)]),
+    "b200_index_create_ivfpq": (_i, [_i, _i, _i, _i, _vp, _vp, _i, C.POINTER(_vp)]),
+    "b200_index_add_codes": (_i, [_vp, _vp, _i64, _i, _vp]),
+    "b200_index_set_pretransform": (_i, [_vp, _i, _vp, _vp]),
+    "b200_index_pq_m": (_i, [_vp]),
     "b200_index_destroy": (_i, [_vp]),
     "b200_index_reserve": (_i, [_vp, _i64]),
     "b200_index_add_f16": (_i, [_vp, _vp, _i64, _i]),

@@ -1,4 +1,4 @@
-// The index handle behind b200_index* (flat and IVF-Flat share the row store and the top-k tail).
+// The index handle behind b200_index* (flat, IVF-Flat and IVF-PQ share the row store and the top-k tail).
 #pragma once
 #include "common.cuh"
 #include <map>
@@ -6,7 +6,9 @@
 #include <vector>
 
 struct b200_index {
-  int d = 0;
+  int d = 0;                // width of the stored space (IVF-PQ: the code space, after any pre-transform)
+  int d_in = 0;             // width of a query and of a reconstructed row (== d unless a pre-transform is set)
+  int row_bytes = 0;        // bytes per stored row: 2 * d (fp16 rows) or the 16-byte padded code pitch (IVF-PQ)
   int device = 0;
   int sms = 132;
   int64_t ntotal = 0;
@@ -37,6 +39,15 @@ struct b200_index {
   std::vector<uint32_t> pending_lists;   // explicit list of every pending row (0xFFFFFFFF: assign by max inner product)
   uint32_t* id_to_slot = nullptr;         // device [ntotal]: inverse of row_ids, rebuilt whenever the store changes
 
+  // IVF-PQ (8-bit codes): `rows` holds M code bytes per row at a pitch of row_bytes, list after list
+  int pq_M = 0;                     // 0 = not IVF-PQ
+  bool pq_by_residual = true;
+  float* pq_centroids = nullptr;    // device [nlist, d] fp32 (dis0 and decoding; never the fp16 copy)
+  float* pq_codebook = nullptr;     // device [M, 256, d / M] fp32
+  float* pt_A = nullptr;            // device [d, d_in] fp32: q' = A q + b; null = no pre-transform
+  float* pt_b = nullptr;            // device [d] fp32
+  bool pt_orthonormal = false;      // rows of A orthonormal: reconstruct may apply A^T (y - b)
+
   // scratch
   void* ws[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // 0: scan internals; 1..3: callers; 4,5: hi-only mode
   size_t ws_bytes[6] = {0, 0, 0, 0, 0, 0};
@@ -63,6 +74,7 @@ struct b200_index {
   int last_scan_launches = 0;
   // {kernel, queries per pass, 16-byte chunks per lane, ring stages} of the last eager exhaustive scan;
   // kernel: 0 register FMA, 1 staged FMA (bulk-copy ring), 2 wgmma split, 3 wgmma hi-only.  -1 before any scan.
+  // kernel 4: IVF-PQ list scan {4, sub-quantisers per CTA, CTAs per cluster, candidate warps per CTA}.
   int last_scan_plan[4] = {-1, -1, -1, -1};
 };
 

@@ -25,6 +25,12 @@ int range_scan(b200_index* idx, const __half* rows, int64_t n, const float* d_q,
                unsigned int cap, unsigned int* d_count, cudaStream_t st);
 int ivf_range_scan(b200_index* idx, const float* d_q, float thresh, unsigned long long* d_out, unsigned int cap,
                    unsigned int* d_count, cudaStream_t st);
+// IVF-PQ (knn_ivfpq.cu)
+int ivfpq_search_keys(b200_index* idx, const float* d_q, int nq, int k, unsigned long long* d_keys, cudaStream_t st);
+int ivfpq_range_scan(b200_index* idx, const float* d_q, float thresh, unsigned long long* d_out, unsigned int cap,
+                     unsigned int* d_count, cudaStream_t st);
+int ivfpq_decode(b200_index* idx, const unsigned long long* keys, const int64_t* ids, int64_t count, float* d_R,
+                 cudaStream_t st);
 
 __global__ void f32_to_f16_kernel(const float* __restrict__ in, __half* __restrict__ out, int64_t count) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -153,14 +159,21 @@ static int search_device_impl(b200_index* idx, const float* d_q, int nq, int k, 
   void* ws = nullptr;
   B200_TRY(index_ws(idx, 1, (size_t)nq * k * 8, &ws));
   unsigned long long* keys = (unsigned long long*)ws;
-  if (idx->nlist > 0) {
+  if (idx->pq_M > 0) {
+    B200_CHECK(!d_R || !idx->pt_A || idx->pt_orthonormal, B200_ERR_UNSUPPORTED,
+               "search_and_reconstruct: the pre-transform matrix is not orthonormal, so rows cannot be mapped back");
+    B200_TRY(ivf_finalize(idx));
+    B200_TRY(ivfpq_search_keys(idx, d_q, nq, k, keys, st));
+  } else if (idx->nlist > 0) {
     B200_TRY(ivf_finalize(idx));
     B200_TRY(ivf_search_keys(idx, d_q, nq, k, keys, st));   // keys carry insertion ids, not slots
   } else {
     B200_TRY(scan_topk_keys(idx, idx->rows, idx->ntotal, d_q, nq, k, keys, st));
   }
   B200_TRY(decode_keys(keys, (int64_t)nq * k, idx->id_base, nullptr, d_D, d_I, st));
-  if (d_R) {
+  if (d_R && idx->pq_M > 0) {
+    B200_TRY(ivfpq_decode(idx, keys, nullptr, (int64_t)nq * k, d_R, st));
+  } else if (d_R) {
     const int64_t count = (int64_t)nq * k;
     gather_rows_from_keys_kernel<<<(unsigned)((count + 7) / 8), 256, 0, st>>>(idx->rows, idx->d, keys,
                                                                                idx->id_to_slot, count, d_R);
@@ -205,6 +218,8 @@ int b200_index_create_flat(int d, int device, b200_index** out) {
   B200_CHECK(idx != nullptr, B200_ERR_OOM, "create_flat: host allocation failed");
   if (const char* e = getenv("B200_GRAPHS")) idx->use_graphs = atoi(e) != 0;
   idx->d = d;
+  idx->d_in = d;
+  idx->row_bytes = 2 * d;
   idx->device = device;
   idx->sms = sm_count(device);
   *out = idx;
@@ -256,6 +271,8 @@ int b200_index_reserve(b200_index* idx, int64_t n) {
 
 static int add_rows(b200_index* idx, const void* rows, int64_t n, int on_device, bool f32) {
   B200_CHECK(idx && (rows || n == 0) && n >= 0, B200_ERR_INVALID, "add: bad argument");
+  B200_CHECK(idx->pq_M == 0, B200_ERR_UNSUPPORTED,
+             "add: an IVF-PQ index takes PQ codes (b200_index_add_codes); there is no encoder for float rows");
   if (n == 0) return B200_OK;
   idx->graph_epoch++;
   DeviceGuard g(idx->device);
@@ -315,6 +332,8 @@ int b200_index_add_f32(b200_index* idx, const float* rows, int64_t n, int rows_o
 int b200_index_add_assigned_f16(b200_index* idx, const void* rows, int64_t n, int rows_on_device, const int32_t* h_lists) {
   B200_CHECK(idx && h_lists, B200_ERR_INVALID, "add_assigned: bad argument");
   B200_CHECK(idx->nlist > 0, B200_ERR_STATE, "add_assigned: not an IVF index");
+  B200_CHECK(idx->pq_M == 0, B200_ERR_UNSUPPORTED,
+             "add_assigned: an IVF-PQ index takes PQ codes (b200_index_add_codes); there is no encoder for float rows");
   for (int64_t i = 0; i < n; i++)
     B200_CHECK(h_lists[i] >= 0 && h_lists[i] < idx->nlist, B200_ERR_INVALID, "add_assigned: row %lld has list %d of %d",
                (long long)i, h_lists[i], idx->nlist);
@@ -327,6 +346,8 @@ int b200_index_add_assigned_f16(b200_index* idx, const void* rows, int64_t n, in
 
 int b200_index_add_synthetic(b200_index* idx, int64_t n, int64_t row0, const b200_synth_spec* spec) {
   B200_CHECK(idx && spec && n >= 0, B200_ERR_INVALID, "add_synthetic: bad argument");
+  B200_CHECK(idx->pq_M == 0, B200_ERR_UNSUPPORTED,
+             "add_synthetic: an IVF-PQ index takes PQ codes (b200_index_add_codes); there is no encoder for float rows");
   if (n == 0) return B200_OK;
   idx->graph_epoch++;
   DeviceGuard g(idx->device);
@@ -347,7 +368,8 @@ int b200_index_finalize(b200_index* idx) {
 }
 
 int64_t b200_index_ntotal(const b200_index* idx) { return idx ? idx->ntotal + idx->npending : -1; }
-int b200_index_d(const b200_index* idx) { return idx ? idx->d : -1; }
+int b200_index_d(const b200_index* idx) { return idx ? idx->d_in : -1; }
+int b200_index_pq_m(const b200_index* idx) { return idx ? idx->pq_M : -1; }
 int b200_index_nlist(const b200_index* idx) { return idx ? idx->nlist : -1; }
 
 int b200_index_set_id_base(b200_index* idx, int64_t id_base) {
@@ -411,7 +433,7 @@ static int scratch_release(b200_index* idx, cudaStream_t st) {
 static int search_graph(b200_index* idx, const float* d_q, int nq, int k, float* d_D, int64_t* d_I, float* d_R,
                         cudaStream_t st) {
   constexpr int GRAPH_MAX_NQ = 4;
-  const size_t r_bytes = d_R ? (size_t)nq * k * idx->d * 4 : 0;
+  const size_t r_bytes = d_R ? (size_t)nq * k * idx->d_in * 4 : 0;
   if (!idx->use_graphs || nq < 1 || nq > GRAPH_MAX_NQ || k > 2048 || r_bytes > (8u << 20) || idx->npending > 0) return 0;
   cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
   B200_CUDA(cudaStreamIsCapturing(st, &cs));
@@ -425,7 +447,7 @@ static int search_graph(b200_index* idx, const float* d_q, int nq, int k, float*
   }
   if (sg.seen < 1) { sg.seen++; return 0; }        // first call of a shape runs eagerly (workspaces, attributes, events)
   // fixed buffers
-  const size_t qb = (size_t)GRAPH_MAX_NQ * idx->d * 4;
+  const size_t qb = (size_t)GRAPH_MAX_NQ * idx->d_in * 4;
   if (idx->g_q_cap < qb) {
     if (idx->g_q) B200_CUDA(cudaFree(idx->g_q));
     B200_CUDA(cudaMalloc((void**)&idx->g_q, qb));
@@ -468,7 +490,7 @@ static int search_graph(b200_index* idx, const float* d_q, int nq, int k, float*
     if (ie != cudaSuccess) { cudaGetLastError(); sg.exec = nullptr; idx->use_graphs = false; return 0; }
     sg.kernels = (int)(g_launches.load() - l0);
   }
-  B200_CUDA(cudaMemcpyAsync(idx->g_q, d_q, (size_t)nq * idx->d * 4, cudaMemcpyDeviceToDevice, st));
+  B200_CUDA(cudaMemcpyAsync(idx->g_q, d_q, (size_t)nq * idx->d_in * 4, cudaMemcpyDeviceToDevice, st));
   B200_CUDA(cudaGraphLaunch(sg.exec, st));
   B200_CUDA(cudaMemcpyAsync(d_D, idx->g_D, (size_t)nq * k * 4, cudaMemcpyDeviceToDevice, st));
   B200_CUDA(cudaMemcpyAsync(d_I, idx->g_I, (size_t)nq * k * 8, cudaMemcpyDeviceToDevice, st));
@@ -501,8 +523,8 @@ int b200_index_search(b200_index* idx, const float* h_q, int nq, int k, float* h
   B200_CHECK(h_q && h_D && h_I, B200_ERR_INVALID, "search: null buffer");
   std::lock_guard<std::mutex> lock(idx->mu);
   DeviceGuard g(idx->device);
-  const size_t qb = (size_t)nq * idx->d * 4, db = (size_t)nq * k * 4, ib = (size_t)nq * k * 8;
-  const size_t rb = h_R ? (size_t)nq * k * idx->d * 4 : 0;
+  const size_t qb = (size_t)nq * idx->d_in * 4, db = (size_t)nq * k * 4, ib = (size_t)nq * k * 8;
+  const size_t rb = h_R ? (size_t)nq * k * idx->d_in * 4 : 0;
   auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
   void* ws = nullptr;
   B200_TRY(index_ws(idx, 2, al(qb) + al(db) + al(ib) + al(rb), &ws));
@@ -528,7 +550,7 @@ int b200_index_range_search(b200_index* idx, const float* h_q, float thresh, int
   B200_CHECK(cap < (1ll << 31), B200_ERR_INVALID, "range_search: cap too large");
   std::lock_guard<std::mutex> lock(idx->mu);
   DeviceGuard g(idx->device);
-  const size_t qb = ((size_t)idx->d * 4 + 255) & ~(size_t)255;
+  const size_t qb = ((size_t)idx->d_in * 4 + 255) & ~(size_t)255;
   void* ws = nullptr;
   B200_TRY(index_ws(idx, 2, qb + 256 + (size_t)cap * 8 + (size_t)cap * 12, &ws));
   float* d_q = (float*)ws;
@@ -537,8 +559,11 @@ int b200_index_range_search(b200_index* idx, const float* h_q, float thresh, int
   float* d_D = (float*)(d_keys + cap);
   int64_t* d_I = (int64_t*)((char*)d_D + (((size_t)cap * 4 + 7) & ~(size_t)7));
   B200_TRY(scratch_acquire(idx, 0));
-  B200_CUDA(cudaMemcpyAsync(d_q, h_q, (size_t)idx->d * 4, cudaMemcpyHostToDevice, 0));
-  if (idx->nlist > 0) {
+  B200_CUDA(cudaMemcpyAsync(d_q, h_q, (size_t)idx->d_in * 4, cudaMemcpyHostToDevice, 0));
+  if (idx->pq_M > 0) {
+    B200_TRY(ivf_finalize(idx));
+    B200_TRY(ivfpq_range_scan(idx, d_q, thresh, d_keys, (unsigned int)cap, d_count, 0));
+  } else if (idx->nlist > 0) {
     B200_TRY(ivf_finalize(idx));
     B200_TRY(ivf_range_scan(idx, d_q, thresh, d_keys, (unsigned int)cap, d_count, 0));
   } else {
@@ -562,6 +587,13 @@ int b200_index_reconstruct_device(b200_index* idx, const int64_t* d_ids, int64_t
   B200_CHECK(idx && d_ids && d_R && n >= 0, B200_ERR_INVALID, "reconstruct: bad argument");
   if (n == 0) return B200_OK;
   DeviceGuard g(idx->device);
+  if (idx->pq_M > 0) {
+    std::lock_guard<std::mutex> lock(idx->mu);
+    B200_CHECK(!idx->pt_A || idx->pt_orthonormal, B200_ERR_UNSUPPORTED,
+               "reconstruct: the pre-transform matrix is not orthonormal, so rows cannot be mapped back");
+    B200_TRY(ivf_finalize(idx));
+    return ivfpq_decode(idx, nullptr, d_ids, n, d_R, (cudaStream_t)stream);
+  }
   const uint32_t* id_to_slot = nullptr;
   if (idx->nlist > 0) {
     std::lock_guard<std::mutex> lock(idx->mu);

@@ -276,11 +276,13 @@ static ivf_assign_fn pick_ivf_assign(int ch) {
 int ivf_create(b200_index* idx, int nlist, const float* h_centroids) {
   idx->nlist = nlist;
   idx->nprobe = 1;
-  const size_t count = (size_t)nlist * idx->d;
-  B200_CUDA(cudaMalloc((void**)&idx->centroids, count * sizeof(__half)));
-  std::vector<__half> tmp(count);
-  for (size_t i = 0; i < count; i++) tmp[i] = __float2half_rn(h_centroids[i]);
-  B200_CUDA(cudaMemcpy(idx->centroids, tmp.data(), count * sizeof(__half), cudaMemcpyHostToDevice));
+  if (h_centroids) {   // IVF-PQ passes none: its coarse step and dis0 use the fp32 centroids (knn_ivfpq.cu)
+    const size_t count = (size_t)nlist * idx->d;
+    B200_CUDA(cudaMalloc((void**)&idx->centroids, count * sizeof(__half)));
+    std::vector<__half> tmp(count);
+    for (size_t i = 0; i < count; i++) tmp[i] = __float2half_rn(h_centroids[i]);
+    B200_CUDA(cudaMemcpy(idx->centroids, tmp.data(), count * sizeof(__half), cudaMemcpyHostToDevice));
+  }
   B200_CUDA(cudaMalloc((void**)&idx->list_offsets, (size_t)(nlist + 1) * sizeof(int64_t)));
   B200_CUDA(cudaMemset(idx->list_offsets, 0, (size_t)(nlist + 1) * sizeof(int64_t)));
   idx->h_list_offsets.assign(nlist + 1, 0);
@@ -293,6 +295,10 @@ void ivf_free(b200_index* idx) {
   if (idx->row_ids) cudaFree(idx->row_ids);
   if (idx->pending) cudaFree(idx->pending);
   if (idx->id_to_slot) cudaFree(idx->id_to_slot);
+  if (idx->pq_centroids) cudaFree(idx->pq_centroids);
+  if (idx->pq_codebook) cudaFree(idx->pq_codebook);
+  if (idx->pt_A) cudaFree(idx->pt_A);
+  if (idx->pt_b) cudaFree(idx->pt_b);
 }
 
 // Sort (list, src) pairs by list (stable) and derive list offsets; `lists`/`src` are device arrays of n.
@@ -341,9 +347,12 @@ static int build_id_to_slot(b200_index* idx) {
   return B200_OK;
 }
 
+// Rows are moved as row_bytes / 16 chunks of 16 bytes: fp16 rows (IVF-Flat) and padded code rows (IVF-PQ) alike.
+// IVF-PQ rows always carry an explicit list, so only IVF-Flat rows are assigned by inner product.
 int ivf_finalize(b200_index* idx) {
   if (idx->npending == 0) return B200_OK;
-  const int d = idx->d, cpr = d / 8, ch = (cpr + 31) / 32;
+  const int d = idx->d, ch = (d / 8 + 31) / 32;
+  const int64_t rb = idx->row_bytes, cpr = rb / 16;
   const int64_t nold = idx->ntotal, nnew = idx->npending, n = nold + nnew;
   B200_CHECK(n < (1ll << 32), B200_ERR_UNSUPPORTED, "ivf: a shard holds at most 2^32 rows");
   uint32_t *lists = nullptr, *src = nullptr;
@@ -353,11 +362,13 @@ int ivf_finalize(b200_index* idx) {
     expand_offsets_kernel<<<idx->nlist, 256>>>(idx->list_offsets, idx->nlist, lists);
     B200_LAUNCH_OK();
   }
-  ivf_assign_fn afn = pick_ivf_assign(ch);
-  B200_CHECK(afn != nullptr, B200_ERR_UNSUPPORTED, "ivf: unsupported dimension %d", d);
-  afn<<<(unsigned)((nnew + 7) / 8), 256>>>(reinterpret_cast<const uint4*>(idx->pending), nnew, cpr,
-                                           reinterpret_cast<const uint4*>(idx->centroids), idx->nlist, lists + nold);
-  B200_LAUNCH_OK();
+  if (idx->pq_M == 0) {
+    ivf_assign_fn afn = pick_ivf_assign(ch);
+    B200_CHECK(afn != nullptr, B200_ERR_UNSUPPORTED, "ivf: unsupported dimension %d", d);
+    afn<<<(unsigned)((nnew + 7) / 8), 256>>>(reinterpret_cast<const uint4*>(idx->pending), nnew, d / 8,
+                                             reinterpret_cast<const uint4*>(idx->centroids), idx->nlist, lists + nold);
+    B200_LAUNCH_OK();
+  }
   if (!idx->pending_lists.empty()) {
     // rows added with an explicit list (an index file's own inverted lists) keep it
     idx->pending_lists.resize((size_t)nnew, 0xFFFFFFFFu);
@@ -377,10 +388,10 @@ int ivf_finalize(b200_index* idx) {
   B200_TRY(sort_by_list(idx, lists, src, n, &sorted_src, &to_free));
   __half* nrows = nullptr;
   uint32_t* nids = nullptr;
-  B200_CUDA(cudaMalloc((void**)&nrows, (size_t)n * d * 2));
+  B200_CUDA(cudaMalloc((void**)&nrows, (size_t)n * rb));
   B200_CUDA(cudaMalloc((void**)&nids, (size_t)n * 4));
   gather_sorted_rows_kernel<<<(unsigned)((n + 7) / 8), 256>>>(
-      reinterpret_cast<const uint4*>(idx->rows), reinterpret_cast<const uint4*>(idx->pending), nold, sorted_src, n, cpr,
+      reinterpret_cast<const uint4*>(idx->rows), reinterpret_cast<const uint4*>(idx->pending), nold, sorted_src, n, (int)cpr,
       reinterpret_cast<uint4*>(nrows), idx->row_ids, nids);
   B200_LAUNCH_OK();
   B200_CUDA(cudaDeviceSynchronize());

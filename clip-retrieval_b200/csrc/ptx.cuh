@@ -67,6 +67,26 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// ---- thread-block clusters / distributed shared memory ---------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// The shared::cluster address of `smem_addr` (a shared::cta address of this CTA's layout) in CTA `rank` of the cluster.
+__device__ __forceinline__ uint32_t mapa_shared(uint32_t smem_addr, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
+  return r;
+}
+__device__ __forceinline__ void st_shared_cluster_f32(uint32_t cluster_addr, float v) {
+  asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(cluster_addr), "f"(v) : "memory");
+}
+// Every thread of every CTA of the cluster: stores before the arrive are visible to loads after the wait.
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+
 // Barrier `id` (1..15; 0 is __syncthreads) over `count` threads, e.g. the 128 of one warpgroup.
 __device__ __forceinline__ void named_barrier_sync(uint32_t id, uint32_t count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");

@@ -95,8 +95,8 @@ int b200_sharded_create(b200_index* const* shards, int nshards, b200_sharded** o
   B200_CHECK(shards && out && nshards >= 1 && nshards <= 64, B200_ERR_INVALID, "sharded_create: bad argument");
   for (int i = 0; i < nshards; i++) {
     B200_CHECK(shards[i] != nullptr, B200_ERR_INVALID, "sharded_create: shard %d is null", i);
-    B200_CHECK(shards[i]->d == shards[0]->d, B200_ERR_INVALID, "sharded_create: shard %d has d=%d, shard 0 has d=%d", i,
-               shards[i]->d, shards[0]->d);
+    B200_CHECK(shards[i]->d_in == shards[0]->d_in, B200_ERR_INVALID, "sharded_create: shard %d has d=%d, shard 0 has d=%d",
+               i, shards[i]->d_in, shards[0]->d_in);
     for (int j = 0; j < i; j++)
       B200_CHECK(shards[j]->device != shards[i]->device, B200_ERR_INVALID,
                  "sharded_create: shards %d and %d share device %d (one shard per GPU)", j, i, shards[i]->device);
@@ -158,7 +158,7 @@ int b200_sharded_search(b200_sharded* h, void* const* comms, const float* h_q, i
   B200_CHECK(h_q && h_D && h_I, B200_ERR_INVALID, "sharded_search: null buffer");
   std::lock_guard<std::mutex> lock(h->mu);
   ShardedState& s = h->s;
-  const int G = s.n, d = h->shards[0]->d;
+  const int G = s.n, d = h->shards[0]->d_in;   // query width
   const size_t q_bytes = (size_t)nq * d * 4;
   const size_t block = (((size_t)nq * k * 12) + 255) & ~(size_t)255;   // [I int64 nq*k | D f32 nq*k], padded
   NcclApi* nccl = nullptr;

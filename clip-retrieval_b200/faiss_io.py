@@ -7,16 +7,24 @@ documented layout; it is UNVERIFIED against files written by FAISS itself — th
 own writer.  Supported (inner-product metric only — the reference builds `metric_type="ip"` indices):
     IxFI / IxF2 / IxFl   IndexFlat                      -> rows fp32
     IxSQ                 IndexScalarQuantizer, QT_fp16  -> rows fp16
-    IwFl                 IndexIVFFlat (quantizer IndexFlat, ArrayInvertedLists)
+    IwFl                 IndexIVFFlat (ArrayInvertedLists)
     IwSq                 IndexIVFScalarQuantizer, QT_fp16, by_residual = false
+    IwPQ                 IndexIVFPQ, 8-bit codes (ArrayInvertedLists)  -> codes uint8 [n, M], served from the codes
+    IHNf                 IndexHNSWFlat as the coarse quantiser of an IVF index: the graph is skipped, its storage
+                         rows are the centroids (this engine probes the centroids exactly)
+    IxPT                 IndexPreTransform with ONE LinearTransform (LTra: an OPQ matrix; rrot) around an IwPQ
     IxMp / IxM2          IndexIDMap / IDMap2 around one of the above
-Anything else (PQ / OPQ / HNSW codes — what autofaiss picks for billion-scale sets — on-disk inverted lists) raises
-NotImplementedError naming the fourcc: those store quantised CODES, which an exact fp16 engine cannot serve
-bit-compatibly; re-index from the embedding shards instead (`load_index(<folder of .npy>)`).
+That covers what autofaiss writes for large collections, `OPQ{M}_{d},IVF{nlist}_HNSW32,PQ{M}x8`.  Still unsupported,
+with NotImplementedError naming the fourcc: a top-level HNSW index, a flat IndexPQ (IxPq), 4-bit or fast-scan PQ,
+IVF refinement (IwQR), on-disk inverted lists (ilod) and longer transform chains; re-index from the embedding
+shards (`load_index(<folder of .npy>)`) or rebuild as one of the above.
 
 Layout (little endian): fourcc u32; header = d i32, ntotal i64, dummy i64 x2, is_trained u8, metric_type i32
 (0 = inner product, 1 = L2; metric_arg f32 follows when metric_type > 1); vectors are `size u64` + payload.
+The file is parsed through a read-only memory map, so a multi-GB code file is not read into memory before the codes
+are gathered into list order.
 """
+import mmap
 import struct
 
 import numpy as np
@@ -78,6 +86,7 @@ def _read_sq(r):
 
 
 def _read_invlists(r, nlist_expected, code_dtype, d):
+    """Inverted lists of `d` entries of `code_dtype` per row: (sizes, rows [n, d] in list order, ids)."""
     tag = _fourcc_str(r.take("I"))
     if tag == "il00":
         raise ValueError("index has no inverted lists")
@@ -106,21 +115,52 @@ def _read_invlists(r, nlist_expected, code_dtype, d):
     return sizes, rows, ids
 
 
+def _read_quantizer(r):
+    """The coarse quantiser of an IVF index: a flat index, or an IndexHNSWFlat whose storage holds the centroids."""
+    if _fourcc_str(struct.unpack_from("<I", r.b, r.o)[0]) != "IHNf":
+        return _read_index(r)
+    r.take("I")
+    _header(r)
+    r.vec(np.float64)                    # assign_probas
+    r.vec(np.int32)                      # cum_nneighbor_per_level
+    r.vec(np.int32)                      # levels
+    r.vec(np.uint64)                     # offsets
+    r.vec(np.int32)                      # neighbors
+    r.take("iiiii")                      # entry_point, max_level, efConstruction, efSearch, upper_beam
+    return _read_index(r)
+
+
+def _read_linear_transform(r):
+    """One VectorTransform of a pre-transform chain: (A [d_out, d_in] fp32, b [d_out] or None)."""
+    tag = _fourcc_str(r.take("I"))
+    if tag not in ("LTra", "rrot"):
+        raise NotImplementedError("pre-transform %r: only a linear transform (LTra, e.g. an OPQ matrix) or a random "
+                                  "rotation (rrot) is supported by load_index" % tag)
+    have_bias = r.take("B")
+    A = np.array(r.vec(np.float32))
+    b = np.array(r.vec(np.float32))
+    d_in, d_out = r.take("i"), r.take("i")
+    r.take("B")                          # is_trained
+    if A.size != d_in * d_out or (have_bias and b.size != d_out):
+        raise ValueError("linear transform: A has %d entries, b %d, for d_in=%d d_out=%d" % (A.size, b.size, d_in, d_out))
+    return A.reshape(d_out, d_in), (b if have_bias else None)
+
+
 def _read_index(r):
     tag = _fourcc_str(r.take("I"))
     if tag in ("IxFI", "IxF2", "IxFl"):
         d, ntotal, _, metric = _header(r)
         xb = r.vec(np.float32)           # codes as bytes / 4 == floats: the count is in 4-byte units either way
-        return {"kind": "flat", "d": d, "ntotal": ntotal, "metric": metric, "rows": xb.reshape(ntotal, d), "ids": None}
+        return {"kind": "flat", "d": d, "ntotal": ntotal, "metric": metric, "rows": np.array(xb.reshape(ntotal, d)), "ids": None}
     if tag == "IxSQ":
         d, ntotal, _, metric = _header(r)
         _read_sq(r)
         codes = r.vec(np.uint8)
-        return {"kind": "flat", "d": d, "ntotal": ntotal, "metric": metric, "rows": codes.view(np.float16).reshape(ntotal, d), "ids": None}
+        return {"kind": "flat", "d": d, "ntotal": ntotal, "metric": metric, "rows": np.array(codes.view(np.float16).reshape(ntotal, d)), "ids": None}
     if tag in ("IwFl", "IwSq"):
         d, ntotal, _, metric = _header(r)
         nlist, nprobe = r.take("Q"), r.take("Q")
-        quant = _read_index(r)
+        quant = _read_quantizer(r)
         if quant["kind"] != "flat":
             raise NotImplementedError("IVF coarse quantiser %r: only a flat quantiser is supported" % quant["kind"])
         dm_type = r.take("b")
@@ -139,6 +179,47 @@ def _read_index(r):
         sizes, rows, ids = _read_invlists(r, nlist, dt, d)
         return {"kind": "ivfflat", "d": d, "ntotal": ntotal, "metric": metric, "nlist": int(nlist), "nprobe": int(nprobe),
                 "centroids": np.asarray(quant["rows"], dtype=np.float32), "list_sizes": sizes, "rows": rows, "ids": ids}
+    if tag == "IwPQ":
+        d, ntotal, _, metric = _header(r)
+        nlist, nprobe = r.take("Q"), r.take("Q")
+        quant = _read_quantizer(r)
+        if quant["kind"] != "flat":
+            raise NotImplementedError("IVF coarse quantiser %r: only a flat or HNSW-flat quantiser is supported" % quant["kind"])
+        dm_type = r.take("b")
+        r.vec(np.int64)                  # direct map array
+        if dm_type == 2:
+            raise NotImplementedError("IVF direct map stored as a hash table")
+        by_residual = bool(r.take("B"))
+        code_size = r.take("Q")
+        pq_d, M, nbits = r.take("Q"), r.take("Q"), r.take("Q")
+        codebook = r.vec(np.float32)
+        if nbits != 8:
+            raise NotImplementedError("PQ with %d-bit codes: only 8-bit codes (PQ{M}x8) are served" % nbits)
+        if pq_d != d or M < 1 or d % M:
+            raise ValueError("PQ d=%d M=%d for an index of d=%d (M must divide d)" % (pq_d, M, d))
+        if code_size != M:
+            raise ValueError("IVF-PQ code size %d for M=%d (8-bit codes take M bytes)" % (code_size, M))
+        if codebook.size != M * 256 * (d // M):
+            raise ValueError("PQ codebook holds %d floats, expected %d" % (codebook.size, M * 256 * (d // M)))
+        sizes, codes, ids = _read_invlists(r, nlist, np.uint8, M)
+        return {"kind": "ivfpq", "d": d, "ntotal": ntotal, "metric": metric, "nlist": int(nlist), "nprobe": int(nprobe),
+                "M": int(M), "by_residual": by_residual, "centroids": np.array(quant["rows"], dtype=np.float32),
+                "codebook": np.array(codebook).reshape(M, 256, d // M), "list_sizes": sizes, "codes": codes, "ids": ids,
+                "transform": None}
+    if tag == "IxPT":
+        _header(r)
+        nt = r.take("i")
+        if nt != 1:
+            raise NotImplementedError("pre-transform chain of %d transforms: load_index serves exactly one linear "
+                                      "transform around an IVF-PQ index" % nt)
+        A, b = _read_linear_transform(r)
+        sub = _read_index(r)
+        if sub["kind"] != "ivfpq":
+            raise NotImplementedError("pre-transform around a %r index: load_index serves it around IVF-PQ only" % sub["kind"])
+        if A.shape[0] != sub["d"]:
+            raise ValueError("pre-transform outputs d=%d, the index holds d=%d" % (A.shape[0], sub["d"]))
+        sub["transform"] = (A, b)
+        return sub
     if tag in ("IxMp", "IxM2"):
         d, ntotal, _, metric = _header(r)
         sub = _read_index(r)
@@ -149,15 +230,19 @@ def _read_index(r):
             sub["ids"] = np.asarray(id_map)[sub["ids"]]
         return sub
     raise NotImplementedError(
-        "FAISS index type %r is not readable: it stores quantised codes or a graph (PQ / OPQ / HNSW / pre-transform "
-        "chains, which autofaiss selects for large sets); this engine serves exact fp16 rows — rebuild from the "
-        "embedding shards with load_index(<folder of .npy>) or build_ivf_index" % tag)
+        "FAISS index type %r is not readable: this engine serves flat, IVF-Flat and IVF-PQ (8-bit codes, flat or HNSW "
+        "coarse quantiser, at most one OPQ / rotation pre-transform) files; a top-level HNSW index, a flat PQ index, "
+        "4-bit / fast-scan PQ, refinement and on-disk lists are not served — rebuild as one of those types, or "
+        "re-index from the embedding shards with load_index(<folder of .npy>) or build_ivf_index" % tag)
 
 
 def read_faiss_index(path):
     """Parse a FAISS index file into plain arrays (see the module docstring for the supported types)."""
     with open(path, "rb") as f:
-        buf = f.read()
+        if f.seek(0, 2) == 0:
+            raise ValueError("%s is empty" % path)
+        buf = mmap.mmap(f.fileno(), 0, access=mmap.ACCESS_READ)
+    # every returned array is a copy (the map closes when the last view made while parsing goes away)
     info = _read_index(_R(buf))
     if info["metric"] != METRIC_INNER_PRODUCT:
         raise NotImplementedError("FAISS index with metric %d: the search path is inner product (cosine on normalised rows)" % info["metric"])
@@ -247,5 +332,90 @@ def write_ivfflat(path, centroids, rows, assign, ids=None, nprobe=1, fp16=False,
             out.append(rows[sel].tobytes())
             out.append(ids[sel].tobytes())
             off += m
+    with open(path, "wb") as f:
+        f.write(b"".join(out))
+
+
+def _w_invlists(out, nlist, code_size, codes, ids, assign, sparse_sizes):
+    out.append(struct.pack("<I", _fourcc("ilar")))
+    out.append(struct.pack("<QQ", nlist, code_size))
+    assign = np.asarray(assign, dtype=np.int64)
+    sizes = np.bincount(assign, minlength=nlist).astype(np.uint64)
+    if sparse_sizes:
+        out.append(struct.pack("<I", _fourcc("sprs")))
+        nz = np.nonzero(sizes)[0]
+        _w_vec(out, np.stack([nz.astype(np.uint64), sizes[nz]], axis=1).reshape(-1))
+    else:
+        out.append(struct.pack("<I", _fourcc("full")))
+        _w_vec(out, sizes)
+    order = np.argsort(assign, kind="stable")
+    off = 0
+    for l in range(nlist):
+        m = int(sizes[l])
+        if m:
+            sel = order[off:off + m]
+            out.append(codes[sel].tobytes())
+            out.append(ids[sel].tobytes())
+            off += m
+
+
+def _w_hnsw_flat(out, centroids):
+    """An IndexHNSWFlat over the centroids: a one-level graph whose neighbour slots are empty (-1); readers skip it."""
+    nlist, d = centroids.shape
+    out.append(struct.pack("<I", _fourcc("IHNf")))
+    _w_header(out, d, nlist, METRIC_INNER_PRODUCT)
+    _w_vec(out, np.array([1.0], np.float64))                        # assign_probas
+    _w_vec(out, np.array([0, 64], np.int32))                        # cum_nneighbor_per_level (2 * HNSW32 at level 0)
+    _w_vec(out, np.ones(nlist, np.int32))                           # levels
+    _w_vec(out, (np.arange(nlist + 1) * 64).astype(np.uint64))      # offsets
+    _w_vec(out, np.full(nlist * 64, -1, np.int32))                  # neighbors
+    out.append(struct.pack("<iiiii", 0, 0, 40, 16, 1))              # entry_point, max_level, efConstruction, efSearch, upper_beam
+    out.append(struct.pack("<I", _fourcc("IxFI")))
+    _w_header(out, d, nlist, METRIC_INNER_PRODUCT)
+    _w_vec(out, centroids.reshape(-1))
+
+
+def write_ivfpq(path, centroids, codebook, codes, assign, ids=None, nprobe=1, by_residual=True, transform=None,
+                transform_tag="LTra", hnsw=False, sparse_sizes=False, id_map=None, nbits=8, code_size=None, pq_d=None):
+    """IndexIVFPQ in the layout read above (test fixtures).  codebook [M, 256, d / M]; codes [n, M] uint8 with list
+    `assign[i]`; transform = (A [d, d_in], b or None) wraps it in IxPT (`transform_tag` LTra or rrot); hnsw = an IHNf
+    quantiser; id_map wraps everything in IxMp.  nbits / code_size / pq_d override the header fields (refusal tests)."""
+    centroids = np.ascontiguousarray(centroids, dtype=np.float32)
+    codebook = np.ascontiguousarray(codebook, dtype=np.float32)
+    codes = np.ascontiguousarray(codes, dtype=np.uint8)
+    nlist, d = centroids.shape
+    n, M = codes.shape
+    ids = np.arange(n, dtype=np.int64) if ids is None else np.asarray(ids, dtype=np.int64)
+    out = []
+    if id_map is not None:
+        out.append(struct.pack("<I", _fourcc("IxMp")))
+        _w_header(out, transform[0].shape[1] if transform is not None else d, n, METRIC_INNER_PRODUCT)
+    if transform is not None:
+        A, b = transform
+        A = np.ascontiguousarray(A, dtype=np.float32)
+        out.append(struct.pack("<I", _fourcc("IxPT")))
+        _w_header(out, A.shape[1], n, METRIC_INNER_PRODUCT)
+        out.append(struct.pack("<i", 1))
+        out.append(struct.pack("<IB", _fourcc(transform_tag), 0 if b is None else 1))
+        _w_vec(out, A.reshape(-1))
+        _w_vec(out, np.zeros(0, np.float32) if b is None else np.asarray(b, np.float32))
+        out.append(struct.pack("<iiB", A.shape[1], A.shape[0], 1))
+    out.append(struct.pack("<I", _fourcc("IwPQ")))
+    _w_header(out, d, n, METRIC_INNER_PRODUCT)
+    out.append(struct.pack("<QQ", nlist, nprobe))
+    if hnsw:
+        _w_hnsw_flat(out, centroids)
+    else:
+        out.append(struct.pack("<I", _fourcc("IxFI")))
+        _w_header(out, d, nlist, METRIC_INNER_PRODUCT)
+        _w_vec(out, centroids.reshape(-1))
+    out.append(struct.pack("<b", 0))
+    _w_vec(out, np.zeros(0, np.int64))
+    out.append(struct.pack("<BQ", 1 if by_residual else 0, M if code_size is None else code_size))
+    out.append(struct.pack("<QQQ", d if pq_d is None else pq_d, M, nbits))
+    _w_vec(out, codebook.reshape(-1))
+    _w_invlists(out, nlist, M if code_size is None else code_size, codes, ids, assign, sparse_sizes)
+    if id_map is not None:
+        _w_vec(out, np.asarray(id_map, dtype=np.int64))
     with open(path, "wb") as f:
         f.write(b"".join(out))

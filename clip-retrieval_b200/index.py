@@ -237,7 +237,8 @@ class _IndexBase:
 
     def last_scan_plan(self):
         """(kernel, queries per pass, chunks per lane, ring stages) of the last eager exhaustive scan; kernel 0 =
-        register FMA, 1 = FMA through the bulk-copy ring, 2 = wgmma split, 3 = wgmma hi-only (include/b200clip.h)."""
+        register FMA, 1 = FMA through the bulk-copy ring, 2 = wgmma split, 3 = wgmma hi-only; an IVF-PQ search reports
+        (4, sub-quantisers per CTA, CTAs per cluster, candidate warps) (include/b200clip.h)."""
         plan = np.zeros(4, dtype=np.int32)
         check(lib.b200_index_last_scan_plan(self._h, plan.ctypes.data), "last_scan_plan")
         return tuple(int(v) for v in plan)
@@ -259,20 +260,9 @@ class B200FlatIndex(_IndexBase):
         check(lib.b200_index_create_flat(int(d), int(device), C.byref(self._h)), "create_flat")
 
 
-class B200IVFFlatIndex(_IndexBase):
-    """IVF-Flat, inner product, fp16 rows (FAISS "IVF{nlist},SQfp16" / IndexIVFFlat semantics).
-
-    `nprobe` is the knob the reference touches through faiss.extract_index_ivf(index).nprobe
-    (clip_back.py:357-361,368-369)."""
-
-    def __init__(self, d, nlist, centroids, device=0):
-        super().__init__()
-        self._id_base = 0
-        self.device = device
-        c = np.ascontiguousarray(centroids, dtype=np.float32)
-        if c.shape != (nlist, d):
-            raise ValueError("centroids must be [%d, %d], got %r" % (nlist, d, c.shape))
-        check(lib.b200_index_create_ivfflat(int(d), int(nlist), c.ctypes.data, int(device), C.byref(self._h)), "create_ivfflat")
+class _IVFBase(_IndexBase):
+    """What every inverted-file index shares: `nprobe` (the knob the reference touches through
+    faiss.extract_index_ivf(index).nprobe, clip_back.py:357-361,368-369), the lists and finalize."""
 
     @property
     def nlist(self):
@@ -289,6 +279,27 @@ class B200IVFFlatIndex(_IndexBase):
     def finalize(self):
         check(lib.b200_index_finalize(self._h), "finalize")
 
+    def invlists(self):
+        """(sizes [nlist], ids concatenated list after list) — what
+        ivf_metadata_ordering.get_old_to_new_mapping reads from FAISS invlists (:46-64)."""
+        sizes = np.zeros(self.nlist, dtype=np.int64)
+        ids = np.zeros(self.ntotal, dtype=np.int64)
+        check(lib.b200_index_ivf_lists(self._h, sizes.ctypes.data, ids.ctypes.data), "ivf_lists")
+        return sizes, ids
+
+
+class B200IVFFlatIndex(_IVFBase):
+    """IVF-Flat, inner product, fp16 rows (FAISS "IVF{nlist},SQfp16" / IndexIVFFlat semantics)."""
+
+    def __init__(self, d, nlist, centroids, device=0):
+        super().__init__()
+        self._id_base = 0
+        self.device = device
+        c = np.ascontiguousarray(centroids, dtype=np.float32)
+        if c.shape != (nlist, d):
+            raise ValueError("centroids must be [%d, %d], got %r" % (nlist, d, c.shape))
+        check(lib.b200_index_create_ivfflat(int(d), int(nlist), c.ctypes.data, int(device), C.byref(self._h)), "create_ivfflat")
+
     def add_with_lists(self, x, lists):
         """Append fp16 rows keeping an EXPLICIT inverted list per row (what an existing FAISS IVF file holds)."""
         x = np.ascontiguousarray(x, dtype=np.float16)
@@ -297,13 +308,67 @@ class B200IVFFlatIndex(_IndexBase):
             raise ValueError("add_with_lists: expected rows [n, %d] and lists [n]" % self.d)
         check(lib.b200_index_add_assigned_f16(self._h, x.ctypes.data, x.shape[0], 0, lists.ctypes.data), "add_assigned")
 
-    def invlists(self):
-        """(sizes [nlist], ids concatenated list after list) — what
-        ivf_metadata_ordering.get_old_to_new_mapping reads from FAISS invlists (:46-64)."""
-        sizes = np.zeros(self.nlist, dtype=np.int64)
-        ids = np.zeros(self.ntotal, dtype=np.int64)
-        check(lib.b200_index_ivf_lists(self._h, sizes.ctypes.data, ids.ctypes.data), "ivf_lists")
-        return sizes, ids
+
+class B200IVFPQIndex(_IVFBase):
+    """IVF-PQ with 8-bit codes, inner product (FAISS IndexIVFPQ, optionally behind an OPQ / rotation pre-transform:
+    what autofaiss writes as `OPQ{M}_{d},IVF{nlist}_HNSW32,PQ{M}x8`).  Scores are dis0 + the sum of the M table
+    entries of a row's codes, in fp32 (DESIGN.md §5); the coarse step is exact where FAISS's HNSW quantiser is not.
+
+    centroids: [nlist, d] fp32; codebook: [M, 256, d / M] fp32.  Rows are added as codes (`add_codes`): this
+    engine has no PQ encoder."""
+
+    def __init__(self, d, nlist, M, centroids, codebook, by_residual=True, device=0):
+        super().__init__()
+        self._id_base = 0
+        self._d_code = int(d)
+        self.device = device
+        c = np.ascontiguousarray(centroids, dtype=np.float32)
+        if c.shape != (nlist, d):
+            raise ValueError("centroids must be [%d, %d], got %r" % (nlist, d, c.shape))
+        if M < 1 or d % M:
+            raise ValueError("M=%d must divide d=%d" % (M, d))
+        cb = np.ascontiguousarray(codebook, dtype=np.float32)
+        if cb.shape != (M, 256, d // M):
+            raise ValueError("codebook must be [%d, 256, %d], got %r" % (M, d // M, cb.shape))
+        check(lib.b200_index_create_ivfpq(int(d), int(nlist), int(M), 1 if by_residual else 0, c.ctypes.data, cb.ctypes.data,
+                                          int(device), C.byref(self._h)), "create_ivfpq")
+
+    @property
+    def M(self):
+        return int(lib.b200_index_pq_m(self._h))
+
+    def add(self, x):
+        raise NotImplementedError("IVF-PQ: this engine has no PQ encoder; add codes with add_codes(codes, lists)")
+
+    def add_synthetic(self, n, spec, row0=0):
+        raise NotImplementedError("IVF-PQ: this engine has no PQ encoder; add codes with add_codes(codes, lists)")
+
+    def add_codes(self, codes, lists):
+        """Append code rows [n, M] uint8 (numpy, or a CUDA uint8 torch tensor) with their inverted lists [n]."""
+        lists = np.ascontiguousarray(lists, dtype=np.int32)
+        M = self.M
+        if _is_torch(codes):
+            codes = codes.contiguous()
+            if codes.dim() != 2 or codes.shape[1] != M or lists.shape != (codes.shape[0],) or str(codes.dtype) != "torch.uint8":
+                raise ValueError("add_codes: expected uint8 codes [n, %d] and lists [n]" % M)
+            check(lib.b200_index_add_codes(self._h, codes.data_ptr(), codes.shape[0], 1 if codes.is_cuda else 0,
+                                           lists.ctypes.data), "add_codes")
+            return
+        codes = np.ascontiguousarray(codes, dtype=np.uint8)
+        if codes.ndim != 2 or codes.shape[1] != M or lists.shape != (codes.shape[0],):
+            raise ValueError("add_codes: expected codes [n, %d] and lists [n]" % M)
+        check(lib.b200_index_add_codes(self._h, codes.ctypes.data, codes.shape[0], 0, lists.ctypes.data), "add_codes")
+
+    def set_pretransform(self, A, b=None):
+        """Queries become A q (+ b), A [d, d_in] fp32; `d` then reports d_in (the width a caller passes)."""
+        A = np.ascontiguousarray(A, dtype=np.float32)
+        if A.ndim != 2 or A.shape[0] != self._d_code:
+            raise ValueError("set_pretransform: A must be [%d, d_in], got %r" % (self._d_code, A.shape))
+        bb = None if b is None else np.ascontiguousarray(b, dtype=np.float32).reshape(-1)
+        if bb is not None and bb.shape != (A.shape[0],):
+            raise ValueError("set_pretransform: b must be [%d]" % A.shape[0])
+        check(lib.b200_index_set_pretransform(self._h, int(A.shape[1]), A.ctypes.data, None if bb is None else bb.ctypes.data),
+              "set_pretransform")
 
 
 def list_embedding_shards(path):
@@ -326,8 +391,10 @@ def load_index(path, enable_faiss_memory_mapping=False, device=0):
     sorted file order, which is the global row id order (SURVEY.md Appendix C).  The rows go
     straight to HBM; `enable_faiss_memory_mapping` is accepted for signature parity and ignored.
     A FAISS index file (what the reference passes: `image.index`, or a folder holding `populated.index`) is read by
-    faiss_io.read_faiss_index when it is a flat / fp16 / IVF-Flat inner-product index (the types that store rows);
-    quantised-code indices raise NotImplementedError with the way out.
+    faiss_io.read_faiss_index when it is a flat / fp16 / IVF-Flat inner-product index, or an IVF-PQ one (8-bit codes,
+    flat or HNSW coarse quantiser, optionally behind one OPQ / rotation pre-transform and an id map: what autofaiss
+    writes for large collections) served from its codes; the file's nprobe is kept.  Other types raise
+    NotImplementedError naming what is missing.
     """
     del enable_faiss_memory_mapping
     from . import faiss_io
@@ -445,6 +512,19 @@ def index_from_faiss(info, device=0):
         step = 1 << 20
         for s in range(0, rows.shape[0], step):
             index.add(np.ascontiguousarray(rows[s:s + step]))
+    elif info["kind"] == "ivfpq":
+        index = B200IVFPQIndex(d, info["nlist"], info["M"], info["centroids"], info["codebook"],
+                               by_residual=info["by_residual"], device=device)
+        if info.get("transform") is not None:
+            A, b = info["transform"]
+            index.set_pretransform(A, b)
+        lists = np.repeat(np.arange(info["nlist"], dtype=np.int32), info["list_sizes"])
+        codes = info["codes"]
+        step = 1 << 22   # rows per host-to-device chunk: the codes may be a memory map of a multi-GB file
+        for s in range(0, codes.shape[0], step):
+            index.add_codes(np.ascontiguousarray(codes[s:s + step]), lists[s:s + step])
+        index.nprobe = max(1, info["nprobe"])
+        index.finalize()
     else:
         index = B200IVFFlatIndex(d, info["nlist"], info["centroids"], device=device)
         lists = np.repeat(np.arange(info["nlist"], dtype=np.int32), info["list_sizes"])

@@ -77,6 +77,21 @@ int b200_index_create_flat(int d, int device, b200_index** out);
 /* IVF-Flat: `h_centroids` is [nlist, d] fp32 on the host (rounded to fp16 inside, as the stored
  * rows are).  Rows are assigned to the centroid of maximum inner product (FAISS IVF, IP metric). */
 int b200_index_create_ivfflat(int d, int nlist, const float* h_centroids, int device, b200_index** out);
+/* IVF-PQ with 8-bit codes (FAISS IndexIVFPQ, inner product): `h_centroids` [nlist, d] fp32 (kept in fp32: they give
+ * dis0), `h_codebook` [M, 256, d / M] fp32; 1 <= M <= 256, M divides d.  by_residual: score = q.c_l + ADC(codes), else
+ * ADC(codes) alone.  Rows enter through b200_index_add_codes only (there is no encoder). */
+int b200_index_create_ivfpq(int d, int nlist, int M, int by_residual, const float* h_centroids,
+                            const float* h_codebook, int device, b200_index** out);
+/* IVF-PQ only: append n code rows ([n, M] uint8) with their inverted lists (h_lists[i] in [0, nlist)); insertion ids
+ * continue from ntotal. */
+int b200_index_add_codes(b200_index* idx, const uint8_t* codes, int64_t n, int codes_on_device, const int32_t* h_lists);
+/* IVF-PQ only: queries are d_in wide and searched as q' = A q (+ b), A [d, d_in] fp32 row-major, b [d] or NULL (FAISS
+ * IndexPreTransform with one LinearTransform: an OPQ matrix or a random rotation).  Reconstruction returns
+ * A^T (y - b), which needs orthonormal rows of A (checked here within 4e-5, as FAISS does); otherwise reconstruct and
+ * search with rows return B200_ERR_UNSUPPORTED while search itself works.  b200_index_d reports d_in afterwards. */
+int b200_index_set_pretransform(b200_index* idx, int d_in, const float* h_A, const float* h_b);
+/* M of an IVF-PQ index; 0 for the other kinds. */
+int b200_index_pq_m(const b200_index* idx);
 int b200_index_destroy(b200_index* idx);
 
 /* Pre-size the row store (rows); avoids regrowth copies for large shards. */
@@ -114,7 +129,8 @@ int b200_index_last_hi_only_fallbacks(const b200_index* idx);
 /* Plan of the last exhaustive scan launched eagerly on this handle (flat search, or the coarse step of an
  * IVF search): h_plan[4] = {kernel, queries per pass, 16-byte chunks per lane = ceil(d / 256), ring stages}.
  * kernel: 0 register FMA scan, 1 FMA scan through the bulk-copy ring, 2 wgmma split (hi/lo) scan, 3 wgmma
- * hi-only scan (queries whose proof fails are re-run in split mode).  All -1 before the first scan.  A
+ * hi-only scan (queries whose proof fails are re-run in split mode).  An IVF-PQ search reports its list scan as
+ * {4, sub-quantisers per CTA, CTAs per cluster, candidate warps per CTA}.  All -1 before the first scan.  A
  * replayed CUDA graph runs no host code and leaves it unchanged. */
 int b200_index_last_scan_plan(const b200_index* idx, int32_t* h_plan);
 /* IVF introspection used by ivf_metadata_ordering.get_old_to_new_mapping
