@@ -314,8 +314,8 @@ class B200IVFPQIndex(_IVFBase):
     what autofaiss writes as `OPQ{M}_{d},IVF{nlist}_HNSW32,PQ{M}x8`).  Scores are dis0 + the sum of the M table
     entries of a row's codes, in fp32 (DESIGN.md §5); the coarse step is exact where FAISS's HNSW quantiser is not.
 
-    centroids: [nlist, d] fp32; codebook: [M, 256, d / M] fp32.  Rows are added as codes (`add_codes`): this
-    engine has no PQ encoder."""
+    centroids: [nlist, d] fp32; codebook: [M, 256, d / M] fp32.  Rows are added as codes (`add_codes`); `encode`
+    makes the codes and lists of float rows on the GPU: `index.add_codes(*index.encode(x))`."""
 
     def __init__(self, d, nlist, M, centroids, codebook, by_residual=True, device=0):
         super().__init__()
@@ -338,10 +338,40 @@ class B200IVFPQIndex(_IVFBase):
         return int(lib.b200_index_pq_m(self._h))
 
     def add(self, x):
-        raise NotImplementedError("IVF-PQ: this engine has no PQ encoder; add codes with add_codes(codes, lists)")
+        raise NotImplementedError("IVF-PQ: add() takes no float rows; run the encoder first: add_codes(*index.encode(x))")
 
     def add_synthetic(self, n, spec, row0=0):
-        raise NotImplementedError("IVF-PQ: this engine has no PQ encoder; add codes with add_codes(codes, lists)")
+        raise NotImplementedError("IVF-PQ: add_synthetic() takes no float rows; run the encoder first: "
+                                  "add_codes(*index.encode(x))")
+
+    def encode(self, x, chunk=1 << 18):
+        """(codes, lists) of rows x [n, d] (fp16 / fp32, numpy or a CUDA tensor; d = the query width, d_in once a
+        pre-transform is set), computed on the GPU (C ABI `b200_index_encode_device`): the list of maximum inner
+        product with the fp32 centroids, then per sub-quantiser the nearest codeword (squared L2) of the residual.
+        codes: uint8 [n, M], numpy for numpy input, a CUDA tensor for CUDA input; lists: numpy int64 [n]."""
+        torch = _torch()
+        M, d = self.M, self.d
+        on_dev = _is_torch(x) and x.is_cuda
+        if not _is_torch(x):
+            x = np.asarray(x)
+            if x.dtype not in (np.float16, np.float32):
+                x = x.astype(np.float32)
+        if x.ndim != 2 or x.shape[1] != d:
+            raise ValueError("encode: expected rows [n, %d], got %r" % (d, tuple(x.shape)))
+        n = int(x.shape[0])
+        dev = x.device if on_dev else torch.device("cuda", self.device)
+        codes_d = torch.empty((n, M), dtype=torch.uint8, device=dev)
+        lists = np.empty(n, np.int64)
+        lists_d = torch.empty(min(n, chunk), dtype=torch.int32, device=dev)
+        st = torch.cuda.current_stream(dev).cuda_stream
+        for s in range(0, n, chunk):
+            e = min(n, s + chunk)
+            xc = x[s:e] if _is_torch(x) else torch.from_numpy(np.ascontiguousarray(x[s:e]))
+            xc = xc.to(device=dev, dtype=torch.float32).contiguous()
+            check(lib.b200_index_encode_device(self._h, xc.data_ptr(), e - s, lists_d.data_ptr(), None,
+                                               codes_d[s:e].data_ptr(), st), "encode")
+            lists[s:e] = lists_d[:e - s].cpu().numpy()
+        return (codes_d if on_dev else codes_d.cpu().numpy()), lists
 
     def add_codes(self, codes, lists):
         """Append code rows [n, M] uint8 (numpy, or a CUDA uint8 torch tensor) with their inverted lists [n]."""
@@ -450,6 +480,83 @@ def train_kmeans(rows, nlist, niter=10, seed=1234, spherical=False, device=0):
                                     1 if spherical else 0, C.c_void_p(cent.ctypes.data), C.c_void_p(sizes.ctypes.data),
                                     dev.index or 0), "kmeans_train")
     return cent, sizes
+
+
+def train_pq(x, M, niter=25, seed=1234, device=0):
+    """PQ codebook training on the GPU (C ABI `b200_pq_train_f32`): M independent Lloyd k-means of 256 codewords on
+    the sub-vectors of x [n, d] (fp16 / fp32, numpy or CUDA tensor; n >= 256, M divides d), seeded as `train_kmeans`.
+    Returns (codebook np.float32 [M, 256, d / M], sizes np.int64 [M, 256])."""
+    torch = _torch()
+    t = x.detach() if _is_torch(x) else torch.from_numpy(np.ascontiguousarray(x))
+    dev = t.device if t.is_cuda else torch.device("cuda", device)
+    t = t.to(device=dev, dtype=torch.float32).contiguous()
+    n, d = t.shape
+    if M < 1 or d % M:
+        raise ValueError("train_pq: M=%d must divide d=%d" % (M, d))
+    cb = np.empty((M, 256, d // M), np.float32)
+    sizes = np.empty((M, 256), np.int64)
+    check(lib.b200_pq_train_f32(C.c_void_p(t.data_ptr()), n, d, int(M), int(niter), C.c_uint64(seed),
+                                C.c_void_p(cb.ctypes.data), C.c_void_p(sizes.ctypes.data), dev.index or 0), "pq_train")
+    return cb, sizes
+
+
+PQ_TRAIN_MAX_ROWS = 65536   # FAISS: max_points_per_centroid (256) x 256 codewords
+
+
+def train_ivfpq(rows, nlist, M, niter=10, pq_niter=25, by_residual=True, seed=1234, device=0):
+    """IVF-PQ training: the coarse quantiser by `train_kmeans` on the rows as fp16, then the PQ by `train_pq` on the
+    residuals (the rows themselves without `by_residual`) of at most 65 536 rows picked one per stride (seeded).
+    Separate from building so that range shards can be encoded against one replicated quantiser.
+    Returns (centroids np.float32 [nlist, d], codebook np.float32 [M, 256, d / M])."""
+    torch = _torch()
+    t = rows.detach() if _is_torch(rows) else torch.from_numpy(np.ascontiguousarray(rows))
+    dev = t.device if t.is_cuda else torch.device("cuda", device)
+    n, d = t.shape
+    if M < 1 or d % M:
+        raise ValueError("train_ivfpq: M=%d must divide d=%d" % (M, d))
+    cent, _ = train_kmeans(t, nlist, niter=niter, seed=seed, device=dev.index or 0)
+    ns = min(n, PQ_TRAIN_MAX_ROWS)
+    pick = torch.from_numpy(stride_picks(n, ns, seed)).to(t.device)
+    sample = t[pick].to(device=dev, dtype=torch.float32).contiguous()
+    if by_residual:
+        tmp = B200IVFPQIndex(d, nlist, M, cent, np.zeros((M, 256, d // M), np.float32), device=dev.index or 0)
+        res = torch.empty_like(sample)
+        st = torch.cuda.current_stream(dev).cuda_stream
+        check(lib.b200_index_encode_device(tmp._h, sample.data_ptr(), ns, None, res.data_ptr(), None, st), "encode")
+        sample = res
+    cb, _ = train_pq(sample, M, niter=pq_niter, seed=seed, device=dev.index or 0)
+    return cent, cb
+
+
+def build_ivfpq_index(rows, nlist, M, niter=10, pq_niter=25, by_residual=True, seed=1234, nprobe=1, device=0,
+                      chunk=1 << 20):
+    """train + create + encode + add_codes + finalize: an IVF-PQ index over `rows` (fp16 / fp32, numpy or CUDA),
+    the IVF-PQ counterpart of `build_ivf_index` (autofaiss's "IVF{nlist},PQ{M}x8" without the OPQ step)."""
+    cent, cb = train_ivfpq(rows, nlist, M, niter=niter, pq_niter=pq_niter, by_residual=by_residual, seed=seed,
+                           device=device)
+    dev = rows.device.index if _is_torch(rows) and rows.is_cuda else device
+    idx = B200IVFPQIndex(cent.shape[1], nlist, M, cent, cb, by_residual=by_residual, device=dev or 0)
+    for s in range(0, rows.shape[0], chunk):
+        idx.add_codes(*idx.encode(rows[s:s + chunk]))
+    idx.finalize()
+    idx.nprobe = nprobe
+    return idx
+
+
+def stride_picks(n, count, seed):
+    """One seeded row per stride: row lo_i + mix(seed ^ i * 0xD1342543DE82EF95) % (hi_i - lo_i) of the i-th of `count`
+    equal strides of n rows (the initial-centroid rule of `b200_kmeans_train_f16` and `b200_pq_train_f32`)."""
+    i = np.arange(count, dtype=np.uint64)
+    lo = (np.arange(count, dtype=object) * n // count).astype(np.int64)
+    hi = (np.arange(1, count + 1, dtype=object) * n // count).astype(np.int64)
+    span = np.maximum(1, hi - lo).astype(np.uint64)
+    with np.errstate(over="ignore"):
+        x = np.uint64(seed) ^ (i * np.uint64(0xD1342543DE82EF95))
+        x = x + np.uint64(0x9E3779B97F4A7C15)
+        x = (x ^ (x >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+        x = (x ^ (x >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+        x = x ^ (x >> np.uint64(31))
+    return lo + (x % span).astype(np.int64)
 
 
 def build_ivf_index(rows, nlist, niter=10, seed=1234, nprobe=1, device=0):

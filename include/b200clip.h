@@ -79,7 +79,8 @@ int b200_index_create_flat(int d, int device, b200_index** out);
 int b200_index_create_ivfflat(int d, int nlist, const float* h_centroids, int device, b200_index** out);
 /* IVF-PQ with 8-bit codes (FAISS IndexIVFPQ, inner product): `h_centroids` [nlist, d] fp32 (kept in fp32: they give
  * dis0), `h_codebook` [M, 256, d / M] fp32; 1 <= M <= 256, M divides d.  by_residual: score = q.c_l + ADC(codes), else
- * ADC(codes) alone.  Rows enter through b200_index_add_codes only (there is no encoder). */
+ * ADC(codes) alone.  Rows enter as codes through b200_index_add_codes; b200_index_encode_device makes those codes
+ * (and lists) from float rows. */
 int b200_index_create_ivfpq(int d, int nlist, int M, int by_residual, const float* h_centroids,
                             const float* h_codebook, int device, b200_index** out);
 /* IVF-PQ only: append n code rows ([n, M] uint8) with their inverted lists (h_lists[i] in [0, nlist)); insertion ids
@@ -92,6 +93,21 @@ int b200_index_add_codes(b200_index* idx, const uint8_t* codes, int64_t n, int c
 int b200_index_set_pretransform(b200_index* idx, int d_in, const float* h_A, const float* h_b);
 /* M of an IVF-PQ index; 0 for the other kinds. */
 int b200_index_pq_m(const b200_index* idx);
+/* IVF-PQ only: encode n fp32 rows d_x [n, width] (width = d_in when a pre-transform is set, else d; 16-byte aligned
+ * without a pre-transform) on `stream`, asynchronously.  x' = A x + b (or x); d_lists [n] = argmax_l x'.c_l over the
+ * fp32 centroids, ties to the lower list; d_residuals [n, d] = x' - c_list in fp32 (x' without by_residual);
+ * d_codes [n, M] (unpadded) = per sub-quantiser the codeword of least fp32 sum of squared differences, ties to the
+ * lower index.  Each output may be NULL.  Rows go through in chunks, so the scratch is bounded whatever n is.
+ * `b200_index_add_codes(idx, codes, n, 1, lists)` then appends the rows. */
+int b200_index_encode_device(b200_index* idx, const float* d_x, int64_t n, int32_t* d_lists, float* d_residuals,
+                             uint8_t* d_codes, void* stream);
+/* PQ training: M independent Lloyd k-means of 256 codewords (squared L2) on the sub-vectors of d_x [n, d] fp32 (device).
+ * Initial codewords: one seeded pick per stride of the rows (as b200_kmeans_train_f16), the same for every m; each
+ * codeword = mean of its rows added in ascending row order in fp32; an empty codeword takes a perturbed copy of the
+ * largest one of the same m.  h_codebook [M, 256, d / M] fp32, h_sizes [M, 256] rows per codeword under the result
+ * (or NULL).  Needs n >= 256, M dividing d, M * n < 2^31. */
+int b200_pq_train_f32(const float* d_x, int64_t n, int d, int M, int niter, uint64_t seed, float* h_codebook,
+                      int64_t* h_sizes, int device);
 int b200_index_destroy(b200_index* idx);
 
 /* Pre-size the row store (rows); avoids regrowth copies for large shards. */
