@@ -1,6 +1,7 @@
 // The index handle behind b200_index* (flat, IVF-Flat and IVF-PQ share the row store and the top-k tail).
 #pragma once
 #include "common.cuh"
+#include <algorithm>
 #include <map>
 #include <mutex>
 #include <vector>
@@ -82,9 +83,105 @@ namespace b200 {
 inline cudaError_t index_record(b200_index* idx, cudaEvent_t e, cudaStream_t st) {
   return idx->capturing ? cudaEventRecordWithFlags(e, st, cudaEventRecordExternal) : cudaEventRecord(e, st);
 }
+// Scan timing: one event pair around the row-scan launches of a query batch (read by b200_index_last_scan_ms).
+inline int scan_timer_begin(b200_index* idx, cudaStream_t st) {
+  if ((int)idx->ev.size() < idx->ev_used + 2) {
+    cudaEvent_t a, b;
+    B200_CUDA(cudaEventCreate(&a));
+    B200_CUDA(cudaEventCreate(&b));
+    idx->ev.push_back(a);
+    idx->ev.push_back(b);
+  }
+  B200_CUDA(index_record(idx, idx->ev[idx->ev_used], st));
+  return B200_OK;
+}
+inline int scan_timer_end(b200_index* idx, cudaStream_t st) {
+  B200_CUDA(index_record(idx, idx->ev[idx->ev_used + 1], st));
+  idx->ev_used += 2;
+  return B200_OK;
+}
+
+inline int next_pow2(int x) {
+  int p = 1;
+  while (p < x) p <<= 1;
+  return p;
+}
+
+// Segments per probed list: enough CTAs over the `work_items` (query, probe) pairs of a launch to reach
+// `target_ctas`, at most 32, and no segment shorter than about `min_rows` rows of the longest list.
+inline int list_segments(const b200_index* idx, int target_ctas, int64_t work_items, int min_rows) {
+  const int64_t segs = std::min<int64_t>(32, std::max<int64_t>(1, (target_ctas + work_items - 1) / work_items));
+  return (int)std::max<int64_t>(1, std::min<int64_t>(segs, (idx->max_list + min_rows - 1) / min_rows));
+}
+
+// ---- knn_scan.cu ------------------------------------------------------------------------------------
 int index_ws(b200_index* idx, int slot, size_t bytes, void** out);
 // Row scan + top-k of nq queries against rows [0, n) of `rows` (row-major fp16, d columns).
 // Writes, per query, k sorted keys (local row ids) into d_keys_out [nq, k].
 int scan_topk_keys(b200_index* idx, const __half* rows, int64_t n, const float* d_q, int nq, int k,
                    unsigned long long* d_keys_out, cudaStream_t st);
+// One query: appends up to `cap` keys to d_out, *d_count receives the number of hits (may exceed cap).
+int range_scan(b200_index* idx, const __half* rows, int64_t n, const float* d_q, float thresh, unsigned long long* d_out,
+               unsigned int cap, unsigned int* d_count, cudaStream_t st);
+// keys -> (D, I): key 0 -> (-FLT_MAX, -1); `slot_to_id` (or null) maps the key's id before id_base is added.
+int decode_keys(const unsigned long long* keys, int64_t count, int64_t id_base, const uint32_t* slot_to_id, float* D,
+                int64_t* I, cudaStream_t st);
+
+// The select tail of every search: M candidate keys per query -> the k best, sorted.  Level 1 cuts the candidates
+// into `slices` chunks of about C keys and keeps k of each; level 2 merges the slices * k survivors in one block
+// with a C2-entry buffer.
+constexpr size_t SELECT_SMEM_MAX = 200 * 1024;   // shared memory of one select block; bounds C, hence k
+inline int select_buffer(int k) { return std::max(2048, next_pow2(2 * k)); }   // C: entries of a block's sort buffer
+struct SelectPlan {
+  int64_t M = 0;
+  int k = 0, C = 0, slices = 0, C2 = 0;
+  size_t keys(int nq) const { return (size_t)nq * (M + (int64_t)slices * k); }   // scratch: candidates + level-1 output
+};
+// Fails with B200_ERR_UNSUPPORTED when k is beyond what one select block holds.
+int plan_select(int64_t M, int k, SelectPlan* p);
+// cand [nq, M] -> out [nq, k] through tmp [nq, slices * k]: two topk_select_kernel launches.
+int select_topk(const SelectPlan& p, const unsigned long long* cand, unsigned long long* tmp, unsigned long long* out,
+                int nq, cudaStream_t st);
+// One launch of topk_select_kernel: grid (slices, nq), the k best of each slice of the M keys of a query.
+int launch_topk_select(const unsigned long long* in, int64_t in_stride_q, int64_t M, int k, int C,
+                       unsigned long long* out, int64_t out_stride_q, int slices, int nq, cudaStream_t st);
+
+// ---- knn_mma.cu: batched scan on the tensor cores, same contract as scan_topk_keys ---------------------
+int scan_topk_keys_mma(b200_index* idx, const __half* rows, int64_t n, const float* d_q, int nq, int k,
+                       unsigned long long* d_keys_out, cudaStream_t st);
+
+// ---- knn_ivf.cu ---------------------------------------------------------------------------------------
+int ivf_create(b200_index* idx, int nlist, const float* h_centroids);
+int ivf_finalize(b200_index* idx);
+int ivf_add_synthetic(b200_index* idx, int64_t n, int64_t row0, const b200_synth_spec* spec);
+int ivf_search_keys(b200_index* idx, const float* d_q, int nq, int k, unsigned long long* d_keys, cudaStream_t st);
+int ivf_lists(b200_index* idx, int64_t* h_sizes, int64_t* h_ids);
+void ivf_free(b200_index* idx);
+// One query (device pointer): (score, slot) keys of every probed row above `thresh`; *d_count = number of hits.
+int ivf_range_scan(b200_index* idx, const float* d_q, float thresh, unsigned long long* d_out, unsigned int cap,
+                   unsigned int* d_count, cudaStream_t st);
+// Room for `need` rows of row_bytes in idx->pending (contents kept).  `amortised`: grow by at least half the
+// capacity, for callers that add a few rows at a time; otherwise exactly to `need`.
+int grow_pending(b200_index* idx, int64_t need, bool amortised);
+
+// ---- knn_ivfpq.cu ---------------------------------------------------------------------------------------
+int ivfpq_search_keys(b200_index* idx, const float* d_q, int nq, int k, unsigned long long* d_keys, cudaStream_t st);
+// One query (device pointer): (score, slot) keys of every row of the probed lists scoring strictly above `thresh`.
+int ivfpq_range_scan(b200_index* idx, const float* d_q, float thresh, unsigned long long* d_out, unsigned int cap,
+                     unsigned int* d_count, cudaStream_t st);
+// Rows for keys (search_and_reconstruct) or for ids (reconstruct); exactly one of the two is non-null.
+int ivfpq_decode(b200_index* idx, const unsigned long long* keys, const int64_t* ids, int64_t count, float* d_R,
+                 cudaStream_t st);
+
+// ---- knn_index.cu -----------------------------------------------------------------------------------------
+// packed per-shard blocks [I int64 nq*k | D f32 nq*k | padding], `stride` bytes apart (sharded.cu, sharded.py)
+int merge_packed_launch(const void* d_gathered, int G, size_t stride, int nq, int k, float* d_D, int64_t* d_I,
+                        cudaStream_t st);
+
+// ---- synth.cu: deterministic synthetic rows (OutT = __half or float) -------------------------------------
+template <typename OutT>
+int synth_rows(OutT* d_out, int64_t n, int d, int64_t row0, const b200_synth_spec* spec, cudaStream_t st);
+// out[p] = synthetic row (row0 + src_rows[p])
+int synth_rows_indirect_f16(__half* out, const uint32_t* src_rows, int64_t n, int d, int64_t row0,
+                            const b200_synth_spec* spec, cudaStream_t st);
 }  // namespace b200

@@ -10,28 +10,6 @@
 
 namespace b200 {
 
-int decode_keys(const unsigned long long* keys, int64_t count, int64_t id_base, const uint32_t* slot_to_id, float* D,
-                int64_t* I, cudaStream_t st);
-template <typename OutT>
-int synth_rows(OutT* d_out, int64_t n, int d, int64_t row0, const b200_synth_spec* spec, cudaStream_t st);
-// IVF (knn_ivf.cu)
-int ivf_create(b200_index* idx, int nlist, const float* h_centroids);
-int ivf_finalize(b200_index* idx);
-int ivf_add_synthetic(b200_index* idx, int64_t n, int64_t row0, const b200_synth_spec* spec);
-int ivf_search_keys(b200_index* idx, const float* d_q, int nq, int k, unsigned long long* d_keys, cudaStream_t st);
-int ivf_lists(b200_index* idx, int64_t* h_sizes, int64_t* h_ids);
-void ivf_free(b200_index* idx);
-int range_scan(b200_index* idx, const __half* rows, int64_t n, const float* d_q, float thresh, unsigned long long* d_out,
-               unsigned int cap, unsigned int* d_count, cudaStream_t st);
-int ivf_range_scan(b200_index* idx, const float* d_q, float thresh, unsigned long long* d_out, unsigned int cap,
-                   unsigned int* d_count, cudaStream_t st);
-// IVF-PQ (knn_ivfpq.cu)
-int ivfpq_search_keys(b200_index* idx, const float* d_q, int nq, int k, unsigned long long* d_keys, cudaStream_t st);
-int ivfpq_range_scan(b200_index* idx, const float* d_q, float thresh, unsigned long long* d_out, unsigned int cap,
-                     unsigned int* d_count, cudaStream_t st);
-int ivfpq_decode(b200_index* idx, const unsigned long long* keys, const int64_t* ids, int64_t count, float* d_R,
-                 cudaStream_t st);
-
 __global__ void f32_to_f16_kernel(const float* __restrict__ in, __half* __restrict__ out, int64_t count) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < count) out[i] = __float2half_rn(in[i]);
@@ -280,17 +258,7 @@ static int add_rows(b200_index* idx, const void* rows, int64_t n, int on_device,
   __half* dst;
   if (idx->nlist > 0) {
     // IVF: stage in insertion order until finalize buckets them
-    const int64_t need = idx->npending + n;
-    if (need > idx->pending_cap) {
-      __half* np = nullptr;
-      B200_CUDA(cudaMalloc((void**)&np, (size_t)need * d * sizeof(__half)));
-      if (idx->pending) {
-        B200_CUDA(cudaMemcpy(np, idx->pending, (size_t)idx->npending * d * 2, cudaMemcpyDeviceToDevice));
-        B200_CUDA(cudaFree(idx->pending));
-      }
-      idx->pending = np;
-      idx->pending_cap = need;
-    }
+    B200_TRY(grow_pending(idx, idx->npending + n, false));
     dst = idx->pending + idx->npending * d;
   } else {
     B200_CHECK(idx->ntotal + n < (1ll << 32), B200_ERR_UNSUPPORTED, "add: a shard holds at most 2^32 rows");

@@ -12,18 +12,12 @@
 // ascending id order even when the tied rows sit in different lists (explicit lists of an index file).
 // HBM-bound: bytes per query = nprobe * (N/nlist) * d * 2 (+ nlist * d * 2 for the coarse step).
 #include "index.cuh"
-#include "topk.cuh"
+#include "scan.cuh"
 #include <cub/cub.cuh>
 #include <algorithm>
 
 namespace b200 {
 
-template <typename OutT>
-int synth_rows(OutT* d_out, int64_t n, int d, int64_t row0, const b200_synth_spec* spec, cudaStream_t st);
-int launch_topk_select(const unsigned long long* in, int64_t in_stride_q, int64_t M, int k, int C,
-                       unsigned long long* out, int64_t out_stride_q, int slices, int nq, cudaStream_t st);
-int synth_rows_indirect_f16(__half* out, const uint32_t* src_rows, int64_t n, int d, int64_t row0,
-                            const b200_synth_spec* spec, cudaStream_t st);
 constexpr int SCAN_ALIGN = 4;
 
 // ---- assignment: argmax_c <x, c> --------------------------------------------------------------------
@@ -41,13 +35,7 @@ ivf_assign_kernel(const uint4* __restrict__ X, int64_t n, int cpr, const uint4* 
     const int ci = c * 32 + lane;
     uint4 v = make_uint4(0, 0, 0, 0);
     if (ci < cpr) v = X[row * cpr + ci];
-    const __half2* h2 = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-    for (int j = 0; j < 4; j++) {
-      const float2 t = __half22float2(h2[j]);
-      x[c][2 * j] = t.x;
-      x[c][2 * j + 1] = t.y;
-    }
+    chunk_to_f32(v, x[c]);
   }
   float best = -INFINITY;
   uint32_t best_l = 0;
@@ -59,16 +47,7 @@ ivf_assign_kernel(const uint4* __restrict__ X, int64_t n, int cpr, const uint4* 
 #pragma unroll
         for (int c = 0; c < CH; c++) {
           const int ci = c * 32 + lane;
-          if (ci < cpr) {
-            const uint4 v = Cn[(int64_t)(l0 + u) * cpr + ci];
-            const __half2* h2 = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-            for (int j = 0; j < 4; j++) {
-              const float2 t = __half22float2(h2[j]);
-              acc[u] = fmaf(t.x, x[c][2 * j], acc[u]);
-              acc[u] = fmaf(t.y, x[c][2 * j + 1], acc[u]);
-            }
-          }
+          if (ci < cpr) fma_chunk(Cn[(int64_t)(l0 + u) * cpr + ci], x[c], acc[u]);
         }
       }
     }
@@ -166,33 +145,17 @@ ivf_scan_kernel(const uint4* __restrict__ X, const uint32_t* __restrict__ row_id
   const int p = (blockIdx.x / segs) % nprobe;
   const int q = blockIdx.x / (segs * nprobe);
   unsigned long long* wkeys = s_keys + (size_t)warp * k;
-  for (int i = lane; i < k; i += 32) wkeys[i] = 0ull;
+  warp_lists_clear(wkeys, k, lane);
   __syncwarp();
   const unsigned long long pk = probes[(int64_t)q * nprobe + p];
   unsigned long long worst = 0ull;
   int worst_pos = 0;
   if (pk != 0ull) {
-    const uint32_t l = key_id(pk);
-    const int64_t lbeg = offsets[l], lend = offsets[l + 1];
-    const int64_t len = lend - lbeg;
-    const int64_t per = ((len + segs - 1) / segs + SCAN_ALIGN - 1) / SCAN_ALIGN * SCAN_ALIGN;
-    const int64_t beg = lbeg + (int64_t)seg * per;
-    const int64_t end = beg + per < lend ? beg + per : lend;
+    int64_t beg, end;
+    segment_rows(offsets, key_id(pk), segs, seg, SCAN_ALIGN, beg, end);
     const int d = cpr * 8;
     float qr[CH][8];
-#pragma unroll
-    for (int c = 0; c < CH; c++) {
-      const int ci = c * 32 + lane;
-      if (ci < cpr) {
-        const float4 a = *reinterpret_cast<const float4*>(Q + (size_t)q * d + ci * 8);
-        const float4 b = *reinterpret_cast<const float4*>(Q + (size_t)q * d + ci * 8 + 4);
-        qr[c][0] = a.x; qr[c][1] = a.y; qr[c][2] = a.z; qr[c][3] = a.w;
-        qr[c][4] = b.x; qr[c][5] = b.y; qr[c][6] = b.z; qr[c][7] = b.w;
-      } else {
-#pragma unroll
-        for (int j = 0; j < 8; j++) qr[c][j] = 0.f;
-      }
-    }
+    load_query_slice<CH>(qr, Q + (size_t)q * d, cpr, lane, true);
     for (int64_t r0 = beg + (int64_t)warp * 4; r0 < end; r0 += (int64_t)nwarps * 4) {
       uint4 v[4][CH];
 #pragma unroll
@@ -208,15 +171,7 @@ ivf_scan_kernel(const uint4* __restrict__ X, const uint32_t* __restrict__ row_id
 #pragma unroll
       for (int u = 0; u < 4; u++) {
 #pragma unroll
-        for (int c = 0; c < CH; c++) {
-          const __half2* h2 = reinterpret_cast<const __half2*>(&v[u][c]);
-#pragma unroll
-          for (int j = 0; j < 4; j++) {
-            const float2 t = __half22float2(h2[j]);
-            acc[u] = fmaf(t.x, qr[c][2 * j], acc[u]);
-            acc[u] = fmaf(t.y, qr[c][2 * j + 1], acc[u]);
-          }
-        }
+        for (int c = 0; c < CH; c++) fma_chunk(v[u][c], qr[c], acc[u]);
       }
       warp_transpose_reduce<4>(acc, lane);
       const float s = acc[0];
@@ -227,18 +182,11 @@ ivf_scan_kernel(const uint4* __restrict__ X, const uint32_t* __restrict__ row_id
       const bool reach = live && f32_to_ordered(s) >= (uint32_t)(worst >> 32);
       unsigned long long key = 0ull;
       if (reach) key = make_key(s, __ldg(row_ids + my_r));
-      unsigned pend = __ballot_sync(FULL, reach && key > worst);
-      while (pend) {
-        const int src = __ffs(pend) - 1;
-        pend &= pend - 1;
-        const unsigned long long ckey = __shfl_sync(FULL, key, src);
-        warp_list_insert(wkeys, k, ckey, worst, worst_pos, lane);
-      }
+      warp_offer(wkeys, k, reach && key > worst, key, &worst, &worst_pos, lane);
     }
   }
   __syncwarp();
-  unsigned long long* o = out_keys + (int64_t)q * out_stride_q + ((int64_t)(p * segs + seg) * nwarps + warp) * k;
-  for (int j = lane; j < k; j += 32) o[j] = wkeys[j];
+  warp_list_store(out_keys + (int64_t)q * out_stride_q + ((int64_t)(p * segs + seg) * nwarps + warp) * k, wkeys, k, lane);
 }
 
 typedef void (*ivf_scan_fn)(const uint4*, const uint32_t*, int, const float*, const unsigned long long*, int, int,
@@ -301,28 +249,50 @@ void ivf_free(b200_index* idx) {
   if (idx->pt_b) cudaFree(idx->pt_b);
 }
 
-// Sort (list, src) pairs by list (stable) and derive list offsets; `lists`/`src` are device arrays of n.
-static int sort_by_list(b200_index* idx, uint32_t* lists, uint32_t* src, int64_t n, uint32_t** sorted_src_out,
-                        void** to_free) {
+int grow_pending(b200_index* idx, int64_t need, bool amortised) {
+  if (need <= idx->pending_cap) return B200_OK;
+  const int64_t rb = idx->row_bytes;
+  const int64_t cap = amortised ? std::max(need, idx->pending_cap + idx->pending_cap / 2) : need;
+  void* np = nullptr;
+  B200_CUDA(cudaMalloc(&np, (size_t)cap * rb));
+  if (idx->pending) {
+    B200_CUDA(cudaMemcpy(np, idx->pending, (size_t)idx->npending * rb, cudaMemcpyDeviceToDevice));
+    B200_CUDA(cudaFree(idx->pending));
+  }
+  idx->pending = (__half*)np;
+  idx->pending_cap = cap;
+  return B200_OK;
+}
+
+// Sort (list, src) pairs by list (stable) into (lists2, src2) and derive offsets [nlist + 1] from the sorted lists.
+// As with cub, a null `tmp` only reports the scratch size in tmp_bytes.
+static int sort_pairs_by_list(void* tmp, size_t& tmp_bytes, uint32_t* lists, uint32_t* lists2, uint32_t* src,
+                              uint32_t* src2, int64_t n, int nlist, int64_t* offsets) {
+  int bits = 1;
+  while ((1ll << bits) < nlist) bits++;
+  cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, lists, lists2, src, src2, (int)n, 0, bits);
+  if (!tmp) return B200_OK;
+  count_launch(4);
+  offsets_from_sorted_kernel<<<(nlist + 1 + 255) / 256, 256>>>(lists2, n, nlist, offsets);
+  B200_LAUNCH_OK();
+  return B200_OK;
+}
+
+// The index's own lists: sorts into fresh arrays, sets idx->list_offsets; the caller frees *sorted_src.
+static int sort_by_list(b200_index* idx, uint32_t* lists, uint32_t* src, int64_t n, uint32_t** sorted_src) {
   uint32_t *lists2 = nullptr, *src2 = nullptr;
   B200_CUDA(cudaMalloc((void**)&lists2, (size_t)n * 4));
   B200_CUDA(cudaMalloc((void**)&src2, (size_t)n * 4));
   B200_CHECK(n < (1ll << 31), B200_ERR_UNSUPPORTED, "ivf: at most 2^31 rows per finalize");
-  int bits = 1;
-  while ((1ll << bits) < idx->nlist) bits++;
   size_t tmp_bytes = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, lists, lists2, src, src2, (int)n, 0, bits);
   void* tmp = nullptr;
+  B200_TRY(sort_pairs_by_list(nullptr, tmp_bytes, lists, lists2, src, src2, n, idx->nlist, idx->list_offsets));
   B200_CUDA(cudaMalloc(&tmp, tmp_bytes));
-  cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, lists, lists2, src, src2, (int)n, 0, bits);
-  count_launch(4);
-  offsets_from_sorted_kernel<<<(idx->nlist + 1 + 255) / 256, 256>>>(lists2, n, idx->nlist, idx->list_offsets);
-  B200_LAUNCH_OK();
+  B200_TRY(sort_pairs_by_list(tmp, tmp_bytes, lists, lists2, src, src2, n, idx->nlist, idx->list_offsets));
   B200_CUDA(cudaDeviceSynchronize());
   B200_CUDA(cudaFree(tmp));
   B200_CUDA(cudaFree(lists2));
-  *sorted_src_out = src2;
-  *to_free = src2;
+  *sorted_src = src2;
   return B200_OK;
 }
 
@@ -384,8 +354,7 @@ int ivf_finalize(b200_index* idx) {
   iota_kernel<<<(unsigned)((n + 255) / 256), 256>>>(src, n, 0u);
   B200_LAUNCH_OK();
   uint32_t* sorted_src = nullptr;
-  void* to_free = nullptr;
-  B200_TRY(sort_by_list(idx, lists, src, n, &sorted_src, &to_free));
+  B200_TRY(sort_by_list(idx, lists, src, n, &sorted_src));
   __half* nrows = nullptr;
   uint32_t* nids = nullptr;
   B200_CUDA(cudaMalloc((void**)&nrows, (size_t)n * rb));
@@ -395,7 +364,7 @@ int ivf_finalize(b200_index* idx) {
       reinterpret_cast<uint4*>(nrows), idx->row_ids, nids);
   B200_LAUNCH_OK();
   B200_CUDA(cudaDeviceSynchronize());
-  B200_CUDA(cudaFree(to_free));
+  B200_CUDA(cudaFree(sorted_src));
   B200_CUDA(cudaFree(lists));
   B200_CUDA(cudaFree(src));
   if (idx->rows) B200_CUDA(cudaFree(idx->rows));
@@ -419,17 +388,7 @@ int ivf_add_synthetic(b200_index* idx, int64_t n, int64_t row0, const b200_synth
   const bool by_construction = spec->clustered && spec->nlist == idx->nlist && idx->ntotal == 0 && idx->npending == 0;
   if (!by_construction) {
     // general path: generate in insertion order, bucket at finalize by argmax inner product
-    const int64_t need = idx->npending + n;
-    if (need > idx->pending_cap) {
-      __half* np = nullptr;
-      B200_CUDA(cudaMalloc((void**)&np, (size_t)need * d * 2));
-      if (idx->pending) {
-        B200_CUDA(cudaMemcpy(np, idx->pending, (size_t)idx->npending * d * 2, cudaMemcpyDeviceToDevice));
-        B200_CUDA(cudaFree(idx->pending));
-      }
-      idx->pending = np;
-      idx->pending_cap = need;
-    }
+    B200_TRY(grow_pending(idx, idx->npending + n, false));
     B200_TRY(synth_rows<__half>(idx->pending + idx->npending * d, n, d, row0, spec, 0));
     B200_CUDA(cudaDeviceSynchronize());
     idx->npending += n;
@@ -442,8 +401,7 @@ int ivf_add_synthetic(b200_index* idx, int64_t n, int64_t row0, const b200_synth
   lists_by_construction_kernel<<<(unsigned)((n + 255) / 256), 256>>>(lists, src, n, row0, spec->centroid_seed, spec->nlist);
   B200_LAUNCH_OK();
   uint32_t* sorted_src = nullptr;
-  void* to_free = nullptr;
-  B200_TRY(sort_by_list(idx, lists, src, n, &sorted_src, &to_free));
+  B200_TRY(sort_by_list(idx, lists, src, n, &sorted_src));
   B200_CUDA(cudaFree(lists));
   B200_CUDA(cudaFree(src));
   B200_CUDA(cudaMalloc((void**)&idx->rows, (size_t)n * d * 2));
@@ -454,7 +412,7 @@ int ivf_add_synthetic(b200_index* idx, int64_t n, int64_t row0, const b200_synth
   sorted_src_to_ids_kernel<<<(unsigned)((n + 255) / 256), 256>>>(sorted_src, n, 0u, idx->row_ids);
   B200_LAUNCH_OK();
   B200_CUDA(cudaDeviceSynchronize());
-  B200_CUDA(cudaFree(to_free));
+  B200_CUDA(cudaFree(sorted_src));
   idx->ntotal = n;
   idx->capacity = n;
   B200_TRY(build_id_to_slot(idx));
@@ -469,12 +427,6 @@ int ivf_lists(b200_index* idx, int64_t* h_sizes, int64_t* h_ids) {
     for (int64_t i = 0; i < idx->ntotal; i++) h_ids[i] = idx->id_base + (int64_t)tmp[i];
   }
   return B200_OK;
-}
-
-static int next_pow2(int x) {
-  int p = 1;
-  while (p < x) p <<= 1;
-  return p;
 }
 
 int ivf_search_keys(b200_index* idx, const float* d_q, int nq, int k, unsigned long long* d_keys, cudaStream_t st) {
@@ -492,8 +444,7 @@ int ivf_search_keys(b200_index* idx, const float* d_q, int nq, int k, unsigned l
   int threads = 256;
   while (threads > 64 && (size_t)(threads / 32) * k * 8 > 160 * 1024) threads >>= 1;
   const size_t smem = (size_t)(threads / 32) * k * 8;
-  const int C = std::max(2048, next_pow2(2 * k));
-  B200_CHECK(smem <= 200 * 1024 && (size_t)C * 8 <= 200 * 1024, B200_ERR_UNSUPPORTED, "search: k=%d exceeds the supported maximum (8192)", k);
+  B200_CHECK(smem <= 200 * 1024, B200_ERR_UNSUPPORTED, "search: k=%d exceeds the supported maximum (8192)", k);
   ivf_scan_fn fn = pick_ivf_scan(ch);
   B200_CHECK(fn != nullptr, B200_ERR_UNSUPPORTED, "ivf: unsupported dimension %d", d);
   if (smem > 48 * 1024) B200_CUDA(cudaFuncSetAttribute((const void*)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -502,32 +453,22 @@ int ivf_search_keys(b200_index* idx, const float* d_q, int nq, int k, unsigned l
   for (int q0 = 0; q0 < nq; q0 += QB) {
     const int qb = std::min(QB, nq - q0);
     // enough CTAs to fill the chip twice, segments no shorter than ~256 rows
-    int segs = (int)std::min<int64_t>(32, std::max<int64_t>(1, (2 * idx->sms + (int64_t)qb * nprobe - 1) / ((int64_t)qb * nprobe)));
-    segs = (int)std::max<int64_t>(1, std::min<int64_t>(segs, (idx->max_list + 255) / 256));
+    const int segs = list_segments(idx, 2 * idx->sms, (int64_t)qb * nprobe, 256);
     const int64_t M = (int64_t)nprobe * segs * nwarps * k;
-    int slices = (int)std::min<int64_t>(256, std::max<int64_t>(1, (M + C - 1) / C));   // one sort round per block
-    const int C2 = std::min(C, std::max(next_pow2(2 * k), next_pow2(slices * k)));
+    SelectPlan sel;
+    B200_TRY(plan_select(M, k, &sel));
     void* w0 = nullptr;
-    B200_TRY(index_ws(idx, 0, ((size_t)qb * M + (size_t)qb * slices * k) * 8, &w0));
+    B200_TRY(index_ws(idx, 0, sel.keys(qb) * 8, &w0));
     unsigned long long* k1 = (unsigned long long*)w0;
     unsigned long long* k2 = k1 + (size_t)qb * M;
-    if ((int)idx->ev.size() < idx->ev_used + 2) {
-      cudaEvent_t a, b;
-      B200_CUDA(cudaEventCreate(&a));
-      B200_CUDA(cudaEventCreate(&b));
-      idx->ev.push_back(a);
-      idx->ev.push_back(b);
-    }
-    B200_CUDA(index_record(idx, idx->ev[idx->ev_used], st));
+    B200_TRY(scan_timer_begin(idx, st));
     fn<<<(unsigned)((int64_t)qb * nprobe * segs), threads, smem, st>>>(
         reinterpret_cast<const uint4*>(idx->rows), idx->row_ids, cpr, d_q + (size_t)q0 * d, probes + (size_t)q0 * nprobe,
         nprobe, segs, idx->list_offsets, k, k1, M);
     B200_LAUNCH_OK();
-    B200_CUDA(index_record(idx, idx->ev[idx->ev_used + 1], st));
-    idx->ev_used += 2;
+    B200_TRY(scan_timer_end(idx, st));
     idx->last_scan_launches++;
-    B200_TRY(launch_topk_select(k1, M, M, k, C, k2, (int64_t)slices * k, slices, qb, st));
-    B200_TRY(launch_topk_select(k2, (int64_t)slices * k, (int64_t)slices * k, k, C2, d_keys + (size_t)q0 * k, k, 1, qb, st));
+    B200_TRY(select_topk(sel, k1, k2, d_keys + (size_t)q0 * k, qb, st));
   }
   return B200_OK;
 }
@@ -546,25 +487,10 @@ ivf_range_kernel(const uint4* __restrict__ X, int cpr, const float* __restrict__
   const int p = blockIdx.x / segs;
   const unsigned long long pk = probes[p];
   if (pk == 0ull) return;
-  const uint32_t l = key_id(pk);
-  const int64_t lbeg = offsets[l], lend = offsets[l + 1];
-  const int64_t per = (((lend - lbeg) + segs - 1) / segs + SCAN_ALIGN - 1) / SCAN_ALIGN * SCAN_ALIGN;
-  const int64_t beg = lbeg + (int64_t)seg * per;
-  const int64_t end = beg + per < lend ? beg + per : lend;
+  int64_t beg, end;
+  segment_rows(offsets, key_id(pk), segs, seg, SCAN_ALIGN, beg, end);
   float qr[CH][8];
-#pragma unroll
-  for (int c = 0; c < CH; c++) {
-    const int ci = c * 32 + lane;
-    if (ci < cpr) {
-      const float4 a = *reinterpret_cast<const float4*>(Q + ci * 8);
-      const float4 b = *reinterpret_cast<const float4*>(Q + ci * 8 + 4);
-      qr[c][0] = a.x; qr[c][1] = a.y; qr[c][2] = a.z; qr[c][3] = a.w;
-      qr[c][4] = b.x; qr[c][5] = b.y; qr[c][6] = b.z; qr[c][7] = b.w;
-    } else {
-#pragma unroll
-      for (int j = 0; j < 8; j++) qr[c][j] = 0.f;
-    }
-  }
+  load_query_slice<CH>(qr, Q, cpr, lane, true);
   for (int64_t r0 = beg + (int64_t)warp * 4; r0 < end; r0 += (int64_t)nwarps * 4) {
     float acc[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
@@ -574,21 +500,12 @@ ivf_range_kernel(const uint4* __restrict__ X, int cpr, const float* __restrict__
         const int ci = c * 32 + lane;
         uint4 v = make_uint4(0u, 0u, 0u, 0u);
         if (r0 + u < end && ci < cpr) v = ld_nc_v4(X + (r0 + u) * cpr + ci);
-        const __half2* h2 = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-          const float2 t = __half22float2(h2[j]);
-          acc[u] = fmaf(t.x, qr[c][2 * j], acc[u]);
-          acc[u] = fmaf(t.y, qr[c][2 * j + 1], acc[u]);
-        }
+        fma_chunk(v, qr[c], acc[u]);
       }
     }
     warp_transpose_reduce<4>(acc, lane);
     const int64_t my_r = r0 + (lane >> 3);
-    if ((lane & 7) == 0 && my_r < end && acc[0] > thresh) {
-      const unsigned int pos = atomicAdd(counter, 1u);
-      if (pos < cap) out[pos] = make_key(acc[0], (uint32_t)my_r);
-    }
+    if ((lane & 7) == 0 && my_r < end && acc[0] > thresh) range_append(out, cap, counter, acc[0], (uint32_t)my_r);
   }
 }
 
@@ -620,8 +537,7 @@ int ivf_range_scan(b200_index* idx, const float* d_q, float thresh, unsigned lon
   ivf_range_fn fn = pick_ivf_range(ch);
   B200_CHECK(fn != nullptr, B200_ERR_UNSUPPORTED, "ivf range_search: unsupported dimension %d", d);
   B200_CUDA(cudaMemsetAsync(d_count, 0, sizeof(unsigned int), st));
-  int segs = (int)std::min<int64_t>(32, std::max<int64_t>(1, (2 * idx->sms + nprobe - 1) / nprobe));
-  segs = (int)std::max<int64_t>(1, std::min<int64_t>(segs, (idx->max_list + 255) / 256));
+  const int segs = list_segments(idx, 2 * idx->sms, nprobe, 256);
   fn<<<(unsigned)(nprobe * segs), 256, 0, st>>>(reinterpret_cast<const uint4*>(idx->rows), cpr, d_q, probes, nprobe, segs,
                                                  idx->list_offsets, thresh, d_out, cap, d_count);
   B200_LAUNCH_OK();
@@ -698,11 +614,6 @@ __global__ void kmeans_split_kernel(float* __restrict__ C32, int d, int ci, int 
   }
 }
 
-__global__ void iota_u32_kernel(uint32_t* __restrict__ out, int64_t n) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = (uint32_t)i;
-}
-
 static inline uint64_t kmeans_mix(uint64_t x) {
   x += 0x9E3779B97F4A7C15ull;
   x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
@@ -752,10 +663,8 @@ extern "C" int b200_kmeans_train_f16(const void* d_rows, int64_t n, int d, int n
     B200_CUDA(cudaMemcpy(d_pick, pick.data(), (size_t)nlist * 8, cudaMemcpyHostToDevice));
     kmeans_gather_kernel<<<(unsigned)((count + 255) / 256), 256>>>(X, d, d_pick, nlist, C32);
     B200_LAUNCH_OK();
-    int bits = 1;
-    while ((1ll << bits) < nlist) bits++;
     size_t tmp_bytes = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, assign, assign2, src, src2, (int)n, 0, bits);
+    B200_TRY(sort_pairs_by_list(nullptr, tmp_bytes, assign, assign2, src, src2, n, nlist, d_off));
     B200_TRY(alloc(&tmp, tmp_bytes));
     ivf_assign_fn afn = pick_ivf_assign((cpr + 31) / 32);
     B200_CHECK(afn != nullptr, B200_ERR_UNSUPPORTED, "kmeans_train: d=%d", d);
@@ -767,12 +676,9 @@ extern "C" int b200_kmeans_train_f16(const void* d_rows, int64_t n, int d, int n
       afn<<<(unsigned)((n + 7) / 8), 256>>>(reinterpret_cast<const uint4*>(X), n, cpr, reinterpret_cast<const uint4*>(C16),
                                             nlist, assign);
       B200_LAUNCH_OK();
-      iota_u32_kernel<<<(unsigned)((n + 255) / 256), 256>>>(src, n);
+      iota_kernel<<<(unsigned)((n + 255) / 256), 256>>>(src, n, 0u);
       B200_LAUNCH_OK();
-      cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, assign, assign2, src, src2, (int)n, 0, bits);
-      count_launch(4);
-      offsets_from_sorted_kernel<<<(nlist + 1 + 255) / 256, 256>>>(assign2, n, nlist, d_off);
-      B200_LAUNCH_OK();
+      B200_TRY(sort_pairs_by_list(tmp, tmp_bytes, assign, assign2, src, src2, n, nlist, d_off));
       B200_CUDA(cudaMemcpy(off.data(), d_off, (size_t)(nlist + 1) * 8, cudaMemcpyDeviceToHost));
       if (it == niter) break;   // the last round only refreshes the sizes of the final centroids
       kmeans_update_kernel<<<nlist, 256>>>(X, d, src2, d_off, C32, spherical);

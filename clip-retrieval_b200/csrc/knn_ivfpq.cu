@@ -13,7 +13,7 @@
 // path buckets them as rows of row_bytes, and a row's code bytes load as whole 16-byte vectors.
 #include "index.cuh"
 #include "ptx.cuh"
-#include "topk.cuh"
+#include "scan.cuh"
 #include <float.h>
 #include <algorithm>
 #include <cmath>
@@ -21,21 +21,12 @@
 
 namespace b200 {
 
-int ivf_create(b200_index* idx, int nlist, const float* h_centroids);
-int launch_topk_select(const unsigned long long* in, int64_t in_stride_q, int64_t M, int k, int C,
-                       unsigned long long* out, int64_t out_stride_q, int slices, int nq, cudaStream_t st);
-
 constexpr int PQ_KSUB = 256;
 constexpr int PQ_THREADS = 256;                 // list-scan CTA: 8 warps at most, one code row per thread
 constexpr size_t PQ_SMEM_BUDGET = 200 * 1024;   // shared memory one list-scan CTA may take
 constexpr int PQ_QB = 256;                      // queries per batch (bounds the scratch)
 
 static int pq_pitch(int M) { return (M + 15) / 16 * 16; }
-static int next_pow2(int x) {
-  int p = 1;
-  while (p < x) p <<= 1;
-  return p;
-}
 
 // ---- (0) pre-transform: one warp per (query, output column) -----------------------------------------
 __global__ void pq_pretransform_kernel(const float* __restrict__ X, int nq, int d_in, const float* __restrict__ A,
@@ -131,8 +122,7 @@ ivfpq_scan_kernel(const uint8_t* __restrict__ codes, int pitch, const uint32_t* 
   const float* tq = tables + ((int64_t)q * pitch + m0) * PQ_KSUB;
   for (int i = tid; i < (m1 - m0) * PQ_KSUB; i += nthreads) s_tab[i] = tq[i];
   unsigned long long* wkeys = s_keys + (size_t)warp * k;
-  if (!RANGE)
-    for (int i = lane; i < k; i += 32) wkeys[i] = 0ull;
+  if (!RANGE) warp_lists_clear(wkeys, k, lane);
   if (cs > 1) ptx::cluster_sync();   // every CTA of the cluster runs before the first remote store
   else __syncthreads();
   const uint32_t xchg_remote = cs > 1 ? ptx::mapa_shared(ptx::smem_u32(s_xchg), 0) : 0u;
@@ -143,12 +133,9 @@ ivfpq_scan_kernel(const uint8_t* __restrict__ codes, int pitch, const uint32_t* 
     const int p = item / segs, seg = item % segs;
     const unsigned long long pk = probes[(int64_t)q * nprobe + p];
     if (pk == 0ull) continue;   // uniform over the cluster: same query, same item
-    const uint32_t l = key_id(pk);
     const float dis0 = by_residual ? key_score(pk) : 0.f;
-    const int64_t lbeg = offsets[l], lend = offsets[l + 1];
-    const int64_t per = (lend - lbeg + segs - 1) / segs;
-    const int64_t beg = lbeg + (int64_t)seg * per;
-    const int64_t end = beg + per < lend ? beg + per : lend;
+    int64_t beg, end;
+    segment_rows(offsets, key_id(pk), segs, seg, 1, beg, end);
     for (int64_t r0 = beg; r0 < end; r0 += nthreads) {
       const int64_t r = r0 + tid;
       const bool live = r < end;
@@ -173,29 +160,19 @@ ivfpq_scan_kernel(const uint8_t* __restrict__ codes, int pitch, const uint32_t* 
       }
       if (rank != 0) continue;
       if (RANGE) {
-        if (live && s > thresh) {
-          const unsigned int pos = atomicAdd(counter, 1u);
-          if (pos < cap) out_keys[pos] = make_key(s, (uint32_t)r);
-        }
+        if (live && s > thresh) range_append(out_keys, cap, counter, s, (uint32_t)r);
         continue;
       }
       // Only a row scoring at least the worst kept score can enter the list (as in the IVF-Flat scan).
       const bool reach = live && (s == s) && f32_to_ordered(s) >= (uint32_t)(worst >> 32);
       unsigned long long key = 0ull;
       if (reach) key = make_key(s, __ldg(row_ids + r));
-      unsigned pend = __ballot_sync(FULL, reach && key > worst);
-      while (pend) {
-        const int srcl = __ffs(pend) - 1;
-        pend &= pend - 1;
-        const unsigned long long ckey = __shfl_sync(FULL, key, srcl);
-        warp_list_insert(wkeys, k, ckey, worst, worst_pos, lane);
-      }
+      warp_offer(wkeys, k, reach && key > worst, key, &worst, &worst_pos, lane);
     }
   }
   if (RANGE || rank != 0) return;
   __syncwarp();
-  unsigned long long* o = out_keys + (int64_t)q * out_stride_q + ((int64_t)g * (nthreads >> 5) + warp) * k;
-  for (int j = lane; j < k; j += 32) o[j] = wkeys[j];
+  warp_list_store(out_keys + (int64_t)q * out_stride_q + ((int64_t)g * (nthreads >> 5) + warp) * k, wkeys, k, lane);
 }
 
 // ---- (4) decode: rows for keys (search_and_reconstruct) or ids (reconstruct) ----------------------------
@@ -301,12 +278,16 @@ static int pq_launch_scan(b200_index* idx, bool range, const PqPlan& pl, int nq,
   return B200_OK;
 }
 
-// Coarse select C for k = nprobe (two select levels, as the list scan).
-static int pq_coarse_c(int nprobe) { return std::max(2048, next_pow2(2 * nprobe)); }
+// Select plan of the coarse step: k = nprobe over the nlist scores of a query (two select levels, as the list scan).
+static int pq_coarse_plan(const b200_index* idx, const char* what, int nprobe, SelectPlan* cp) {
+  B200_CHECK((size_t)select_buffer(nprobe) * 8 <= SELECT_SMEM_MAX, B200_ERR_UNSUPPORTED,
+             "ivfpq %s: nprobe=%d exceeds the supported maximum (12800)", what, nprobe);
+  return plan_select(idx->nlist, nprobe, cp);
+}
 
 // Steps (0)-(2) for queries [0, qb) of d_q: probes [qb, nprobe] (keys: fp32 coarse score = dis0, list id) and
 // tables [qb, pitch, 256].  `w0` holds the coarse scores, `w4` the transformed queries and the tables.
-static int pq_prepare(b200_index* idx, const float* d_q, int qb, int nprobe, unsigned long long* probes, char* w0,
+static int pq_prepare(b200_index* idx, const float* d_q, int qb, const SelectPlan& cp, unsigned long long* probes, char* w0,
                       float* w4, float** tables_out, cudaStream_t st) {
   const int d = idx->d, M = idx->pq_M, pitch = idx->row_bytes, nlist = idx->nlist;
   const float* q = d_q;
@@ -323,12 +304,7 @@ static int pq_prepare(b200_index* idx, const float* d_q, int qb, int nprobe, uns
   pq_coarse_kernel<<<dim3((nlist + CQ_T - 1) / CQ_T, (qb + CQ_T - 1) / CQ_T), 256, 0, st>>>(q, qb, idx->pq_centroids, nlist,
                                                                                             d, ck);
   B200_LAUNCH_OK();
-  const int C = pq_coarse_c(nprobe);
-  const int slices = (int)std::min<int64_t>(256, std::max<int64_t>(1, (nlist + C - 1) / C));
-  const int C2 = std::min(C, std::max(next_pow2(2 * nprobe), next_pow2(slices * nprobe)));
-  unsigned long long* ck2 = ck + (size_t)qb * nlist;
-  B200_TRY(launch_topk_select(ck, nlist, nlist, nprobe, C, ck2, (int64_t)slices * nprobe, slices, qb, st));
-  B200_TRY(launch_topk_select(ck2, (int64_t)slices * nprobe, (int64_t)slices * nprobe, nprobe, C2, probes, nprobe, 1, qb, st));
+  B200_TRY(select_topk(cp, ck, ck + (size_t)qb * nlist, probes, qb, st));
   pq_tables_kernel<<<dim3(pitch, qb), PQ_KSUB, 0, st>>>(q, d, M, d / M, idx->pq_codebook, tables);
   B200_LAUNCH_OK();
   *tables_out = tables;
@@ -338,31 +314,22 @@ static int pq_prepare(b200_index* idx, const float* d_q, int qb, int nprobe, uns
 static size_t pq_w4_bytes(const b200_index* idx, int qb) {
   return ((((size_t)qb * idx->d + 63) & ~(size_t)63) + (size_t)qb * idx->row_bytes * PQ_KSUB) * 4;
 }
-static size_t pq_coarse_bytes(const b200_index* idx, int qb, int nprobe) {
-  const int C = pq_coarse_c(nprobe);
-  const int slices = (int)std::min<int64_t>(256, std::max<int64_t>(1, (idx->nlist + C - 1) / C));
-  return ((size_t)qb * idx->nlist + (size_t)qb * slices * nprobe) * 8;
-}
 
 int ivfpq_search_keys(b200_index* idx, const float* d_q, int nq, int k, unsigned long long* d_keys, cudaStream_t st) {
   const int nprobe = std::min(idx->nprobe, idx->nlist);
-  B200_CHECK((size_t)pq_coarse_c(nprobe) * 8 <= 200 * 1024, B200_ERR_UNSUPPORTED,
-             "ivfpq search: nprobe=%d exceeds the supported maximum (12800)", nprobe);
+  SelectPlan cp, sel;
+  B200_TRY(pq_coarse_plan(idx, "search", nprobe, &cp));
   const PqPlan pl = pq_plan(idx->row_bytes, k);
-  const int C = std::max(2048, next_pow2(2 * k));
-  B200_CHECK(pl.warps >= 1 && (size_t)C * 8 <= 200 * 1024, B200_ERR_UNSUPPORTED,
-             "search: k=%d exceeds the supported maximum (8192)", k);
+  B200_CHECK(pl.warps >= 1, B200_ERR_UNSUPPORTED, "search: k=%d exceeds the supported maximum (8192)", k);
   const int qmax = std::min(PQ_QB, nq);
   // clusters per query: enough to fill the chip twice; segments of at least ~PQ_THREADS rows
   const int target = std::max(1, 2 * idx->sms / pl.cs);
-  int segs = (int)std::min<int64_t>(32, std::max<int64_t>(1, (target + (int64_t)qmax * nprobe - 1) / ((int64_t)qmax * nprobe)));
-  segs = (int)std::max<int64_t>(1, std::min<int64_t>(segs, (idx->max_list + PQ_THREADS - 1) / PQ_THREADS));
+  const int segs = list_segments(idx, target, (int64_t)qmax * nprobe, PQ_THREADS);
   const int cpq = (int)std::min<int64_t>((int64_t)nprobe * segs, std::max<int64_t>(1, (target + qmax - 1) / qmax));
   const int64_t Mq = (int64_t)cpq * pl.warps * k;   // candidates per query
-  const int slices = (int)std::min<int64_t>(256, std::max<int64_t>(1, (Mq + C - 1) / C));
-  const int C2 = std::min(C, std::max(next_pow2(2 * k), next_pow2(slices * k)));
+  B200_TRY(plan_select(Mq, k, &sel));
   void *w0 = nullptr, *w3 = nullptr, *w4 = nullptr;
-  B200_TRY(index_ws(idx, 0, std::max(pq_coarse_bytes(idx, qmax, nprobe), ((size_t)qmax * Mq + (size_t)qmax * slices * k) * 8), &w0));
+  B200_TRY(index_ws(idx, 0, std::max(cp.keys(qmax), sel.keys(qmax)) * 8, &w0));
   B200_TRY(index_ws(idx, 3, (size_t)qmax * nprobe * 8, &w3));
   B200_TRY(index_ws(idx, 4, pq_w4_bytes(idx, qmax), &w4));
   unsigned long long* probes = (unsigned long long*)w3;
@@ -370,23 +337,14 @@ int ivfpq_search_keys(b200_index* idx, const float* d_q, int nq, int k, unsigned
   for (int q0 = 0; q0 < nq; q0 += PQ_QB) {
     const int qb = std::min(PQ_QB, nq - q0);
     float* tables = nullptr;
-    B200_TRY(pq_prepare(idx, d_q + (size_t)q0 * idx->d_in, qb, nprobe, probes, (char*)w0, (float*)w4, &tables, st));
+    B200_TRY(pq_prepare(idx, d_q + (size_t)q0 * idx->d_in, qb, cp, probes, (char*)w0, (float*)w4, &tables, st));
     unsigned long long* k1 = (unsigned long long*)w0;
     unsigned long long* k2 = k1 + (size_t)qb * Mq;
-    if ((int)idx->ev.size() < idx->ev_used + 2) {
-      cudaEvent_t a, b;
-      B200_CUDA(cudaEventCreate(&a));
-      B200_CUDA(cudaEventCreate(&b));
-      idx->ev.push_back(a);
-      idx->ev.push_back(b);
-    }
-    B200_CUDA(index_record(idx, idx->ev[idx->ev_used], st));
+    B200_TRY(scan_timer_begin(idx, st));
     B200_TRY(pq_launch_scan(idx, false, pl, qb, tables, probes, nprobe, segs, cpq, k, k1, Mq, 0.f, 0, nullptr, st));
-    B200_CUDA(index_record(idx, idx->ev[idx->ev_used + 1], st));
-    idx->ev_used += 2;
+    B200_TRY(scan_timer_end(idx, st));
     idx->last_scan_launches++;
-    B200_TRY(launch_topk_select(k1, Mq, Mq, k, C, k2, (int64_t)slices * k, slices, qb, st));
-    B200_TRY(launch_topk_select(k2, (int64_t)slices * k, (int64_t)slices * k, k, C2, d_keys + (size_t)q0 * k, k, 1, qb, st));
+    B200_TRY(select_topk(sel, k1, k2, d_keys + (size_t)q0 * k, qb, st));
   }
   idx->last_scan_plan[0] = 4;
   idx->last_scan_plan[1] = pl.mc;
@@ -399,20 +357,19 @@ int ivfpq_search_keys(b200_index* idx, const float* d_q, int nq, int k, unsigned
 int ivfpq_range_scan(b200_index* idx, const float* d_q, float thresh, unsigned long long* d_out, unsigned int cap,
                      unsigned int* d_count, cudaStream_t st) {
   const int nprobe = std::min(idx->nprobe, idx->nlist);
-  B200_CHECK((size_t)pq_coarse_c(nprobe) * 8 <= 200 * 1024, B200_ERR_UNSUPPORTED,
-             "ivfpq range_search: nprobe=%d exceeds the supported maximum (12800)", nprobe);
+  SelectPlan cp;
+  B200_TRY(pq_coarse_plan(idx, "range_search", nprobe, &cp));
   const PqPlan pl = pq_plan(idx->row_bytes, 0);
   void *w0 = nullptr, *w3 = nullptr, *w4 = nullptr;
-  B200_TRY(index_ws(idx, 0, pq_coarse_bytes(idx, 1, nprobe), &w0));
+  B200_TRY(index_ws(idx, 0, cp.keys(1) * 8, &w0));
   B200_TRY(index_ws(idx, 3, (size_t)nprobe * 8, &w3));
   B200_TRY(index_ws(idx, 4, pq_w4_bytes(idx, 1), &w4));
   unsigned long long* probes = (unsigned long long*)w3;
   float* tables = nullptr;
-  B200_TRY(pq_prepare(idx, d_q, 1, nprobe, probes, (char*)w0, (float*)w4, &tables, st));
+  B200_TRY(pq_prepare(idx, d_q, 1, cp, probes, (char*)w0, (float*)w4, &tables, st));
   B200_CUDA(cudaMemsetAsync(d_count, 0, sizeof(unsigned int), st));
   const int target = std::max(1, 2 * idx->sms / pl.cs);
-  int segs = (int)std::min<int64_t>(32, std::max<int64_t>(1, (target + nprobe - 1) / nprobe));
-  segs = (int)std::max<int64_t>(1, std::min<int64_t>(segs, (idx->max_list + PQ_THREADS - 1) / PQ_THREADS));
+  const int segs = list_segments(idx, target, nprobe, PQ_THREADS);
   const int cpq = std::min(nprobe * segs, target);
   return pq_launch_scan(idx, true, pl, 1, tables, probes, nprobe, segs, cpq, 0, d_out, 0, thresh, cap, d_count, st);
 }
@@ -475,18 +432,8 @@ int b200_index_add_codes(b200_index* idx, const uint8_t* codes, int64_t n, int c
   B200_CHECK(idx->ntotal + idx->npending + n < (1ll << 32), B200_ERR_UNSUPPORTED, "add_codes: a shard holds at most 2^32 rows");
   idx->graph_epoch++;
   DeviceGuard g(idx->device);
-  const int64_t rb = idx->row_bytes, need = idx->npending + n;
-  if (need > idx->pending_cap) {
-    const int64_t cap = std::max(need, idx->pending_cap + idx->pending_cap / 2);
-    uint8_t* np = nullptr;
-    B200_CUDA(cudaMalloc((void**)&np, (size_t)cap * rb));
-    if (idx->pending) {
-      B200_CUDA(cudaMemcpy(np, idx->pending, (size_t)idx->npending * rb, cudaMemcpyDeviceToDevice));
-      B200_CUDA(cudaFree(idx->pending));
-    }
-    idx->pending = reinterpret_cast<__half*>(np);
-    idx->pending_cap = cap;
-  }
+  const int64_t rb = idx->row_bytes;
+  B200_TRY(grow_pending(idx, idx->npending + n, true));
   uint8_t* dst = reinterpret_cast<uint8_t*>(idx->pending) + idx->npending * rb;
   if (rb != idx->pq_M) B200_CUDA(cudaMemset(dst, 0, (size_t)n * rb));   // the padding scores as the zero table rows
   B200_CUDA(cudaMemcpy2D(dst, (size_t)rb, codes, (size_t)idx->pq_M, (size_t)idx->pq_M, (size_t)n,

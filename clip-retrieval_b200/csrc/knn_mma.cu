@@ -43,9 +43,6 @@
 
 namespace b200 {
 
-int launch_topk_select(const unsigned long long* in, int64_t in_stride_q, int64_t M, int k, int C,
-                       unsigned long long* out, int64_t out_stride_q, int slices, int nq, cudaStream_t st);
-
 constexpr int MS_BM = 64;        // rows per tile
 constexpr int MS_QG = 128;       // queries per group (256 MMA columns: hi | lo)
 constexpr int MS_BN = 256;
@@ -384,9 +381,6 @@ scan_mma_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
   }
 }
 
-int make_tmap_2d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t rows, uint64_t cols, uint64_t ld_elems,
-                 uint32_t box_rows, uint32_t box_cols);
-
 // One mode of the batched scan: k sorted keys per query into d_keys_out.
 template <bool HILO>
 static int scan_mma_passes(b200_index* idx, const __half* rows, int64_t n, const float* d_q, int nq, int k,
@@ -417,18 +411,10 @@ static int scan_mma_passes(b200_index* idx, const __half* rows, int64_t n, const
     B200_TRY(make_tmap_2d(&tmQ, Qp, 0, (uint64_t)groups * MS_BN, (uint64_t)d, (uint64_t)d, MS_BN, MS_BK));
     const size_t smem = (size_t)MS_STAGES * MS_STAGE_BYTES + (size_t)groups * QG * 8 + 256 + 1024;
     B200_CUDA(cudaFuncSetAttribute(scan_mma_kernel<HILO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    if ((int)idx->ev.size() < idx->ev_used + 2) {
-      cudaEvent_t a, b;
-      B200_CUDA(cudaEventCreate(&a));
-      B200_CUDA(cudaEventCreate(&b));
-      idx->ev.push_back(a);
-      idx->ev.push_back(b);
-    }
     // sampling passes first (strided row tiles), each seeding the next pass's thresholds
     const int64_t row_tiles = (n + MS_BM - 1) / MS_BM;
     const int64_t M = (int64_t)grid * k;
-    int C = 2048;
-    while (C < 2 * k) C <<= 1;
+    const int C = select_buffer(k);
     unsigned long long* keys_q = d_keys_out + (size_t)q0 * k;
     // Pass schedule.  The first pass starts from -inf thresholds, where EVERY score is appended and the
     // buffers are compacted every third tile, so it is kept to one tile per CTA (a sample of ctas*64 rows, no
@@ -440,14 +426,14 @@ static int scan_mma_passes(b200_index* idx, const __half* rows, int64_t n, const
     if (npass == 1 && strides[0] > 64 && row_tiles / 32 >= 2 * ctas) strides[npass++] = 32;
     strides[npass++] = 1;
     bool have_thr = false;
-    B200_CUDA(cudaEventRecord(idx->ev[idx->ev_used], st));
+    B200_TRY(scan_timer_begin(idx, st));
     for (int pi = 0; pi < npass; pi++) {
       const int stride = strides[pi];
       scan_mma_kernel<HILO><<<grid, MS_THREADS, smem, st>>>(tmX, tmQ, n, d, nqb, groups, k, cand, dense, stride,
                                                             have_thr ? thr : nullptr);
       B200_LAUNCH_OK();
       idx->last_scan_launches++;
-      if (stride == 1) B200_CUDA(cudaEventRecord(idx->ev[idx->ev_used + 1], st));
+      if (stride == 1) B200_TRY(scan_timer_end(idx, st));   // the full pass is the last one
       // merge the per-CTA lists: grid*k candidates per query
       B200_TRY(launch_topk_select(dense, M, M, k, C, keys_q, k, 1, nqb, st));
       if (stride > 1) {
@@ -456,7 +442,6 @@ static int scan_mma_passes(b200_index* idx, const __half* rows, int64_t n, const
         have_thr = true;
       }
     }
-    idx->ev_used += 2;
   }
   return B200_OK;
 }
@@ -516,9 +501,7 @@ int scan_topk_keys_mma(b200_index* idx, const __half* rows, int64_t n, const flo
   rescore_kernel<<<(unsigned)((count + 7) / 8), 256, 0, st>>>(reinterpret_cast<const uint4*>(rows), d / 8, d_q, d, approx,
                                                              count, kc, exact);
   B200_LAUNCH_OK();
-  int C = 2048;
-  while (C < 2 * k) C <<= 1;
-  B200_TRY(launch_topk_select(exact, kc, kc, k, C, d_keys_out, k, 1, nq, st));
+  B200_TRY(launch_topk_select(exact, kc, kc, k, select_buffer(k), d_keys_out, k, 1, nq, st));
   verify_kernel<<<(nq + 255) / 256, 256, 0, st>>>(approx, kc, d_keys_out, k, margin, nq, fail_list, fail_count);
   B200_LAUNCH_OK();
   int h_fail = 0;

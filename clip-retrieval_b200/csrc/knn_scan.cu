@@ -8,13 +8,30 @@
 // touched only when a score beats the list's current worst (k*(1+ln(n_warp/k)) times per warp).
 // Algorithmic bytes per launch: n * d * 2 (the row store); everything else is O(grid * k).
 #include "index.cuh"
-#include "topk.cuh"
+#include "scan.cuh"
 #include <float.h>
 #include <algorithm>
 
 namespace b200 {
 
 constexpr int SCAN_U = 4;
+
+// After the transposing reduction of a block of SCAN_U rows x NQ queries starting at row r0: the lanes holding a
+// total offer (score, row) to the list of their query.
+template <int NQ>
+__device__ __forceinline__ void offer_block_scores(float s, int64_t r0, int64_t n, int nq_valid, unsigned long long* wkeys,
+                                                   int k, unsigned long long (&worst)[NQ], int (&worst_pos)[NQ], int lane) {
+  constexpr int SH = 5 - Log2<SCAN_U * NQ>::v;
+  const int vi = lane >> SH;           // value index u*NQ+q held by this lane
+  const int my_q = vi % NQ;
+  const int64_t my_r = r0 + vi / NQ;
+  unsigned long long wq = worst[0];
+#pragma unroll
+  for (int q = 1; q < NQ; q++) if (my_q == q) wq = worst[q];
+  const unsigned long long key = make_key(s, (uint32_t)my_r);
+  const bool live = ((lane & ((1 << SH) - 1)) == 0) && my_r < n && my_q < nq_valid && (s == s);
+  warp_offer<NQ, SH>(wkeys, k, live && key > wq, key, worst, worst_pos, lane);
+}
 
 template <int NQ, int CH>
 __global__ void __launch_bounds__(256)
@@ -23,28 +40,13 @@ flat_scan_kernel(const uint4* __restrict__ X, int64_t n, int cpr, const float* _
   extern __shared__ unsigned long long s_keys[];  // [warps][NQ][k]
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   unsigned long long* wkeys = s_keys + (size_t)warp * NQ * k;
-  for (int i = lane; i < NQ * k; i += 32) wkeys[i] = 0ull;
+  warp_lists_clear(wkeys, NQ * k, lane);
   __syncwarp();
 
-  // This lane's slice of each query: chunks lane, lane+32, ... (8 columns per chunk).
   float qr[NQ][CH][8];
   const int d = cpr * 8;
 #pragma unroll
-  for (int q = 0; q < NQ; q++) {
-#pragma unroll
-    for (int c = 0; c < CH; c++) {
-      const int ci = c * 32 + lane;
-      if (q < nq_valid && ci < cpr) {
-        const float4 a = *reinterpret_cast<const float4*>(Q + (size_t)q * d + ci * 8);
-        const float4 b = *reinterpret_cast<const float4*>(Q + (size_t)q * d + ci * 8 + 4);
-        qr[q][c][0] = a.x; qr[q][c][1] = a.y; qr[q][c][2] = a.z; qr[q][c][3] = a.w;
-        qr[q][c][4] = b.x; qr[q][c][5] = b.y; qr[q][c][6] = b.z; qr[q][c][7] = b.w;
-      } else {
-#pragma unroll
-        for (int j = 0; j < 8; j++) qr[q][c][j] = 0.0f;
-      }
-    }
-  }
+  for (int q = 0; q < NQ; q++) load_query_slice<CH>(qr[q], Q + (size_t)q * d, cpr, lane, q < nq_valid);
 
   unsigned long long worst[NQ];
   int worst_pos[NQ];
@@ -52,7 +54,6 @@ flat_scan_kernel(const uint4* __restrict__ X, int64_t n, int cpr, const float* _
   for (int q = 0; q < NQ; q++) { worst[q] = 0ull; worst_pos[q] = 0; }
 
   constexpr int V = SCAN_U * NQ;
-  constexpr int SH = 5 - Log2<V>::v;
   const int64_t gw = (int64_t)blockIdx.x * nwarps + warp;
   const int64_t total = (int64_t)gridDim.x * nwarps;
   const int64_t nblk = (n + SCAN_U - 1) / SCAN_U;
@@ -76,49 +77,19 @@ flat_scan_kernel(const uint4* __restrict__ X, int64_t n, int cpr, const float* _
     for (int u = 0; u < SCAN_U; u++) {
 #pragma unroll
       for (int c = 0; c < CH; c++) {
-        const __half2* h2 = reinterpret_cast<const __half2*>(&v[u][c]);
         float f[8];
+        chunk_to_f32(v[u][c], f);
 #pragma unroll
-        for (int j = 0; j < 4; j++) {
-          const float2 t = __half22float2(h2[j]);
-          f[2 * j] = t.x; f[2 * j + 1] = t.y;
-        }
-#pragma unroll
-        for (int q = 0; q < NQ; q++) {
-#pragma unroll
-          for (int j = 0; j < 8; j++) acc[u * NQ + q] = fmaf(f[j], qr[q][c][j], acc[u * NQ + q]);
-        }
+        for (int q = 0; q < NQ; q++) fma_chunk(f, qr[q][c], acc[u * NQ + q]);
       }
     }
     warp_transpose_reduce<V>(acc, lane);
-    const float s = acc[0];
-    const int vi = lane >> SH;           // value index u*NQ+q held by this lane
-    const int my_q = vi % NQ;
-    const int64_t my_r = r0 + vi / NQ;
-    unsigned long long wq = worst[0];
-#pragma unroll
-    for (int q = 1; q < NQ; q++) if (my_q == q) wq = worst[q];
-    const unsigned long long key = make_key(s, (uint32_t)my_r);
-    const bool live = ((lane & ((1 << SH) - 1)) == 0) && my_r < n && my_q < nq_valid && (s == s);
-    unsigned pend = __ballot_sync(FULL, live && key > wq);
-    while (pend) {
-      const int src = __ffs(pend) - 1;
-      pend &= pend - 1;
-      const unsigned long long ckey = __shfl_sync(FULL, key, src);
-      const int cq = (src >> SH) % NQ;
-#pragma unroll
-      for (int q = 0; q < NQ; q++)
-        if (cq == q) warp_list_insert(wkeys + q * k, k, ckey, worst[q], worst_pos[q], lane);
-    }
+    offer_block_scores<NQ>(acc[0], r0, n, nq_valid, wkeys, k, worst, worst_pos, lane);
   }
   __syncwarp();
 #pragma unroll
-  for (int q = 0; q < NQ; q++) {
-    if (q < nq_valid) {
-      unsigned long long* o = out_keys + (int64_t)q * out_stride_q + gw * k;
-      for (int j = lane; j < k; j += 32) o[j] = wkeys[q * k + j];
-    }
-  }
+  for (int q = 0; q < NQ; q++)
+    if (q < nq_valid) warp_list_store(out_keys + (int64_t)q * out_stride_q + gw * k, wkeys + q * k, k, lane);
 }
 
 // ---- staged variant: cp.async.bulk ring -------------------------------------------------------------
@@ -199,32 +170,17 @@ flat_scan_staged_kernel(const uint4* __restrict__ X, int64_t n, int cpr, const f
 
   // ---------------- consumers ----------------
   unsigned long long* wkeys = s_keys + (size_t)warp * NQ * k;
-  for (int i = lane; i < NQ * k; i += 32) wkeys[i] = 0ull;
+  warp_lists_clear(wkeys, NQ * k, lane);
   __syncwarp();
   float qr[NQ][CH][8];
   const int d = cpr * 8;
 #pragma unroll
-  for (int q = 0; q < NQ; q++) {
-#pragma unroll
-    for (int c = 0; c < CH; c++) {
-      const int ci = c * 32 + lane;
-      if (q < nq_valid && ci < cpr) {
-        const float4 a = *reinterpret_cast<const float4*>(Q + (size_t)q * d + ci * 8);
-        const float4 b = *reinterpret_cast<const float4*>(Q + (size_t)q * d + ci * 8 + 4);
-        qr[q][c][0] = a.x; qr[q][c][1] = a.y; qr[q][c][2] = a.z; qr[q][c][3] = a.w;
-        qr[q][c][4] = b.x; qr[q][c][5] = b.y; qr[q][c][6] = b.z; qr[q][c][7] = b.w;
-      } else {
-#pragma unroll
-        for (int j = 0; j < 8; j++) qr[q][c][j] = 0.0f;
-      }
-    }
-  }
+  for (int q = 0; q < NQ; q++) load_query_slice<CH>(qr[q], Q + (size_t)q * d, cpr, lane, q < nq_valid);
   unsigned long long worst[NQ];
   int worst_pos[NQ];
 #pragma unroll
   for (int q = 0; q < NQ; q++) { worst[q] = 0ull; worst_pos[q] = 0; }
   constexpr int V = SCAN_U * NQ;
-  constexpr int SH = 5 - Log2<V>::v;
 
   int s = 0;
   uint32_t phase = 0;
@@ -242,18 +198,10 @@ flat_scan_staged_kernel(const uint4* __restrict__ X, int64_t n, int cpr, const f
         const int ci = c * 32 + lane;
         uint4 v = make_uint4(0u, 0u, 0u, 0u);
         if (r0 + u < n && ci < cpr) v = slot[(warp * SCAN_U + u) * cpr + ci];
-        const __half2* h2 = reinterpret_cast<const __half2*>(&v);
         float f[8];
+        chunk_to_f32(v, f);
 #pragma unroll
-        for (int j = 0; j < 4; j++) {
-          const float2 t = __half22float2(h2[j]);
-          f[2 * j] = t.x; f[2 * j + 1] = t.y;
-        }
-#pragma unroll
-        for (int q = 0; q < NQ; q++) {
-#pragma unroll
-          for (int j = 0; j < 8; j++) acc[u * NQ + q] = fmaf(f[j], qr[q][c][j], acc[u * NQ + q]);
-        }
+        for (int q = 0; q < NQ; q++) fma_chunk(f, qr[q][c], acc[u * NQ + q]);
       }
     }
     // the slot's bytes are in registers: hand it back to the producer before the reduction
@@ -262,35 +210,13 @@ flat_scan_staged_kernel(const uint4* __restrict__ X, int64_t n, int cpr, const f
     if (++s == stages) { s = 0; phase ^= 1; }
 
     warp_transpose_reduce<V>(acc, lane);
-    const float sc = acc[0];
-    const int vi = lane >> SH;
-    const int my_q = vi % NQ;
-    const int64_t my_r = r0 + vi / NQ;
-    unsigned long long wq = worst[0];
-#pragma unroll
-    for (int q = 1; q < NQ; q++) if (my_q == q) wq = worst[q];
-    const unsigned long long key = make_key(sc, (uint32_t)my_r);
-    const bool live = ((lane & ((1 << SH) - 1)) == 0) && my_r < n && my_q < nq_valid && (sc == sc);
-    unsigned pend = __ballot_sync(FULL, live && key > wq);
-    while (pend) {
-      const int src = __ffs(pend) - 1;
-      pend &= pend - 1;
-      const unsigned long long ckey = __shfl_sync(FULL, key, src);
-      const int cq = (src >> SH) % NQ;
-#pragma unroll
-      for (int q = 0; q < NQ; q++)
-        if (cq == q) warp_list_insert(wkeys + q * k, k, ckey, worst[q], worst_pos[q], lane);
-    }
+    offer_block_scores<NQ>(acc[0], r0, n, nq_valid, wkeys, k, worst, worst_pos, lane);
   }
   __syncwarp();
   const int64_t gw = (int64_t)blockIdx.x * TS_CONSUMERS + warp;
 #pragma unroll
-  for (int q = 0; q < NQ; q++) {
-    if (q < nq_valid) {
-      unsigned long long* o = out_keys + (int64_t)q * out_stride_q + gw * k;
-      for (int j = lane; j < k; j += 32) o[j] = wkeys[q * k + j];
-    }
-  }
+  for (int q = 0; q < NQ; q++)
+    if (q < nq_valid) warp_list_store(out_keys + (int64_t)q * out_stride_q + gw * k, wkeys + q * k, k, lane);
 }
 
 // Select the k best of M candidate keys per query: grid (slices, nq); every block streams its
@@ -353,10 +279,34 @@ int index_ws(b200_index* idx, int slot, size_t bytes, void** out) {
   return B200_OK;
 }
 
-static int next_pow2(int x) {
-  int p = 1;
-  while (p < x) p <<= 1;
-  return p;
+int launch_topk_select(const unsigned long long* in, int64_t in_stride_q, int64_t M, int k, int C,
+                       unsigned long long* out, int64_t out_stride_q, int slices, int nq, cudaStream_t st) {
+  const size_t sel_smem = (size_t)C * 8;
+  if (sel_smem > 48 * 1024)
+    B200_CUDA(cudaFuncSetAttribute(topk_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
+  topk_select_kernel<<<dim3(slices, nq), 1024, sel_smem, st>>>(in, in_stride_q, M, k, C, out, out_stride_q);
+  B200_LAUNCH_OK();
+  return B200_OK;
+}
+
+int plan_select(int64_t M, int k, SelectPlan* p) {
+  p->M = M;
+  p->k = k;
+  p->C = select_buffer(k);
+  B200_CHECK((size_t)p->C * 8 <= SELECT_SMEM_MAX, B200_ERR_UNSUPPORTED, "search: k=%d exceeds the supported maximum (8192)", k);
+  // level 1: one sort round per block (a block sorts one C-entry chunk of the candidates) — the select of a single
+  // query is latency, not throughput: dependent sort rounds per block are what it costs
+  p->slices = (int)std::min<int64_t>(256, std::max<int64_t>(1, (M + p->C - 1) / p->C));
+  p->C2 = std::min(p->C, std::max(next_pow2(2 * k), next_pow2(p->slices * k)));   // level 2 buffer: slices * k keys
+  return B200_OK;
+}
+
+int select_topk(const SelectPlan& p, const unsigned long long* cand, unsigned long long* tmp, unsigned long long* out,
+                int nq, cudaStream_t st) {
+  const int64_t M2 = (int64_t)p.slices * p.k;
+  // level 1: slices per query; level 2: one block per query
+  B200_TRY(launch_topk_select(cand, p.M, p.M, p.k, p.C, tmp, M2, p.slices, nq, st));
+  return launch_topk_select(tmp, M2, M2, p.k, p.C2, out, p.k, 1, nq, st);
 }
 
 typedef void (*scan_fn)(const uint4*, int64_t, int, const float*, int, int, unsigned long long*, int64_t);
@@ -412,7 +362,6 @@ struct ScanPlan {
   int nqp;       // queries per pass
   int threads;   // block size
   int grid;
-  int C;         // select buffer entries
   size_t smem;
   scan_fn fn;
   staged_fn sfn = nullptr;  // cp.async.bulk ring variant (preferred when it fits)
@@ -430,8 +379,7 @@ static int plan_scan(const b200_index* idx, int k, int nq, ScanPlan* p) {
   const size_t budget = 96 * 1024;  // keeps two blocks per SM
   while (nqp > 1 && (size_t)(threads / 32) * nqp * k * 8 > budget) nqp >>= 1;
   while (threads > 64 && (size_t)(threads / 32) * nqp * k * 8 > 200 * 1024) threads >>= 1;
-  p->C = std::max(2048, next_pow2(2 * k));
-  if ((size_t)(threads / 32) * nqp * k * 8 > 200 * 1024 || (size_t)p->C * 8 > 200 * 1024) {
+  if ((size_t)(threads / 32) * nqp * k * 8 > 200 * 1024) {
     set_error("search: k=%d exceeds the supported maximum (8192)", k);
     return B200_ERR_UNSUPPORTED;
   }
@@ -472,9 +420,6 @@ static int plan_scan(const b200_index* idx, int k, int nq, ScanPlan* p) {
   return B200_OK;
 }
 
-int scan_topk_keys_mma(b200_index* idx, const __half* rows, int64_t n, const float* d_q, int nq, int k,
-                       unsigned long long* d_keys_out, cudaStream_t st);
-
 int scan_topk_keys(b200_index* idx, const __half* rows, int64_t n, const float* d_q, int nq, int k,
                    unsigned long long* d_keys_out, cudaStream_t st) {
   const int d = idx->d;
@@ -489,31 +434,17 @@ int scan_topk_keys(b200_index* idx, const __half* rows, int64_t n, const float* 
   idx->last_scan_plan[3] = p.stages;
   const int64_t total_warps = (int64_t)p.grid * p.warps_out;
   const int64_t M1 = total_warps * k;
-  // level 1: one sort round per block (a block sorts one C-entry chunk of the candidates) — the select of a single
-  // query is latency, not throughput: dependent sort rounds per block are what it costs
-  int slices = (int)std::min<int64_t>(256, std::max<int64_t>(1, (M1 + p.C - 1) / p.C));
-  const int C2 = std::min(p.C, std::max(next_pow2(2 * k), next_pow2(slices * k)));   // level 2 buffer: slices * k keys
+  SelectPlan sel;
+  B200_TRY(plan_select(M1, k, &sel));
   const int QB = 64;  // queries per batch (bounds the scratch)
-  const size_t keys1 = (size_t)QB * M1, keys2 = (size_t)QB * slices * k;
   void* ws = nullptr;
-  B200_TRY(index_ws(idx, 0, (keys1 + keys2) * 8, &ws));
+  B200_TRY(index_ws(idx, 0, sel.keys(QB) * 8, &ws));
   unsigned long long* k1 = (unsigned long long*)ws;
-  unsigned long long* k2 = k1 + keys1;
-  const size_t sel_smem = (size_t)p.C * 8;
-  if (sel_smem > 48 * 1024)
-    B200_CUDA(cudaFuncSetAttribute(topk_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
+  unsigned long long* k2 = k1 + (size_t)QB * M1;
 
   for (int q0 = 0; q0 < nq; q0 += QB) {
     const int qb = std::min(QB, nq - q0);
-    // time the row-scan kernels of this batch
-    if ((int)idx->ev.size() < idx->ev_used + 2) {
-      cudaEvent_t a, b;
-      B200_CUDA(cudaEventCreate(&a));
-      B200_CUDA(cudaEventCreate(&b));
-      idx->ev.push_back(a);
-      idx->ev.push_back(b);
-    }
-    B200_CUDA(index_record(idx, idx->ev[idx->ev_used], st));
+    B200_TRY(scan_timer_begin(idx, st));   // time the row-scan kernels of this batch
     for (int qq = 0; qq < qb; qq += p.nqp) {
       const int valid = std::min(p.nqp, qb - qq);
       const float* qptr = d_q + (size_t)(q0 + qq) * d;
@@ -525,25 +456,9 @@ int scan_topk_keys(b200_index* idx, const __half* rows, int64_t n, const float* 
       B200_LAUNCH_OK();
       idx->last_scan_launches++;
     }
-    B200_CUDA(index_record(idx, idx->ev[idx->ev_used + 1], st));
-    idx->ev_used += 2;
-    // level 1: slices per query; level 2: one block per query
-    topk_select_kernel<<<dim3(slices, qb), 1024, sel_smem, st>>>(k1, M1, M1, k, p.C, k2, (int64_t)slices * k);
-    B200_LAUNCH_OK();
-    topk_select_kernel<<<dim3(1, qb), 1024, (size_t)C2 * 8, st>>>(k2, (int64_t)slices * k, (int64_t)slices * k, k, C2,
-                                                                 d_keys_out + (size_t)q0 * k, k);
-    B200_LAUNCH_OK();
+    B200_TRY(scan_timer_end(idx, st));
+    B200_TRY(select_topk(sel, k1, k2, d_keys_out + (size_t)q0 * k, qb, st));
   }
-  return B200_OK;
-}
-
-int launch_topk_select(const unsigned long long* in, int64_t in_stride_q, int64_t M, int k, int C,
-                       unsigned long long* out, int64_t out_stride_q, int slices, int nq, cudaStream_t st) {
-  const size_t sel_smem = (size_t)C * 8;
-  if (sel_smem > 48 * 1024)
-    B200_CUDA(cudaFuncSetAttribute(topk_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
-  topk_select_kernel<<<dim3(slices, nq), 1024, sel_smem, st>>>(in, in_stride_q, M, k, C, out, out_stride_q);
-  B200_LAUNCH_OK();
   return B200_OK;
 }
 
@@ -569,19 +484,7 @@ range_scan_kernel(const uint4* __restrict__ X, int64_t n, int cpr, const float* 
                   unsigned long long* __restrict__ out, unsigned int cap, unsigned int* __restrict__ counter) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   float qr[CH][8];
-#pragma unroll
-  for (int c = 0; c < CH; c++) {
-    const int ci = c * 32 + lane;
-    if (ci < cpr) {
-      const float4 a = *reinterpret_cast<const float4*>(Q + ci * 8);
-      const float4 b = *reinterpret_cast<const float4*>(Q + ci * 8 + 4);
-      qr[c][0] = a.x; qr[c][1] = a.y; qr[c][2] = a.z; qr[c][3] = a.w;
-      qr[c][4] = b.x; qr[c][5] = b.y; qr[c][6] = b.z; qr[c][7] = b.w;
-    } else {
-#pragma unroll
-      for (int j = 0; j < 8; j++) qr[c][j] = 0.f;
-    }
-  }
+  load_query_slice<CH>(qr, Q, cpr, lane, true);
   const int64_t gw = (int64_t)blockIdx.x * nwarps + warp, total = (int64_t)gridDim.x * nwarps;
   const int64_t nblk = (n + 3) / 4;
   for (int64_t blk = gw; blk < nblk; blk += total) {
@@ -594,21 +497,12 @@ range_scan_kernel(const uint4* __restrict__ X, int64_t n, int cpr, const float* 
         const int ci = c * 32 + lane;
         uint4 v = make_uint4(0u, 0u, 0u, 0u);
         if (r0 + u < n && ci < cpr) v = ld_nc_v4(X + (r0 + u) * cpr + ci);
-        const __half2* h2 = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-          const float2 t = __half22float2(h2[j]);
-          acc[u] = fmaf(t.x, qr[c][2 * j], acc[u]);
-          acc[u] = fmaf(t.y, qr[c][2 * j + 1], acc[u]);
-        }
+        fma_chunk(v, qr[c], acc[u]);
       }
     }
     warp_transpose_reduce<4>(acc, lane);
     const int64_t my_r = r0 + (lane >> 3);
-    if ((lane & 7) == 0 && my_r < n && acc[0] > thresh) {
-      const unsigned int pos = atomicAdd(counter, 1u);
-      if (pos < cap) out[pos] = make_key(acc[0], (uint32_t)my_r);
-    }
+    if ((lane & 7) == 0 && my_r < n && acc[0] > thresh) range_append(out, cap, counter, acc[0], (uint32_t)my_r);
   }
 }
 

@@ -20,9 +20,6 @@
 
 namespace b200 {
 
-int merge_packed_launch(const void* d_gathered, int G, size_t shard_stride_bytes, int nq, int k, float* d_D, int64_t* d_I,
-                        cudaStream_t st);
-
 struct NcclApi {
   void* lib = nullptr;
   int (*AllGather)(const void*, void*, size_t, int, void*, cudaStream_t) = nullptr;
