@@ -186,12 +186,12 @@ struct SpanGuard {
 static int run_linear(b200_clip* m, const CUtensorMap& tmA, const Linear& l, int M, GemmEpilogue ep, cudaStream_t st,
                       int kind = CLS_GEMM) {
   SpanGuard sg(m, kind, st);
-  int bn = gemm_pick_bn(M, l.N, m->sms);
+  int bn = gemm_pick_bn(M, l.N, m->sms, gemm_epilogue_is_plain(ep));
   // row statistics are written per 64-column slot by ONE thread: the narrow tiles split a slot over two warps
   if (ep.stats_out != nullptr && bn < 128) bn = 128;
   ep.bias = l.b;
   m->last_launches++;
-  const CUtensorMap& tmB = bn == 64 ? l.tm64 : (bn == 32 ? l.tm32 : l.tm128);
+  const CUtensorMap& tmB = bn == 64 ? l.tm64 : (bn == 32 ? l.tm32 : l.tm128);   // 256: two 128-row boxes
   return gemm_bf16_launch(tmA, tmB, bn, M, l.N, l.K, ep, st);
 }
 

@@ -66,8 +66,16 @@ int make_tmap_3d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t pla
   return B200_OK;
 }
 
-int gemm_pick_bn(int M, int N, int sms) {
+// 256-wide persistent tiles once the grid has at least one of them per SM.  Measured on an H100 SXM (700 W,
+// tools/gemm_bench.py): at every measured shape from the ViT-H/14 text tower at batch 64 up (156 tiles and more) the
+// 256-wide kernel is faster than the 128-wide one, from 1.28x (c_proj of ViT-L/14 image and of ViT-H/14 text at batch
+// 64) to 1.8x (ViT-L/14 patch embedding, ViT-H/14 text qkv at batch 64); below one tile per SM (batch 8: 20 .. 80 tiles) the 128-, 64- and 32-wide tiles spread the weight read
+// over more SMs and are mostly as fast or faster.
+constexpr long GEMM_WIDE_MIN_TILES_PER_SM = 1;
+
+int gemm_pick_bn(int M, int N, int sms, bool wide) {
   const long mb = (M + GEMM_BM - 1) / GEMM_BM;
+  if (wide && mb * ((N + GEMM_WIDE_BN - 1) / GEMM_WIDE_BN) >= GEMM_WIDE_MIN_TILES_PER_SM * sms) return GEMM_WIDE_BN;
   const long tiles128 = mb * ((N + 127) / 128);
   if (tiles128 < sms && N >= 64) {
     const long tiles64 = mb * ((N + 63) / 64);
@@ -99,9 +107,7 @@ static int launch_bn_spec(const CUtensorMap& tmA, const CUtensorMap& tmB, int M,
 template <int BN>
 static int launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, const GemmEpilogue& ep,
                      cudaStream_t st, bool generic) {
-  const bool plain = !generic && ep.ln_stats == nullptr && ep.stats_out == nullptr && ep.ln_c == nullptr &&
-                     ep.act >= 0 && ep.act <= 2;
-  if (plain) {
+  if (!generic && gemm_epilogue_is_plain(ep)) {
     switch ((ep.act & 3) | (ep.residual ? 4 : 0)) {
       case 0: return launch_bn_spec<BN, 0>(tmA, tmB, M, N, K, ep, st);
       case 1: return launch_bn_spec<BN, 1>(tmA, tmB, M, N, K, ep, st);
@@ -113,6 +119,43 @@ static int launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int 
     }
   }
   return launch_bn_spec<BN, -1>(tmA, tmB, M, N, K, ep, st);
+}
+
+template <int SPEC>
+static int launch_wide_spec(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, const GemmEpilogue& ep,
+                            cudaStream_t st) {
+  static std::atomic<int> grid_of[64];   // per device: co-resident CTAs (0 until the attributes are set)
+  auto kern = gemm_bf16_wgmma_persistent_kernel<SPEC>;
+  int dev = 0;
+  B200_CUDA(cudaGetDevice(&dev));
+  int grid = grid_of[dev & 63].load();
+  if (grid == 0) {
+    B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmWideCfg::SMEM_BYTES));
+    int per_sm = 0;
+    B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, GEMM_WIDE_THREADS, GemmWideCfg::SMEM_BYTES));
+    B200_CHECK(per_sm >= 1, B200_ERR_CUDA, "gemm: the persistent kernel does not fit on an SM");
+    grid = per_sm * sm_count(dev);
+    grid_of[dev & 63].store(grid);
+  }
+  const long tiles = (long)((M + GEMM_BM - 1) / GEMM_BM) * ((N + GEMM_WIDE_BN - 1) / GEMM_WIDE_BN);
+  kern<<<(unsigned)std::min<long>(tiles, grid), GEMM_WIDE_THREADS, GemmWideCfg::SMEM_BYTES, st>>>(tmA, tmB, M, N, K, ep);
+  B200_LAUNCH_OK();
+  return B200_OK;
+}
+
+static int launch_wide(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, const GemmEpilogue& ep,
+                       cudaStream_t st, bool generic) {
+  B200_CHECK(!generic && gemm_epilogue_is_plain(ep), B200_ERR_INVALID,
+             "gemm: 256-wide tiles take the compile-time epilogue flavours only (no LayerNorm fold, row statistics or "
+             "forced run-time flavour)");
+  switch ((ep.act & 3) | (ep.residual ? 4 : 0)) {
+    case 0: return launch_wide_spec<0>(tmA, tmB, M, N, K, ep, st);
+    case 1: return launch_wide_spec<1>(tmA, tmB, M, N, K, ep, st);
+    case 2: return launch_wide_spec<2>(tmA, tmB, M, N, K, ep, st);
+    case 4: return launch_wide_spec<4>(tmA, tmB, M, N, K, ep, st);
+    case 5: return launch_wide_spec<5>(tmA, tmB, M, N, K, ep, st);
+    default: return launch_wide_spec<6>(tmA, tmB, M, N, K, ep, st);
+  }
 }
 
 int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int M, int N, int K,
@@ -128,6 +171,7 @@ int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int
   B200_CHECK(ep.ln_stats == nullptr || (ep.ln_c != nullptr && ep.ln_w > 0 && ep.ln_w % 64 == 0), B200_ERR_INVALID,
              "gemm: folded LayerNorm needs c and a row width that is a multiple of 64 (ln_w=%d)", ep.ln_w);
   B200_CHECK(ep.ln_stats == nullptr || ep.ln_w <= 64 * LN_MAX_SLOTS, B200_ERR_UNSUPPORTED, "gemm: folded LayerNorm supports rows of at most %d columns", 64 * LN_MAX_SLOTS);
+  if (bn == GEMM_WIDE_BN) return launch_wide(tmA, tmB, M, N, K, ep, st, generic);
   if (bn == 128) return launch_bn<128>(tmA, tmB, M, N, K, ep, st, generic);
   if (bn == 64) return launch_bn<64>(tmA, tmB, M, N, K, ep, st, generic);
   if (bn == 32) return launch_bn<32>(tmA, tmB, M, N, K, ep, st, generic);
@@ -140,20 +184,21 @@ int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int
 using namespace b200;
 
 // The stand-alone entries: A [M, K] and W [N, K] contiguous, everything else as the epilogue says.  bn = 0 takes
-// gemm_pick_bn's width (raised to 128 when row statistics are written, as the model does).
+// gemm_pick_bn's width (256 only for the compile-time flavours; raised to 128 when row statistics are written, as the
+// model does).
 static int gemm_entry(const void* d_A, const void* d_W, int M, int N, int K, GemmEpilogue ep, int bn, bool generic,
                       int device, void* stream) {
   B200_CHECK(d_A && d_W && ep.out, B200_ERR_INVALID, "gemm: null operand");
   B200_CHECK(ep.act >= 0 && ep.act <= 2, B200_ERR_INVALID, "gemm: act=%d", ep.act);
-  B200_CHECK(bn == 0 || bn == 32 || bn == 64 || bn == 128, B200_ERR_INVALID, "gemm: unsupported column block %d", bn);
+  B200_CHECK(bn == 0 || bn == 32 || bn == 64 || bn == 128 || bn == GEMM_WIDE_BN, B200_ERR_INVALID, "gemm: unsupported column block %d", bn);
   DeviceGuard g(device);
   if (bn == 0) {
-    bn = gemm_pick_bn(M, N, sm_count(device));
+    bn = gemm_pick_bn(M, N, sm_count(device), !generic && gemm_epilogue_is_plain(ep));
     if (ep.stats_out != nullptr && bn < 128) bn = 128;
   }
   CUtensorMap tmA, tmB;
   B200_TRY(make_tmap_2d(&tmA, d_A, 1, (uint64_t)M, (uint64_t)K, (uint64_t)K, GEMM_BM, GEMM_BK));
-  B200_TRY(make_tmap_2d(&tmB, d_W, 1, (uint64_t)N, (uint64_t)K, (uint64_t)K, (uint32_t)bn, GEMM_BK));
+  B200_TRY(make_tmap_2d(&tmB, d_W, 1, (uint64_t)N, (uint64_t)K, (uint64_t)K, (uint32_t)std::min(bn, 128), GEMM_BK));
   return gemm_bf16_launch(tmA, tmB, bn, M, N, K, ep, (cudaStream_t)stream, generic);
 }
 

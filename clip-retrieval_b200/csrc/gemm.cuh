@@ -341,17 +341,208 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   }
 }
 
+// ---- persistent 128 x 256 tiles for the large-batch shapes ----------------------------------------------------
+// One CTA per SM (384 threads) loops over the tiles blockIdx.x, blockIdx.x + gridDim.x, ... in gemm_tile_coords' order:
+//   warpgroup 0     TMA producer (one issuing thread; its registers go to the consumers): a 128x64 A box and two
+//                   128x64 W boxes per k-block into a 4-stage ring of 48 KB stages.  It runs on into the next tile's
+//                   k-blocks while the consumers are in the epilogue of this one: with one CTA per SM, that is what
+//                   takes the place of the second CTA the 128-wide kernel overlaps its epilogue with.
+//   warpgroups 1-2  consumers, each issuing wgmma m64n256k16 over its 64 rows of the tile (128 fp32 accumulators per
+//                   thread).  Per 64-deep k-block a CTA loads 48 KB for 1024 tensor-pipe clocks of math, against 32 KB
+//                   for 512 at 128 x 128: a third less L2 -> SM traffic per flop.
+// The epilogue runs from the accumulators: each warp passes its 16 x 256 slab through a private 16 x 32 fp32 staging
+// chunk so that its stores run along rows (8 rows x 64 contiguous bytes per warp instruction).  The chunks take 20 KB
+// and leave room for 4 ring stages; a 64 KB bf16 staging tile for coalesced / TMA stores would leave room for 3 (that
+// variant has not been built and measured).  The per-element arithmetic is epi_store8's, so
+// every element is stored with the same bits as by the 128-wide kernel (the same k16 wgmma sequence feeds it).
+// Only the compile-time epilogue flavours (SPEC 0..7); the LayerNorm fold and row statistics stay on the kernel above.
+// A variant with CTA pairs (clusters of 2 along M) multicasting one 128-row W half each was built and measured slower
+// at every bench shape (DESIGN.md §8), so W is loaded per CTA.
+constexpr int GEMM_WIDE_BN = 256;
+constexpr int GEMM_WIDE_THREADS = 384;
+struct GemmWideCfg {
+  static constexpr int STAGES = 4;
+  static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;        // 16 KB
+  static constexpr int B_BYTES = GEMM_WIDE_BN * GEMM_BK * 2;   // 32 KB: two 128-row W boxes
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
+  static constexpr int STG_LD = 40;                            // staging pitch (floats): conflict-free float2 writes and
+                                                               // (with the odd-row order below) float4 reads
+  static constexpr int STG_BYTES = 8 * 16 * STG_LD * 4;        // 8 consumer warps x 16 rows x 32 columns
+  static constexpr int SMEM_BYTES = RING_BYTES + STG_BYTES + 2 * GEMM_WIDE_BN * 4 + 256 + 1024;  // + 2 bias rows, barriers, align
+};
+static_assert(GemmWideCfg::SMEM_BYTES <= 227 * 1024, "the persistent GEMM's shared memory exceeds an SM's");
+
+template <int SPEC>
+__global__ void __launch_bounds__(GEMM_WIDE_THREADS, 1)
+gemm_bf16_wgmma_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M,
+                                  int N, int K, GemmEpilogue ep) {
+  static_assert(SPEC >= 0 && SPEC < 8, "compile-time epilogue flavours only");
+  using Cfg = GemmWideCfg;
+  constexpr int STAGES = Cfg::STAGES;
+  constexpr int BN = GEMM_WIDE_BN;
+  constexpr bool HAS_RES = ((SPEC >> 2) & 1) != 0;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw_addr = ptx::smem_u32(smem_raw);
+  uint8_t* base = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
+  uint8_t* sA = base;
+  uint8_t* sB = base + STAGES * Cfg::A_BYTES;
+  float* s_stg = reinterpret_cast<float*>(base + Cfg::RING_BYTES);
+  float* s_bias = s_stg + Cfg::STG_BYTES / 4;   // [2][BN]: alternate tiles, so one tile's epilogue never races the next fill
+  uint64_t* full = reinterpret_cast<uint64_t*>(s_bias + 2 * BN);
+  uint64_t* empty = full + STAGES;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int mb = (M + GEMM_BM - 1) / GEMM_BM, nb = (N + BN - 1) / BN, kb = (K + GEMM_BK - 1) / GEMM_BK;
+  const int tiles = mb * nb;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; s++) {
+      ptx::mbar_init(&full[s], 1);
+      ptx::mbar_init(&empty[s], 8);  // one arrive per consumer warp
+    }
+    ptx::fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    // ---------------- TMA producer ----------------
+    ptx::setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      ptx::prefetch_tensormap(&tmA);
+      ptx::prefetch_tensormap(&tmB);
+      int it = 0;   // k-blocks issued by this CTA over all its tiles: the ring position
+      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        int m_blk, n_blk;
+        gemm_tile_coords(tile, mb, nb, m_blk, n_blk);
+        for (int kbi = 0; kbi < kb; kbi++, it++) {
+          const int stage = it % STAGES;
+          if (it >= STAGES) ptx::mbar_wait(&empty[stage], ((it / STAGES) - 1) & 1);
+          ptx::mbar_arrive_expect_tx(&full[stage], Cfg::STAGE_BYTES);
+          uint8_t* b = sB + stage * Cfg::B_BYTES;
+          ptx::tma_load_2d(sA + stage * Cfg::A_BYTES, &tmA, &full[stage], kbi * GEMM_BK, m_blk * GEMM_BM);
+          ptx::tma_load_2d(b, &tmB, &full[stage], kbi * GEMM_BK, n_blk * BN);
+          ptx::tma_load_2d(b + Cfg::B_BYTES / 2, &tmB, &full[stage], kbi * GEMM_BK, n_blk * BN + 128);
+        }
+      }
+    }
+    return;
+  }
+
+  // ---------------- consumers (warps 4..11) ----------------
+  ptx::setmaxnreg_inc<232>();
+  const int cw = warp - 4;                  // consumer warp 0..7
+  const int wg = cw >> 2;                   // rows wg*64 .. wg*64+63 of the tile
+  const int ct = threadIdx.x - 128;         // 0..255
+  const int fr = lane >> 2, fc = lane & 3;  // accumulator fragment: rows fr, fr + 8 of the warp's 16; columns 8 j + 2 fc
+  float* stg = s_stg + cw * 16 * Cfg::STG_LD;
+  float acc[BN / 2];
+  int it = 0;
+  for (int tile = blockIdx.x, local = 0; tile < tiles; tile += gridDim.x, local++) {
+    int m_blk, n_blk;
+    gemm_tile_coords(tile, mb, nb, m_blk, n_blk);
+    const int n0 = n_blk * BN;
+    float* bias_t = s_bias + (local & 1) * BN;
+    bias_t[ct] = (ep.bias != nullptr && n0 + ct < N) ? ep.bias[n0 + ct] : 0.0f;
+    if (HAS_RES) {
+      // the residual rows of the tile are brought to L2 while the k-loop runs (two 128-byte lines per thread)
+      const int row = m_blk * GEMM_BM + (ct >> 1);
+      const int col = (ct & 1) * 128;
+      if (row < M) {
+        const EpiRow er = epi_row(ep, row, n0);
+        if (n0 + col < N) ptx::prefetch_l2(er.res_ptr + col);
+        if (n0 + col + 64 < N) ptx::prefetch_l2(er.res_ptr + col + 64);
+      }
+    }
+    ptx::named_barrier_sync(1, 256);   // bias_t is filled
+
+    for (int kbi = 0; kbi < kb; kbi++, it++) {
+      const int stage = it % STAGES;
+      ptx::mbar_wait(&full[stage], (it / STAGES) & 1);
+      ptx::wgmma_fence();
+      const uint64_t da = ptx::wgmma_desc_k_sw128(ptx::smem_u32(sA + stage * Cfg::A_BYTES + wg * 64 * 128));
+      const uint64_t db = ptx::wgmma_desc_k_sw128(ptx::smem_u32(sB + stage * Cfg::B_BYTES));
+#pragma unroll
+      for (int k = 0; k < GEMM_BK / GEMM_MMA_K; k++)
+        ptx::wgmma_bf16<BN>(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kbi | k) != 0 ? 1u : 0u);
+      ptx::wgmma_commit();
+      // the group of the previous k-block has completed: its ring slot may be refilled
+      ptx::wgmma_wait<1>();
+      if (kbi > 0 && lane == 0) ptx::mbar_arrive(&empty[(it - 1) % STAGES]);
+    }
+    ptx::wgmma_wait<0>();
+    ptx::fence_regs(acc);
+    if (lane == 0) ptx::mbar_arrive(&empty[(it - 1) % STAGES]);
+
+    // ---------------- epilogue: 8 chunks of 32 columns ----------------
+    // after the staging round trip, lane (fr, fc) holds columns 8 fc .. 8 fc + 7 of the chunk for rows fr and fr + 8
+    const int row0 = m_blk * GEMM_BM + wg * 64 + (cw & 3) * 16 + fr;
+    bool ok[2];
+    EpiRow er[2];
+#pragma unroll
+    for (int q = 0; q < 2; q++) {
+      ok[q] = row0 + 8 * q < M;
+      er[q] = epi_row(ep, ok[q] ? row0 + 8 * q : 0, n0);
+    }
+    uint4 res[2][2];   // [chunk parity][q]: the next chunk's residual is loaded while this one is stored
+    auto load_res = [&](int c, uint4 (&r)[2]) {
+#pragma unroll
+      for (int q = 0; q < 2; q++) {
+        const int col = c * 32 + fc * 8;
+        r[q] = (HAS_RES && ok[q] && n0 + col < N) ? *reinterpret_cast<const uint4*>(er[q].res_ptr + col)
+                                                   : make_uint4(0u, 0u, 0u, 0u);
+      }
+    };
+    load_res(0, res[0]);
+#pragma unroll
+    for (int c = 0; c < BN / 32; c++) {
+      if (c + 1 < BN / 32) load_res(c + 1, res[(c + 1) & 1]);
+      __syncwarp();
+#pragma unroll
+      for (int jj = 0; jj < 4; jj++) {
+        const int j = 4 * c + jj;
+        *reinterpret_cast<float2*>(stg + fr * Cfg::STG_LD + 8 * jj + 2 * fc) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(stg + (fr + 8) * Cfg::STG_LD + 8 * jj + 2 * fc) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      }
+      __syncwarp();
+#pragma unroll
+      for (int q = 0; q < 2; q++) {
+        const int col = c * 32 + fc * 8;
+        if (ok[q] && n0 + col < N) {
+          // odd rows read their two halves in the other order: rows fr and fr + 1 (40 floats apart) then hit
+          // disjoint banks within a quarter-warp
+          const float* src = stg + (fr + 8 * q) * Cfg::STG_LD + fc * 8;
+          const int sw = (fr & 1) * 4;
+          const float4 h0 = *reinterpret_cast<const float4*>(src + sw);
+          const float4 h1 = *reinterpret_cast<const float4*>(src + (4 - sw));
+          const float4 u = sw ? h1 : h0, v = sw ? h0 : h1;
+          const uint32_t r8[8] = {__float_as_uint(u.x), __float_as_uint(u.y), __float_as_uint(u.z), __float_as_uint(u.w),
+                                  __float_as_uint(v.x), __float_as_uint(v.y), __float_as_uint(v.z), __float_as_uint(v.w)};
+          float st_s = 0.f, st_q = 0.f;
+          epi_store8<SPEC>(ep, er[q], r8, bias_t, nullptr, col, n0, res[c & 1][q], 0.f, st_s, st_q);
+        }
+      }
+    }
+  }
+}
+
 // host side (gemm.cu)
 int make_tmap_2d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t rows, uint64_t cols, uint64_t ld_elems,
                  uint32_t box_rows, uint32_t box_cols);
 int make_tmap_3d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t planes, uint64_t rows, uint64_t cols,
                  uint64_t ld_row, uint64_t ld_plane, uint32_t box_rows, uint32_t box_cols);
-// tmB must have boxes of bn rows x 64 columns.  generic = true launches the run-time epilogue flavour (SPEC = -1)
-// even where a compile-time flavour applies (the tests check that both store the same bits).
+// tmB must have boxes of bn rows x 64 columns (128 rows for bn = 256).  generic = true launches the run-time epilogue
+// flavour (SPEC = -1) even where a compile-time flavour applies (the tests check that both store the same bits).
+// bn = 256 (the persistent kernel) takes the compile-time flavours only: B200_ERR_INVALID for generic, ln_stats or
+// stats_out.
 int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int M, int N, int K,
                      const GemmEpilogue& ep, cudaStream_t st, bool generic = false);
-// Pick the column-block width for a GEMM with N output columns (128, or 64 / 32 when the grid would be
-// under-filled).
-int gemm_pick_bn(int M, int N, int sms);
+// true when a compile-time epilogue flavour covers `ep` (no LayerNorm fold, no row statistics)
+inline bool gemm_epilogue_is_plain(const GemmEpilogue& ep) {
+  return ep.ln_stats == nullptr && ep.stats_out == nullptr && ep.ln_c == nullptr && ep.act >= 0 && ep.act <= 2;
+}
+// Pick the column-block width for a GEMM with N output columns: 256 (persistent kernel) for large grids when `wide`
+// (the epilogue is plain), else 128, or 64 / 32 when the grid would be under-filled.
+int gemm_pick_bn(int M, int N, int sms, bool wide);
 
 }  // namespace b200

@@ -277,7 +277,9 @@ int b200_gemm_bf16_device(const void* d_A, const void* d_W, const float* d_bias,
  * result is rstd * (x W'^T - mean * ln_c) + d, with mean / rstd (eps 1e-5) combined from ln_w / 64 (mean, M2)
  * float2 records per row.  stats_out != NULL: one (mean, M2) float2 record per 64 stored columns of every row
  * (needs N % 64 == 0 and 128-wide column blocks).
- * bn: 0 = the width the library picks (128 whenever stats_out is set), else 32, 64 or 128.
+ * bn: 0 = the width the library picks (128 whenever stats_out is set), else 32, 64, 128 or 256.  256 is the
+ * persistent 128 x 256 kernel of the large-batch shapes: it takes the compile-time epilogue flavours only, and is
+ * refused (B200_ERR_INVALID) with force_generic, stats_out or ln_stats.
  * force_generic != 0: the epilogue flavour that decides every feature at run time, even where a compile-time
  * flavour exists; both store the same bits. */
 typedef struct b200_gemm_epilogue {
