@@ -121,45 +121,71 @@ static int launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int 
   return launch_bn_spec<BN, -1>(tmA, tmB, M, N, K, ep, st);
 }
 
-template <int SPEC>
-static int launch_wide_spec(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, const GemmEpilogue& ep,
-                            cudaStream_t st) {
+template <int SPEC, class Cfg>
+static int launch_wide_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
+                           const CUtensorMap& tmR, int M, int N, int K, const GemmEpilogue& ep, cudaStream_t st) {
   static std::atomic<int> grid_of[64];   // per device: co-resident CTAs (0 until the attributes are set)
-  auto kern = gemm_bf16_wgmma_persistent_kernel<SPEC>;
+  auto kern = gemm_bf16_wgmma_persistent_kernel<SPEC, Cfg>;
   int dev = 0;
   B200_CUDA(cudaGetDevice(&dev));
   int grid = grid_of[dev & 63].load();
   if (grid == 0) {
-    B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmWideCfg::SMEM_BYTES));
+    B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     int per_sm = 0;
-    B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, GEMM_WIDE_THREADS, GemmWideCfg::SMEM_BYTES));
+    B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, GEMM_WIDE_THREADS, Cfg::SMEM_BYTES));
     B200_CHECK(per_sm >= 1, B200_ERR_CUDA, "gemm: the persistent kernel does not fit on an SM");
     grid = per_sm * sm_count(dev);
     grid_of[dev & 63].store(grid);
   }
   const long tiles = (long)((M + GEMM_BM - 1) / GEMM_BM) * ((N + GEMM_WIDE_BN - 1) / GEMM_WIDE_BN);
-  kern<<<(unsigned)std::min<long>(tiles, grid), GEMM_WIDE_THREADS, GemmWideCfg::SMEM_BYTES, st>>>(tmA, tmB, M, N, K, ep);
+  kern<<<(unsigned)std::min<long>(tiles, grid), GEMM_WIDE_THREADS, Cfg::SMEM_BYTES, st>>>(tmA, tmB, tmC, tmR, M, N, K,
+                                                                                        ep);
   B200_LAUNCH_OK();
   return B200_OK;
 }
 
+// The TMA-store epilogue (3-stage ring) where every CTA has at least this many tiles; fewer tiles, and the row maps,
+// take the register-store epilogue (4-stage ring).  Measured on an H100 SXM (700 W): the TMA stores won at every
+// ViT-L/14 batch-1024 layer GEMM (14 tiles per CTA and more), but at the ViT-H/14 text tower at batch 64 (1.2 - 4.7 tiles
+// per CTA) `bench.py --workload e2e` was about 2 % slower with them (DESIGN.md §8).
+constexpr long GEMM_WIDE_TMA_MIN_TILES_PER_CTA = 8;
+
+// The TMA-store epilogue takes output (and residual) tensor maps of [M, N] with their own leading dimensions, so the
+// stores are clipped at M and N; one encode per map per launch.  force_tma: whatever the grid (tests).
+template <int SPEC>
+static int launch_wide_spec(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, const GemmEpilogue& ep,
+                            cudaStream_t st, bool force_tma) {
+  CUtensorMap tmC{}, tmR{};
+  int dev = 0;
+  B200_CUDA(cudaGetDevice(&dev));
+  const long tiles = (long)((M + GEMM_BM - 1) / GEMM_BM) * ((N + GEMM_WIDE_BN - 1) / GEMM_WIDE_BN);
+  const bool row_map = ep.out_group > 0 || ep.res_row_mod > 0;
+  if (row_map || (!force_tma && tiles < GEMM_WIDE_TMA_MIN_TILES_PER_CTA * sm_count(dev)))
+    return launch_wide_cfg<SPEC, GemmWideRegCfg>(tmA, tmB, tmC, tmR, M, N, K, ep, st);
+  B200_TRY(make_tmap_2d(&tmC, ep.out, 1, (uint64_t)M, (uint64_t)N, (uint64_t)ep.out_ld, GEMM_WIDE_BOX, GEMM_WIDE_BOX));
+  if (ep.residual != nullptr)
+    B200_TRY(make_tmap_2d(&tmR, ep.residual, 1, (uint64_t)M, (uint64_t)N, (uint64_t)ep.res_ld, GEMM_WIDE_BOX,
+                          GEMM_WIDE_BOX));
+  return launch_wide_cfg<SPEC, GemmWideTmaCfg>(tmA, tmB, tmC, tmR, M, N, K, ep, st);
+}
+
 static int launch_wide(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, const GemmEpilogue& ep,
-                       cudaStream_t st, bool generic) {
+                       cudaStream_t st, bool generic, bool force_tma) {
   B200_CHECK(!generic && gemm_epilogue_is_plain(ep), B200_ERR_INVALID,
              "gemm: 256-wide tiles take the compile-time epilogue flavours only (no LayerNorm fold, row statistics or "
              "forced run-time flavour)");
   switch ((ep.act & 3) | (ep.residual ? 4 : 0)) {
-    case 0: return launch_wide_spec<0>(tmA, tmB, M, N, K, ep, st);
-    case 1: return launch_wide_spec<1>(tmA, tmB, M, N, K, ep, st);
-    case 2: return launch_wide_spec<2>(tmA, tmB, M, N, K, ep, st);
-    case 4: return launch_wide_spec<4>(tmA, tmB, M, N, K, ep, st);
-    case 5: return launch_wide_spec<5>(tmA, tmB, M, N, K, ep, st);
-    default: return launch_wide_spec<6>(tmA, tmB, M, N, K, ep, st);
+    case 0: return launch_wide_spec<0>(tmA, tmB, M, N, K, ep, st, force_tma);
+    case 1: return launch_wide_spec<1>(tmA, tmB, M, N, K, ep, st, force_tma);
+    case 2: return launch_wide_spec<2>(tmA, tmB, M, N, K, ep, st, force_tma);
+    case 4: return launch_wide_spec<4>(tmA, tmB, M, N, K, ep, st, force_tma);
+    case 5: return launch_wide_spec<5>(tmA, tmB, M, N, K, ep, st, force_tma);
+    default: return launch_wide_spec<6>(tmA, tmB, M, N, K, ep, st, force_tma);
   }
 }
 
 int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int M, int N, int K,
-                     const GemmEpilogue& ep, cudaStream_t st, bool generic) {
+                     const GemmEpilogue& ep, cudaStream_t st, bool generic, bool force_tma_epilogue) {
   B200_CHECK(M >= 1 && N >= 8 && K >= 8 && N % 8 == 0 && K % 8 == 0, B200_ERR_INVALID,
              "gemm: need M>=1 and N, K multiples of 8 (M=%d N=%d K=%d)", M, N, K);
   B200_CHECK(ep.out != nullptr && ep.out_ld % 8 == 0 && ((uintptr_t)ep.out & 15) == 0, B200_ERR_INVALID,
@@ -171,7 +197,7 @@ int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int
   B200_CHECK(ep.ln_stats == nullptr || (ep.ln_c != nullptr && ep.ln_w > 0 && ep.ln_w % 64 == 0), B200_ERR_INVALID,
              "gemm: folded LayerNorm needs c and a row width that is a multiple of 64 (ln_w=%d)", ep.ln_w);
   B200_CHECK(ep.ln_stats == nullptr || ep.ln_w <= 64 * LN_MAX_SLOTS, B200_ERR_UNSUPPORTED, "gemm: folded LayerNorm supports rows of at most %d columns", 64 * LN_MAX_SLOTS);
-  if (bn == GEMM_WIDE_BN) return launch_wide(tmA, tmB, M, N, K, ep, st, generic);
+  if (bn == GEMM_WIDE_BN) return launch_wide(tmA, tmB, M, N, K, ep, st, generic, force_tma_epilogue);
   if (bn == 128) return launch_bn<128>(tmA, tmB, M, N, K, ep, st, generic);
   if (bn == 64) return launch_bn<64>(tmA, tmB, M, N, K, ep, st, generic);
   if (bn == 32) return launch_bn<32>(tmA, tmB, M, N, K, ep, st, generic);
@@ -187,7 +213,7 @@ using namespace b200;
 // gemm_pick_bn's width (256 only for the compile-time flavours; raised to 128 when row statistics are written, as the
 // model does).
 static int gemm_entry(const void* d_A, const void* d_W, int M, int N, int K, GemmEpilogue ep, int bn, bool generic,
-                      int device, void* stream) {
+                      int device, void* stream, bool force_tma_epilogue = false) {
   B200_CHECK(d_A && d_W && ep.out, B200_ERR_INVALID, "gemm: null operand");
   B200_CHECK(ep.act >= 0 && ep.act <= 2, B200_ERR_INVALID, "gemm: act=%d", ep.act);
   B200_CHECK(bn == 0 || bn == 32 || bn == 64 || bn == 128 || bn == GEMM_WIDE_BN, B200_ERR_INVALID, "gemm: unsupported column block %d", bn);
@@ -199,7 +225,7 @@ static int gemm_entry(const void* d_A, const void* d_W, int M, int N, int K, Gem
   CUtensorMap tmA, tmB;
   B200_TRY(make_tmap_2d(&tmA, d_A, 1, (uint64_t)M, (uint64_t)K, (uint64_t)K, GEMM_BM, GEMM_BK));
   B200_TRY(make_tmap_2d(&tmB, d_W, 1, (uint64_t)N, (uint64_t)K, (uint64_t)K, (uint32_t)std::min(bn, 128), GEMM_BK));
-  return gemm_bf16_launch(tmA, tmB, bn, M, N, K, ep, (cudaStream_t)stream, generic);
+  return gemm_bf16_launch(tmA, tmB, bn, M, N, K, ep, (cudaStream_t)stream, generic, force_tma_epilogue);
 }
 
 extern "C" int b200_gemm_bf16_device(const void* d_A, const void* d_W, const float* d_bias, const void* d_residual,
@@ -231,5 +257,6 @@ extern "C" int b200_gemm_bf16_ex_device(const void* d_A, const void* d_W, void* 
   ep.ln_c = e->ln_c;
   ep.ln_w = e->ln_w;
   ep.stats_out = (float2*)e->stats_out;
-  return gemm_entry(d_A, d_W, M, N, K, ep, bn, force_generic != 0, device, stream);
+  // bit 1: the persistent kernel's TMA-store epilogue whatever the grid size (the tests reach it at small shapes)
+  return gemm_entry(d_A, d_W, M, N, K, ep, bn, (force_generic & ~2) != 0, device, stream, (force_generic & 2) != 0);
 }

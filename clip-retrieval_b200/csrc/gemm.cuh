@@ -138,6 +138,15 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
   return __bfloat1622float2(v);
 }
 
+// act(pre) + residual, pre = accumulator + bias (or the folded LayerNorm's value): the per-element arithmetic of every
+// epilogue, rounded to bf16 by the caller (pack_bf16x2).  __fadd_rn: never contracted with the activation's last
+// multiply into an FMA — every epilogue flavour (run-time or compile-time, either kernel) rounds the same way and stays
+// bit-identical to the others.
+__device__ __forceinline__ float epi_apply(float pre, int act, bool has_res, float res) {
+  const float v = act_apply(pre, act);
+  return has_res ? __fadd_rn(v, res) : v;
+}
+
 // bias + activation + residual + bf16 store of 8 consecutive columns (col = offset inside the tile)
 // `rr` = the residual's 8 values, loaded before the accumulator is read so that their HBM latency does not sit in
 // the middle of the epilogue.
@@ -154,21 +163,14 @@ __device__ __forceinline__ void epi_store8(const GemmEpilogue& ep, const EpiRow&
   const bool use_ln = SPEC < 0 && ep.ln_stats != nullptr;
   const bool use_stats = SPEC < 0 && ep.stats_out != nullptr;
   const bool has_res = SPEC >= 0 ? ((SPEC >> 2) & 1) != 0 : er.res_ptr != nullptr;
+  const float2 a = unpack_bf16x2(rr.x), b = unpack_bf16x2(rr.y), cc = unpack_bf16x2(rr.z), dd = unpack_bf16x2(rr.w);
+  const float res[8] = {a.x, a.y, b.x, b.y, cc.x, cc.y, dd.x, dd.y};
   float v[8];
-  if (use_ln) {
 #pragma unroll
-    for (int j = 0; j < 8; j++)
-      v[j] = act_apply(fmaf(__uint_as_float(r8[j]), er.ln_a, fmaf(er.ln_b, s_c[col + j], s_bias[col + j])), act);
-  } else {
-#pragma unroll
-    for (int j = 0; j < 8; j++) v[j] = act_apply(__uint_as_float(r8[j]) + s_bias[col + j], act);
-  }
-  if (has_res) {
-    const float2 a = unpack_bf16x2(rr.x), b = unpack_bf16x2(rr.y), cc = unpack_bf16x2(rr.z), dd = unpack_bf16x2(rr.w);
-    // __fadd_rn: never contracted with the activation's last multiply into an FMA — every epilogue flavour (run-time or
-    // compile-time) rounds the same way and stays bit-identical to the others
-    v[0] = __fadd_rn(v[0], a.x); v[1] = __fadd_rn(v[1], a.y); v[2] = __fadd_rn(v[2], b.x); v[3] = __fadd_rn(v[3], b.y);
-    v[4] = __fadd_rn(v[4], cc.x); v[5] = __fadd_rn(v[5], cc.y); v[6] = __fadd_rn(v[6], dd.x); v[7] = __fadd_rn(v[7], dd.y);
+  for (int j = 0; j < 8; j++) {
+    const float pre = use_ln ? fmaf(__uint_as_float(r8[j]), er.ln_a, fmaf(er.ln_b, s_c[col + j], s_bias[col + j]))
+                             : __uint_as_float(r8[j]) + s_bias[col + j];
+    v[j] = epi_apply(pre, act, has_res, res[j]);
   }
   uint4 o;
   o.x = pack_bf16x2(v[0], v[1]);
@@ -343,54 +345,87 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 
 // ---- persistent 128 x 256 tiles for the large-batch shapes ----------------------------------------------------
 // One CTA per SM (384 threads) loops over the tiles blockIdx.x, blockIdx.x + gridDim.x, ... in gemm_tile_coords' order:
-//   warpgroup 0     TMA producer (one issuing thread; its registers go to the consumers): a 128x64 A box and two
-//                   128x64 W boxes per k-block into a 4-stage ring of 48 KB stages.  It runs on into the next tile's
-//                   k-blocks while the consumers are in the epilogue of this one: with one CTA per SM, that is what
-//                   takes the place of the second CTA the 128-wide kernel overlaps its epilogue with.
+//   warpgroup 0     thread 0, the k-block producer (its registers go to the consumers): a 128x64 A box and two
+//                   128x64 W boxes per k-block into a ring of 48 KB stages.  It runs on into the next tile's k-blocks
+//                   while the consumers are in the epilogue of this one.
+//                   thread 32, the staging thread (TMA-store epilogue): loads the residual boxes of a tile into the
+//                   bf16 staging tile while the consumers are still in its k-loop, stores the finished tile by TMA, and
+//                   hands the staging tile back once those stores have read it.
 //   warpgroups 1-2  consumers, each issuing wgmma m64n256k16 over its 64 rows of the tile (128 fp32 accumulators per
 //                   thread).  Per 64-deep k-block a CTA loads 48 KB for 1024 tensor-pipe clocks of math, against 32 KB
 //                   for 512 at 128 x 128: a third less L2 -> SM traffic per flop.
-// The epilogue runs from the accumulators: each warp passes its 16 x 256 slab through a private 16 x 32 fp32 staging
-// chunk so that its stores run along rows (8 rows x 64 contiguous bytes per warp instruction).  The chunks take 20 KB
-// and leave room for 4 ring stages; a 64 KB bf16 staging tile for coalesced / TMA stores would leave room for 3 (that
-// variant has not been built and measured).  The per-element arithmetic is epi_store8's, so
-// every element is stored with the same bits as by the 128-wide kernel (the same k16 wgmma sequence feeds it).
+// Epilogue (TMA store, every GEMM without a row map): each consumer converts its accumulators in fragment layout,
+// act(acc + bias) + residual (epi_apply), and writes bf16 pairs into its warpgroup's half of the staging tile, four
+// 64 x 64 boxes in the 128B-swizzled layout of the output tensor map (the residual, loaded there by TMA, is read from
+// and overwritten in place).  Then fence.proxy.async, one arrive per thread on the warpgroup's stg_full barrier, and
+// straight on into the next tile's k-loop: the staging thread issues the TMA stores, which drain behind that k-loop, and
+// the consumers wait for the staging tile (stg_ready) only at their next epilogue.  The premise: every CTA reaches
+// its epilogues at about the same moment, so stores from registers stall all SMs at once behind a burst of 8.6 MB
+// (17 MB with the residual read).  Measured (tools/gemm_bench.py --ksweep, DESIGN.md §8): the fixed cost per tile fell
+// by half or more for the plain and GELU epilogues, and less with a residual; the rest is the consumers' conversion work.
+// The TMA-store epilogue is taken from 8 tiles per CTA up (gemm.cu): below that its 3-stage ring costs more than the
+// overlap saves.
+// Row maps (out_group / res_row_mod: the patch embedding, one GEMM per image tower) and small grids keep a
+// register-store epilogue with a 4-stage ring:
+// each warp passes its 16 x 256 slab through a private 16 x 32 fp32 staging chunk so that its stores run along rows.
+// Both epilogues compute every element with epi_apply, so outputs are bit-identical to the 128-wide kernel's (the
+// same k16 wgmma sequence feeds it).
 // Only the compile-time epilogue flavours (SPEC 0..7); the LayerNorm fold and row statistics stay on the kernel above.
 // A variant with CTA pairs (clusters of 2 along M) multicasting one 128-row W half each was built and measured slower
 // at every bench shape (DESIGN.md §8), so W is loaded per CTA.
 constexpr int GEMM_WIDE_BN = 256;
 constexpr int GEMM_WIDE_THREADS = 384;
+constexpr int GEMM_WIDE_BOX = 64;   // rows and columns of a TMA box of the output / residual maps (128 bytes per row)
+// STAGES_: ring depth.  STG_BOXES_: 64-column boxes of each warpgroup's 64 rows in the bf16 staging tile (4: the whole
+// 128 x 256 tile; 2: half of it, staged and stored in two passes per tile), or 0 for the register-store epilogue.
+template <int STAGES_, int STG_BOXES_>
 struct GemmWideCfg {
-  static constexpr int STAGES = 4;
+  static constexpr int STAGES = STAGES_;
+  static constexpr int STG_BOXES = STG_BOXES_;
   static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;        // 16 KB
   static constexpr int B_BYTES = GEMM_WIDE_BN * GEMM_BK * 2;   // 32 KB: two 128-row W boxes
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
-  static constexpr int STG_LD = 40;                            // staging pitch (floats): conflict-free float2 writes and
-                                                               // (with the odd-row order below) float4 reads
-  static constexpr int STG_BYTES = 8 * 16 * STG_LD * 4;        // 8 consumer warps x 16 rows x 32 columns
-  static constexpr int SMEM_BYTES = RING_BYTES + STG_BYTES + 2 * GEMM_WIDE_BN * 4 + 256 + 1024;  // + 2 bias rows, barriers, align
+  static constexpr int BOX_BYTES = GEMM_WIDE_BOX * GEMM_WIDE_BOX * 2;   // 8 KB, 1024-byte aligned (the swizzle atom)
+  static constexpr int STG_LD = 40;   // register-store epilogue: fp32 chunk pitch (floats), conflict-free float2 writes
+                                      // and (with the odd-row order below) float4 reads
+  static constexpr int STG_BYTES = STG_BOXES > 0 ? 2 * STG_BOXES * BOX_BYTES     // two warpgroups' boxes
+                                                 : 8 * 16 * STG_LD * 4;           // 8 consumer warps x 16 x 32 fp32
+  static constexpr int PASSES = STG_BOXES > 0 ? 4 / STG_BOXES : 1;   // staging passes per tile
+  // Two bias rows (alternate tiles, so one tile's epilogue never races the next fill) where they fit; the half-tile
+  // variant with its 4-stage ring has room for one, refilled behind a barrier.
+  static constexpr int BIAS_ROWS = STG_BOXES == 2 ? 1 : 2;
+  // + bias rows, 16 mbarriers, and the slack to align the ring to 1024 bytes
+  static constexpr int SMEM_BYTES = RING_BYTES + STG_BYTES + BIAS_ROWS * GEMM_WIDE_BN * 4 + 128 + 1024;
+  // STG_BOXES = 2 (4-stage ring, half a tile in two passes) fits in 231 552 B but failed a bit-identity check at
+  // M = 1, N = 264 when first run, and is not used (DESIGN.md §8)
+  static_assert(STG_BOXES == 0 || STG_BOXES == 4, "the staging tile holds a whole tile");
+  static_assert(SMEM_BYTES <= 227 * 1024, "the persistent GEMM's shared memory exceeds an SM's");
 };
-static_assert(GemmWideCfg::SMEM_BYTES <= 227 * 1024, "the persistent GEMM's shared memory exceeds an SM's");
+using GemmWideTmaCfg = GemmWideCfg<3, 4>;       // 144 KB ring + 64 KB staging tile
+using GemmWideRegCfg = GemmWideCfg<4, 0>;       // 192 KB ring + 20 KB of fp32 chunks
 
-template <int SPEC>
+template <int SPEC, class Cfg>
 __global__ void __launch_bounds__(GEMM_WIDE_THREADS, 1)
-gemm_bf16_wgmma_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M,
-                                  int N, int K, GemmEpilogue ep) {
+gemm_bf16_wgmma_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR,
+                                  int M, int N, int K, GemmEpilogue ep) {
   static_assert(SPEC >= 0 && SPEC < 8, "compile-time epilogue flavours only");
-  using Cfg = GemmWideCfg;
   constexpr int STAGES = Cfg::STAGES;
   constexpr int BN = GEMM_WIDE_BN;
   constexpr bool HAS_RES = ((SPEC >> 2) & 1) != 0;
+  constexpr bool TMA_EPI = Cfg::STG_BOXES > 0;   // tmC (and with a residual tmR) are read only then
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = ptx::smem_u32(smem_raw);
   uint8_t* base = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
   uint8_t* sA = base;
   uint8_t* sB = base + STAGES * Cfg::A_BYTES;
-  float* s_stg = reinterpret_cast<float*>(base + Cfg::RING_BYTES);
-  float* s_bias = s_stg + Cfg::STG_BYTES / 4;   // [2][BN]: alternate tiles, so one tile's epilogue never races the next fill
-  uint64_t* full = reinterpret_cast<uint64_t*>(s_bias + 2 * BN);
+  uint8_t* s_stg = base + Cfg::RING_BYTES;         // 1024-byte aligned: RING_BYTES is a multiple of 16 KB
+  float* s_bias = reinterpret_cast<float*>(s_stg + Cfg::STG_BYTES);   // [BIAS_ROWS][BN]
+  uint64_t* full = reinterpret_cast<uint64_t*>(s_bias + Cfg::BIAS_ROWS * BN);
   uint64_t* empty = full + STAGES;
+  uint64_t* stg_ready = empty + STAGES;   // [2] per warpgroup: its staging boxes may be written (residual landed)
+  uint64_t* stg_full = stg_ready + 2;     // [2] per warpgroup: its staging boxes hold the finished tile
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int mb = (M + GEMM_BM - 1) / GEMM_BM, nb = (N + BN - 1) / BN, kb = (K + GEMM_BK - 1) / GEMM_BK;
@@ -401,14 +436,18 @@ gemm_bf16_wgmma_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const
       ptx::mbar_init(&full[s], 1);
       ptx::mbar_init(&empty[s], 8);  // one arrive per consumer warp
     }
+    for (int g = 0; g < 2; g++) {
+      ptx::mbar_init(&stg_ready[g], 1);
+      ptx::mbar_init(&stg_full[g], 128);   // every thread of the warpgroup, after its fence.proxy.async
+    }
     ptx::fence_barrier_init();
   }
   __syncthreads();
 
   if (warp < 4) {
-    // ---------------- TMA producer ----------------
     ptx::setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
+      // ---------------- TMA producer ----------------
       ptx::prefetch_tensormap(&tmA);
       ptx::prefetch_tensormap(&tmB);
       int it = 0;   // k-blocks issued by this CTA over all its tiles: the ring position
@@ -425,6 +464,57 @@ gemm_bf16_wgmma_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const
           ptx::tma_load_2d(b + Cfg::B_BYTES / 2, &tmB, &full[stage], kbi * GEMM_BK, n_blk * BN + 128);
         }
       }
+    } else if (TMA_EPI && threadIdx.x == 32) {
+      // ---------------- staging thread: residual loads and output stores ----------------
+      ptx::prefetch_tensormap(&tmC);
+      if (HAS_RES) ptx::prefetch_tensormap(&tmR);
+      // Boxes of warpgroup g in staging pass `pass` of `tile` that lie inside M and N (the others are neither loaded
+      // nor stored): the first one covers columns c0 + pass * STG_BOXES * 64.
+      auto live_boxes = [&](int m_blk, int c0, int pass, int g) {
+        if (m_blk * GEMM_BM + g * GEMM_WIDE_BOX >= M) return 0;
+        return max(0, min(Cfg::STG_BOXES, (N - c0 + GEMM_WIDE_BOX - 1) / GEMM_WIDE_BOX - pass * Cfg::STG_BOXES));
+      };
+      // Hands warpgroup g's staging boxes to its consumers for a pass: with the residual loaded into them, else at once.
+      auto open = [&](int tile, int pass, int g) {
+        if (tile >= tiles) return;
+        if (!HAS_RES) {
+          ptx::mbar_arrive(&stg_ready[g]);
+          return;
+        }
+        int m_blk, n_blk;
+        gemm_tile_coords(tile, mb, nb, m_blk, n_blk);
+        const int boxes = live_boxes(m_blk, n_blk * BN, pass, g);
+        ptx::mbar_arrive_expect_tx(&stg_ready[g], boxes * Cfg::BOX_BYTES);
+        for (int b = 0; b < boxes; b++)
+          ptx::tma_load_2d(s_stg + (g * Cfg::STG_BOXES + b) * Cfg::BOX_BYTES, &tmR, &stg_ready[g],
+                           n_blk * BN + (pass * Cfg::STG_BOXES + b) * GEMM_WIDE_BOX, m_blk * GEMM_BM + g * GEMM_WIDE_BOX);
+      };
+      open(blockIdx.x, 0, 0);
+      open(blockIdx.x, 0, 1);
+      int ph = 0;   // staging passes completed: the phase of stg_full
+      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        int m_blk, n_blk;
+        gemm_tile_coords(tile, mb, nb, m_blk, n_blk);
+        const int c0 = n_blk * BN;
+        for (int pass = 0; pass < Cfg::PASSES; pass++, ph++) {
+          for (int g = 0; g < 2; g++) {
+            ptx::mbar_wait(&stg_full[g], ph & 1);
+            const int boxes = live_boxes(m_blk, c0, pass, g);
+            for (int b = 0; b < boxes; b++)
+              ptx::tma_store_2d(&tmC, s_stg + (g * Cfg::STG_BOXES + b) * Cfg::BOX_BYTES,
+                                c0 + (pass * Cfg::STG_BOXES + b) * GEMM_WIDE_BOX, m_blk * GEMM_BM + g * GEMM_WIDE_BOX);
+            ptx::bulk_commit_group();
+          }
+          // once the stores have read a warpgroup's boxes, they take the next pass's residual
+          const int next_tile = pass + 1 < Cfg::PASSES ? tile : tile + gridDim.x;
+          const int next_pass = pass + 1 < Cfg::PASSES ? pass + 1 : 0;
+          ptx::bulk_wait_group_read<1>();
+          open(next_tile, next_pass, 0);
+          ptx::bulk_wait_group_read<0>();
+          open(next_tile, next_pass, 1);
+        }
+      }
+      ptx::bulk_wait_group<0>();
     }
     return;
   }
@@ -435,16 +525,16 @@ gemm_bf16_wgmma_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const
   const int wg = cw >> 2;                   // rows wg*64 .. wg*64+63 of the tile
   const int ct = threadIdx.x - 128;         // 0..255
   const int fr = lane >> 2, fc = lane & 3;  // accumulator fragment: rows fr, fr + 8 of the warp's 16; columns 8 j + 2 fc
-  float* stg = s_stg + cw * 16 * Cfg::STG_LD;
   float acc[BN / 2];
   int it = 0;
   for (int tile = blockIdx.x, local = 0; tile < tiles; tile += gridDim.x, local++) {
     int m_blk, n_blk;
     gemm_tile_coords(tile, mb, nb, m_blk, n_blk);
     const int n0 = n_blk * BN;
-    float* bias_t = s_bias + (local & 1) * BN;
+    float* bias_t = s_bias + (local % Cfg::BIAS_ROWS) * BN;
+    if (Cfg::BIAS_ROWS == 1 && local > 0) ptx::named_barrier_sync(1, 256);   // the last tile's epilogue has read it
     bias_t[ct] = (ep.bias != nullptr && n0 + ct < N) ? ep.bias[n0 + ct] : 0.0f;
-    if (HAS_RES) {
+    if (HAS_RES && !TMA_EPI) {
       // the residual rows of the tile are brought to L2 while the k-loop runs (two 128-byte lines per thread)
       const int row = m_blk * GEMM_BM + (ct >> 1);
       const int col = (ct & 1) * 128;
@@ -474,52 +564,80 @@ gemm_bf16_wgmma_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const
     ptx::fence_regs(acc);
     if (lane == 0) ptx::mbar_arrive(&empty[(it - 1) % STAGES]);
 
-    // ---------------- epilogue: 8 chunks of 32 columns ----------------
-    // after the staging round trip, lane (fr, fc) holds columns 8 fc .. 8 fc + 7 of the chunk for rows fr and fr + 8
-    const int row0 = m_blk * GEMM_BM + wg * 64 + (cw & 3) * 16 + fr;
-    bool ok[2];
-    EpiRow er[2];
+    if constexpr (TMA_EPI) {
+      // ---------------- epilogue: fragments into the swizzled staging boxes, stored by the staging thread ----------
+      // Row r of a box is 128 bytes; its 16-byte chunk q lies at chunk q ^ (r % 8) (128B swizzle).  Lane (fr, fc)
+      // writes columns 8 j + 2 fc, +1 of rows fr and fr + 8 (both = fr mod 8): per instruction the 8 rows of a warp hit
+      // 8 different chunks, so the 32 lanes cover the 32 banks once.
+      // With half a tile staged, columns 0..127 go first; the second pass waits until their stores have read them.
+      uint8_t* stg = s_stg + wg * Cfg::STG_BOXES * Cfg::BOX_BYTES + ((cw & 3) * 16 + fr) * 128 + 4 * fc;
 #pragma unroll
-    for (int q = 0; q < 2; q++) {
-      ok[q] = row0 + 8 * q < M;
-      er[q] = epi_row(ep, ok[q] ? row0 + 8 * q : 0, n0);
-    }
-    uint4 res[2][2];   // [chunk parity][q]: the next chunk's residual is loaded while this one is stored
-    auto load_res = [&](int c, uint4 (&r)[2]) {
+      for (int pass = 0; pass < Cfg::PASSES; pass++) {
+        ptx::mbar_wait(&stg_ready[wg], (local * Cfg::PASSES + pass) & 1);
+#pragma unroll
+        for (int jj = 0; jj < Cfg::STG_BOXES * 8; jj++) {
+          const int j = pass * Cfg::STG_BOXES * 8 + jj;   // 8-column group of the tile
+          const float2 bb = *reinterpret_cast<const float2*>(bias_t + 8 * j + 2 * fc);
+#pragma unroll
+          for (int h = 0; h < 2; h++) {
+            uint32_t* p = reinterpret_cast<uint32_t*>(stg + (jj >> 3) * Cfg::BOX_BYTES + h * 8 * 128 + (((jj & 7) ^ fr) << 4));
+            const float2 r = HAS_RES ? unpack_bf16x2(*p) : make_float2(0.f, 0.f);
+            *p = pack_bf16x2(epi_apply(acc[4 * j + 2 * h] + bb.x, SPEC & 3, HAS_RES, r.x),
+                             epi_apply(acc[4 * j + 2 * h + 1] + bb.y, SPEC & 3, HAS_RES, r.y));
+          }
+        }
+        ptx::fence_proxy_async();   // the TMA stores (async proxy) read what these generic stores wrote
+        ptx::mbar_arrive(&stg_full[wg]);
+      }
+    } else {
+      // ---------------- epilogue: register stores through a per-warp fp32 chunk, 8 chunks of 32 columns -----------
+      // after the staging round trip, lane (fr, fc) holds columns 8 fc .. 8 fc + 7 of the chunk for rows fr and fr + 8
+      float* stg = reinterpret_cast<float*>(s_stg) + cw * 16 * Cfg::STG_LD;
+      const int row0 = m_blk * GEMM_BM + wg * 64 + (cw & 3) * 16 + fr;
+      bool ok[2];
+      EpiRow er[2];
 #pragma unroll
       for (int q = 0; q < 2; q++) {
-        const int col = c * 32 + fc * 8;
-        r[q] = (HAS_RES && ok[q] && n0 + col < N) ? *reinterpret_cast<const uint4*>(er[q].res_ptr + col)
-                                                   : make_uint4(0u, 0u, 0u, 0u);
+        ok[q] = row0 + 8 * q < M;
+        er[q] = epi_row(ep, ok[q] ? row0 + 8 * q : 0, n0);
       }
-    };
-    load_res(0, res[0]);
+      uint4 res[2][2];   // [chunk parity][q]: the next chunk's residual is loaded while this one is stored
+      auto load_res = [&](int c, uint4 (&r)[2]) {
 #pragma unroll
-    for (int c = 0; c < BN / 32; c++) {
-      if (c + 1 < BN / 32) load_res(c + 1, res[(c + 1) & 1]);
-      __syncwarp();
+        for (int q = 0; q < 2; q++) {
+          const int col = c * 32 + fc * 8;
+          r[q] = (HAS_RES && ok[q] && n0 + col < N) ? *reinterpret_cast<const uint4*>(er[q].res_ptr + col)
+                                                     : make_uint4(0u, 0u, 0u, 0u);
+        }
+      };
+      load_res(0, res[0]);
 #pragma unroll
-      for (int jj = 0; jj < 4; jj++) {
-        const int j = 4 * c + jj;
-        *reinterpret_cast<float2*>(stg + fr * Cfg::STG_LD + 8 * jj + 2 * fc) = make_float2(acc[4 * j], acc[4 * j + 1]);
-        *reinterpret_cast<float2*>(stg + (fr + 8) * Cfg::STG_LD + 8 * jj + 2 * fc) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-      }
-      __syncwarp();
+      for (int c = 0; c < BN / 32; c++) {
+        if (c + 1 < BN / 32) load_res(c + 1, res[(c + 1) & 1]);
+        __syncwarp();
 #pragma unroll
-      for (int q = 0; q < 2; q++) {
-        const int col = c * 32 + fc * 8;
-        if (ok[q] && n0 + col < N) {
-          // odd rows read their two halves in the other order: rows fr and fr + 1 (40 floats apart) then hit
-          // disjoint banks within a quarter-warp
-          const float* src = stg + (fr + 8 * q) * Cfg::STG_LD + fc * 8;
-          const int sw = (fr & 1) * 4;
-          const float4 h0 = *reinterpret_cast<const float4*>(src + sw);
-          const float4 h1 = *reinterpret_cast<const float4*>(src + (4 - sw));
-          const float4 u = sw ? h1 : h0, v = sw ? h0 : h1;
-          const uint32_t r8[8] = {__float_as_uint(u.x), __float_as_uint(u.y), __float_as_uint(u.z), __float_as_uint(u.w),
-                                  __float_as_uint(v.x), __float_as_uint(v.y), __float_as_uint(v.z), __float_as_uint(v.w)};
-          float st_s = 0.f, st_q = 0.f;
-          epi_store8<SPEC>(ep, er[q], r8, bias_t, nullptr, col, n0, res[c & 1][q], 0.f, st_s, st_q);
+        for (int jj = 0; jj < 4; jj++) {
+          const int j = 4 * c + jj;
+          *reinterpret_cast<float2*>(stg + fr * Cfg::STG_LD + 8 * jj + 2 * fc) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(stg + (fr + 8) * Cfg::STG_LD + 8 * jj + 2 * fc) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+        __syncwarp();
+#pragma unroll
+        for (int q = 0; q < 2; q++) {
+          const int col = c * 32 + fc * 8;
+          if (ok[q] && n0 + col < N) {
+            // odd rows read their two halves in the other order: rows fr and fr + 1 (40 floats apart) then hit
+            // disjoint banks within a quarter-warp
+            const float* src = stg + (fr + 8 * q) * Cfg::STG_LD + fc * 8;
+            const int sw = (fr & 1) * 4;
+            const float4 h0 = *reinterpret_cast<const float4*>(src + sw);
+            const float4 h1 = *reinterpret_cast<const float4*>(src + (4 - sw));
+            const float4 u = sw ? h1 : h0, v = sw ? h0 : h1;
+            const uint32_t r8[8] = {__float_as_uint(u.x), __float_as_uint(u.y), __float_as_uint(u.z), __float_as_uint(u.w),
+                                    __float_as_uint(v.x), __float_as_uint(v.y), __float_as_uint(v.z), __float_as_uint(v.w)};
+            float st_s = 0.f, st_q = 0.f;
+            epi_store8<SPEC>(ep, er[q], r8, bias_t, nullptr, col, n0, res[c & 1][q], 0.f, st_s, st_q);
+          }
         }
       }
     }
@@ -534,9 +652,9 @@ int make_tmap_3d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t pla
 // tmB must have boxes of bn rows x 64 columns (128 rows for bn = 256).  generic = true launches the run-time epilogue
 // flavour (SPEC = -1) even where a compile-time flavour applies (the tests check that both store the same bits).
 // bn = 256 (the persistent kernel) takes the compile-time flavours only: B200_ERR_INVALID for generic, ln_stats or
-// stats_out.
+// stats_out.  It stores by TMA from 8 tiles per CTA up (or with force_tma_epilogue), else from registers.
 int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int M, int N, int K,
-                     const GemmEpilogue& ep, cudaStream_t st, bool generic = false);
+                     const GemmEpilogue& ep, cudaStream_t st, bool generic = false, bool force_tma_epilogue = false);
 // true when a compile-time epilogue flavour covers `ep` (no LayerNorm fold, no row statistics)
 inline bool gemm_epilogue_is_plain(const GemmEpilogue& ep) {
   return ep.ln_stats == nullptr && ep.stats_out == nullptr && ep.ln_c == nullptr && ep.act >= 0 && ep.act <= 2;

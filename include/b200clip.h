@@ -280,8 +280,9 @@ int b200_gemm_bf16_device(const void* d_A, const void* d_W, const float* d_bias,
  * bn: 0 = the width the library picks (128 whenever stats_out is set), else 32, 64, 128 or 256.  256 is the
  * persistent 128 x 256 kernel of the large-batch shapes: it takes the compile-time epilogue flavours only, and is
  * refused (B200_ERR_INVALID) with force_generic, stats_out or ln_stats.
- * force_generic != 0: the epilogue flavour that decides every feature at run time, even where a compile-time
- * flavour exists; both store the same bits. */
+ * force_generic bit 0 (or any value other than 2): the epilogue flavour that decides every feature at run time,
+ * even where a compile-time flavour exists; both store the same bits.  force_generic == 2: with bn = 256, the TMA-store
+ * epilogue whatever the grid size (the library takes it from 8 tiles per SM up); the same bits again. */
 typedef struct b200_gemm_epilogue {
   const float* bias;        /* [N] fp32 or NULL */
   const void* residual;     /* bf16, added after the activation, or NULL; may equal the output (in-place update) */

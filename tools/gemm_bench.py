@@ -11,6 +11,14 @@ TFLOP/s (2 M N K) and the fraction of the 989 TFLOP/s BF16 data-sheet rate, whic
 launched, and, as a reference for what this card reaches on the shape, torch.matmul in bf16 (cuBLAS; not a code path
 of the library).  Shapes: the eight ViT-L/14 layer GEMMs at batch 1024 and its patch embedding, the ViT-H/14 text
 tower at batches 1, 8 and 64, and the ViT-B/32 image tower at batch 1024.  A width the library refuses prints "-".
+
+  python tools/gemm_bench.py --ksweep [--json OUT]
+
+splits the persistent kernel's time into k-loop and per-tile fixed cost: M = 1024 * 257 (ViT-L/14 image rows at batch
+1024), N in {1024, 3072, 4096}, K in {256, 512, 1024, 2048, 4096}, bn forced to 256, for the plain (bias), quick-GELU
+and in-place residual epilogues.  Per (N, flavour) it fits ms = waves * (a * k_blocks + b), waves = ceil(tiles / grid),
+by least squares and prints a (us per 64-deep k-block), b (us per tile) and b / a (the fixed cost in k-blocks), with
+the card's name, power limit and the SM clock sampled during each timed replay.
 """
 import argparse
 import json
@@ -48,11 +56,98 @@ def shapes():
     return out
 
 
+def sm_clock():
+    return subprocess.run(["nvidia-smi", "--query-gpu=clocks.sm", "--format=csv,noheader"], capture_output=True,
+                          text=True, check=True).stdout.strip().splitlines()[0]
+
+
+def graph_ms(fn, iters, during=None):
+    """ms per call of fn(stream) over one replay of a CUDA graph of `iters` calls (after warm-up); `during()` is called
+    on the host while the timed replay runs."""
+    import torch
+
+    for _ in range(3):
+        fn(torch.cuda.current_stream().cuda_stream)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        cap = torch.cuda.current_stream().cuda_stream
+        for _ in range(iters):
+            fn(cap)
+    graph.replay()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    e0.record()
+    graph.replay()
+    e1.record()
+    if during is not None:
+        during()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / iters
+
+
+KSWEEP_M = 1024 * 257
+KSWEEP_N = (1024, 3072, 4096)
+KSWEEP_K = (256, 512, 1024, 2048, 4096)
+KSWEEP_FLAVOURS = (("plain", 0, False), ("quick-gelu", 1, False), ("residual", 0, True))
+
+
+def ksweep(args, name, power):
+    import numpy as np
+    import torch
+    from clip_retrieval_b200._lib import lib, check, GemmEpilogueC
+
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    M = KSWEEP_M
+    t = {}   # (N, flavour, K) -> ms
+    clocks = []
+    for K in KSWEEP_K:
+        g = torch.Generator(device="cuda").manual_seed(K)
+        A = (torch.randn(M, K, device="cuda", generator=g, dtype=torch.bfloat16) * 0.5)
+        for N in KSWEEP_N:
+            W = (torch.randn(N, K, device="cuda", generator=g, dtype=torch.bfloat16) * K ** -0.5)
+            bias = torch.randn(N, device="cuda", generator=g)
+            out = torch.randn(M, N, device="cuda", generator=g, dtype=torch.bfloat16)
+            for fl, act, res in KSWEEP_FLAVOURS:
+                ep = GemmEpilogueC(bias.data_ptr(), out.data_ptr() if res else None, 0, 0, 0, 0, 0, act, None, None, 0,
+                                   None)
+
+                def launch(s, ep=ep):
+                    check(lib.b200_gemm_bf16_ex_device(A.data_ptr(), W.data_ptr(), out.data_ptr(), M, N, K, ep, 256, 0,
+                                                       0, s), "gemm")
+
+                est = graph_ms(launch, 2)
+                # the timed replay lasts about 200 ms: the SM clock is sampled while it runs
+                t[(N, fl, K)] = graph_ms(launch, max(3, min(500, int(200.0 / est))), lambda: clocks.append(sm_clock()))
+                print("N=%-5d K=%-5d %-10s %8.4f ms  (SM clock %s)" % (N, K, fl, t[(N, fl, K)], clocks[-1]), flush=True)
+            del W, bias, out
+        del A
+        torch.cuda.empty_cache()
+    print("card: %s, power limit %s, SM clock sampled during the timings %s .. %s"
+          % (name, power, min(clocks, key=lambda c: int(c.split()[0])), max(clocks, key=lambda c: int(c.split()[0]))))
+    print("%-5s %-10s %12s %12s %10s" % ("N", "flavour", "a us/kblk", "b us/tile", "b/a kblk"))
+    fits = []
+    for N in KSWEEP_N:
+        tiles = ((M + 127) // 128) * ((N + 255) // 256)
+        waves = -(-tiles // min(tiles, sms))
+        for fl, _, _ in KSWEEP_FLAVOURS:
+            kblk = np.array([K / 64.0 for K in KSWEEP_K])
+            y = np.array([t[(N, fl, K)] * 1e3 / waves for K in KSWEEP_K])   # us per wave
+            a, b = np.polyfit(kblk, y, 1)
+            fits.append({"N": N, "flavour": fl, "a_us_per_kblock": a, "b_us_per_tile": b, "b_over_a": b / a})
+            print("%-5d %-10s %12.3f %12.3f %10.2f" % (N, fl, a, b, b / a))
+    if args.json:
+        with open(args.json, "w") as f:
+            json.dump({"device": name, "power_limit": power, "sm_clocks": clocks, "M": M, "sms": sms,
+                       "ms": [{"N": N, "flavour": fl, "K": K, "ms": v} for (N, fl, K), v in t.items()], "fits": fits},
+                      f, indent=1)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--only", default=None, help="only shapes whose name contains this")
     ap.add_argument("--json", default=None)
+    ap.add_argument("--ksweep", action="store_true", help="fit the persistent kernel's k-loop and per-tile costs")
     args = ap.parse_args()
     import torch
     import clip_retrieval_b200  # noqa: F401
@@ -62,6 +157,8 @@ def main():
         raise SystemExit("gemm_bench.py needs a CUDA device")
     name, power, clock = card()
     print("card: %s, power limit %s, max SM clock %s" % (name, power, clock))
+    if args.ksweep:
+        return ksweep(args, name, power)
     rows = []
     for sname, M, N, K, act, res, group in shapes():
         if args.only and args.only not in sname:
@@ -85,21 +182,7 @@ def main():
             return lib.b200_gemm_bf16_ex_device(A.data_ptr(), W.data_ptr(), out.data_ptr(), M, N, K, ep, bn, 0, 0, s)
 
         def timed(fn):
-            for _ in range(3):
-                fn(torch.cuda.current_stream().cuda_stream)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                cap = torch.cuda.current_stream().cuda_stream
-                for _ in range(iters):
-                    fn(cap)
-            graph.replay()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            torch.cuda.synchronize()
-            e0.record()
-            graph.replay()
-            e1.record()
-            torch.cuda.synchronize()
-            return e0.elapsed_time(e1) / iters
+            return graph_ms(fn, iters)
 
         r = {"shape": sname, "M": M, "N": N, "K": K}
         for label, bn in (("bn128", 128), ("bn256", 256), ("auto", 0)):
