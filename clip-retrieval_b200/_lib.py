@@ -55,6 +55,24 @@ class ClipConfigC(C.Structure):
     ]
 
 
+class TextEncoderConfigC(C.Structure):
+    _fields_ = [
+        ("layers", C.c_int32),
+        ("width", C.c_int32),
+        ("heads", C.c_int32),
+        ("ffn", C.c_int32),
+        ("vocab_size", C.c_int32),
+        ("max_positions", C.c_int32),
+        ("type_vocab_size", C.c_int32),
+        ("position_offset", C.c_int32),
+        ("layer_norm_eps", C.c_float),
+        ("out_dim", C.c_int32),
+        ("proj_bias", C.c_int32),
+        ("max_batch", C.c_int32),
+        ("max_tokens", C.c_int32),
+    ]
+
+
 class TensorViewC(C.Structure):
     _fields_ = [
         ("name", C.c_char_p),
@@ -157,6 +175,16 @@ PROTOTYPES = {
     "b200_mlp_destroy": (_i, [_vp]),
     "b200_mlp_load_layer": (_i, [_vp, _i, _vp, _vp]),
     "b200_mlp_forward_device": (_i, [_vp, _vp, _i, _vp, _vp]),
+    "b200_text_encoder_create": (_i, [C.POINTER(TextEncoderConfigC), _i, C.POINTER(_vp)]),
+    "b200_text_encoder_destroy": (_i, [_vp]),
+    "b200_text_encoder_load_weights": (_i, [_vp, C.POINTER(TensorViewC), _i]),
+    "b200_text_encoder_encode_device": (_i, [_vp, _vp, _vp, _i, _i, _vp, _i, _i, _vp]),
+    "b200_text_encoder_encode": (_i, [_vp, _vp, _vp, _i, _i, _vp, _i, _i]),
+    "b200_text_encoder_last_timing": (_i, [_vp, C.POINTER(C.c_float), C.POINTER(C.c_int)]),
+    "b200_text_encoder_set_profiling": (_i, [_vp, _i]),
+    "b200_layernorm_eps_bf16_device": (_i, [_vp, _vp, _vp, _vp, _i64, _i, C.c_float, _i, _vp]),
+    "b200_attention_len_bf16_device": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "b200_encoder_embed_bf16_device": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, C.c_float, _vp, _i, _i, _i, _i, _i, _vp]),
 }
 
 for _name, (_res, _args) in PROTOTYPES.items():

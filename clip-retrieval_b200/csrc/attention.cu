@@ -3,6 +3,8 @@
 // of one head sit in shared memory (padded rows, conflict-free ldmatrix), each warp owns 16 query
 // rows at a time and runs the flash-style online softmax in fp32 registers.
 // First version on mma.sync.m16n8k16 (bf16 in, fp32 accumulate); 4% of the forward's flops.
+// Per-sample key lengths (len[b] in 1..T) as in attention_wgmma.cu: keys >= len[b] are staged as zeros and masked,
+// the key loop stops at the 32-key block holding len[b] - 1, and rows >= len[b] are written as zeros.
 #include "embed_kernels.cuh"
 
 namespace b200 {
@@ -34,7 +36,7 @@ constexpr int ATT_KB = 32;  // keys per inner block
 template <int HD>
 __global__ void __launch_bounds__(256)
 attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ out, int T, int w, float scale_log2e,
-                 int causal) {
+                 int causal, const int* __restrict__ len) {
   constexpr int LDS = HD + 8;  // padded row (elements): 144 B / 176 B rows -> conflict-free ldmatrix
   extern __shared__ __align__(16) unsigned char att_smem[];
   __nv_bfloat16* sK = reinterpret_cast<__nv_bfloat16*>(att_smem);
@@ -42,6 +44,8 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
   __nv_bfloat16* sV = sK + (size_t)Tp * LDS;
 
   const int h = blockIdx.x, b = blockIdx.y;
+  const int L = len != nullptr ? min(max(len[b], 1), T) : T;   // keys of this sample
+  const int Lp = (L + ATT_KB - 1) / ATT_KB * ATT_KB;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   const size_t ld = (size_t)3 * w;
   const __nv_bfloat16* base = qkv + (size_t)b * T * ld + (size_t)h * HD;
@@ -51,7 +55,7 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
   for (int i = threadIdx.x; i < Tp * CPR; i += blockDim.x) {
     const int t = i / CPR, c = i - t * CPR;
     uint4 kv = make_uint4(0, 0, 0, 0), vv = make_uint4(0, 0, 0, 0);
-    if (t < T) {
+    if (t < L) {
       kv = *reinterpret_cast<const uint4*>(base + (size_t)t * ld + w + c * 8);
       vv = *reinterpret_cast<const uint4*>(base + (size_t)t * ld + 2 * w + c * 8);
     }
@@ -60,7 +64,7 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
   }
   __syncthreads();
 
-  const int qblocks = (T + 15) / 16;
+  const int qblocks = (L + 15) / 16;
   const uint32_t sK_u = (uint32_t)__cvta_generic_to_shared(sK);
   const uint32_t sV_u = (uint32_t)__cvta_generic_to_shared(sV);
 
@@ -81,7 +85,7 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
     for (int i = 0; i < HD / 8; i++) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
     float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
 
-    const int kend = causal ? min(Tp, (qb * 16 + 16 + ATT_KB - 1) / ATT_KB * ATT_KB) : Tp;
+    const int kend = causal ? min(Lp, (qb * 16 + 16 + ATT_KB - 1) / ATT_KB * ATT_KB) : Lp;
     for (int kb = 0; kb < kend; kb += ATT_KB) {
       float s[ATT_KB / 8][4];
 #pragma unroll
@@ -113,8 +117,8 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
 #pragma unroll
         for (int e = 0; e < 2; e++) {
           const int kk = key + e;
-          const bool dead0 = kk >= T || (causal && kk > r0);
-          const bool dead1 = kk >= T || (causal && kk > r1);
+          const bool dead0 = kk >= L || (causal && kk > r0);
+          const bool dead1 = kk >= L || (causal && kk > r1);
           if (dead0) s[nt][e] = -INFINITY;
           if (dead1) s[nt][2 + e] = -INFINITY;
           bm0 = fmaxf(bm0, s[nt][e]);
@@ -171,15 +175,19 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
 #pragma unroll
     for (int i = 0; i < HD / 8; i++) {
       const int col = i * 8 + (lane & 3) * 2;
-      if (r0 < T) *reinterpret_cast<uint32_t*>(ob + (size_t)r0 * w + col) = pack2(o[i][0] * i0, o[i][1] * i0);
-      if (r1 < T) *reinterpret_cast<uint32_t*>(ob + (size_t)r1 * w + col) = pack2(o[i][2] * i1, o[i][3] * i1);
+      if (r0 < T) *reinterpret_cast<uint32_t*>(ob + (size_t)r0 * w + col) = r0 < L ? pack2(o[i][0] * i0, o[i][1] * i0) : 0u;
+      if (r1 < T) *reinterpret_cast<uint32_t*>(ob + (size_t)r1 * w + col) = r1 < L ? pack2(o[i][2] * i1, o[i][3] * i1) : 0u;
     }
   }
+  // rows of the 16-row query blocks past the sample's keys (none without lengths)
+  __nv_bfloat16* ob = out + (size_t)b * T * w + (size_t)h * HD;
+  for (int i = qblocks * 16 * CPR + (int)threadIdx.x; i < T * CPR; i += blockDim.x)
+    *reinterpret_cast<uint4*>(ob + (size_t)(i / CPR) * w + (i % CPR) * 8) = make_uint4(0u, 0u, 0u, 0u);
 }
 
 template <int HD>
 static int launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int heads, int w, int causal,
-                            cudaStream_t st) {
+                            cudaStream_t st, const int* len) {
   const int Tp = (T + ATT_KB - 1) / ATT_KB * ATT_KB;
   const size_t smem = (size_t)2 * Tp * (HD + 8) * sizeof(__nv_bfloat16);
   B200_CHECK(smem <= 200 * 1024, B200_ERR_UNSUPPORTED, "attention: sequence length %d too long for the small-T kernel", T);
@@ -188,19 +196,20 @@ static int launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B,
   const float scale_log2e = (1.0f / sqrtf((float)HD)) * 1.4426950408889634f;
   const int qblocks = (T + 15) / 16;
   const int threads = qblocks >= 8 ? 256 : (qblocks >= 4 ? 128 : 64);
-  kern<<<dim3(heads, B), threads, smem, st>>>(qkv, out, T, w, scale_log2e, causal);
+  kern<<<dim3(heads, B), threads, smem, st>>>(qkv, out, T, w, scale_log2e, causal, len);
   B200_LAUNCH_OK();
   return B200_OK;
 }
 
-int attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int heads, int w, int causal, cudaStream_t st) {
+int attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int heads, int w, int causal, cudaStream_t st,
+              const int* len) {
   B200_CHECK(heads > 0 && w % heads == 0, B200_ERR_INVALID, "attention: width %d not divisible by heads %d", w, heads);
   if (B == 0) return B200_OK;
   const int hd = w / heads;
-  if (hd == 64) return launch_attention<64>(qkv, out, B, T, heads, w, causal, st);
-  if (hd == 80) return launch_attention<80>(qkv, out, B, T, heads, w, causal, st);
-  if (hd == 96) return launch_attention<96>(qkv, out, B, T, heads, w, causal, st);
-  if (hd == 128) return launch_attention<128>(qkv, out, B, T, heads, w, causal, st);
+  if (hd == 64) return launch_attention<64>(qkv, out, B, T, heads, w, causal, st, len);
+  if (hd == 80) return launch_attention<80>(qkv, out, B, T, heads, w, causal, st, len);
+  if (hd == 96) return launch_attention<96>(qkv, out, B, T, heads, w, causal, st, len);
+  if (hd == 128) return launch_attention<128>(qkv, out, B, T, heads, w, causal, st, len);
   set_error("attention: head dimension %d not supported (64, 80, 96, 128)", hd);
   return B200_ERR_UNSUPPORTED;
 }

@@ -15,6 +15,11 @@
 // before the softmax of block j, so the tensor cores work on it while the warpgroup computes exponentials.  Only the
 // last key block of a tile (the end of the sequence, or the causal diagonal) is masked, and it is computed on
 // N = 16 * ceil(keys / 16) columns and as many k16 steps of P V.
+//
+// With per-sample key lengths (len[b] in 1..T, the key-padding mask of a bidirectional encoder) a sample sees keys
+// < len[b] only: the key blocks at or past len[b] are not loaded, the query tiles wholly past it are not computed, and
+// every row >= len[b] of the output is written as zeros.  len == nullptr is len[b] = T, and then the arithmetic and the
+// stores are the ones of the kernel without lengths.
 #include "embed_kernels.cuh"
 #include "gemm.cuh"
 #include "ptx.cuh"
@@ -121,7 +126,7 @@ __device__ __forceinline__ void attw_quad_transpose(const uint32_t (&a)[4], uint
 
 __global__ void __launch_bounds__(ATTW_THREADS, 2)
 attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __restrict__ out, int T, int w,
-                       float scale_log2e, int causal) {
+                       float scale_log2e, int causal, const int* __restrict__ len) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t pad = (1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u;
   uint8_t* base = smem_raw + pad;
@@ -135,6 +140,8 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16*
   uint64_t* barQ = bar + 2 * ATTW_MAX_KB;
 
   const int h = blockIdx.x, b = blockIdx.y;
+  const int L = len != nullptr ? min(max(len[b], 1), T) : T;   // keys of this sample
+  const int nlb = (L + ATTW_BK - 1) / ATTW_BK;      // key blocks loaded and query tiles computed
   // the warpgroup index through a shuffle: the compiler then knows it is uniform across the warp, and so is every
   // branch around a wgmma that depends on it (else it serialises the wgmmas)
   const int wg = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 7, 0);
@@ -155,21 +162,21 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16*
   __syncthreads();
   if (threadIdx.x == 0) {
     load_q(0);
-    if (nkb > 1) load_q(1);
-    for (int j = 0; j < nkb; j++) {
+    if (nlb > 1) load_q(1);
+    for (int j = 0; j < nlb; j++) {
       ptx::mbar_arrive_expect_tx(barK + j, ATTW_TILE);
       ptx::tma_load_3d(sK + j * ATTW_TILE, &tmQKV, barK + j, ck, j * ATTW_BK, b);
       ptx::mbar_arrive_expect_tx(barV + j, ATTW_TILE);
       ptx::tma_load_3d(sV + j * ATTW_TILE, &tmQKV, barV + j, cv, j * ATTW_BK, b);
     }
-    for (int t = 2; t < nkb && t < ATTW_QSLOTS; t++) load_q(t);
+    for (int t = 2; t < nlb && t < ATTW_QSLOTS; t++) load_q(t);
   }
 
   __nv_bfloat16* ob = out + (int64_t)b * T * w + h * ATTW_HD;
-  for (int t = wg; t < nkb; t += 2) {
+  for (int t = wg; t < nlb; t += 2) {
     const int slot = 2 * wg + ((t >> 1) & 1);
     const int q0 = t * ATTW_BQ;
-    const int kend = causal ? min(T, q0 + ATTW_BQ) : T;       // keys this tile can see
+    const int kend = causal ? min(L, q0 + ATTW_BQ) : L;       // keys this tile can see
     const int nkt = (kend + ATTW_BK - 1) / ATTW_BK;
     const int last_cols = 16 * ((kend - (nkt - 1) * ATTW_BK + 15) / 16);
     const int r_lo = q0 + 16 * warp + (lane >> 2);
@@ -198,7 +205,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16*
       if (last) {
         // the tile's last Q K^T is done: once every warp of the warpgroup is here, the Q slot can be refilled
         ptx::named_barrier_sync(1 + wg, 128);
-        if (tid == 0 && t + ATTW_QSLOTS < nkb) load_q(t + ATTW_QSLOTS);
+        if (tid == 0 && t + ATTW_QSLOTS < nlb) load_q(t + ATTW_QSLOTS);
         attw_softmax<true>(s, o, r, lane, j * ATTW_BK, kend, r_lo, causal, scale_log2e);
       } else {
         attw_softmax<false>(s, o, r, lane, j * ATTW_BK, kend, r_lo, causal, scale_log2e);
@@ -249,10 +256,15 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16*
 #pragma unroll
         for (int k = 0; k < 4; k++) a[k] = attw_pack(o[4 * (4 * g + k) + 2 * half] * inv, o[4 * (4 * g + k) + 2 * half + 1] * inv);
         attw_quad_transpose(a, c, q);
-        if (row < T) *reinterpret_cast<uint4*>(ob + (int64_t)row * w + 8 * (4 * g + q)) = make_uint4(c[0], c[1], c[2], c[3]);
+        if (row < T)
+          *reinterpret_cast<uint4*>(ob + (int64_t)row * w + 8 * (4 * g + q)) =
+              row < L ? make_uint4(c[0], c[1], c[2], c[3]) : make_uint4(0u, 0u, 0u, 0u);
       }
     }
   }
+  // rows of the query tiles past the sample's keys (none without lengths): 8 x 16-byte stores per row of the head
+  for (int i = nlb * ATTW_BQ * 8 + (int)threadIdx.x; i < T * 8; i += ATTW_THREADS)
+    *reinterpret_cast<uint4*>(ob + (int64_t)(i >> 3) * w + 8 * (i & 7)) = make_uint4(0u, 0u, 0u, 0u);
 }
 
 bool attention_wgmma_supported(int T, int heads, int w) {
@@ -260,7 +272,7 @@ bool attention_wgmma_supported(int T, int heads, int w) {
 }
 
 int attention_wgmma(const CUtensorMap& tmQKV, __nv_bfloat16* out, int B, int T, int heads, int w, int causal,
-                    cudaStream_t st) {
+                    cudaStream_t st, const int* len) {
   B200_CHECK(attention_wgmma_supported(T, heads, w), B200_ERR_UNSUPPORTED,
              "attention_wgmma: head dim 64 and T <= %d only (T=%d heads=%d w=%d)", ATTW_MAX_T, T, heads, w);
   if (B == 0) return B200_OK;
@@ -273,7 +285,7 @@ int attention_wgmma(const CUtensorMap& tmQKV, __nv_bfloat16* out, int B, int T, 
     configured.fetch_or(1ull << (dev & 63));
   }
   const float scale_log2e = 0.125f * 1.4426950408889634f;   // hd^-0.5 * log2(e)
-  attention_wgmma_kernel<<<dim3(heads, B), ATTW_THREADS, attw_smem_bytes(T), st>>>(tmQKV, out, T, w, scale_log2e, causal);
+  attention_wgmma_kernel<<<dim3(heads, B), ATTW_THREADS, attw_smem_bytes(T), st>>>(tmQKV, out, T, w, scale_log2e, causal, len);
   B200_LAUNCH_OK();
   return B200_OK;
 }

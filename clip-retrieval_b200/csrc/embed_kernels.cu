@@ -108,7 +108,7 @@ constexpr int LN_MAXC = 8;  // 16-byte chunks per lane: w <= 2048
 template <int CPL>          // chunks per lane actually present: ceil(w / 256)
 __global__ void __launch_bounds__(256)
 layernorm_kernel(const __nv_bfloat16* __restrict__ in, int64_t in_ld, __nv_bfloat16* __restrict__ out, int64_t out_ld,
-                 const float* __restrict__ gamma, const float* __restrict__ beta, int64_t rows, int w) {
+                 const float* __restrict__ gamma, const float* __restrict__ beta, int64_t rows, int w, float eps) {
   // persistent warps: row = gwarp, gwarp + total, ...; the next row's 16-byte chunks are loaded
   // before the current row is reduced and stored, so a warp always has a row in flight.
   const int lane = threadIdx.x & 31;
@@ -179,7 +179,7 @@ layernorm_kernel(const __nv_bfloat16* __restrict__ in, int64_t in_ld, __nv_bfloa
     }
 #pragma unroll
     for (int o = 16; o >= 1; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-    const float rstd = rsqrtf(ss / (float)w + 1e-5f);
+    const float rstd = rsqrtf(ss / (float)w + eps);
     __nv_bfloat16* dst = out + row * out_ld;
 #pragma unroll
     for (int c = 0; c < CPL; c++) {
@@ -200,19 +200,23 @@ layernorm_kernel(const __nv_bfloat16* __restrict__ in, int64_t in_ld, __nv_bfloa
 }
 int layernorm_rows(const __nv_bfloat16* in, int64_t in_ld, __nv_bfloat16* out, int64_t out_ld, const float* gamma,
                    const float* beta, int64_t rows, int w, cudaStream_t st) {
+  return layernorm_rows_eps(in, in_ld, out, out_ld, gamma, beta, rows, w, 1e-5f, st);
+}
+int layernorm_rows_eps(const __nv_bfloat16* in, int64_t in_ld, __nv_bfloat16* out, int64_t out_ld, const float* gamma,
+                       const float* beta, int64_t rows, int w, float eps, cudaStream_t st) {
   B200_CHECK(w % 8 == 0 && w <= LN_MAXC * 256, B200_ERR_UNSUPPORTED, "layernorm: width %d (need %%8, <= 2048)", w);
   if (rows == 0) return B200_OK;
   // persistent: enough blocks to fill the chip, each warp strides over rows
   const unsigned grid = (unsigned)std::min<int64_t>((rows + 7) / 8, (int64_t)132 * 6);
   switch ((w / 8 + 31) / 32) {
-    case 1: layernorm_kernel<1><<<grid, 256, 0, st>>>(in, in_ld, out, out_ld, gamma, beta, rows, w); break;
-    case 2: layernorm_kernel<2><<<grid, 256, 0, st>>>(in, in_ld, out, out_ld, gamma, beta, rows, w); break;
-    case 3: layernorm_kernel<3><<<grid, 256, 0, st>>>(in, in_ld, out, out_ld, gamma, beta, rows, w); break;
-    case 4: layernorm_kernel<4><<<grid, 256, 0, st>>>(in, in_ld, out, out_ld, gamma, beta, rows, w); break;
-    case 5: layernorm_kernel<5><<<grid, 256, 0, st>>>(in, in_ld, out, out_ld, gamma, beta, rows, w); break;
-    case 6: layernorm_kernel<6><<<grid, 256, 0, st>>>(in, in_ld, out, out_ld, gamma, beta, rows, w); break;
-    case 7: layernorm_kernel<7><<<grid, 256, 0, st>>>(in, in_ld, out, out_ld, gamma, beta, rows, w); break;
-    default: layernorm_kernel<8><<<grid, 256, 0, st>>>(in, in_ld, out, out_ld, gamma, beta, rows, w); break;
+    case 1: layernorm_kernel<1><<<grid, 256, 0, st>>>(in, in_ld, out, out_ld, gamma, beta, rows, w, eps); break;
+    case 2: layernorm_kernel<2><<<grid, 256, 0, st>>>(in, in_ld, out, out_ld, gamma, beta, rows, w, eps); break;
+    case 3: layernorm_kernel<3><<<grid, 256, 0, st>>>(in, in_ld, out, out_ld, gamma, beta, rows, w, eps); break;
+    case 4: layernorm_kernel<4><<<grid, 256, 0, st>>>(in, in_ld, out, out_ld, gamma, beta, rows, w, eps); break;
+    case 5: layernorm_kernel<5><<<grid, 256, 0, st>>>(in, in_ld, out, out_ld, gamma, beta, rows, w, eps); break;
+    case 6: layernorm_kernel<6><<<grid, 256, 0, st>>>(in, in_ld, out, out_ld, gamma, beta, rows, w, eps); break;
+    case 7: layernorm_kernel<7><<<grid, 256, 0, st>>>(in, in_ld, out, out_ld, gamma, beta, rows, w, eps); break;
+    default: layernorm_kernel<8><<<grid, 256, 0, st>>>(in, in_ld, out, out_ld, gamma, beta, rows, w, eps); break;
   }
   B200_LAUNCH_OK();
   return B200_OK;
@@ -388,6 +392,139 @@ int pool_ln_proj_norm(const __nv_bfloat16* x, int T, int w, const int* pool_idx,
   const size_t smem = (size_t)(w + D) * sizeof(float);
   B200_CHECK(smem <= 48 * 1024, B200_ERR_UNSUPPORTED, "pool_proj: width+embed_dim too large");
   pool_proj_kernel<<<B, 256, smem, st>>>(x, T, w, pool_idx, gamma, beta, proj, D, out, out_f16, normalize);
+  B200_LAUNCH_OK();
+  return B200_OK;
+}
+
+// ---- BERT-family encoders (text_encoder.cu) --------------------------------------------------------------
+// Embedding + LayerNorm: one block per row, 8 columns per thread in registers between the two passes.
+__global__ void __launch_bounds__(256)
+encoder_embed_kernel(const int64_t* __restrict__ ids, const __nv_bfloat16* __restrict__ word,
+                     const float* __restrict__ tt0, const float* __restrict__ pos, int pos_off,
+                     const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
+                     __nv_bfloat16* __restrict__ x, int T, int w, int vocab) {
+  __shared__ float red[8];
+  const int64_t r = blockIdx.x;
+  const int t = (int)(r % T);
+  const int c = threadIdx.x;          // 8-column chunk
+  const bool live = c * 8 < w;
+  int64_t tok = ids[r];
+  if (tok < 0) tok = 0;
+  if (tok >= vocab) tok = vocab - 1;
+  float v[8];
+  float part = 0.f;
+  if (live) {
+    const uint4 e = *reinterpret_cast<const uint4*>(word + tok * w + c * 8);
+    const __nv_bfloat162* e2 = reinterpret_cast<const __nv_bfloat162*>(&e);
+    const float* pr = pos + (size_t)(pos_off + t) * w + c * 8;
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      const float2 f = __bfloat1622float2(e2[j]);
+      float a = f.x, b = f.y;
+      if (tt0 != nullptr) { a = a + tt0[c * 8 + 2 * j]; b = b + tt0[c * 8 + 2 * j + 1]; }
+      v[2 * j] = a + pr[2 * j];
+      v[2 * j + 1] = b + pr[2 * j + 1];
+    }
+#pragma unroll
+    for (int j = 0; j < 8; j++) part += v[j];
+  }
+  const float mean = block_sum(part, red) / (float)w;
+  part = 0.f;
+  if (live) {
+#pragma unroll
+    for (int j = 0; j < 8; j++) part += (v[j] - mean) * (v[j] - mean);
+  }
+  const float rstd = rsqrtf(block_sum(part, red) / (float)w + eps);
+  if (live) {
+    uint32_t o[4];
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      const int k = c * 8 + 2 * j;
+      __nv_bfloat162 h = __floats2bfloat162_rn((v[2 * j] - mean) * rstd * gamma[k] + beta[k],
+                                               (v[2 * j + 1] - mean) * rstd * gamma[k + 1] + beta[k + 1]);
+      o[j] = *reinterpret_cast<uint32_t*>(&h);
+    }
+    *reinterpret_cast<uint4*>(x + r * w + c * 8) = make_uint4(o[0], o[1], o[2], o[3]);
+  }
+}
+int encoder_embed(const int64_t* ids, const __nv_bfloat16* word, const float* tt0, const float* pos, int pos_off,
+                  const float* gamma, const float* beta, float eps, __nv_bfloat16* x, int B, int T, int w, int vocab,
+                  cudaStream_t st) {
+  B200_CHECK(w % 8 == 0 && w <= 2048, B200_ERR_UNSUPPORTED, "encoder_embed: width %d (need %%8, <= 2048)", w);
+  if (B == 0) return B200_OK;
+  const int threads = (w / 8 + 31) / 32 * 32;
+  encoder_embed_kernel<<<(unsigned)((int64_t)B * T), threads, 0, st>>>(ids, word, tt0, pos, pos_off, gamma, beta, eps,
+                                                                       x, T, w, vocab);
+  B200_LAUNCH_OK();
+  return B200_OK;
+}
+
+// Masked mean + projection, split like pool_proj_split_kernel: a block owns 64 output columns of one sample, forms
+// the mean row itself (one thread per column, tokens in ascending order) and splits the projection over 4 quarters
+// of the reduction dimension.
+__global__ void __launch_bounds__(256)
+masked_mean_proj_kernel(const __nv_bfloat16* __restrict__ x, int T, int w, const int* __restrict__ len,
+                        const float* __restrict__ projT, const float* __restrict__ bias, int D,
+                        float* __restrict__ feat) {
+  extern __shared__ float sm[];
+  float* s_row = sm;                // [w]
+  float* s_part = sm + w;           // [4][64]
+  const int b = blockIdx.y, j0 = blockIdx.x * 64;
+  const int L = min(max(len[b], 1), T);
+  const __nv_bfloat16* src = x + (size_t)b * T * w;
+  for (int j = threadIdx.x; j < w; j += blockDim.x) {
+    float acc = 0.f;
+    for (int t = 0; t < L; t++) acc += __bfloat162float(src[(size_t)t * w + j]);
+    s_row[j] = acc / (float)L;
+  }
+  __syncthreads();
+  const int jj = threadIdx.x & 63, quarter = threadIdx.x >> 6;
+  const int j = j0 + jj;
+  const int per = (w + 3) / 4, i0 = quarter * per, i1 = min(w, i0 + per);
+  float acc0 = 0.f, acc1 = 0.f;
+  if (j < D) {
+    int i = i0;
+    for (; i + 1 < i1; i += 2) {
+      acc0 = fmaf(s_row[i], projT[(size_t)i * D + j], acc0);
+      acc1 = fmaf(s_row[i + 1], projT[(size_t)(i + 1) * D + j], acc1);
+    }
+    if (i < i1) acc0 = fmaf(s_row[i], projT[(size_t)i * D + j], acc0);
+  }
+  s_part[quarter * 64 + jj] = acc0 + acc1;
+  __syncthreads();
+  if (quarter == 0 && j < D) {
+    const float f = (s_part[jj] + s_part[64 + jj]) + (s_part[128 + jj] + s_part[192 + jj]);
+    feat[(size_t)b * D + j] = bias != nullptr ? f + bias[j] : f;
+  }
+}
+
+// clip_back.py normalized(): a / |a|, with |a| == 0 replaced by 1 (a zero row stays zero, never NaN).
+__global__ void __launch_bounds__(256)
+feat_normalized_cast_kernel(const float* __restrict__ feat, int D, void* __restrict__ out, int out_f16, int normalize) {
+  __shared__ float red[8];
+  const int b = blockIdx.x;
+  float part = 0.f;
+  for (int j = threadIdx.x; j < D; j += blockDim.x) {
+    const float v = feat[(size_t)b * D + j];
+    part += v * v;
+  }
+  float nrm = sqrtf(block_sum(part, red));
+  if (!normalize || nrm == 0.f) nrm = 1.f;
+  for (int j = threadIdx.x; j < D; j += blockDim.x) {
+    const float v = feat[(size_t)b * D + j] / nrm;
+    if (out_f16) reinterpret_cast<__half*>(out)[(size_t)b * D + j] = __float2half_rn(v);
+    else reinterpret_cast<float*>(out)[(size_t)b * D + j] = v;
+  }
+}
+
+int masked_mean_proj_norm(const __nv_bfloat16* x, int T, int w, const int* len, const float* projT, const float* bias,
+                          int D, float* feat, void* out, int out_f16, int normalize, int B, cudaStream_t st) {
+  if (B == 0) return B200_OK;
+  const size_t smem = (size_t)(w + 256) * sizeof(float);
+  B200_CHECK(smem <= 48 * 1024, B200_ERR_UNSUPPORTED, "masked_mean_proj: width %d too large", w);
+  masked_mean_proj_kernel<<<dim3((D + 63) / 64, B), 256, smem, st>>>(x, T, w, len, projT, bias, D, feat);
+  B200_LAUNCH_OK();
+  feat_normalized_cast_kernel<<<B, 256, 0, st>>>(feat, D, out, out_f16, normalize);
   B200_LAUNCH_OK();
   return B200_OK;
 }

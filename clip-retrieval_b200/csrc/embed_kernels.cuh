@@ -17,22 +17,39 @@ int text_embed(const int64_t* tokens, const __nv_bfloat16* tok_emb, const float*
 // rows of `w` bf16 elements, in_ld/out_ld in elements; in == out allowed.
 int layernorm_rows(const __nv_bfloat16* in, int64_t in_ld, __nv_bfloat16* out, int64_t out_ld, const float* gamma,
                    const float* beta, int64_t rows, int w, cudaStream_t st);
+// The same LayerNorm with the epsilon as an argument (BERT-family encoders carry it in their config: 1e-5, 1e-12).
+int layernorm_rows_eps(const __nv_bfloat16* in, int64_t in_ld, __nv_bfloat16* out, int64_t out_ld, const float* gamma,
+                       const float* beta, int64_t rows, int w, float eps, cudaStream_t st);
 // (mean, M2) per 64-column slot of every row of x [rows, w] (w % 64 == 0): seeds GemmEpilogue::ln_stats.
 int row_stats(const __nv_bfloat16* x, int64_t rows, int w, float2* stats, cudaStream_t st);
 // K4: multi-head attention over the fused qkv buffer [B*T, 3w] -> out [B*T, w]; causal for text.  mma.sync kernel
 // (attention.cu) for the head dimensions the wgmma kernel does not take (80, 96, 128).
-int attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int heads, int w, int causal, cudaStream_t st);
+// len (device int32 [B], values 1..T, or nullptr = T): sample b attends to its keys < len[b], and its rows >= len[b]
+// of `out` are zeros — the key-padding mask of a bidirectional encoder (both kernels).
+int attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int heads, int w, int causal, cudaStream_t st,
+              const int* len = nullptr);
 // K4 on wgmma (attention_wgmma.cu) for head dim 64, T <= 320: tmQKV is a 3-D map over the qkv buffer seen as
 // [samples >= B, T, 3w] (make_tmap_3d, row pitch 3w, plane pitch T * 3w) with boxes of 64 tokens x 64 columns (128B
 // swizzle); a box is clipped at token T of its sample, so keys and values past the end read as zeros.
 bool attention_wgmma_supported(int T, int heads, int w);
 int attention_wgmma(const CUtensorMap& tmQKV, __nv_bfloat16* out, int B, int T, int heads, int w, int causal,
-                    cudaStream_t st);
+                    cudaStream_t st, const int* len = nullptr);
 // K8/K10/K11: pooled row (x[b*T + pool_index(b)]) -> LN -> @ proj [w, D] -> optional L2 normalise
 // -> fp16 or fp32.  pool_idx == nullptr pools token 0 (vision); else row pool_idx[b] (text EOT).
 int pool_ln_proj_norm(const __nv_bfloat16* x, int T, int w, const int* pool_idx, const float* gamma, const float* beta,
                       const __nv_bfloat16* proj, int D, void* out, int out_f16, int normalize, int B, cudaStream_t st,
                       float* feat_scratch = nullptr);   // fp32 [B, D]: when given, the projection is split over D / 64 blocks per sample
+// BERT-family embedding: x[b*T + t, :] = LN_eps((word[ids[b,t]] + tt0) + pos[pos_off + t]) in fp32, stored bf16
+// (HF's order of additions; tt0 = token-type row 0, or nullptr when the model has no token types).  word bf16
+// [vocab, w]; tt0, pos, gamma, beta fp32.  Ids outside [0, vocab) are clamped.
+int encoder_embed(const int64_t* ids, const __nv_bfloat16* word, const float* tt0, const float* pos, int pos_off,
+                  const float* gamma, const float* beta, float eps, __nv_bfloat16* x, int B, int T, int w, int vocab,
+                  cudaStream_t st);
+// Masked mean pool + projection + normalise: m = (sum over t < len[b], ascending, of x[b*T + t, :] in fp32) / len[b];
+// f = m @ projT [w, D] fp32 (+ bias[D] fp32 | nullptr) into feat fp32 [B, D] (blocks of 64 output columns per
+// sample); out = f / (normalize ? (|f| == 0 ? 1 : |f|) : 1) as fp16 or fp32 (clip_back.py normalized()).
+int masked_mean_proj_norm(const __nv_bfloat16* x, int T, int w, const int* len, const float* projT, const float* bias,
+                          int D, float* feat, void* out, int out_f16, int normalize, int B, cudaStream_t st);
 // argmax(tokens, dim=-1) (first maximum) -> pool_idx[b]
 int token_argmax(const int64_t* tokens, int* pool_idx, int B, int T, cudaStream_t st);
 

@@ -6,12 +6,15 @@ carries `image_tensor` fp32 [B,3,S,S], `text_tokens` int [B,77], `image_filename
 `metadata`, with embeddings as np.float16 [B, D] arrays owned by Python (the writer keeps them
 until flush: writer.py:43-56).  H2D copy, forward, L2-normalise, fp16 cast and D2H copy happen
 inside one C-ABI call per modality (b200_clip_encode_image / b200_clip_encode_text).
+With `use_mclip=True` the captions go through the multilingual encoder of `mclip_model` instead (mclip.py), and
+`text_embs` are float32 normalized() rows as in the reference.
 
 Extension (SURVEY §8(f) row 1): when the batch carries `image_rgb8` (a list of decoded uint8 HWC
 images of any size — what a reader yields if its `preprocess` is `to_rgb8` instead of the torchvision
 transform) instead of `image_tensor`, Resize/CenterCrop/ToTensor/Normalize run on the GPU
 (`B200Preprocess`, bit-exact with the host transform) and feed the image tower in place.
 """
+from .mclip import build_mclip
 from .model import load_clip
 from .preprocess import B200Preprocess
 
@@ -35,11 +38,12 @@ class ClipMapper:
         self.enable_text = enable_text
         self.enable_metadata = enable_metadata
         self.use_mclip = use_mclip
+        self.mclip = None
         if use_mclip:
-            # reference: SentenceTransformer(mclip_model).encode on raw strings (mapper.py:44-47,62-63);
-            # a different model family on a CPU library — outside the B200 hot path (SURVEY.md §3.2).
-            raise NotImplementedError("use_mclip=True (M-CLIP / sentence_transformers) is outside the b200clip embed path")
-        del mclip_model
+            # reference: SentenceTransformer(mclip_model).encode on the raw captions, then normalized()
+            # (mapper.py:44-47,62-63): the text tower is replaced by the GPU encoder of that folder.  A name that is
+            # no known encoder and no local folder raises NotImplementedError before anything is loaded.
+            self.mclip = build_mclip(mclip_model, clip_cache_path, max_batch=max(int(warmup_batch_size), 32))
         self.device = "cuda"
         model, _, _ = load_clip(
             clip_model=clip_model,
@@ -67,7 +71,10 @@ class ClipMapper:
                 image_embs = self.model.embed_image(item["image_tensor"])
             image_filename = item["image_filename"]
         if self.enable_text:
-            text_embs = self.model.embed_text(item["text_tokens"])
+            if self.use_mclip:
+                text_embs = self.mclip.embed(item["text"])       # float32, as the reference's mclip path
+            else:
+                text_embs = self.model.embed_text(item["text_tokens"])
             text = item["text"]
         if self.enable_metadata:
             metadata = item["metadata"]

@@ -252,32 +252,8 @@ class B200Clip:
     # ---- weights ----
     def load_state_dict(self, sd):
         """sd: name -> torch tensor / numpy array (fp32 or fp16), OpenAI/open_clip key layout."""
-        torch = _torch()
-        views = (_lib.TensorViewC * len(sd))()
-        keep = []
-        n = 0
-        for name, t in sd.items():
-            if _is_torch(t):
-                t = t.detach().cpu()
-                if t.dtype not in (torch.float32, torch.float16):
-                    t = t.float()
-                a = t.contiguous().numpy()
-            else:
-                a = np.ascontiguousarray(t)
-                if a.dtype not in (np.float32, np.float16):
-                    a = a.astype(np.float32)
-            if a.ndim > 4:
-                continue
-            keep.append(a)
-            v = views[n]
-            v.name = name.encode()
-            v.data = a.ctypes.data
-            v.dtype = 0 if a.dtype == np.float32 else 1
-            v.ndim = a.ndim
-            for i, s in enumerate(a.shape):
-                v.shape[i] = s
-            n += 1
-        check(lib.b200_clip_load_weights(self._h, views, n), "clip_load_weights")
+        views, keep = _tensor_views(sd)
+        check(lib.b200_clip_load_weights(self._h, views, len(keep)), "clip_load_weights")
         return self
 
     # ---- reference model contract ----
@@ -358,6 +334,35 @@ class B200Clip:
 
 def _is_torch(x):
     return type(x).__module__.startswith("torch")
+
+
+def _tensor_views(sd):
+    """b200_tensor_view array over a state_dict (fp32 / fp16 host copies; tensors of more than 4 dimensions are
+    skipped) and the arrays it points into, which the caller keeps alive for the duration of the call."""
+    torch = _torch()
+    views = (_lib.TensorViewC * len(sd))()
+    keep = []
+    for name, t in sd.items():
+        if _is_torch(t):
+            t = t.detach().cpu()
+            if t.dtype not in (torch.float32, torch.float16):
+                t = t.float()
+            a = t.contiguous().numpy()
+        else:
+            a = np.ascontiguousarray(t)
+            if a.dtype not in (np.float32, np.float16):
+                a = a.astype(np.float32)
+        if a.ndim > 4:
+            continue
+        v = views[len(keep)]
+        keep.append(a)
+        v.name = name.encode()
+        v.data = a.ctypes.data
+        v.dtype = 0 if a.dtype == np.float32 else 1
+        v.ndim = a.ndim
+        for i, s in enumerate(a.shape):
+            v.shape[i] = s
+    return views, keep
 
 
 # ---- preprocess / tokenizer (returned by load_clip for signature parity; reader-side, CPU) ----------

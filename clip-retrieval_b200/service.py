@@ -24,8 +24,9 @@ class ClipResource:
 
     def __init__(self, model, tokenizer=None, preprocess=None, image_index=None, text_index=None, device=None,
                  metadata_provider=None, columns_to_return=None, safety_model=None, violence_detector=None,
-                 aesthetic_embeddings=None, ivf_old_to_new_mapping=None):
+                 aesthetic_embeddings=None, ivf_old_to_new_mapping=None, model_txt_mclip=None):
         self.model = model
+        self.model_txt_mclip = model_txt_mclip   # mclip.load_mclip(...) for use_mclip queries, or None
         self.tokenizer = tokenizer
         self.preprocess = preprocess
         self.image_index = image_index
@@ -48,13 +49,22 @@ class B200KnnService:
 
     # ---- compute_query (clip_back.py:207-255) -------------------------------------------------------
     def compute_query_device(self, clip_resource, text_input=None, image_input=None, embedding_input=None,
-                             text_tokens=None, aesthetic_score=None, aesthetic_weight=None):
+                             text_tokens=None, aesthetic_score=None, aesthetic_weight=None, use_mclip=False,
+                             mclip_tokens=None):
         """Normalised fp32 query [n, D] as a CUDA tensor.  `text_tokens` (int [n, 77]) bypasses the tokenizer
-        (benchmarks: no BPE vocabulary exists offline); `image_input` is a PIL image or a preprocessed tensor."""
+        (benchmarks: no BPE vocabulary exists offline); `image_input` is a PIL image or a preprocessed tensor.
+        `use_mclip`: the text goes through `clip_resource.model_txt_mclip` (clip_back.py:222-224); `mclip_tokens` =
+        (ids [n, T], lengths [n]) bypasses its tokenizer."""
         import torch
 
         model = clip_resource.model
-        if text_tokens is not None or (text_input is not None and text_input != ""):
+        if use_mclip and (mclip_tokens is not None or (text_input is not None and text_input != "")):
+            if clip_resource.model_txt_mclip is None:
+                raise ValueError("use_mclip=True but this ClipResource has no model_txt_mclip "
+                                 "(ClipResource(..., model_txt_mclip=load_mclip(clip_model)))")
+            texts = None if mclip_tokens is not None else ([text_input] if isinstance(text_input, str) else list(text_input))
+            q = clip_resource.model_txt_mclip.embed_device(texts, mclip_tokens)
+        elif text_tokens is not None or (text_input is not None and text_input != ""):
             if text_tokens is None:
                 text_tokens = clip_resource.tokenizer([text_input] if isinstance(text_input, str) else list(text_input))
             q = model.embed_text_device(torch.as_tensor(text_tokens).to(model.device), dtype=torch.float32)
@@ -78,12 +88,11 @@ class B200KnnService:
 
     def compute_query(self, clip_resource, text_input, image_input, image_url_input, embedding_input, use_mclip,
                       aesthetic_score, aesthetic_weight):
-        if use_mclip:
-            raise NotImplementedError("use_mclip=True (M-CLIP / sentence_transformers) is outside the b200clip embed path")
         if image_url_input is not None and image_input is None and (text_input is None or text_input == ""):
             raise NotImplementedError("image_url input needs network access (download_image, clip_back.py:238-239)")
         return self.compute_query_device(clip_resource, text_input, image_input, embedding_input,
-                                         aesthetic_score=aesthetic_score, aesthetic_weight=aesthetic_weight).cpu().numpy()
+                                         aesthetic_score=aesthetic_score, aesthetic_weight=aesthetic_weight,
+                                         use_mclip=use_mclip).cpu().numpy()
 
     # ---- post_filter (clip_back.py:326-341) on the device ----------------------------------------------
     def post_filter_device(self, safety_model, embeddings, deduplicate, use_safety_model, use_violence_detector,
@@ -177,16 +186,15 @@ class B200KnnService:
     def query(self, text_input=None, image_input=None, image_url_input=None, embedding_input=None, modality="image",
               num_images=100, num_result_ids=100, indice_name=None, use_mclip=False, deduplicate=True,
               use_safety_model=False, use_violence_detector=False, aesthetic_score=None, aesthetic_weight=None,
-              text_tokens=None):
-        if text_input is None and image_input is None and image_url_input is None and embedding_input is None and text_tokens is None:
+              text_tokens=None, mclip_tokens=None):
+        if (text_input is None and image_input is None and image_url_input is None and embedding_input is None
+                and text_tokens is None and mclip_tokens is None):
             raise ValueError("must fill one of text, image and image url input")
-        if use_mclip:
-            raise NotImplementedError("use_mclip=True (M-CLIP / sentence_transformers) is outside the b200clip embed path")
         if indice_name is None:
             indice_name = next(iter(self.clip_resources.keys()))
         clip_resource = self.clip_resources[indice_name]
         query = self.compute_query_device(clip_resource, text_input, image_input, embedding_input, text_tokens,
-                                          aesthetic_score, aesthetic_weight)
+                                          aesthetic_score, aesthetic_weight, use_mclip, mclip_tokens)
         distances, indices = self.knn_search(query, modality=modality, num_result_ids=num_result_ids,
                                              clip_resource=clip_resource, deduplicate=deduplicate,
                                              use_safety_model=use_safety_model, use_violence_detector=use_violence_detector)

@@ -309,6 +309,62 @@ int b200_layernorm_bf16_device(const void* d_in, void* d_out, const float* d_gam
                                int64_t rows, int w, int device, void* stream);
 int b200_attention_bf16_device(const void* d_qkv, void* d_out, int B, int T, int heads, int w, int causal,
                                int device, void* stream);
+/* ------------------------------------------------------------------------------------------
+ * Multilingual text towers (use_mclip).  Replaces the M-CLIP text model of the query service
+ * (clip_back.py:222-224,836-859: XLM-RoBERTa-Large + mean pool + LinearTransformation) and the
+ * SentenceTransformer of the mapper (mapper.py:44-47,62-63: DistilBERT + mean pool + Dense), each
+ * followed by normalized().  A BERT-family encoder: bidirectional attention under a key-padding mask,
+ * post-LayerNorm blocks, erf GELU, masked mean pooling, a linear projection.  Head dimension 64.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct b200_text_encoder b200_text_encoder;
+
+typedef struct b200_text_encoder_config {
+  int32_t layers, width, heads, ffn;
+  int32_t vocab_size;
+  int32_t max_positions;     /* rows of the position table */
+  int32_t type_vocab_size;   /* rows of the token-type table; 0 = the model has none (DistilBERT) */
+  int32_t position_offset;   /* position id of token t is position_offset + t (XLM-R: pad_token_id + 1 = 2) */
+  float   layer_norm_eps;    /* from the model config (XLM-R-Large 1e-5, DistilBERT 1e-12) */
+  int32_t out_dim;           /* projection output dimension */
+  int32_t proj_bias;         /* 1: the projection has a bias */
+  int32_t max_batch;         /* samples per forward (larger calls run in chunks) */
+  int32_t max_tokens;        /* longest T of a call (<= 512, position_offset + max_tokens <= max_positions) */
+} b200_text_encoder_config;
+
+int b200_text_encoder_create(const b200_text_encoder_config* cfg, int device, b200_text_encoder** out);
+int b200_text_encoder_destroy(b200_text_encoder* m);
+/* Weights in the HuggingFace BERT / XLM-RoBERTa key layout without a model prefix:
+ * embeddings.{word,position,token_type}_embeddings.weight, embeddings.LayerNorm.{weight,bias},
+ * encoder.layer.N.attention.self.{query,key,value}.{weight,bias}, encoder.layer.N.attention.output.dense.*,
+ * encoder.layer.N.attention.output.LayerNorm.*, encoder.layer.N.intermediate.dense.*, encoder.layer.N.output.dense.*,
+ * encoder.layer.N.output.LayerNorm.*, and projection.weight [out_dim, width] (+ projection.bias).  Only row 0 of
+ * the token-type table is used.  Missing or mis-shaped tensors are an error. */
+int b200_text_encoder_load_weights(b200_text_encoder* m, const b200_tensor_view* tensors, int n);
+/* d_ids int64 [B, T] right-padded, d_len int32 [B] with values 1..T (tokens of each sample; the others are never
+ * attended to nor pooled).  d_out [B, out_dim] fp16 or fp32; normalize: 0 raw projected features, 1 normalized()
+ * (a / |a|, a zero row stays zero).  Asynchronous on `stream`. */
+int b200_text_encoder_encode_device(b200_text_encoder* m, const int64_t* d_ids, const int32_t* d_len, int B, int T,
+                                    void* d_out, int out_dtype, int normalize, void* stream);
+/* Host-buffer variant (lengths checked on the host); returns after the result is in h_out. */
+int b200_text_encoder_encode(b200_text_encoder* m, const int64_t* h_ids, const int32_t* h_len, int B, int T,
+                             void* h_out, int out_dtype, int normalize);
+/* Per-kernel-class device time of the encode calls since profiling was switched on or since the previous read:
+ * ms_by_class[4] = gemm, attention, layernorm, other (embedding, pooling); *launches = kernels of the last call. */
+int b200_text_encoder_last_timing(b200_text_encoder* m, float* ms_by_class, int* launches);
+int b200_text_encoder_set_profiling(b200_text_encoder* m, int on);
+
+/* Stand-alone entries of the encoder kernels, for their parity tests: LayerNorm with an explicit epsilon;
+ * non-causal attention where sample b sees its keys < d_len[b] (int32, 1..T) and its rows >= d_len[b] are zeros;
+ * the embedding x = LN_eps((word[id] + tt0) + pos[position_offset + t]) (d_word bf16 [vocab, w], d_tt0 fp32 [w] or
+ * NULL, d_pos fp32, output bf16 [B*T, w]). */
+int b200_layernorm_eps_bf16_device(const void* d_in, void* d_out, const float* d_gamma, const float* d_beta,
+                                   int64_t rows, int w, float eps, int device, void* stream);
+int b200_attention_len_bf16_device(const void* d_qkv, const int32_t* d_len, void* d_out, int B, int T, int heads,
+                                   int w, int device, void* stream);
+int b200_encoder_embed_bf16_device(const int64_t* d_ids, const void* d_word, const float* d_tt0, const float* d_pos,
+                                   int position_offset, const float* d_gamma, const float* d_beta, float eps,
+                                   void* d_out, int B, int T, int w, int vocab, int device, void* stream);
+
 /* ---- image transform in front of the embed path (SURVEY §8(f) row 1) ----------------------------
  * Replaces `preprocess(PIL.Image)` as the reference calls it per image on the host
  * (clip_retrieval/clip_inference/reader.py:98-106,158-165; the object `load_clip` returns,
