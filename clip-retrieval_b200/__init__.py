@@ -9,7 +9,9 @@ Everything numeric runs in the CUDA library `lib/libb200clip.so` (C ABI in inclu
 there is no CPU fallback: importing works without a GPU, calling compute without one raises.
 """
 from ._lib import lib, B200Error, library_path, launch_count  # noqa: F401
-from .index import B200FlatIndex, B200IVFFlatIndex, B200IVFPQIndex, SynthSpec, load_index, merge_shard_results, merge_packed_results, train_kmeans, build_ivf_index, train_pq, train_ivfpq, build_ivfpq_index  # noqa: F401
+from .index import B200FlatIndex, B200IVFFlatIndex, B200IVFPQIndex, SynthSpec, load_index, merge_shard_results, merge_packed_results, train_kmeans, build_ivf_index, train_pq, train_ivfpq, build_ivfpq_index, train_opq  # noqa: F401
+from .clip_index import clip_index, build_index, parse_index_key, default_index_key, default_nprobe  # noqa: F401
+from .faiss_io import write_index  # noqa: F401
 
 from .model import B200Clip, ClipArch, Tower, ARCHS, load_clip, synthetic_state_dict, convert_hf_state_dict  # noqa: F401,E402
 from .preprocess import B200Preprocess, to_rgb8  # noqa: F401,E402
@@ -23,6 +25,7 @@ __all__ = [
     "B200Clip", "ClipArch", "Tower", "ARCHS", "load_clip", "synthetic_state_dict", "convert_hf_state_dict", "ClipMapper", "get_non_uniques", "get_violent_items", "dedup_mask", "H14NsfwDetector", "get_unsafe_items", "B200Preprocess", "to_rgb8", "B200KnnService", "ClipResource", "MicroBatcher", "ShardedIndex", "B200ShardedIndex", "shard_range",
     "lib", "B200Error", "library_path", "launch_count",
     "B200FlatIndex", "B200IVFFlatIndex", "B200IVFPQIndex", "SynthSpec", "load_index", "merge_shard_results", "train_kmeans", "build_ivf_index",
-    "train_pq", "train_ivfpq", "build_ivfpq_index",
+    "train_pq", "train_ivfpq", "build_ivfpq_index", "train_opq", "clip_index", "build_index", "parse_index_key",
+    "default_index_key", "default_nprobe", "write_index",
     "B200TextEncoder", "EncoderArch", "MCLIP_ARCHS", "MclipTextModel", "load_mclip",
 ]

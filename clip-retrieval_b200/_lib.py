@@ -117,6 +117,12 @@ PROTOTYPES = {
     "b200_index_pq_m": (_i, [_vp]),
     "b200_index_encode_device": (_i, [_vp, _vp, _i64, _vp, _vp, _vp, _vp]),
     "b200_pq_train_f32": (_i, [_vp, _i64, _i, _i, _i, C.c_uint64, _vp, _vp, _i]),
+    "b200_opq_train_f32": (_i, [_vp, _i64, _i, _i, _i, _i, _i, _i, C.c_uint64, _vp, _vp, _vp, _i]),
+    "b200_rows_pretransform_device": (_i, [_vp, _i64, _i, _vp, _vp, _i, _vp, _i, _i, _vp]),
+    "b200_opq_cross_f32_device": (_i, [_vp, _i64, _i, _vp, _vp, _i, _i, _vp, _i, _vp]),
+    "b200_opq_polar_f32_device": (_i, [_vp, _i, _i, _vp, _i, _vp]),
+    "b200_index_get_quantizer": (_i, [_vp, _vp, _vp, _vp, _vp, _vp]),
+    "b200_index_copy_rows": (_i, [_vp, _i64, _i64, _vp, _vp]),
     "b200_index_destroy": (_i, [_vp]),
     "b200_index_reserve": (_i, [_vp, _i64]),
     "b200_index_add_f16": (_i, [_vp, _vp, _i64, _i]),

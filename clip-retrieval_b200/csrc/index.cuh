@@ -173,6 +173,17 @@ int ivfpq_range_scan(b200_index* idx, const float* d_q, float thresh, unsigned l
 int ivfpq_decode(b200_index* idx, const unsigned long long* keys, const int64_t* ids, int64_t count, float* d_R,
                  cudaStream_t st);
 
+// ---- pq_encode.cu: the PQ pieces OPQ training (opq_train.cu) reuses ---------------------------------------
+// Y [n, d] = X [n, d_in] A^T (+ b): the row pre-transform of encode.
+int pq_pretransform(const float* X, int64_t n, int d_in, const float* A, const float* b, int d, float* Y, cudaStream_t st);
+// codes [n, M] of rows X [n, d] against the codebook (no residual).
+int pq_codes(const float* X, int64_t n, int d, int M, const float* cb, uint8_t* codes, cudaStream_t st);
+// Initial codebook [M, 256, d / M] of b200_pq_train_f32: sub-vectors of one seeded pick per stride of the rows.
+int pq_init_codebook(const float* d_x, int64_t n, int d, int M, uint64_t seed, float* cb);
+// The Lloyd iterations of b200_pq_train_f32, started from the device codebook `cb` (updated in place).
+// codes_out (device [n, M] or null) receives the codes of the final codebook; h_sizes [M, 256] (or null) its sizes.
+int pq_train_loop(const float* d_x, int64_t n, int d, int M, int niter, float* cb, uint8_t* codes_out, int64_t* h_sizes);
+
 // ---- knn_index.cu -----------------------------------------------------------------------------------------
 // packed per-shard blocks [I int64 nq*k | D f32 nq*k | padding], `stride` bytes apart (sharded.cu, sharded.py)
 int merge_packed_launch(const void* d_gathered, int G, size_t stride, int nq, int k, float* d_D, int64_t* d_I,

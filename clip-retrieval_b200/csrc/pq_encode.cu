@@ -25,9 +25,10 @@ constexpr int64_t PE_CHUNK = 32768;   // rows per encode chunk: bounds the scrat
 
 // ---- (1) row pre-transform: Y[n, d] = X[n, d_in] A^T (+ b), 64 x 64 tiles, 4 x 4 per thread ---------------------
 constexpr int PT_T = 64, PT_K = 16;
+template <typename OutT>   // float (encode) or __half (training rows a caller keeps in fp16)
 __global__ void __launch_bounds__(256)
 pq_rows_pretransform_kernel(const float* __restrict__ X, int64_t n, int d_in, const float* __restrict__ A,
-                            const float* __restrict__ b, int d, float* __restrict__ Y) {
+                            const float* __restrict__ b, int d, OutT* __restrict__ Y) {
   __shared__ float sx[PT_K][PT_T + 1], sa[PT_K][PT_T + 1];
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   const int i0 = blockIdx.x * PT_T;
@@ -58,7 +59,7 @@ pq_rows_pretransform_kernel(const float* __restrict__ X, int64_t n, int d_in, co
     for (int v = 0; v < 4; v++) {
       const int64_t r = r0 + ty + 16 * u;
       const int i = i0 + tx + 16 * v;
-      if (r < n && i < d) Y[r * d + i] = b ? acc[u][v] + b[i] : acc[u][v];
+      if (r < n && i < d) Y[r * d + i] = (OutT)(b ? acc[u][v] + b[i] : acc[u][v]);
     }
 }
 
@@ -299,24 +300,43 @@ static int launch_code(const float* X, int64_t n, int d, int M, const float* cb,
   return B200_OK;
 }
 
-}  // namespace b200
+int pq_codes(const float* X, int64_t n, int d, int M, const float* cb, uint8_t* codes, cudaStream_t st) {
+  return launch_code(X, n, d, M, cb, nullptr, nullptr, nullptr, codes, st);
+}
 
-using namespace b200;
+int pq_pretransform(const float* X, int64_t n, int d_in, const float* A, const float* b, int d, float* Y, cudaStream_t st) {
+  if (n == 0) return B200_OK;
+  pq_rows_pretransform_kernel<float><<<dim3((d + PT_T - 1) / PT_T, (unsigned)((n + PT_T - 1) / PT_T)), 256, 0, st>>>(
+      X, n, d_in, A, b, d, Y);
+  B200_LAUNCH_OK();
+  return B200_OK;
+}
 
-extern "C" {
+int pq_init_codebook(const float* d_x, int64_t n, int d, int M, uint64_t seed, float* cb) {
+  // one seeded pick inside each of 256 equal strides of the rows (oracle/kmeans_ref.initial_picks)
+  std::vector<int64_t> pick(PE_KSUB);
+  for (int i = 0; i < PE_KSUB; i++) {
+    const int64_t lo = (int64_t)(((__int128)i * n) / PE_KSUB), hi = (int64_t)(((__int128)(i + 1) * n) / PE_KSUB);
+    const uint64_t span = (uint64_t)std::max<int64_t>(1, hi - lo);
+    pick[i] = lo + (int64_t)(pq_mix(seed ^ ((uint64_t)i * 0xD1342543DE82EF95ull)) % span);
+  }
+  int64_t* d_pick = nullptr;
+  B200_CUDA(cudaMalloc((void**)&d_pick, PE_KSUB * 8));
+  int rc = [&]() -> int {
+    B200_CUDA(cudaMemcpy(d_pick, pick.data(), PE_KSUB * 8, cudaMemcpyHostToDevice));
+    pq_gather_kernel<<<(unsigned)(((int64_t)PE_KSUB * d + 255) / 256), 256>>>(d_x, d, d / M, d_pick, cb);
+    B200_LAUNCH_OK();
+    return B200_OK;
+  }();
+  cudaDeviceSynchronize();
+  cudaFree(d_pick);
+  return rc;
+}
 
-int b200_pq_train_f32(const float* d_x, int64_t n, int d, int M, int niter, uint64_t seed, float* h_codebook,
-                      int64_t* h_sizes, int device) {
-  B200_CHECK(d_x && h_codebook, B200_ERR_INVALID, "pq_train: null argument");
-  B200_CHECK(d >= 1 && M >= 1 && M <= d && d % M == 0, B200_ERR_INVALID, "pq_train: M=%d must divide d=%d", M, d);
-  B200_CHECK(n >= PE_KSUB, B200_ERR_INVALID, "pq_train: n=%lld training rows; 256 codewords need at least 256",
-             (long long)n);
-  B200_CHECK((int64_t)M * n < (1ll << 31) && niter >= 0, B200_ERR_INVALID,
-             "pq_train: M * n = %lld must stay below 2^31 (niter=%d)", (long long)M * n, niter);
-  DeviceGuard g(device);
+int pq_train_loop(const float* d_x, int64_t n, int d, int M, int niter, float* cb, uint8_t* codes_out, int64_t* h_sizes) {
   const int dsub = d / M, nb = M * PE_KSUB;
   const int64_t count = (int64_t)M * n;
-  float* cb = nullptr; int64_t *d_pick = nullptr, *d_off = nullptr; uint8_t* codes = nullptr;
+  int64_t* d_off = nullptr; uint8_t* codes = codes_out;
   uint32_t *keys = nullptr, *keys2 = nullptr, *rows = nullptr, *rows2 = nullptr;
   int* d_splits = nullptr;
   void* tmp = nullptr;
@@ -327,25 +347,13 @@ int b200_pq_train_f32(const float* d_x, int64_t n, int d, int M, int niter, uint
     return B200_OK;
   };
   int rc = [&]() -> int {
-    B200_TRY(alloc((void**)&cb, (size_t)PE_KSUB * d * 4));
-    B200_TRY(alloc((void**)&d_pick, PE_KSUB * 8));
     B200_TRY(alloc((void**)&d_off, (size_t)(nb + 1) * 8));
-    B200_TRY(alloc((void**)&codes, (size_t)count));
+    if (!codes) B200_TRY(alloc((void**)&codes, (size_t)count));
     B200_TRY(alloc((void**)&keys, (size_t)count * 4));
     B200_TRY(alloc((void**)&keys2, (size_t)count * 4));
     B200_TRY(alloc((void**)&rows, (size_t)count * 4));
     B200_TRY(alloc((void**)&rows2, (size_t)count * 4));
     B200_TRY(alloc((void**)&d_splits, (size_t)nb * 3 * 4));
-    // initial codewords: one seeded pick inside each of 256 equal strides of the rows (oracle/kmeans_ref.initial_picks)
-    std::vector<int64_t> pick(PE_KSUB);
-    for (int i = 0; i < PE_KSUB; i++) {
-      const int64_t lo = (int64_t)(((__int128)i * n) / PE_KSUB), hi = (int64_t)(((__int128)(i + 1) * n) / PE_KSUB);
-      const uint64_t span = (uint64_t)std::max<int64_t>(1, hi - lo);
-      pick[i] = lo + (int64_t)(pq_mix(seed ^ ((uint64_t)i * 0xD1342543DE82EF95ull)) % span);
-    }
-    B200_CUDA(cudaMemcpy(d_pick, pick.data(), PE_KSUB * 8, cudaMemcpyHostToDevice));
-    pq_gather_kernel<<<(unsigned)(((int64_t)PE_KSUB * d + 255) / 256), 256>>>(d_x, d, dsub, d_pick, cb);
-    B200_LAUNCH_OK();
     int bits = 1;
     while ((1ll << bits) < nb) bits++;
     size_t tmp_bytes = 0;
@@ -363,7 +371,7 @@ int b200_pq_train_f32(const float* d_x, int64_t n, int d, int M, int niter, uint
       pq_offsets_kernel<<<(nb + 1 + 255) / 256, 256>>>(keys2, count, nb, d_off);
       B200_LAUNCH_OK();
       B200_CUDA(cudaMemcpy(off.data(), d_off, (size_t)(nb + 1) * 8, cudaMemcpyDeviceToHost));
-      if (it == niter) break;   // the last round only refreshes the sizes of the final codewords
+      if (it == niter) break;   // the last round only refreshes the codes and sizes of the final codewords
       pq_update_kernel<<<nb, ublock>>>(d_x, d, dsub, rows2, d_off, cb);
       B200_LAUNCH_OK();
       // empty codewords: per m, split the (currently) largest one, ties to the lower id; sizes halve as in FAISS
@@ -388,7 +396,6 @@ int b200_pq_train_f32(const float* d_x, int64_t n, int d, int M, int niter, uint
         B200_LAUNCH_OK();
       }
     }
-    B200_CUDA(cudaMemcpy(h_codebook, cb, (size_t)PE_KSUB * d * 4, cudaMemcpyDeviceToHost));
     if (h_sizes)
       for (int b = 0; b < nb; b++) h_sizes[b] = off[b + 1] - off[b];
     return B200_OK;
@@ -396,6 +403,51 @@ int b200_pq_train_f32(const float* d_x, int64_t n, int d, int M, int niter, uint
   cudaDeviceSynchronize();
   for (void* p : frees) cudaFree(p);
   return rc;
+}
+
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+int b200_pq_train_f32(const float* d_x, int64_t n, int d, int M, int niter, uint64_t seed, float* h_codebook,
+                      int64_t* h_sizes, int device) {
+  B200_CHECK(d_x && h_codebook, B200_ERR_INVALID, "pq_train: null argument");
+  B200_CHECK(d >= 1 && M >= 1 && M <= d && d % M == 0, B200_ERR_INVALID, "pq_train: M=%d must divide d=%d", M, d);
+  B200_CHECK(n >= PE_KSUB, B200_ERR_INVALID, "pq_train: n=%lld training rows; 256 codewords need at least 256",
+             (long long)n);
+  B200_CHECK((int64_t)M * n < (1ll << 31) && niter >= 0, B200_ERR_INVALID,
+             "pq_train: M * n = %lld must stay below 2^31 (niter=%d)", (long long)M * n, niter);
+  DeviceGuard g(device);
+  float* cb = nullptr;
+  B200_CUDA(cudaMalloc((void**)&cb, (size_t)PE_KSUB * d * 4));
+  int rc = [&]() -> int {
+    B200_TRY(pq_init_codebook(d_x, n, d, M, seed, cb));
+    B200_TRY(pq_train_loop(d_x, n, d, M, niter, cb, nullptr, h_sizes));
+    B200_CUDA(cudaMemcpy(h_codebook, cb, (size_t)PE_KSUB * d * 4, cudaMemcpyDeviceToHost));
+    return B200_OK;
+  }();
+  cudaDeviceSynchronize();
+  cudaFree(cb);
+  return rc;
+}
+
+int b200_rows_pretransform_device(const float* d_x, int64_t n, int d_in, const float* d_A, const float* d_b, int d_out,
+                                  void* d_y, int out_fp16, int device, void* stream) {
+  B200_CHECK(n >= 0 && (n == 0 || (d_x && d_A && d_y)) && d_in >= 1 && d_out >= 1, B200_ERR_INVALID,
+             "rows_pretransform: bad argument");
+  B200_CHECK(n < (1ll << 31) * PT_T, B200_ERR_INVALID, "rows_pretransform: n=%lld rows in one call", (long long)n);
+  if (n == 0) return B200_OK;
+  DeviceGuard g(device);
+  cudaStream_t st = (cudaStream_t)stream;
+  const dim3 grid((d_out + PT_T - 1) / PT_T, (unsigned)((n + PT_T - 1) / PT_T));
+  if (out_fp16)
+    pq_rows_pretransform_kernel<__half><<<grid, 256, 0, st>>>(d_x, n, d_in, d_A, d_b, d_out, (__half*)d_y);
+  else
+    pq_rows_pretransform_kernel<float><<<grid, 256, 0, st>>>(d_x, n, d_in, d_A, d_b, d_out, (float*)d_y);
+  B200_LAUNCH_OK();
+  return B200_OK;
 }
 
 int b200_index_encode_device(b200_index* idx, const float* d_x, int64_t n, int32_t* d_lists, float* d_residuals,
@@ -420,7 +472,7 @@ int b200_index_encode_device(b200_index* idx, const float* d_x, int64_t n, int32
       const float* x = d_x + r0 * d_in;
       if (idx->pt_A) {
         float* xt = reinterpret_cast<float*>(scratch);
-        pq_rows_pretransform_kernel<<<dim3((d + PT_T - 1) / PT_T, (unsigned)((m_ + PT_T - 1) / PT_T)), 256, 0, st>>>(
+        pq_rows_pretransform_kernel<float><<<dim3((d + PT_T - 1) / PT_T, (unsigned)((m_ + PT_T - 1) / PT_T)), 256, 0, st>>>(
             x, m_, d_in, idx->pt_A, idx->pt_b, d, xt);
         B200_LAUNCH_OK();
         x = xt;

@@ -1,10 +1,10 @@
-"""Reader (and a minimal writer) of FAISS index files for `load_index` (clip_retrieval/clip_back.py:589-596 reads
+"""Reader and writer of FAISS index files for `load_index` and `clip_index` (clip_retrieval/clip_back.py:589-596 reads
 `image.index` / `text.index` with `faiss.read_index`).
 
 FAISS is not installable offline and /root/reference holds no index file, so this module restates the published
 serialisation of faiss/impl/index_write.cpp / index_read.cpp (faiss-cpu >= 1.7.2, requirements.txt:8) from its
-documented layout; it is UNVERIFIED against files written by FAISS itself — the tests round-trip this module's
-own writer.  Supported (inner-product metric only — the reference builds `metric_type="ip"` indices):
+documented layout; it is UNVERIFIED against FAISS itself, in both directions — the tests round-trip this module's
+own writers (`write_index` for a built index, the array writers below for test fixtures).  Supported (inner-product metric only — the reference builds `metric_type="ip"` indices):
     IxFI / IxF2 / IxFl   IndexFlat                      -> rows fp32
     IxSQ                 IndexScalarQuantizer, QT_fp16  -> rows fp16
     IwFl                 IndexIVFFlat (ArrayInvertedLists)
@@ -258,7 +258,22 @@ def looks_like_faiss_index(path):
     return len(head) == 4 and head[:2] in (b"Ix", b"Iw", b"IH", b"Ib", b"IB", b"IR", b"I2", b"IL")
 
 
-# ---- writer (fixtures for the tests; the same layout) -----------------------------------------------------
+# ---- writer: the same layout; the fixture writers (numpy arrays, for the tests) and write_index (a built index)
+# share every record helper below --------------------------------------------------------------------------------
+class _FileSink:
+    """What the record helpers append to when writing straight to a file (the fixture writers collect a list)."""
+
+    def __init__(self, f):
+        self.f = f
+
+    def append(self, b):
+        self.f.write(b)
+
+
+def _w_fourcc(out, tag):
+    out.append(struct.pack("<I", _fourcc(tag)))
+
+
 def _w_header(out, d, ntotal, metric):
     out.append(struct.pack("<iqqqBi", d, ntotal, 1 << 20, 1 << 20, 1, metric))
 
@@ -269,21 +284,88 @@ def _w_vec(out, a):
     out.append(a.tobytes())
 
 
+def _w_sq_fp16(out, d):
+    """ScalarQuantizer QT_fp16 of width d (no trained parameters)."""
+    out.append(struct.pack("<iifQQ", QT_FP16, 0, 0.0, d, 2 * d))
+    _w_vec(out, np.zeros(0, np.float32))
+
+
+def _w_flat_quantizer(out, centroids):
+    """The coarse quantiser as an IndexFlatIP (IxFI) over the centroids."""
+    nlist, d = centroids.shape
+    _w_fourcc(out, "IxFI")
+    _w_header(out, d, nlist, METRIC_INNER_PRODUCT)
+    _w_vec(out, np.ascontiguousarray(centroids, dtype=np.float32).reshape(-1))
+
+
+def _w_ivf_head(out, tag, d, n, nprobe, centroids, hnsw=False):
+    """IndexIVF common part: header, nlist / nprobe, coarse quantiser, an empty direct map."""
+    _w_fourcc(out, tag)
+    _w_header(out, d, n, METRIC_INNER_PRODUCT)
+    out.append(struct.pack("<QQ", centroids.shape[0], nprobe))
+    if hnsw:
+        _w_hnsw_flat(out, centroids)
+    else:
+        _w_flat_quantizer(out, centroids)
+    out.append(struct.pack("<b", 0))
+    _w_vec(out, np.zeros(0, np.int64))
+
+
+def _w_pretransform(out, A, b, n, tag="LTra"):
+    """IndexPreTransform head with one LinearTransform (A [d_out, d_in], b [d_out] or None); the sub-index follows."""
+    A = np.ascontiguousarray(A, dtype=np.float32)
+    _w_fourcc(out, "IxPT")
+    _w_header(out, A.shape[1], n, METRIC_INNER_PRODUCT)
+    out.append(struct.pack("<i", 1))
+    out.append(struct.pack("<IB", _fourcc(tag), 0 if b is None else 1))
+    _w_vec(out, A.reshape(-1))
+    _w_vec(out, np.zeros(0, np.float32) if b is None else np.asarray(b, np.float32))
+    out.append(struct.pack("<iiB", A.shape[1], A.shape[0], 1))
+
+
+def _w_invlists_head(out, nlist, code_size, sizes, sparse_sizes=False):
+    """ArrayInvertedLists up to the list contents (then per non-empty list: its codes, then its int64 ids)."""
+    sizes = np.asarray(sizes).astype(np.uint64)
+    out.append(struct.pack("<I", _fourcc("ilar")))
+    out.append(struct.pack("<QQ", nlist, code_size))
+    if sparse_sizes:
+        out.append(struct.pack("<I", _fourcc("sprs")))
+        nz = np.nonzero(sizes)[0]
+        _w_vec(out, np.stack([nz.astype(np.uint64), sizes[nz]], axis=1).reshape(-1))
+    else:
+        out.append(struct.pack("<I", _fourcc("full")))
+        _w_vec(out, sizes)
+
+
+def _w_invlists(out, nlist, code_size, codes, ids, assign, sparse_sizes):
+    assign = np.asarray(assign, dtype=np.int64)
+    sizes = np.bincount(assign, minlength=nlist).astype(np.uint64)
+    _w_invlists_head(out, nlist, code_size, sizes, sparse_sizes)
+    order = np.argsort(assign, kind="stable")
+    off = 0
+    for l in range(nlist):
+        m = int(sizes[l])
+        if m:
+            sel = order[off:off + m]
+            out.append(codes[sel].tobytes())
+            out.append(ids[sel].tobytes())
+            off += m
+
+
 def write_flat(path, rows, metric=METRIC_INNER_PRODUCT, fp16=False, id_map=None):
     rows = np.ascontiguousarray(rows, dtype=np.float16 if fp16 else np.float32)
     n, d = rows.shape
     out = []
     if id_map is not None:
-        out.append(struct.pack("<I", _fourcc("IxMp")))
+        _w_fourcc(out, "IxMp")
         _w_header(out, d, n, metric)
     if fp16:
-        out.append(struct.pack("<I", _fourcc("IxSQ")))
+        _w_fourcc(out, "IxSQ")
         _w_header(out, d, n, metric)
-        out.append(struct.pack("<iifQQ", QT_FP16, 0, 0.0, d, 2 * d))
-        _w_vec(out, np.zeros(0, np.float32))
+        _w_sq_fp16(out, d)
         _w_vec(out, rows.view(np.uint8).reshape(-1))
     else:
-        out.append(struct.pack("<I", _fourcc({0: "IxFI", 1: "IxF2"}.get(metric, "IxFl"))))
+        _w_fourcc(out, {0: "IxFI", 1: "IxF2"}.get(metric, "IxFl"))
         _w_header(out, d, n, metric)
         _w_vec(out, rows.reshape(-1))
     if id_map is not None:
@@ -298,65 +380,16 @@ def write_ivfflat(path, centroids, rows, assign, ids=None, nprobe=1, fp16=False,
     nlist, d = centroids.shape
     n = rows.shape[0]
     ids = np.arange(n, dtype=np.int64) if ids is None else np.asarray(ids, dtype=np.int64)
-    out = [struct.pack("<I", _fourcc("IwSq" if fp16 else "IwFl"))]
-    _w_header(out, d, n, METRIC_INNER_PRODUCT)
-    out.append(struct.pack("<QQ", nlist, nprobe))
-    out.append(struct.pack("<I", _fourcc("IxFI")))
-    _w_header(out, d, nlist, METRIC_INNER_PRODUCT)
-    _w_vec(out, centroids.reshape(-1))
-    out.append(struct.pack("<b", 0))
-    _w_vec(out, np.zeros(0, np.int64))
+    out = []
+    _w_ivf_head(out, "IwSq" if fp16 else "IwFl", d, n, nprobe, centroids)
     if fp16:
-        out.append(struct.pack("<iifQQ", QT_FP16, 0, 0.0, d, 2 * d))
-        _w_vec(out, np.zeros(0, np.float32))
+        _w_sq_fp16(out, d)
         out.append(struct.pack("<QB", 2 * d, 0))
     else:
         out.append(struct.pack("<Q", 4 * d))
-    out.append(struct.pack("<I", _fourcc("ilar")))
-    out.append(struct.pack("<QQ", nlist, rows.dtype.itemsize * d))
-    assign = np.asarray(assign, dtype=np.int64)
-    sizes = np.bincount(assign, minlength=nlist).astype(np.uint64)
-    if sparse_sizes:
-        out.append(struct.pack("<I", _fourcc("sprs")))
-        nz = np.nonzero(sizes)[0]
-        _w_vec(out, np.stack([nz.astype(np.uint64), sizes[nz]], axis=1).reshape(-1))
-    else:
-        out.append(struct.pack("<I", _fourcc("full")))
-        _w_vec(out, sizes)
-    order = np.argsort(assign, kind="stable")
-    off = 0
-    for l in range(nlist):
-        m = int(sizes[l])
-        if m:
-            sel = order[off:off + m]
-            out.append(rows[sel].tobytes())
-            out.append(ids[sel].tobytes())
-            off += m
+    _w_invlists(out, nlist, rows.dtype.itemsize * d, rows, ids, assign, sparse_sizes)
     with open(path, "wb") as f:
         f.write(b"".join(out))
-
-
-def _w_invlists(out, nlist, code_size, codes, ids, assign, sparse_sizes):
-    out.append(struct.pack("<I", _fourcc("ilar")))
-    out.append(struct.pack("<QQ", nlist, code_size))
-    assign = np.asarray(assign, dtype=np.int64)
-    sizes = np.bincount(assign, minlength=nlist).astype(np.uint64)
-    if sparse_sizes:
-        out.append(struct.pack("<I", _fourcc("sprs")))
-        nz = np.nonzero(sizes)[0]
-        _w_vec(out, np.stack([nz.astype(np.uint64), sizes[nz]], axis=1).reshape(-1))
-    else:
-        out.append(struct.pack("<I", _fourcc("full")))
-        _w_vec(out, sizes)
-    order = np.argsort(assign, kind="stable")
-    off = 0
-    for l in range(nlist):
-        m = int(sizes[l])
-        if m:
-            sel = order[off:off + m]
-            out.append(codes[sel].tobytes())
-            out.append(ids[sel].tobytes())
-            off += m
 
 
 def _w_hnsw_flat(out, centroids):
@@ -370,9 +403,14 @@ def _w_hnsw_flat(out, centroids):
     _w_vec(out, (np.arange(nlist + 1) * 64).astype(np.uint64))      # offsets
     _w_vec(out, np.full(nlist * 64, -1, np.int32))                  # neighbors
     out.append(struct.pack("<iiiii", 0, 0, 40, 16, 1))              # entry_point, max_level, efConstruction, efSearch, upper_beam
-    out.append(struct.pack("<I", _fourcc("IxFI")))
-    _w_header(out, d, nlist, METRIC_INNER_PRODUCT)
-    _w_vec(out, centroids.reshape(-1))
+    _w_flat_quantizer(out, centroids)
+
+
+def _w_ivfpq_params(out, d, M, by_residual, codebook, nbits=8, code_size=None, pq_d=None):
+    """What IwPQ adds after the IVF head: by_residual, code size, the ProductQuantizer."""
+    out.append(struct.pack("<BQ", 1 if by_residual else 0, M if code_size is None else code_size))
+    out.append(struct.pack("<QQQ", d if pq_d is None else pq_d, M, nbits))
+    _w_vec(out, np.ascontiguousarray(codebook, dtype=np.float32).reshape(-1))
 
 
 def write_ivfpq(path, centroids, codebook, codes, assign, ids=None, nprobe=1, by_residual=True, transform=None,
@@ -388,34 +426,116 @@ def write_ivfpq(path, centroids, codebook, codes, assign, ids=None, nprobe=1, by
     ids = np.arange(n, dtype=np.int64) if ids is None else np.asarray(ids, dtype=np.int64)
     out = []
     if id_map is not None:
-        out.append(struct.pack("<I", _fourcc("IxMp")))
+        _w_fourcc(out, "IxMp")
         _w_header(out, transform[0].shape[1] if transform is not None else d, n, METRIC_INNER_PRODUCT)
     if transform is not None:
-        A, b = transform
-        A = np.ascontiguousarray(A, dtype=np.float32)
-        out.append(struct.pack("<I", _fourcc("IxPT")))
-        _w_header(out, A.shape[1], n, METRIC_INNER_PRODUCT)
-        out.append(struct.pack("<i", 1))
-        out.append(struct.pack("<IB", _fourcc(transform_tag), 0 if b is None else 1))
-        _w_vec(out, A.reshape(-1))
-        _w_vec(out, np.zeros(0, np.float32) if b is None else np.asarray(b, np.float32))
-        out.append(struct.pack("<iiB", A.shape[1], A.shape[0], 1))
-    out.append(struct.pack("<I", _fourcc("IwPQ")))
-    _w_header(out, d, n, METRIC_INNER_PRODUCT)
-    out.append(struct.pack("<QQ", nlist, nprobe))
-    if hnsw:
-        _w_hnsw_flat(out, centroids)
-    else:
-        out.append(struct.pack("<I", _fourcc("IxFI")))
-        _w_header(out, d, nlist, METRIC_INNER_PRODUCT)
-        _w_vec(out, centroids.reshape(-1))
-    out.append(struct.pack("<b", 0))
-    _w_vec(out, np.zeros(0, np.int64))
-    out.append(struct.pack("<BQ", 1 if by_residual else 0, M if code_size is None else code_size))
-    out.append(struct.pack("<QQQ", d if pq_d is None else pq_d, M, nbits))
-    _w_vec(out, codebook.reshape(-1))
+        _w_pretransform(out, transform[0], transform[1], n, transform_tag)
+    _w_ivf_head(out, "IwPQ", d, n, nprobe, centroids, hnsw=hnsw)
+    _w_ivfpq_params(out, d, M, by_residual, codebook, nbits, code_size, pq_d)
     _w_invlists(out, nlist, M if code_size is None else code_size, codes, ids, assign, sparse_sizes)
     if id_map is not None:
         _w_vec(out, np.asarray(id_map, dtype=np.int64))
     with open(path, "wb") as f:
         f.write(b"".join(out))
+
+
+class _StoreReader:
+    """Sequential reads of an index's row store (or of its slot ids) through a window of `chunk` slots."""
+
+    def __init__(self, index, chunk, width, ids):
+        self.index, self.chunk, self.width, self.ids = index, max(1, int(chunk)), width, ids
+        self.w0 = self.w1 = 0
+        self.buf = None
+
+    def write(self, out, a, b):
+        from ._lib import lib, check
+
+        while a < b:
+            if not (self.w0 <= a < self.w1):
+                self.w0, self.w1 = a, min(self.index.ntotal, a + self.chunk)
+                m = self.w1 - self.w0
+                if self.ids:
+                    self.buf = np.empty(m, np.int64)
+                    check(lib.b200_index_copy_rows(self.index._h, self.w0, m, None, self.buf.ctypes.data), "copy_rows")
+                else:
+                    self.buf = np.empty((m, self.width), np.uint8)
+                    check(lib.b200_index_copy_rows(self.index._h, self.w0, m, self.buf.ctypes.data, None), "copy_rows")
+            e = min(b, self.w1)
+            out.append(self.buf[a - self.w0:e - self.w0])
+            a = e
+
+
+def write_index(index, path, chunk_bytes=1 << 26):
+    """Write a built index as a FAISS index file, the file `load_index` (and clip back's faiss.read_index) opens.
+
+        B200FlatIndex       -> IxSQ, QT_fp16
+        B200IVFFlatIndex    -> IwSq, QT_fp16, by_residual = false
+        B200IVFPQIndex      -> IwPQ (8-bit codes); with a pre-transform, inside one IxPT holding an LTra
+        index_from_faiss's id-mapped wrapper -> IxMp around the above
+
+    Rows are fp16 in this engine, so a flat or IVF-Flat index is always written as its SQfp16 form.  The coarse
+    quantiser is always written as a flat IndexFlatIP (IxFI), also for an index built from an `_HNSW32` key: building
+    an HNSW graph is out of scope, and FAISS then probes the centroids exactly, as this engine does.  IVF indices are
+    finalized first.  The row / code store is streamed to the file `chunk_bytes` at a time (ids alike), so host memory
+    stays bounded by the chunk, not by the index.  Refuses other objects and an index whose id_base is not 0.
+    The layout restates FAISS's index_write.cpp and is UNVERIFIED against FAISS itself (see the module docstring)."""
+    from ._lib import lib, check
+    from .index import B200FlatIndex, B200IVFFlatIndex, B200IVFPQIndex, _IdMapped
+
+    id_map = None
+    inner = index
+    if isinstance(index, _IdMapped):
+        inner, id_map = index._index, index._map
+    if not isinstance(inner, (B200FlatIndex, B200IVFFlatIndex, B200IVFPQIndex)):
+        raise TypeError("write_index: %s is not an index of this engine (flat, IVF-Flat, IVF-PQ or an id-mapped one)"
+                        % type(index).__name__)
+    if inner.id_base != 0:
+        raise ValueError("write_index: id_base=%d; a FAISS file numbers its rows from 0 (write each shard's index "
+                         "before setting id_base, or wrap it in an id map)" % inner.id_base)
+    if not isinstance(inner, B200FlatIndex):
+        inner.finalize()
+    info = np.zeros(8, np.int32)
+    check(lib.b200_index_get_quantizer(inner._h, None, None, None, None, info.ctypes.data), "get_quantizer")
+    nlist, M, by_residual, has_A, has_b, d, d_in, nprobe = (int(v) for v in info)
+    n = inner.ntotal
+    width = M if M else 2 * d
+    chunk = max(1, chunk_bytes // width)
+    with open(path, "wb") as f:
+        out = _FileSink(f)
+        if id_map is not None:
+            _w_fourcc(out, "IxMp")
+            _w_header(out, d_in, n, METRIC_INNER_PRODUCT)
+        if nlist == 0:
+            _w_fourcc(out, "IxSQ")
+            _w_header(out, d, n, METRIC_INNER_PRODUCT)
+            _w_sq_fp16(out, d)
+            out.append(struct.pack("<Q", n * width))
+            _StoreReader(inner, chunk, width, False).write(out, 0, n)
+        else:
+            cent = np.empty((nlist, d), np.float32)
+            cb = np.empty((M, 256, d // M), np.float32) if M else None
+            A = np.empty((d, d_in), np.float32) if has_A else None
+            b = np.empty(d, np.float32) if has_b else None
+            ptr = lambda a: None if a is None else a.ctypes.data  # noqa: E731
+            check(lib.b200_index_get_quantizer(inner._h, ptr(cent), ptr(cb), ptr(A), ptr(b), None), "get_quantizer")
+            if A is not None:
+                _w_pretransform(out, A, b, n)
+            if M:
+                _w_ivf_head(out, "IwPQ", d, n, nprobe, cent)
+                _w_ivfpq_params(out, d, M, by_residual, cb)
+            else:
+                _w_ivf_head(out, "IwSq", d, n, nprobe, cent)
+                _w_sq_fp16(out, d)
+                out.append(struct.pack("<QB", 2 * d, 0))
+            sizes = np.zeros(nlist, np.int64)
+            check(lib.b200_index_ivf_lists(inner._h, sizes.ctypes.data, None), "ivf_lists")
+            _w_invlists_head(out, nlist, width, sizes)
+            rows, ids = _StoreReader(inner, chunk, width, False), _StoreReader(inner, chunk, width, True)
+            off = 0
+            for m in sizes.tolist():
+                if m:
+                    rows.write(out, off, off + m)
+                    ids.write(out, off, off + m)
+                    off += m
+        if id_map is not None:
+            _w_vec(out, np.asarray(id_map, dtype=np.int64))

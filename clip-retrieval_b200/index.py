@@ -503,39 +503,134 @@ def train_pq(x, M, niter=25, seed=1234, device=0):
 PQ_TRAIN_MAX_ROWS = 65536   # FAISS: max_points_per_centroid (256) x 256 codewords
 
 
-def train_ivfpq(rows, nlist, M, niter=10, pq_niter=25, by_residual=True, seed=1234, device=0):
+def train_ivfpq(rows, nlist, M, niter=10, pq_niter=25, by_residual=True, seed=1234, device=0, A=None):
     """IVF-PQ training: the coarse quantiser by `train_kmeans` on the rows as fp16, then the PQ by `train_pq` on the
     residuals (the rows themselves without `by_residual`) of at most 65 536 rows picked one per stride (seeded).
+    With a pre-transform A [d_out, d] both are trained on A x (FAISS IndexPreTransform::train order): the k-means rows
+    are rotated chunk by chunk straight into one fp16 copy, the PQ sample in fp32.
     Separate from building so that range shards can be encoded against one replicated quantiser.
-    Returns (centroids np.float32 [nlist, d], codebook np.float32 [M, 256, d / M])."""
+    Returns (centroids np.float32 [nlist, d], codebook np.float32 [M, 256, d / M]) in the pre-transformed width."""
     torch = _torch()
     t = rows.detach() if _is_torch(rows) else torch.from_numpy(np.ascontiguousarray(rows))
     dev = t.device if t.is_cuda else torch.device("cuda", device)
     n, d = t.shape
+    if A is not None:
+        d = int(np.asarray(A).shape[0])
     if M < 1 or d % M:
         raise ValueError("train_ivfpq: M=%d must divide d=%d" % (M, d))
-    cent, _ = train_kmeans(t, nlist, niter=niter, seed=seed, device=dev.index or 0)
+    coarse = t if A is None else pretransform_rows(t, A, dtype="float16", device=dev.index or 0)
+    cent, _ = train_kmeans(coarse, nlist, niter=niter, seed=seed, device=dev.index or 0)
+    del coarse
     ns = min(n, PQ_TRAIN_MAX_ROWS)
     pick = torch.from_numpy(stride_picks(n, ns, seed)).to(t.device)
     sample = t[pick].to(device=dev, dtype=torch.float32).contiguous()
+    if A is not None:
+        sample = pretransform_rows(sample, A, device=dev.index or 0)
+    return cent, train_pq_residuals(sample, cent, M, pq_niter=pq_niter, by_residual=by_residual, seed=seed,
+                                    device=dev.index or 0)
+
+
+def train_pq_residuals(sample, cent, M, pq_niter=25, by_residual=True, seed=1234, device=0):
+    """The PQ step of `train_ivfpq`: `train_pq` on the residuals of `sample` (a CUDA fp32 tensor [n, d]) to their
+    nearest of the centroids [nlist, d] (the rows themselves without `by_residual`).  Returns the codebook."""
+    torch = _torch()
+    nlist, d = np.asarray(cent).shape
     if by_residual:
-        tmp = B200IVFPQIndex(d, nlist, M, cent, np.zeros((M, 256, d // M), np.float32), device=dev.index or 0)
+        tmp = B200IVFPQIndex(d, nlist, M, cent, np.zeros((M, 256, d // M), np.float32), device=device)
         res = torch.empty_like(sample)
-        st = torch.cuda.current_stream(dev).cuda_stream
-        check(lib.b200_index_encode_device(tmp._h, sample.data_ptr(), ns, None, res.data_ptr(), None, st), "encode")
+        st = torch.cuda.current_stream(sample.device).cuda_stream
+        check(lib.b200_index_encode_device(tmp._h, sample.data_ptr(), sample.shape[0], None, res.data_ptr(), None, st),
+              "encode")
         sample = res
-    cb, _ = train_pq(sample, M, niter=pq_niter, seed=seed, device=dev.index or 0)
-    return cent, cb
+    cb, _ = train_pq(sample, M, niter=pq_niter, seed=seed, device=device)
+    return cb
+
+
+OPQ_PHASES = ("rotate", "pq", "cross", "svd")
+
+
+def train_opq(rows, M, d_out=None, niter=50, niter_pq=4, niter_pq_0=40, seed=1234, device=0, phases=False):
+    """OPQ rotation training on the GPU (C ABI `b200_opq_train_f32`; FAISS OPQMatrix::train, DESIGN §5 (xiii)):
+    A [d_out, d_in] fp32 with orthonormal rows such that the M-way PQ of A x loses less than that of x.  rows: the
+    training rows [n, d_in] (fp16 / fp32, numpy or CUDA), 256 <= n <= 65 536 (pick them with `stride_picks`); d_out
+    defaults to d_in and may not exceed it; M divides d_out.  Starts from the polar factor of a seeded Gaussian matrix
+    (this project's rule, not FAISS's RNG); each iteration trains the PQ on x A^T (`niter_pq_0` Lloyd iterations the
+    first time, `niter_pq` from the previous codebook after that) and sets A to the polar factor of decode(codes)^T X.
+    Returns (A np.float32 [d_out, d_in], objective np.float32 [niter]: |x A^T - decode(codes)|^2 / n per iteration,
+    before that iteration's rotation update); with phases=True also {phase: ms} over OPQ_PHASES, each phase timed
+    between device synchronisations."""
+    torch = _torch()
+    t = rows.detach() if _is_torch(rows) else torch.from_numpy(np.ascontiguousarray(rows))
+    dev = t.device if t.is_cuda else torch.device("cuda", device)
+    t = t.to(device=dev, dtype=torch.float32).contiguous()
+    n, d_in = t.shape
+    d_out = d_in if d_out is None else int(d_out)
+    if d_out > d_in:
+        raise ValueError("train_opq: d_out=%d > d_in=%d (the rotation can only keep or reduce the width)" % (d_out, d_in))
+    if M < 1 or d_out % M:
+        raise ValueError("train_opq: M=%d must divide d_out=%d" % (M, d_out))
+    A = np.empty((d_out, d_in), np.float32)
+    obj = np.empty(max(0, int(niter)), np.float32)
+    ph = np.zeros(4, np.float32)
+    check(lib.b200_opq_train_f32(C.c_void_p(t.data_ptr()), n, d_in, d_out, int(M), int(niter), int(niter_pq),
+                                 int(niter_pq_0), C.c_uint64(seed), C.c_void_p(A.ctypes.data),
+                                 C.c_void_p(obj.ctypes.data) if obj.size else None,
+                                 C.c_void_p(ph.ctypes.data) if phases else None, dev.index or 0), "opq_train")
+    if phases:
+        return A, obj, dict(zip(OPQ_PHASES, (float(v) for v in ph)))
+    return A, obj
+
+
+def pretransform_rows(rows, A, b=None, dtype="float32", device=0, chunk=1 << 18):
+    """A x (+ b) for rows [n, d_in] (fp16 / fp32, numpy or CUDA) as a CUDA tensor [n, d_out] of `dtype` ("float32" or
+    "float16"), by the encoder's pre-transform kernel (C ABI `b200_rows_pretransform_device`): the rows an index with
+    this pre-transform quantises.  Rows go through `chunk` at a time, so besides the output the device holds one fp32
+    chunk; numpy rows are uploaded chunk by chunk."""
+    torch = _torch()
+    A = np.ascontiguousarray(A, dtype=np.float32)
+    d_out, d_in = A.shape
+    if rows.shape[1] != d_in:
+        raise ValueError("pretransform_rows: rows are %d wide, A expects %d" % (rows.shape[1], d_in))
+    dev = torch.device("cuda", device)
+    fp16 = dtype in ("float16", "f16", torch.float16)
+    Ad = torch.from_numpy(A).to(dev)
+    bd = None if b is None else torch.from_numpy(np.ascontiguousarray(b, dtype=np.float32).reshape(-1)).to(dev)
+    n = int(rows.shape[0])
+    out = torch.empty((n, d_out), dtype=torch.float16 if fp16 else torch.float32, device=dev)
+    st = torch.cuda.current_stream(dev).cuda_stream
+    for s in range(0, n, chunk):
+        e = min(n, s + chunk)
+        xc = rows[s:e] if _is_torch(rows) else torch.from_numpy(np.array(rows[s:e]))
+        xc = xc.to(device=dev, dtype=torch.float32).contiguous()
+        check(lib.b200_rows_pretransform_device(xc.data_ptr(), e - s, d_in, Ad.data_ptr(),
+                                                None if bd is None else bd.data_ptr(), d_out, out[s:e].data_ptr(),
+                                                1 if fp16 else 0, dev.index or 0, st), "pretransform")
+    return out
 
 
 def build_ivfpq_index(rows, nlist, M, niter=10, pq_niter=25, by_residual=True, seed=1234, nprobe=1, device=0,
-                      chunk=1 << 20):
+                      chunk=1 << 20, opq_dim=None, opq_niter=50):
     """train + create + encode + add_codes + finalize: an IVF-PQ index over `rows` (fp16 / fp32, numpy or CUDA),
-    the IVF-PQ counterpart of `build_ivf_index` (autofaiss's "IVF{nlist},PQ{M}x8" without the OPQ step)."""
-    cent, cb = train_ivfpq(rows, nlist, M, niter=niter, pq_niter=pq_niter, by_residual=by_residual, seed=seed,
-                           device=device)
+    the IVF-PQ counterpart of `build_ivf_index` (autofaiss's "IVF{nlist},PQ{M}x8").
+
+    opq_dim (default None: no rotation) adds the OPQ step, autofaiss's "OPQ{M}_{opq_dim},IVF{nlist},PQ{M}x8": an OPQ
+    rotation A [opq_dim, d] is trained (`train_opq`, M sub-quantisers) on at most 65 536 rows picked by `stride_picks`,
+    then the coarse quantiser and the PQ are trained on A x (`train_ivfpq(A=...)`: FAISS IndexPreTransform::train
+    order; the k-means rows take one extra fp16 copy of [n, opq_dim] on the device), A becomes the index's
+    pre-transform and rows are encoded through it."""
+    torch = _torch()
     dev = rows.device.index if _is_torch(rows) and rows.is_cuda else device
+    A = None
+    if opq_dim is not None:
+        n = rows.shape[0]
+        t = rows.detach() if _is_torch(rows) else torch.from_numpy(np.ascontiguousarray(rows))
+        pick = torch.from_numpy(stride_picks(n, min(n, PQ_TRAIN_MAX_ROWS), seed)).to(t.device)
+        A, _ = train_opq(t[pick], M, d_out=opq_dim, niter=opq_niter, seed=seed, device=dev or 0)
+    cent, cb = train_ivfpq(rows, nlist, M, niter=niter, pq_niter=pq_niter, by_residual=by_residual, seed=seed,
+                           device=device, A=A)
     idx = B200IVFPQIndex(cent.shape[1], nlist, M, cent, cb, by_residual=by_residual, device=dev or 0)
+    if A is not None:
+        idx.set_pretransform(A)
     for s in range(0, rows.shape[0], chunk):
         idx.add_codes(*idx.encode(rows[s:s + chunk]))
     idx.finalize()

@@ -108,6 +108,29 @@ int b200_index_encode_device(b200_index* idx, const float* d_x, int64_t n, int32
  * (or NULL).  Needs n >= 256, M dividing d, M * n < 2^31. */
 int b200_pq_train_f32(const float* d_x, int64_t n, int d, int M, int niter, uint64_t seed, float* h_codebook,
                       int64_t* h_sizes, int device);
+/* OPQ training (FAISS OPQMatrix::train, DESIGN §5 (xiii)): a rotation h_A [d_out, d_in] fp32 with orthonormal rows
+ * (d_out <= d_in, M divides d_out) for the rows d_x [n, d_in] fp32 (device, 256 <= n <= 65536).  The start is the polar
+ * factor of a seeded Gaussian matrix; each of `niter` iterations trains the PQ on the rotated rows (niter_pq_0 Lloyd
+ * iterations from b200_pq_train_f32's seeded picks the first time, then niter_pq from the previous codebook), records
+ * |x A^T - decode(codes)|^2 / n in h_objective[it] (or NULL), and sets A to the polar factor U V^T of
+ * G = decode(codes)^T X (fp64 SVD).  The SVD is cuSOLVER's, resolved at run time: without libcusolver.so.11 the call
+ * returns B200_ERR_UNSUPPORTED.  Deterministic: the same bits on every run.  h_phase_ms[4] (or NULL: no extra
+ * synchronisation) receives the milliseconds spent in {rotating the rows, PQ training and objective, cross matrix,
+ * SVD and polar product (the initial rotation included)}, measured between device synchronisations. */
+int b200_opq_train_f32(const float* d_x, int64_t n, int d_in, int d_out, int M, int niter, int niter_pq, int niter_pq_0,
+                       uint64_t seed, float* h_A, float* h_objective, float* h_phase_ms, int device);
+/* The cross-matrix step of OPQ training alone: d_G [d_out, d_in] fp32 = Y^T X over the n <= 65536 rows, Y = the rows d_codes
+ * [n, M] decode to under d_codebook [M, 256, d_out / M].  fp32 fma over fixed chunks of 1024 rows (ascending rows within
+ * a chunk), the chunk partials added in chunk order. */
+int b200_opq_cross_f32_device(const float* d_x, int64_t n, int d_in, const uint8_t* d_codes, const float* d_codebook,
+                              int d_out, int M, float* d_G, int device, void* stream);
+/* Rows d_y [n, d_out] = d_x [n, d_in] A^T (+ b), all fp32 on the device (A [d_out, d_in], b [d_out] or NULL), by the
+ * kernel b200_index_encode_device pre-transforms with; d_y is fp32, or fp16 (rounded to nearest) with out_fp16. */
+int b200_rows_pretransform_device(const float* d_x, int64_t n, int d_in, const float* d_A, const float* d_b, int d_out,
+                                  void* d_y, int out_fp16, int device, void* stream);
+/* The polar step alone: d_A [d_out, d_in] fp32 = U V^T for d_G = U S V^T [d_out, d_in] fp32 (d_out <= d_in), from the
+ * fp64 SVD.  Synchronises the stream. */
+int b200_opq_polar_f32_device(const float* d_G, int d_out, int d_in, float* d_A, int device, void* stream);
 int b200_index_destroy(b200_index* idx);
 
 /* Pre-size the row store (rows); avoids regrowth copies for large shards. */
@@ -152,6 +175,16 @@ int b200_index_last_scan_plan(const b200_index* idx, int32_t* h_plan);
 /* IVF introspection used by ivf_metadata_ordering.get_old_to_new_mapping
  * (ivf_metadata_ordering.py:46-64): sizes[nlist] and, list after list, the ids in list order. */
 int b200_index_ivf_lists(b200_index* idx, int64_t* h_sizes, int64_t* h_ids);
+/* What a FAISS index writer needs of the quantiser.  h_info[8] = {nlist, M (0 unless IVF-PQ), by_residual,
+ * has pre-transform A, has b, d (stored width), d_in (query width), nprobe}.  Each other output may be NULL:
+ * h_centroids [nlist, d] fp32 (IVF-Flat: its fp16 centroids widened), h_codebook [M, 256, d / M], h_A [d, d_in],
+ * h_b [d]. */
+int b200_index_get_quantizer(b200_index* idx, float* h_centroids, float* h_codebook, float* h_A, float* h_b,
+                             int32_t* h_info);
+/* Rows [s0, s0 + n) of the store in store order (flat: insertion order; IVF: list order, after the pending rows are
+ * bucketed as b200_index_finalize does), unpadded: 2 d bytes of fp16 per row, or M code bytes.  h_ids [n] (or NULL)
+ * receives each slot's id (id_base + insertion id).  Either output may be NULL. */
+int b200_index_copy_rows(b200_index* idx, int64_t s0, int64_t n, void* h_rows, int64_t* h_ids);
 
 /* index.search_and_reconstruct(x, k) / index.search(x, k) with HOST buffers (the call the
  * reference makes): h_q fp32 [nq, d]; h_D fp32 [nq, k]; h_I int64 [nq, k]; h_R fp32 [nq, k, d] or

@@ -10,6 +10,15 @@ FP32 data-sheet rate of the H100 SXM: the assignment is bound by FP32 FMA issue 
 memory, four 16-byte loads per 64 FMAs), so that is the bound its fraction names.  The coarse quantiser is trained on
 the first `--train-rows` rows (`train_kmeans`), the PQ on the residuals of at most 65 536 of them (`train_ivfpq`).
 8 rows of every shape are checked against tests/pq_train_ref.check_encode.
+
+    python tools/ivfpq_build_bench.py --opq [--d 768] [--M 64] [--opq-niter 50]
+
+`--opq` times OPQ training instead (`train_opq`, C ABI `b200_opq_train_f32`) on 65 536 anisotropic rows (a decaying
+spectrum under a random rotation, made on the host from `--seed`): one JSON line per M with the training time split
+into rotate (x A^T) / PQ (Lloyd iterations and the objective) / cross (G = Y^T X: 2 * n * d_in * d_out flops per
+iteration, against the FP32 data-sheet rate) / SVD (fp64 cuSOLVER SVD and the polar product), each phase measured
+between device synchronisations; the first and last objective; and the PQ error of the sample with and without the
+rotation (plain PQ trained by `train_pq` with as many Lloyd iterations as OPQ ran in all).
 """
 import argparse
 import json
@@ -33,6 +42,51 @@ def card():
     return name, power
 
 
+def opq_main(a):
+    import torch
+    import clip_retrieval_b200 as m
+
+    name, power = card()
+    n, d = m.index.PQ_TRAIN_MAX_ROWS, a.d
+    rng = np.random.default_rng(a.seed)
+    q, _ = np.linalg.qr(rng.standard_normal((d, d)))
+    X = torch.from_numpy(((rng.standard_normal((n, d)) * np.exp(-np.arange(d) / (d / 8))) @ q.T).astype(np.float32))
+    X = X.cuda()
+    Xn = X.cpu().numpy().astype(np.float64)
+
+    def pq_error(rows, cb):
+        M = cb.shape[0]
+        codes, _ = m.B200IVFPQIndex(rows.shape[1], 1, M, np.zeros((1, rows.shape[1]), np.float32), cb,
+                                    by_residual=False).encode(rows)
+        codes = codes.cpu().numpy()
+        Y = np.concatenate([cb[j][codes[:, j]] for j in range(M)], axis=1)
+        return float(((rows.cpu().numpy().astype(np.float64) - Y) ** 2).sum() / rows.shape[0])
+
+    for M in (int(x) for x in a.M.split(",")):
+        m.train_opq(X[:4096], M, niter=1, niter_pq_0=1)       # warm-up: module load, cuSOLVER handle
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        A, obj, ph = m.train_opq(X, M, niter=a.opq_niter, seed=a.seed, phases=True)
+        total = time.perf_counter() - t0
+        lloyd = 40 + (a.opq_niter - 1) * 4
+        cb, _ = m.train_pq(X, M, niter=lloyd, seed=a.seed)
+        plain = pq_error(X, cb)
+        Xr = m.index.pretransform_rows(X, A)
+        cbr, _ = m.train_pq(Xr, M, niter=a.pq_niter, seed=a.seed)
+        cross_flops = 2.0 * n * d * d * a.opq_niter
+        rec = {"mode": "opq", "M": M, "rows": n, "d": d, "niter": a.opq_niter, "train_s": round(total, 3),
+               "phase_ms": {k: round(v, 1) for k, v in ph.items()},
+               "cross_flops_per_s": cross_flops / (ph["cross"] / 1e3) if ph["cross"] > 0 else None,
+               "cross_fp32_datasheet_fraction": cross_flops / (ph["cross"] / 1e3) / FP32_FLOPS if ph["cross"] > 0 else None,
+               "objective_first": float(obj[0]), "objective_last": float(obj[-1]),
+               "pq_error_plain": plain, "pq_error_opq_codebook": float(obj[-1]),
+               "pq_error_opq_retrained": pq_error(Xr, cbr), "plain_pq_lloyd_iterations": lloyd,
+               "gpu": name, "power_limit": power}
+        print(json.dumps(rec), flush=True)
+        del Xr
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", type=int, default=10_000_000)
@@ -44,7 +98,13 @@ def main():
     ap.add_argument("--pq-niter", type=int, default=25)
     ap.add_argument("--chunk", type=int, default=1 << 20)
     ap.add_argument("--seed", type=int, default=1234)
+    ap.add_argument("--opq", action="store_true", help="time OPQ training instead of the IVF-PQ build")
+    ap.add_argument("--opq-niter", type=int, default=50)
     a = ap.parse_args()
+    if a.opq:
+        if a.M == ap.get_default("M"):
+            a.M = "64"
+        return opq_main(a)
     import torch
     import clip_retrieval_b200 as m
     import pq_train_ref as P
