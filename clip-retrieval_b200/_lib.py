@@ -93,10 +93,10 @@ class GemmEpilogueC(C.Structure):
         ("out_ld", C.c_int64),
         ("out_group", C.c_int32),
         ("act", C.c_int32),
-        ("ln_stats", C.c_void_p),
-        ("ln_c", C.c_void_p),
-        ("ln_w", C.c_int32),
-        ("stats_out", C.c_void_p),
+        ("reserved0", C.c_void_p),
+        ("reserved1", C.c_void_p),
+        ("reserved2", C.c_int32),
+        ("reserved3", C.c_void_p),
     ]
 
 
@@ -164,7 +164,6 @@ PROTOTYPES = {
     "b200_attention_bf16_device": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "b200_gemm_bf16_device": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "b200_gemm_bf16_ex_device": (_i, [_vp, _vp, _vp, _i, _i, _i, C.POINTER(GemmEpilogueC), _i, _i, _i, _vp]),
-    "b200_row_stats_bf16_device": (_i, [_vp, _i64, _i, _vp, _i, _vp]),
     "b200_index_last_hi_only_fallbacks": (_i, [_vp]),
     "b200_index_last_scan_plan": (_i, [_vp, _vp]),
     "b200_kmeans_train_f16": (_i, [_vp, _i64, _i, _i, _i, C.c_uint64, _i, _vp, _vp, _i]),

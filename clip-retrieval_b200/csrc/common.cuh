@@ -67,6 +67,29 @@ struct DeviceGuard {
 
 int sm_count(int device);
 
+// Buffers a handle shares between calls: calls hold the handle's mutex while they enqueue, acquire() before their
+// first launch and release() after their last.  A call on a different stream than the previous one first waits (event)
+// for the previous call's kernels, so in-flight work never sees its buffers reused.
+struct StreamFence {
+  cudaEvent_t ev = nullptr;   // recorded after the last call's launches
+  cudaStream_t last = nullptr;
+  bool used = false;
+  ~StreamFence() {
+    if (ev) cudaEventDestroy(ev);
+  }
+  int acquire(cudaStream_t st) {
+    if (!ev) B200_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    if (used && last != st) B200_CUDA(cudaStreamWaitEvent(st, ev, 0));
+    return B200_OK;
+  }
+  int release(cudaStream_t st) {
+    B200_CUDA(cudaEventRecord(ev, st));
+    last = st;
+    used = true;
+    return B200_OK;
+  }
+};
+
 // ---- device helpers ---------------------------------------------------------------------------
 __device__ __forceinline__ uint4 ld_nc_v4(const uint4* p) {
   uint4 r;

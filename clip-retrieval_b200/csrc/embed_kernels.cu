@@ -222,38 +222,6 @@ int layernorm_rows_eps(const __nv_bfloat16* in, int64_t in_ld, __nv_bfloat16* ou
   return B200_OK;
 }
 
-// ---- row statistics for the folded LayerNorm (gemm.cuh GemmEpilogue::ln_stats) ---------------------------
-// One (mean, M2) record per 64-column slot of every row — what the residual GEMM epilogues write for the rows they
-// produce; this kernel seeds the records for a residual stream that did not come out of a GEMM (after ln_pre in the
-// vision tower, after the token + positional embedding in the text tower).  One warp per row.
-__global__ void __launch_bounds__(256)
-row_stats_kernel(const __nv_bfloat16* __restrict__ x, int64_t rows, int w, float2* __restrict__ stats) {
-  const int lane = threadIdx.x & 31;
-  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (row >= rows) return;
-  const int slots = w >> 6;
-  for (int s = 0; s < slots; s++) {
-    // two values per lane
-    const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(x + row * w + s * 64 + lane * 2);
-    const float2 f = __bfloat1622float2(v);
-    float sum = f.x + f.y;
-#pragma unroll
-    for (int o = 16; o >= 1; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    const float mean = sum * (1.0f / 64.0f);
-    float m2 = (f.x - mean) * (f.x - mean) + (f.y - mean) * (f.y - mean);
-#pragma unroll
-    for (int o = 16; o >= 1; o >>= 1) m2 += __shfl_xor_sync(0xffffffffu, m2, o);
-    if (lane == 0) stats[row * slots + s] = make_float2(mean, m2);
-  }
-}
-int row_stats(const __nv_bfloat16* x, int64_t rows, int w, float2* stats, cudaStream_t st) {
-  B200_CHECK(w % 64 == 0, B200_ERR_UNSUPPORTED, "row_stats: width %d is not a multiple of 64", w);
-  if (rows == 0) return B200_OK;
-  row_stats_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(x, rows, w, stats);
-  B200_LAUNCH_OK();
-  return B200_OK;
-}
-
 // ---- K8/K10/K11: pooled LN + projection + L2 normalise + cast --------------------------------------
 __device__ __forceinline__ float block_sum(float v, float* red) {
 #pragma unroll

@@ -20,8 +20,6 @@ int layernorm_rows(const __nv_bfloat16* in, int64_t in_ld, __nv_bfloat16* out, i
 // The same LayerNorm with the epsilon as an argument (BERT-family encoders carry it in their config: 1e-5, 1e-12).
 int layernorm_rows_eps(const __nv_bfloat16* in, int64_t in_ld, __nv_bfloat16* out, int64_t out_ld, const float* gamma,
                        const float* beta, int64_t rows, int w, float eps, cudaStream_t st);
-// (mean, M2) per 64-column slot of every row of x [rows, w] (w % 64 == 0): seeds GemmEpilogue::ln_stats.
-int row_stats(const __nv_bfloat16* x, int64_t rows, int w, float2* stats, cudaStream_t st);
 // K4: multi-head attention over the fused qkv buffer [B*T, 3w] -> out [B*T, w]; causal for text.  mma.sync kernel
 // (attention.cu) for the head dimensions the wgmma kernel does not take (80, 96, 128).
 // len (device int32 [B], values 1..T, or nullptr = T): sample b attends to its keys < len[b], and its rows >= len[b]

@@ -73,9 +73,9 @@ int make_tmap_3d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t pla
 // over more SMs and are mostly as fast or faster.
 constexpr long GEMM_WIDE_MIN_TILES_PER_SM = 1;
 
-int gemm_pick_bn(int M, int N, int sms, bool wide) {
+int gemm_pick_bn(int M, int N, int sms) {
   const long mb = (M + GEMM_BM - 1) / GEMM_BM;
-  if (wide && mb * ((N + GEMM_WIDE_BN - 1) / GEMM_WIDE_BN) >= GEMM_WIDE_MIN_TILES_PER_SM * sms) return GEMM_WIDE_BN;
+  if (mb * ((N + GEMM_WIDE_BN - 1) / GEMM_WIDE_BN) >= GEMM_WIDE_MIN_TILES_PER_SM * sms) return GEMM_WIDE_BN;
   const long tiles128 = mb * ((N + 127) / 128);
   if (tiles128 < sms && N >= 64) {
     const long tiles64 = mb * ((N + 63) / 64);
@@ -102,23 +102,18 @@ static int launch_bn_spec(const CUtensorMap& tmA, const CUtensorMap& tmB, int M,
   return B200_OK;
 }
 
-// the epilogue flavour (activation | residual << 2) fixed at compile time unless the LayerNorm fold or the row
-// statistics are in use
+// the epilogue flavour (activation | residual << 2) fixed at compile time; gemm_bf16_launch has checked ep.act
 template <int BN>
 static int launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, const GemmEpilogue& ep,
-                     cudaStream_t st, bool generic) {
-  if (!generic && gemm_epilogue_is_plain(ep)) {
-    switch ((ep.act & 3) | (ep.residual ? 4 : 0)) {
-      case 0: return launch_bn_spec<BN, 0>(tmA, tmB, M, N, K, ep, st);
-      case 1: return launch_bn_spec<BN, 1>(tmA, tmB, M, N, K, ep, st);
-      case 2: return launch_bn_spec<BN, 2>(tmA, tmB, M, N, K, ep, st);
-      case 4: return launch_bn_spec<BN, 4>(tmA, tmB, M, N, K, ep, st);
-      case 5: return launch_bn_spec<BN, 5>(tmA, tmB, M, N, K, ep, st);
-      case 6: return launch_bn_spec<BN, 6>(tmA, tmB, M, N, K, ep, st);
-      default: break;
-    }
+                     cudaStream_t st) {
+  switch (ep.act | (ep.residual ? 4 : 0)) {
+    case 0: return launch_bn_spec<BN, 0>(tmA, tmB, M, N, K, ep, st);
+    case 1: return launch_bn_spec<BN, 1>(tmA, tmB, M, N, K, ep, st);
+    case 2: return launch_bn_spec<BN, 2>(tmA, tmB, M, N, K, ep, st);
+    case 4: return launch_bn_spec<BN, 4>(tmA, tmB, M, N, K, ep, st);
+    case 5: return launch_bn_spec<BN, 5>(tmA, tmB, M, N, K, ep, st);
+    default: return launch_bn_spec<BN, 6>(tmA, tmB, M, N, K, ep, st);
   }
-  return launch_bn_spec<BN, -1>(tmA, tmB, M, N, K, ep, st);
 }
 
 template <int SPEC, class Cfg>
@@ -170,11 +165,8 @@ static int launch_wide_spec(const CUtensorMap& tmA, const CUtensorMap& tmB, int 
 }
 
 static int launch_wide(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, const GemmEpilogue& ep,
-                       cudaStream_t st, bool generic, bool force_tma) {
-  B200_CHECK(!generic && gemm_epilogue_is_plain(ep), B200_ERR_INVALID,
-             "gemm: 256-wide tiles take the compile-time epilogue flavours only (no LayerNorm fold, row statistics or "
-             "forced run-time flavour)");
-  switch ((ep.act & 3) | (ep.residual ? 4 : 0)) {
+                       cudaStream_t st, bool force_tma) {
+  switch (ep.act | (ep.residual ? 4 : 0)) {
     case 0: return launch_wide_spec<0>(tmA, tmB, M, N, K, ep, st, force_tma);
     case 1: return launch_wide_spec<1>(tmA, tmB, M, N, K, ep, st, force_tma);
     case 2: return launch_wide_spec<2>(tmA, tmB, M, N, K, ep, st, force_tma);
@@ -185,22 +177,18 @@ static int launch_wide(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, in
 }
 
 int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int M, int N, int K,
-                     const GemmEpilogue& ep, cudaStream_t st, bool generic, bool force_tma_epilogue) {
+                     const GemmEpilogue& ep, cudaStream_t st, bool force_tma_epilogue) {
   B200_CHECK(M >= 1 && N >= 8 && K >= 8 && N % 8 == 0 && K % 8 == 0, B200_ERR_INVALID,
              "gemm: need M>=1 and N, K multiples of 8 (M=%d N=%d K=%d)", M, N, K);
   B200_CHECK(ep.out != nullptr && ep.out_ld % 8 == 0 && ((uintptr_t)ep.out & 15) == 0, B200_ERR_INVALID,
              "gemm: output must be 16-byte aligned with ld %% 8 == 0");
   B200_CHECK(ep.residual == nullptr || (ep.res_ld % 8 == 0 && ((uintptr_t)ep.residual & 15) == 0), B200_ERR_INVALID,
              "gemm: residual must be 16-byte aligned with ld %% 8 == 0");
-  B200_CHECK(ep.stats_out == nullptr || (N % 64 == 0 && bn >= 128), B200_ERR_INVALID,
-             "gemm: row statistics need N %% 64 == 0 and tiles of at least 128 columns (N=%d, bn=%d)", N, bn);
-  B200_CHECK(ep.ln_stats == nullptr || (ep.ln_c != nullptr && ep.ln_w > 0 && ep.ln_w % 64 == 0), B200_ERR_INVALID,
-             "gemm: folded LayerNorm needs c and a row width that is a multiple of 64 (ln_w=%d)", ep.ln_w);
-  B200_CHECK(ep.ln_stats == nullptr || ep.ln_w <= 64 * LN_MAX_SLOTS, B200_ERR_UNSUPPORTED, "gemm: folded LayerNorm supports rows of at most %d columns", 64 * LN_MAX_SLOTS);
-  if (bn == GEMM_WIDE_BN) return launch_wide(tmA, tmB, M, N, K, ep, st, generic, force_tma_epilogue);
-  if (bn == 128) return launch_bn<128>(tmA, tmB, M, N, K, ep, st, generic);
-  if (bn == 64) return launch_bn<64>(tmA, tmB, M, N, K, ep, st, generic);
-  if (bn == 32) return launch_bn<32>(tmA, tmB, M, N, K, ep, st, generic);
+  B200_CHECK(ep.act >= 0 && ep.act <= 2, B200_ERR_INVALID, "gemm: act=%d", ep.act);
+  if (bn == GEMM_WIDE_BN) return launch_wide(tmA, tmB, M, N, K, ep, st, force_tma_epilogue);
+  if (bn == 128) return launch_bn<128>(tmA, tmB, M, N, K, ep, st);
+  if (bn == 64) return launch_bn<64>(tmA, tmB, M, N, K, ep, st);
+  if (bn == 32) return launch_bn<32>(tmA, tmB, M, N, K, ep, st);
   set_error("gemm: unsupported column block %d", bn);
   return B200_ERR_INVALID;
 }
@@ -210,22 +198,17 @@ int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int
 using namespace b200;
 
 // The stand-alone entries: A [M, K] and W [N, K] contiguous, everything else as the epilogue says.  bn = 0 takes
-// gemm_pick_bn's width (256 only for the compile-time flavours; raised to 128 when row statistics are written, as the
-// model does).
-static int gemm_entry(const void* d_A, const void* d_W, int M, int N, int K, GemmEpilogue ep, int bn, bool generic,
-                      int device, void* stream, bool force_tma_epilogue = false) {
+// gemm_pick_bn's width.
+static int gemm_entry(const void* d_A, const void* d_W, int M, int N, int K, const GemmEpilogue& ep, int bn, int device,
+                      void* stream, bool force_tma_epilogue = false) {
   B200_CHECK(d_A && d_W && ep.out, B200_ERR_INVALID, "gemm: null operand");
-  B200_CHECK(ep.act >= 0 && ep.act <= 2, B200_ERR_INVALID, "gemm: act=%d", ep.act);
   B200_CHECK(bn == 0 || bn == 32 || bn == 64 || bn == 128 || bn == GEMM_WIDE_BN, B200_ERR_INVALID, "gemm: unsupported column block %d", bn);
   DeviceGuard g(device);
-  if (bn == 0) {
-    bn = gemm_pick_bn(M, N, sm_count(device), !generic && gemm_epilogue_is_plain(ep));
-    if (ep.stats_out != nullptr && bn < 128) bn = 128;
-  }
+  if (bn == 0) bn = gemm_pick_bn(M, N, sm_count(device));
   CUtensorMap tmA, tmB;
   B200_TRY(make_tmap_2d(&tmA, d_A, 1, (uint64_t)M, (uint64_t)K, (uint64_t)K, GEMM_BM, GEMM_BK));
   B200_TRY(make_tmap_2d(&tmB, d_W, 1, (uint64_t)N, (uint64_t)K, (uint64_t)K, (uint32_t)std::min(bn, 128), GEMM_BK));
-  return gemm_bf16_launch(tmA, tmB, bn, M, N, K, ep, (cudaStream_t)stream, generic, force_tma_epilogue);
+  return gemm_bf16_launch(tmA, tmB, bn, M, N, K, ep, (cudaStream_t)stream, force_tma_epilogue);
 }
 
 extern "C" int b200_gemm_bf16_device(const void* d_A, const void* d_W, const float* d_bias, const void* d_residual,
@@ -237,12 +220,16 @@ extern "C" int b200_gemm_bf16_device(const void* d_A, const void* d_W, const flo
   ep.out = (__nv_bfloat16*)d_C;
   ep.out_ld = N;
   ep.act = act;
-  return gemm_entry(d_A, d_W, M, N, K, ep, 0, false, device, stream);
+  return gemm_entry(d_A, d_W, M, N, K, ep, 0, device, stream);
 }
 
 extern "C" int b200_gemm_bf16_ex_device(const void* d_A, const void* d_W, void* d_C, int M, int N, int K,
-                                        const b200_gemm_epilogue* e, int bn, int force_generic, int device, void* stream) {
+                                        const b200_gemm_epilogue* e, int bn, int flags, int device, void* stream) {
   B200_CHECK(e != nullptr, B200_ERR_INVALID, "gemm: null epilogue");
+  // bit 1: the persistent kernel's TMA-store epilogue whatever the grid size (the tests reach it at small shapes)
+  B200_CHECK((flags & ~2) == 0, B200_ERR_INVALID, "gemm: flags=%d (only bit 1 is defined)", flags);
+  B200_CHECK(!e->reserved0 && !e->reserved1 && e->reserved2 == 0 && !e->reserved3, B200_ERR_INVALID,
+             "gemm: the reserved members of b200_gemm_epilogue must be zero (the LayerNorm fold was removed)");
   GemmEpilogue ep;
   ep.bias = e->bias;
   ep.residual = (const __nv_bfloat16*)e->residual;
@@ -253,10 +240,5 @@ extern "C" int b200_gemm_bf16_ex_device(const void* d_A, const void* d_W, void* 
   ep.out_ld = e->out_ld > 0 ? e->out_ld : N;
   ep.out_group = e->out_group;
   ep.act = e->act;
-  ep.ln_stats = (const float2*)e->ln_stats;
-  ep.ln_c = e->ln_c;
-  ep.ln_w = e->ln_w;
-  ep.stats_out = (float2*)e->stats_out;
-  // bit 1: the persistent kernel's TMA-store epilogue whatever the grid size (the tests reach it at small shapes)
-  return gemm_entry(d_A, d_W, M, N, K, ep, bn, (force_generic & ~2) != 0, device, stream, (force_generic & 2) != 0);
+  return gemm_entry(d_A, d_W, M, N, K, ep, bn, device, stream, (flags & 2) != 0);
 }

@@ -38,46 +38,13 @@ struct GemmEpilogue {
   int64_t out_ld = 0;
   int out_group = 0;                        // > 0: out row = (row / g) * (g + 1) + 1 + row % g  (cls slot)
   int act = ACT_NONE;
-  // LayerNorm folded into this GEMM (K5/K6 of SURVEY §2.2 without a separate normalisation pass): A is the RAW
-  // residual stream x and the weights carry gamma (W'[n,k] = W[n,k] * gamma[k]), so
-  //   LN(x) W^T + b = rstd * (x W'^T - mean * c) + d,   c[n] = sum_k W'[n,k],  d[n] = sum_k beta[k] W[n,k] + b[n].
-  // ln_stats: per row, ln_w / 64 records (mean, M2) of 64-column slots of x, written by the producer's epilogue
-  // (stats_out below); ln_c = c (fp32 [N]); `bias` then points at d.
-  const float2* ln_stats = nullptr;
-  const float* ln_c = nullptr;
-  int ln_w = 0;
-  // Row statistics of what this epilogue stores (bf16-rounded), one (mean, M2) record per 64 output columns:
-  // stats_out[row * (N / 64) + slot].  Set on the GEMMs that write the residual stream.
-  float2* stats_out = nullptr;
 };
 
 // Per-row constants of the epilogue, computed once per tile.
 struct EpiRow {
   __nv_bfloat16* out_ptr;
   const __nv_bfloat16* res_ptr;
-  float ln_a, ln_b;        // folded LayerNorm: value = acc * ln_a + (ln_b * c[col] + d[col]);  (1, 0) when off
 };
-// (mean, rstd) of a row from its 64-column slot records (Chan's combination of equal-sized groups).  Every record
-// load is issued before the first is used: consuming them one by one pays the L2 latency `slots` times per row.
-constexpr int LN_MAX_SLOTS = 24;   // row width <= 1536
-__device__ __forceinline__ void ln_row_coeffs(const float2* __restrict__ rec, int slots, int w, float& a, float& b) {
-  float2 v[LN_MAX_SLOTS];
-#pragma unroll
-  for (int i = 0; i < LN_MAX_SLOTS; i++) v[i] = i < slots ? __ldg(rec + i) : make_float2(0.f, 0.f);
-  float msum = 0.f;
-#pragma unroll
-  for (int i = 0; i < LN_MAX_SLOTS; i++) msum += v[i].x;
-  const float mean = msum / (float)slots;
-  float m2 = 0.f;
-#pragma unroll
-  for (int i = 0; i < LN_MAX_SLOTS; i++) {
-    const float dm = v[i].x - mean;
-    m2 += i < slots ? v[i].y + 64.0f * dm * dm : 0.f;
-  }
-  const float rstd = rsqrtf(fmaxf(m2 / (float)w, 0.f) + 1e-5f);
-  a = rstd;
-  b = -mean * rstd;
-}
 __device__ __forceinline__ EpiRow epi_row(const GemmEpilogue& ep, int row, int n0) {
   EpiRow r;
   int64_t out_row = row;
@@ -86,8 +53,6 @@ __device__ __forceinline__ EpiRow epi_row(const GemmEpilogue& ep, int row, int n
   if (ep.res_row_mod > 0) res_row = ep.res_row_off + row % ep.res_row_mod;
   r.out_ptr = ep.out + out_row * ep.out_ld + n0;
   r.res_ptr = ep.residual ? ep.residual + res_row * ep.res_ld + n0 : nullptr;
-  r.ln_a = 1.0f;
-  r.ln_b = 0.0f;
   return r;
 }
 
@@ -104,7 +69,7 @@ struct GemmCfg {
   static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
   static constexpr int STG_LD = BN + 4;   // fp32 staging row pitch (floats): conflict-free 16-byte row reads
   static_assert(GEMM_BM * STG_LD * 4 <= RING_BYTES, "the accumulator staging tile reuses the ring");
-  static constexpr int SMEM_BYTES = RING_BYTES + 2 * BN * 4 + 256 + 1024;  // ring + bias + LN c + barriers + align slack
+  static constexpr int SMEM_BYTES = RING_BYTES + BN * 4 + 256 + 1024;  // ring + bias + barriers + align slack
 };
 
 __device__ __forceinline__ void gemm_tile_coords(int tile, int mb, int nb, int& m_blk, int& n_blk) {
@@ -138,10 +103,9 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
   return __bfloat1622float2(v);
 }
 
-// act(pre) + residual, pre = accumulator + bias (or the folded LayerNorm's value): the per-element arithmetic of every
-// epilogue, rounded to bf16 by the caller (pack_bf16x2).  __fadd_rn: never contracted with the activation's last
-// multiply into an FMA — every epilogue flavour (run-time or compile-time, either kernel) rounds the same way and stays
-// bit-identical to the others.
+// act(pre) + residual, pre = accumulator + bias: the per-element arithmetic of every epilogue, rounded to bf16 by the
+// caller (pack_bf16x2).  __fadd_rn: never contracted with the activation's last multiply into an FMA — every epilogue
+// (either kernel, register or TMA store) rounds the same way and stays bit-identical to the others.
 __device__ __forceinline__ float epi_apply(float pre, int act, bool has_res, float res) {
   const float v = act_apply(pre, act);
   return has_res ? __fadd_rn(v, res) : v;
@@ -150,77 +114,37 @@ __device__ __forceinline__ float epi_apply(float pre, int act, bool has_res, flo
 // bias + activation + residual + bf16 store of 8 consecutive columns (col = offset inside the tile)
 // `rr` = the residual's 8 values, loaded before the accumulator is read so that their HBM latency does not sit in
 // the middle of the epilogue.
-// s_bias = bias (or the folded LayerNorm's d), s_c = the folded LayerNorm's c (read only when ep.ln_stats is set).
-// st_k / st_s / st_q: running shifted sums of the stored values for the row statistics (ep.stats_out).
-// SPEC: -1 = every feature decided at run time; 0..7 = activation | residual << 2 fixed at compile time (no LayerNorm
-// fold, no row statistics): the generic flavour carries a run-time activation switch around an inlined
-// erff for every element plus the fold / statistics paths.
+// SPEC = activation | residual << 2, fixed at compile time.
 template <int SPEC>
-__device__ __forceinline__ void epi_store8(const GemmEpilogue& ep, const EpiRow& er, const uint32_t* r8,
-                                           const float* s_bias, const float* s_c, int col, int n0, const uint4& rr,
-                                           float st_k, float& st_s, float& st_q) {
-  const int act = SPEC >= 0 ? (SPEC & 3) : ep.act;
-  const bool use_ln = SPEC < 0 && ep.ln_stats != nullptr;
-  const bool use_stats = SPEC < 0 && ep.stats_out != nullptr;
-  const bool has_res = SPEC >= 0 ? ((SPEC >> 2) & 1) != 0 : er.res_ptr != nullptr;
+__device__ __forceinline__ void epi_store8(const EpiRow& er, const uint32_t* r8, const float* s_bias, int col,
+                                           const uint4& rr) {
+  constexpr int act = SPEC & 3;
+  constexpr bool has_res = ((SPEC >> 2) & 1) != 0;
   const float2 a = unpack_bf16x2(rr.x), b = unpack_bf16x2(rr.y), cc = unpack_bf16x2(rr.z), dd = unpack_bf16x2(rr.w);
   const float res[8] = {a.x, a.y, b.x, b.y, cc.x, cc.y, dd.x, dd.y};
   float v[8];
 #pragma unroll
-  for (int j = 0; j < 8; j++) {
-    const float pre = use_ln ? fmaf(__uint_as_float(r8[j]), er.ln_a, fmaf(er.ln_b, s_c[col + j], s_bias[col + j]))
-                             : __uint_as_float(r8[j]) + s_bias[col + j];
-    v[j] = epi_apply(pre, act, has_res, res[j]);
-  }
+  for (int j = 0; j < 8; j++) v[j] = epi_apply(__uint_as_float(r8[j]) + s_bias[col + j], act, has_res, res[j]);
   uint4 o;
   o.x = pack_bf16x2(v[0], v[1]);
   o.y = pack_bf16x2(v[2], v[3]);
   o.z = pack_bf16x2(v[4], v[5]);
   o.w = pack_bf16x2(v[6], v[7]);
   *reinterpret_cast<uint4*>(er.out_ptr + col) = o;
-  if (use_stats) {
-    // statistics of the values as stored (bf16), shifted by the slot's first value to keep the sums small
-    const float2 f0 = unpack_bf16x2(o.x), f1 = unpack_bf16x2(o.y), f2 = unpack_bf16x2(o.z), f3 = unpack_bf16x2(o.w);
-    const float e[8] = {f0.x - st_k, f0.y - st_k, f1.x - st_k, f1.y - st_k, f2.x - st_k, f2.y - st_k, f3.x - st_k, f3.y - st_k};
-#pragma unroll
-    for (int j = 0; j < 8; j++) {
-      st_s += e[j];
-      st_q = fmaf(e[j], e[j], st_q);
-    }
-  }
 }
 
-// One 32-column chunk `c` of the tile for this thread's row: the four 8-column groups, and (stats_out) the
-// (mean, M2) record of a completed 64-column slot (chunks 2j, 2j+1).
+// One 32-column chunk `c` of the tile for this thread's row: the four 8-column groups.
 template <int SPEC>
-__device__ __forceinline__ void epi_chunk(const GemmEpilogue& ep, const EpiRow& er, const uint32_t* r, const float* s_bias,
-                                          const float* s_c, int c, int n0, int N, int row, const uint4* res4, float& st_k,
-                                          float& st_s, float& st_q) {
-  const bool use_stats = SPEC < 0 && ep.stats_out != nullptr;
-  if (use_stats && (c & 1) == 0) {
-    // shift = what the first column of the slot will store (bf16): recomputed here, cheap
-    st_s = 0.f;
-    st_q = 0.f;
-    float v0;
-    const int col = c * 32;
-    if (ep.ln_stats != nullptr) v0 = act_apply(fmaf(__uint_as_float(r[0]), er.ln_a, fmaf(er.ln_b, s_c[col], s_bias[col])), ep.act);
-    else v0 = act_apply(__uint_as_float(r[0]) + s_bias[col], ep.act);
-    if (er.res_ptr) v0 = __fadd_rn(v0, unpack_bf16x2(res4[0].x).x);
-    st_k = __bfloat162float(__float2bfloat16_rn(v0));
-  }
+__device__ __forceinline__ void epi_chunk(const EpiRow& er, const uint32_t* r, const float* s_bias, int c, int n0, int N,
+                                          const uint4* res4) {
 #pragma unroll
   for (int g = 0; g < 4; g++) {
     const int col = c * 32 + g * 8;
-    if (n0 + col < N) epi_store8<SPEC>(ep, er, r + g * 8, s_bias, s_c, col, n0, res4[g], st_k, st_s, st_q);
-  }
-  if (use_stats && (c & 1) == 1 && n0 + c * 32 < N) {
-    const float mean = st_k + st_s * (1.0f / 64.0f);
-    const float m2 = fmaxf(st_q - st_s * st_s * (1.0f / 64.0f), 0.f);
-    ep.stats_out[(int64_t)row * (N >> 6) + ((n0 + c * 32) >> 6)] = make_float2(mean, m2);
+    if (n0 + col < N) epi_store8<SPEC>(er, r + g * 8, s_bias, col, res4[g]);
   }
 }
 
-template <int BN, int SPEC = -1>
+template <int BN, int SPEC>
 __global__ void __launch_bounds__(GEMM_THREADS, 2)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N,
                        int K, GemmEpilogue ep) {
@@ -232,8 +156,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   uint8_t* sA = base;
   uint8_t* sB = base + STAGES * Cfg::A_BYTES;
   float* s_bias = reinterpret_cast<float*>(base + Cfg::RING_BYTES);
-  float* s_c = s_bias + BN;
-  uint64_t* full = reinterpret_cast<uint64_t*>(s_c + BN);
+  uint64_t* full = reinterpret_cast<uint64_t*>(s_bias + BN);
   uint64_t* empty = full + STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -249,10 +172,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     }
     ptx::fence_barrier_init();
   }
-  for (int j = threadIdx.x; j < BN; j += GEMM_THREADS) {
+  for (int j = threadIdx.x; j < BN; j += GEMM_THREADS)
     s_bias[j] = (ep.bias != nullptr && n0 + j < N) ? ep.bias[n0 + j] : 0.0f;
-    if (SPEC < 0) s_c[j] = (ep.ln_c != nullptr && n0 + j < N) ? ep.ln_c[n0 + j] : 0.0f;
-  }
   __syncthreads();
 
   if (warp == GEMM_WARP_TMA) {
@@ -315,16 +236,14 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   const bool row_ok = row < M;
   constexpr int CPW = BN >= 64 ? BN / 64 : 1;   // 32-column chunks per epilogue warp
   if (!row_ok || half * CPW * 32 >= BN) return;  // BN = 32: the second warp of each quarter has no columns
-  EpiRow er = epi_row(ep, row, n0);
-  if (SPEC < 0 && ep.ln_stats != nullptr) ln_row_coeffs(ep.ln_stats + (int64_t)row * (ep.ln_w >> 6), ep.ln_w >> 6, ep.ln_w, er.ln_a, er.ln_b);
-  float st_k = 0.f, st_s = 0.f, st_q = 0.f;
+  const EpiRow er = epi_row(ep, row, n0);
   uint4 res[CPW][4];
 #pragma unroll
   for (int ci = 0; ci < CPW; ci++) {
 #pragma unroll
     for (int g = 0; g < 4; g++) {
       const int col = (half * CPW + ci) * 32 + g * 8;
-      const bool want = SPEC >= 0 ? ((SPEC >> 2) & 1) != 0 : er.res_ptr != nullptr;
+      constexpr bool want = ((SPEC >> 2) & 1) != 0;
       res[ci][g] = (want && n0 + col < N) ? *reinterpret_cast<const uint4*>(er.res_ptr + col) : make_uint4(0u, 0u, 0u, 0u);
     }
   }
@@ -339,7 +258,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       r[4 * i] = __float_as_uint(v.x); r[4 * i + 1] = __float_as_uint(v.y);
       r[4 * i + 2] = __float_as_uint(v.z); r[4 * i + 3] = __float_as_uint(v.w);
     }
-    epi_chunk<SPEC>(ep, er, r, s_bias, s_c, c, n0, N, row, res[ci], st_k, st_s, st_q);
+    epi_chunk<SPEC>(er, r, s_bias, c, n0, N, res[ci]);
   }
 }
 
@@ -370,7 +289,6 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 // each warp passes its 16 x 256 slab through a private 16 x 32 fp32 staging chunk so that its stores run along rows.
 // Both epilogues compute every element with epi_apply, so outputs are bit-identical to the 128-wide kernel's (the
 // same k16 wgmma sequence feeds it).
-// Only the compile-time epilogue flavours (SPEC 0..7); the LayerNorm fold and row statistics stay on the kernel above.
 // A variant with CTA pairs (clusters of 2 along M) multicasting one 128-row W half each was built and measured slower
 // at every bench shape (DESIGN.md §8), so W is loaded per CTA.
 constexpr int GEMM_WIDE_BN = 256;
@@ -410,7 +328,6 @@ __global__ void __launch_bounds__(GEMM_WIDE_THREADS, 1)
 gemm_bf16_wgmma_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                                   const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR,
                                   int M, int N, int K, GemmEpilogue ep) {
-  static_assert(SPEC >= 0 && SPEC < 8, "compile-time epilogue flavours only");
   constexpr int STAGES = Cfg::STAGES;
   constexpr int BN = GEMM_WIDE_BN;
   constexpr bool HAS_RES = ((SPEC >> 2) & 1) != 0;
@@ -635,8 +552,7 @@ gemm_bf16_wgmma_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const
             const float4 u = sw ? h1 : h0, v = sw ? h0 : h1;
             const uint32_t r8[8] = {__float_as_uint(u.x), __float_as_uint(u.y), __float_as_uint(u.z), __float_as_uint(u.w),
                                     __float_as_uint(v.x), __float_as_uint(v.y), __float_as_uint(v.z), __float_as_uint(v.w)};
-            float st_s = 0.f, st_q = 0.f;
-            epi_store8<SPEC>(ep, er[q], r8, bias_t, nullptr, col, n0, res[c & 1][q], 0.f, st_s, st_q);
+            epi_store8<SPEC>(er[q], r8, bias_t, col, res[c & 1][q]);
           }
         }
       }
@@ -649,18 +565,13 @@ int make_tmap_2d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t row
                  uint32_t box_rows, uint32_t box_cols);
 int make_tmap_3d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t planes, uint64_t rows, uint64_t cols,
                  uint64_t ld_row, uint64_t ld_plane, uint32_t box_rows, uint32_t box_cols);
-// tmB must have boxes of bn rows x 64 columns (128 rows for bn = 256).  generic = true launches the run-time epilogue
-// flavour (SPEC = -1) even where a compile-time flavour applies (the tests check that both store the same bits).
-// bn = 256 (the persistent kernel) takes the compile-time flavours only: B200_ERR_INVALID for generic, ln_stats or
-// stats_out.  It stores by TMA from 8 tiles per CTA up (or with force_tma_epilogue), else from registers.
+// tmB must have boxes of bn rows x 64 columns (128 rows for bn = 256).  The epilogue flavour (activation | residual
+// << 2) is a template argument of the kernel: ep.act outside 0..2 is B200_ERR_INVALID.  bn = 256 (the persistent
+// kernel) stores by TMA from 8 tiles per CTA up (or with force_tma_epilogue), else from registers.
 int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int M, int N, int K,
-                     const GemmEpilogue& ep, cudaStream_t st, bool generic = false, bool force_tma_epilogue = false);
-// true when a compile-time epilogue flavour covers `ep` (no LayerNorm fold, no row statistics)
-inline bool gemm_epilogue_is_plain(const GemmEpilogue& ep) {
-  return ep.ln_stats == nullptr && ep.stats_out == nullptr && ep.ln_c == nullptr && ep.act >= 0 && ep.act <= 2;
-}
-// Pick the column-block width for a GEMM with N output columns: 256 (persistent kernel) for large grids when `wide`
-// (the epilogue is plain), else 128, or 64 / 32 when the grid would be under-filled.
-int gemm_pick_bn(int M, int N, int sms, bool wide);
+                     const GemmEpilogue& ep, cudaStream_t st, bool force_tma_epilogue = false);
+// Pick the column-block width for a GEMM with N output columns: 256 (persistent kernel) for large grids, else 128,
+// or 64 / 32 when the grid would be under-filled.
+int gemm_pick_bn(int M, int N, int sms);
 
 }  // namespace b200

@@ -53,9 +53,7 @@ struct b200_index {
   void* ws[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // 0: scan internals; 1..3: callers; 4,5: hi-only mode
   size_t ws_bytes[6] = {0, 0, 0, 0, 0, 0};
   std::mutex mu;             // every search entry (host and device) holds it while it enqueues work
-  cudaEvent_t scratch_ev = nullptr;   // recorded after the last search's launches: the next search on ANOTHER
-  cudaStream_t scratch_stream = nullptr;   // stream waits on it before it reuses ws[] / norm_bound[]
-  bool scratch_used = false;
+  b200::StreamFence scratch; // orders the searches that reuse ws[] / norm_bound[] / timing events across streams
 
   // Serving shape (nq <= 4: clip_back.py:362 issues one query): the launches of a search are captured once per
   // (nq, k, nprobe, reconstruct) into a CUDA graph over fixed buffers and replayed; any mutation of the index bumps

@@ -226,7 +226,6 @@ int b200_index_destroy(b200_index* idx) {
   for (float* b : idx->norm_bound)
     if (b) cudaFree(b);
   for (auto e : idx->ev) cudaEventDestroy(e);
-  if (idx->scratch_ev) cudaEventDestroy(idx->scratch_ev);
   for (auto& kv : idx->graphs) if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
   if (idx->cap_stream) cudaStreamDestroy(idx->cap_stream);
   if (idx->g_q) cudaFree(idx->g_q);
@@ -381,21 +380,6 @@ int b200_index_ivf_lists(b200_index* idx, int64_t* h_sizes, int64_t* h_ids) {
   return ivf_lists(idx, h_sizes, h_ids);
 }
 
-// The per-index scratch (ws[], norm_bound[], timing events) is shared by every search on the handle.  Calls are
-// serialised on idx->mu while they enqueue; a call on a different stream than the previous one first makes
-// its stream wait for the previous call's kernels (event), so in-flight work never sees its buffers reused.
-static int scratch_acquire(b200_index* idx, cudaStream_t st) {
-  if (!idx->scratch_ev) B200_CUDA(cudaEventCreateWithFlags(&idx->scratch_ev, cudaEventDisableTiming));
-  if (idx->scratch_used && idx->scratch_stream != st) B200_CUDA(cudaStreamWaitEvent(st, idx->scratch_ev, 0));
-  return B200_OK;
-}
-static int scratch_release(b200_index* idx, cudaStream_t st) {
-  B200_CUDA(cudaEventRecord(idx->scratch_ev, st));
-  idx->scratch_stream = st;
-  idx->scratch_used = true;
-  return B200_OK;
-}
-
 // nq <= 4 through a replayed CUDA graph: returns 1 when the search was served from a graph, 0 when the caller must
 // launch eagerly (first sighting of the shape, graphs disabled, stream already capturing), < 0 on error.
 static int search_graph(b200_index* idx, const float* d_q, int nq, int k, float* d_D, int64_t* d_I, float* d_R,
@@ -472,7 +456,7 @@ int b200_index_search_device(b200_index* idx, const float* d_q, int nq, int k, f
   B200_CHECK(idx, B200_ERR_INVALID, "search: null index");
   std::lock_guard<std::mutex> lock(idx->mu);
   DeviceGuard g(idx->device);
-  B200_TRY(scratch_acquire(idx, (cudaStream_t)stream));
+  B200_TRY(idx->scratch.acquire((cudaStream_t)stream));
   int rc = B200_OK;
   if (d_q && d_D && d_I && nq >= 1 && k >= 1 && ((uintptr_t)d_q & 15) == 0) {
     if (idx->nlist > 0) B200_TRY(ivf_finalize(idx));
@@ -480,7 +464,7 @@ int b200_index_search_device(b200_index* idx, const float* d_q, int nq, int k, f
   }
   if (rc == 0) rc = search_device_impl(idx, d_q, nq, k, d_D, d_I, d_R, (cudaStream_t)stream);
   else if (rc == 1) rc = B200_OK;
-  B200_TRY(scratch_release(idx, (cudaStream_t)stream));
+  B200_TRY(idx->scratch.release((cudaStream_t)stream));
   return rc;
 }
 
@@ -501,10 +485,10 @@ int b200_index_search(b200_index* idx, const float* h_q, int nq, int k, float* h
   float* d_D = (float*)p; p += al(db);
   int64_t* d_I = (int64_t*)p; p += al(ib);
   float* d_R = h_R ? (float*)p : nullptr;
-  B200_TRY(scratch_acquire(idx, 0));
+  B200_TRY(idx->scratch.acquire(0));
   B200_CUDA(cudaMemcpyAsync(d_q, h_q, qb, cudaMemcpyHostToDevice, 0));
   B200_TRY(search_device_impl(idx, d_q, nq, k, d_D, d_I, d_R, 0));   // legacy stream: never captured
-  B200_TRY(scratch_release(idx, 0));
+  B200_TRY(idx->scratch.release(0));
   B200_CUDA(cudaMemcpyAsync(h_D, d_D, db, cudaMemcpyDeviceToHost, 0));
   B200_CUDA(cudaMemcpyAsync(h_I, d_I, ib, cudaMemcpyDeviceToHost, 0));
   if (h_R) B200_CUDA(cudaMemcpyAsync(h_R, d_R, rb, cudaMemcpyDeviceToHost, 0));
@@ -526,7 +510,7 @@ int b200_index_range_search(b200_index* idx, const float* h_q, float thresh, int
   unsigned long long* d_keys = (unsigned long long*)((char*)ws + qb + 256);
   float* d_D = (float*)(d_keys + cap);
   int64_t* d_I = (int64_t*)((char*)d_D + (((size_t)cap * 4 + 7) & ~(size_t)7));
-  B200_TRY(scratch_acquire(idx, 0));
+  B200_TRY(idx->scratch.acquire(0));
   B200_CUDA(cudaMemcpyAsync(d_q, h_q, (size_t)idx->d_in * 4, cudaMemcpyHostToDevice, 0));
   if (idx->pq_M > 0) {
     B200_TRY(ivf_finalize(idx));

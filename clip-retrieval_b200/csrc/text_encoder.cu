@@ -13,6 +13,7 @@
 #include "common.cuh"
 #include "embed_kernels.cuh"
 #include "gemm.cuh"
+#include "layers.cuh"
 #include "weights.cuh"
 #include <algorithm>
 #include <map>
@@ -23,15 +24,8 @@
 namespace b200 {
 namespace {
 
-struct EncLinear {
-  __nv_bfloat16* w = nullptr;   // [N, K]
-  float* b = nullptr;           // [N]
-  int N = 0, K = 0;
-  CUtensorMap tm128, tm64, tm32;
-};
-
 struct EncLayer {
-  EncLinear qkv, out, fc1, fc2;
+  Linear qkv, out, fc1, fc2;
   float *ln1_g = nullptr, *ln1_b = nullptr, *ln2_g = nullptr, *ln2_b = nullptr;
 };
 
@@ -44,7 +38,7 @@ struct b200_text_encoder {
   b200_text_encoder_config cfg;
   int device = 0, sms = 132;
   bool loaded = false;
-  std::vector<void*> allocs;
+  b200::DeviceAllocs allocs;
   // weights
   __nv_bfloat16* word = nullptr;   // [vocab, w]
   float* tt0 = nullptr;            // token type 0 [w] or null
@@ -56,73 +50,28 @@ struct b200_text_encoder {
   // activations
   __nv_bfloat16 *x = nullptr, *qkv = nullptr, *a = nullptr, *f = nullptr;
   CUtensorMap tm_x, tm_a, tm_f;
-  std::map<int, CUtensorMap> tm_qkv;   // per T: qkv as [max_batch, T, 3w], boxes of 64 tokens x 64 columns
+  std::map<int, CUtensorMap> tm_qkv;   // per T: make_qkv_map over max_batch samples
   float* feat = nullptr;               // [max_batch, D]
   // staging of the host entry
   int64_t* s_ids = nullptr;
   int* s_len = nullptr;
-  void* s_out = nullptr;
-  std::mutex mu;
-  // timing
-  bool profiling = false;
-  struct Span { int cls; cudaEvent_t a, b; };
-  std::vector<Span> spans;
-  int span_used = 0;
-  int last_launches = 0;
+  float* s_out = nullptr;
+  std::mutex mu;                  // held by both encode entries while they enqueue
+  b200::StreamFence act;          // orders calls on different streams: they share the activation buffers
+  b200::SpanTimer timer;          // timing; timer.launches = kernels of the last encode call
 };
 
 namespace b200 {
 namespace {
 
-template <typename T>
-int enc_alloc(b200_text_encoder* m, T** p, size_t count) {
-  void* q = nullptr;
-  B200_CUDA(cudaMalloc(&q, std::max<size_t>(count, 1) * sizeof(T)));
-  m->allocs.push_back(q);
-  *p = (T*)q;
-  return B200_OK;
-}
-
-int enc_linear(b200_text_encoder* m, EncLinear* l, int N, int K) {
-  l->N = N;
-  l->K = K;
-  B200_TRY(enc_alloc(m, &l->w, (size_t)N * K));
-  B200_TRY(enc_alloc(m, &l->b, (size_t)N));
-  B200_TRY(make_tmap_2d(&l->tm128, l->w, 1, N, K, K, 128, GEMM_BK));
-  B200_TRY(make_tmap_2d(&l->tm64, l->w, 1, N, K, K, 64, GEMM_BK));
-  B200_TRY(make_tmap_2d(&l->tm32, l->w, 1, N, K, K, 32, GEMM_BK));
-  return B200_OK;
-}
-
-struct EncSpan {
-  b200_text_encoder* m; cudaStream_t st; int idx = -1;
-  EncSpan(b200_text_encoder* m_, int cls, cudaStream_t s, int kernels) : m(m_), st(s) {
-    m->last_launches += kernels;
-    if (!m->profiling) return;
-    if (m->span_used == (int)m->spans.size()) {
-      b200_text_encoder::Span sp;
-      if (cudaEventCreate(&sp.a) != cudaSuccess || cudaEventCreate(&sp.b) != cudaSuccess) return;
-      m->spans.push_back(sp);
-    }
-    idx = m->span_used++;
-    m->spans[idx].cls = cls;
-    cudaEventRecord(m->spans[idx].a, st);
-  }
-  ~EncSpan() {
-    if (idx >= 0) cudaEventRecord(m->spans[idx].b, st);
-  }
-};
-
-int enc_gemm(b200_text_encoder* m, const CUtensorMap& tmA, const EncLinear& l, int M, GemmEpilogue ep, cudaStream_t st) {
-  EncSpan sp(m, ENC_GEMM, st, 1);
-  const int bn = gemm_pick_bn(M, l.N, m->sms, gemm_epilogue_is_plain(ep));
-  ep.bias = l.b;
-  const CUtensorMap& tmB = bn == 64 ? l.tm64 : (bn == 32 ? l.tm32 : l.tm128);
-  return gemm_bf16_launch(tmA, tmB, bn, M, l.N, l.K, ep, st);
+int enc_gemm(b200_text_encoder* m, const CUtensorMap& tmA, const Linear& l, int M, const GemmEpilogue& ep,
+             cudaStream_t st) {
+  TimedSpan sp(m->timer, ENC_GEMM, st, 1);
+  return linear_gemm(l, tmA, M, ep, m->sms, st);
 }
 
 int enc_ln(b200_text_encoder* m, const float* g, const float* b, int64_t rows, cudaStream_t st) {
-  EncSpan sp(m, ENC_LN, st, 1);
+  TimedSpan sp(m->timer, ENC_LN, st, 1);
   const int w = m->cfg.width;
   return layernorm_rows_eps(m->x, w, m->x, w, g, b, rows, w, m->cfg.layer_norm_eps, st);
 }
@@ -132,27 +81,24 @@ int enc_forward(b200_text_encoder* m, const int64_t* d_ids, const int* d_len, in
                 int normalize, cudaStream_t st) {
   const b200_text_encoder_config& c = m->cfg;
   const int w = c.width, M = B * T;
-  const bool wg = attention_wgmma_supported(T, c.heads, w);
   const CUtensorMap* tmq = nullptr;
-  if (wg) {
+  if (attention_wgmma_supported(T, c.heads, w)) {
     auto it = m->tm_qkv.find(T);
     if (it == m->tm_qkv.end()) {
       CUtensorMap tm;
-      B200_TRY(make_tmap_3d(&tm, m->qkv, 1, (uint64_t)c.max_batch, (uint64_t)T, 3 * (uint64_t)w, 3 * (uint64_t)w,
-                            (uint64_t)T * 3 * w, 64, 64));
+      B200_TRY(make_qkv_map(&tm, m->qkv, c.max_batch, T, w));
       it = m->tm_qkv.emplace(T, tm).first;
     }
     tmq = &it->second;
   }
-  { EncSpan sp(m, ENC_OTHER, st, 1);
+  { TimedSpan sp(m->timer, ENC_OTHER, st, 1);
     B200_TRY(encoder_embed(d_ids, m->word, m->tt0, m->pos, c.position_offset, m->emb_g, m->emb_b, c.layer_norm_eps,
                            m->x, B, T, w, c.vocab_size, st)); }
   for (const EncLayer& L : m->L) {
     GemmEpilogue e1; e1.out = m->qkv; e1.out_ld = 3 * w;
     B200_TRY(enc_gemm(m, m->tm_x, L.qkv, M, e1, st));
-    { EncSpan sp(m, ENC_ATTN, st, 1);
-      if (wg) B200_TRY(attention_wgmma(*tmq, m->a, B, T, c.heads, w, 0, st, d_len));
-      else B200_TRY(attention(m->qkv, m->a, B, T, c.heads, w, 0, st, d_len)); }
+    { TimedSpan sp(m->timer, ENC_ATTN, st, 1);
+      B200_TRY(qkv_attention(tmq, m->qkv, m->a, B, T, c.heads, w, 0, st, d_len)); }
     GemmEpilogue e2; e2.out = m->x; e2.out_ld = w; e2.residual = m->x; e2.res_ld = w;
     B200_TRY(enc_gemm(m, m->tm_a, L.out, M, e2, st));
     B200_TRY(enc_ln(m, L.ln1_g, L.ln1_b, M, st));
@@ -162,7 +108,7 @@ int enc_forward(b200_text_encoder* m, const int64_t* d_ids, const int* d_len, in
     B200_TRY(enc_gemm(m, m->tm_f, L.fc2, M, e4, st));
     B200_TRY(enc_ln(m, L.ln2_g, L.ln2_b, M, st));
   }
-  EncSpan sp(m, ENC_OTHER, st, 2);
+  TimedSpan sp(m->timer, ENC_OTHER, st, 2);
   return masked_mean_proj_norm(m->x, T, w, d_len, m->projT, m->proj_b, c.out_dim, m->feat, d_out, out_f16, normalize,
                                B, st);
 }
@@ -175,7 +121,7 @@ int enc_encode(b200_text_encoder* m, const int64_t* d_ids, const int* d_len, int
              m->cfg.max_tokens);
   B200_CHECK(out_dtype == B200_OUT_F16 || out_dtype == B200_OUT_F32, B200_ERR_INVALID, "text_encoder: out_dtype %d",
              out_dtype);
-  m->last_launches = 0;
+  m->timer.launches = 0;
   const int mb = m->cfg.max_batch;
   const size_t out_stride = (size_t)m->cfg.out_dim * (out_dtype == B200_OUT_F16 ? 2 : 4);
   for (int b0 = 0; b0 < B; b0 += mb) {
@@ -215,35 +161,34 @@ int b200_text_encoder_create(const b200_text_encoder_config* cfg, int device, b2
   auto build = [&]() -> int {
     const int w = c.width;
     const size_t rows = (size_t)c.max_batch * c.max_tokens;
-    B200_TRY(enc_alloc(m, &m->word, (size_t)c.vocab_size * w));
-    if (c.type_vocab_size > 0) B200_TRY(enc_alloc(m, &m->tt0, (size_t)w));
-    B200_TRY(enc_alloc(m, &m->pos, (size_t)c.max_positions * w));
-    B200_TRY(enc_alloc(m, &m->emb_g, (size_t)w));
-    B200_TRY(enc_alloc(m, &m->emb_b, (size_t)w));
+    DeviceAllocs& al = m->allocs;
+    B200_TRY(al.alloc(&m->word, (size_t)c.vocab_size * w));
+    if (c.type_vocab_size > 0) B200_TRY(al.alloc(&m->tt0, (size_t)w));
+    B200_TRY(al.alloc(&m->pos, (size_t)c.max_positions * w));
+    B200_TRY(al.alloc(&m->emb_g, (size_t)w));
+    B200_TRY(al.alloc(&m->emb_b, (size_t)w));
     m->L.resize(c.layers);
     for (EncLayer& L : m->L) {
-      B200_TRY(enc_linear(m, &L.qkv, 3 * w, w));
-      B200_TRY(enc_linear(m, &L.out, w, w));
-      B200_TRY(enc_linear(m, &L.fc1, c.ffn, w));
-      B200_TRY(enc_linear(m, &L.fc2, w, c.ffn));
-      B200_TRY(enc_alloc(m, &L.ln1_g, (size_t)w)); B200_TRY(enc_alloc(m, &L.ln1_b, (size_t)w));
-      B200_TRY(enc_alloc(m, &L.ln2_g, (size_t)w)); B200_TRY(enc_alloc(m, &L.ln2_b, (size_t)w));
+      B200_TRY(make_linear(al, &L.qkv, 3 * w, w, true));
+      B200_TRY(make_linear(al, &L.out, w, w, true));
+      B200_TRY(make_linear(al, &L.fc1, c.ffn, w, true));
+      B200_TRY(make_linear(al, &L.fc2, w, c.ffn, true));
+      B200_TRY(al.alloc(&L.ln1_g, (size_t)w)); B200_TRY(al.alloc(&L.ln1_b, (size_t)w));
+      B200_TRY(al.alloc(&L.ln2_g, (size_t)w)); B200_TRY(al.alloc(&L.ln2_b, (size_t)w));
     }
-    B200_TRY(enc_alloc(m, &m->projT, (size_t)w * c.out_dim));
-    if (c.proj_bias) B200_TRY(enc_alloc(m, &m->proj_b, (size_t)c.out_dim));
-    B200_TRY(enc_alloc(m, &m->x, rows * w));
-    B200_TRY(enc_alloc(m, &m->qkv, rows * 3 * w));
-    B200_TRY(enc_alloc(m, &m->a, rows * w));
-    B200_TRY(enc_alloc(m, &m->f, rows * c.ffn));
+    B200_TRY(al.alloc(&m->projT, (size_t)w * c.out_dim));
+    if (c.proj_bias) B200_TRY(al.alloc(&m->proj_b, (size_t)c.out_dim));
+    B200_TRY(al.alloc(&m->x, rows * w));
+    B200_TRY(al.alloc(&m->qkv, rows * 3 * w));
+    B200_TRY(al.alloc(&m->a, rows * w));
+    B200_TRY(al.alloc(&m->f, rows * c.ffn));
     B200_TRY(make_tmap_2d(&m->tm_x, m->x, 1, rows, w, w, GEMM_BM, GEMM_BK));
     B200_TRY(make_tmap_2d(&m->tm_a, m->a, 1, rows, w, w, GEMM_BM, GEMM_BK));
     B200_TRY(make_tmap_2d(&m->tm_f, m->f, 1, rows, c.ffn, c.ffn, GEMM_BM, GEMM_BK));
-    B200_TRY(enc_alloc(m, &m->feat, (size_t)c.max_batch * c.out_dim));
-    B200_TRY(enc_alloc(m, &m->s_ids, rows));
-    B200_TRY(enc_alloc(m, &m->s_len, (size_t)c.max_batch));
-    float* so = nullptr;
-    B200_TRY(enc_alloc(m, &so, (size_t)c.max_batch * c.out_dim));
-    m->s_out = so;
+    B200_TRY(al.alloc(&m->feat, (size_t)c.max_batch * c.out_dim));
+    B200_TRY(al.alloc(&m->s_ids, rows));
+    B200_TRY(al.alloc(&m->s_len, (size_t)c.max_batch));
+    B200_TRY(al.alloc(&m->s_out, (size_t)c.max_batch * c.out_dim));
     return B200_OK;
   };
   const int rc = build();
@@ -259,8 +204,7 @@ int b200_text_encoder_destroy(b200_text_encoder* m) {
   if (!m) return B200_OK;
   DeviceGuard g(m->device);
   cudaDeviceSynchronize();
-  for (void* p : m->allocs) cudaFree(p);
-  for (auto& s : m->spans) { cudaEventDestroy(s.a); cudaEventDestroy(s.b); }
+  m->allocs.free_all();
   delete m;
   return B200_OK;
 }
@@ -269,12 +213,7 @@ int b200_text_encoder_load_weights(b200_text_encoder* m, const b200_tensor_view*
   B200_CHECK(m && tensors && n > 0, B200_ERR_INVALID, "text_encoder_load_weights: bad argument");
   DeviceGuard g(m->device);
   Loader ld;
-  for (int i = 0; i < n; i++) {
-    B200_CHECK(tensors[i].name && tensors[i].data && (tensors[i].dtype == 0 || tensors[i].dtype == 1) &&
-                   tensors[i].ndim >= 0 && tensors[i].ndim <= 4,
-               B200_ERR_INVALID, "text_encoder_load_weights: malformed tensor view %d", i);
-    ld.by_name[tensors[i].name] = &tensors[i];
-  }
+  B200_TRY(ld.index(tensors, n));
   const b200_text_encoder_config& c = m->cfg;
   const size_t w = c.width, D = c.out_dim, ffn = c.ffn;
   B200_TRY(ld.put_bf16("embeddings.word_embeddings.weight", m->word, (size_t)c.vocab_size, w, w));
@@ -329,7 +268,11 @@ int b200_text_encoder_encode_device(b200_text_encoder* m, const int64_t* d_ids, 
   B200_CHECK(m, B200_ERR_INVALID, "text_encoder_encode: null handle");
   std::lock_guard<std::mutex> lock(m->mu);
   DeviceGuard g(m->device);
-  return enc_encode(m, d_ids, d_len, B, T, d_out, out_dtype, normalize, (cudaStream_t)stream);
+  const cudaStream_t st = (cudaStream_t)stream;
+  B200_TRY(m->act.acquire(st));
+  const int rc = enc_encode(m, d_ids, d_len, B, T, d_out, out_dtype, normalize, st);
+  B200_TRY(m->act.release(st));
+  return rc;
 }
 
 int b200_text_encoder_encode(b200_text_encoder* m, const int64_t* h_ids, const int32_t* h_len, int B, int T,
@@ -342,6 +285,7 @@ int b200_text_encoder_encode(b200_text_encoder* m, const int64_t* h_ids, const i
                h_len[b], T);
   std::lock_guard<std::mutex> lock(m->mu);
   DeviceGuard g(m->device);
+  B200_TRY(m->act.acquire(nullptr));   // the legacy stream, which does not wait for work on non-blocking streams
   const int mb = m->cfg.max_batch;
   const size_t out_stride = (size_t)m->cfg.out_dim * (out_dtype == B200_OUT_F16 ? 2 : 4);
   int launches = 0;
@@ -350,33 +294,25 @@ int b200_text_encoder_encode(b200_text_encoder* m, const int64_t* h_ids, const i
     B200_CUDA(cudaMemcpy(m->s_ids, h_ids + (size_t)b0 * T, (size_t)nb * T * 8, cudaMemcpyHostToDevice));
     B200_CUDA(cudaMemcpy(m->s_len, h_len + b0, (size_t)nb * 4, cudaMemcpyHostToDevice));
     B200_TRY(enc_encode(m, m->s_ids, m->s_len, nb, T, m->s_out, out_dtype, normalize, nullptr));
-    launches += m->last_launches;
+    launches += m->timer.launches;
     B200_CUDA(cudaMemcpy((char*)h_out + b0 * out_stride, m->s_out, nb * out_stride, cudaMemcpyDeviceToHost));
   }
-  m->last_launches = launches;
+  B200_TRY(m->act.release(nullptr));
+  m->timer.launches = launches;
   return B200_OK;
 }
 
 int b200_text_encoder_set_profiling(b200_text_encoder* m, int on) {
   B200_CHECK(m, B200_ERR_INVALID, "text_encoder_set_profiling: null handle");
-  m->profiling = on != 0;
-  m->span_used = 0;
+  m->timer.set_profiling(on != 0);
   return B200_OK;
 }
 
 int b200_text_encoder_last_timing(b200_text_encoder* m, float* ms_by_class, int* launches) {
   B200_CHECK(m && ms_by_class, B200_ERR_INVALID, "text_encoder_last_timing: null argument");
   DeviceGuard g(m->device);
-  for (int i = 0; i < ENC_CLASSES; i++) ms_by_class[i] = 0.f;
-  for (int i = 0; i < m->span_used; i++) {
-    const auto& s = m->spans[i];
-    B200_CUDA(cudaEventSynchronize(s.b));
-    float t = 0.f;
-    B200_CUDA(cudaEventElapsedTime(&t, s.a, s.b));
-    ms_by_class[s.cls] += t;
-  }
-  if (launches) *launches = m->last_launches;
-  m->span_used = 0;
+  B200_TRY(m->timer.collect(ms_by_class, ENC_CLASSES));
+  if (launches) *launches = m->timer.launches;
   return B200_OK;
 }
 
@@ -392,13 +328,8 @@ int b200_attention_len_bf16_device(const void* d_qkv, const int32_t* d_len, void
                                    int device, void* stream) {
   B200_CHECK(d_qkv && d_len && d_out && B >= 0 && T >= 1, B200_ERR_INVALID, "attention_len: bad argument");
   DeviceGuard g(device);
-  if (B > 0 && attention_wgmma_supported(T, heads, w)) {
-    CUtensorMap tm;
-    B200_TRY(make_tmap_3d(&tm, d_qkv, 1, (uint64_t)B, (uint64_t)T, 3 * (uint64_t)w, 3 * (uint64_t)w, (uint64_t)T * 3 * w,
-                          64, 64));
-    return attention_wgmma(tm, (__nv_bfloat16*)d_out, B, T, heads, w, 0, (cudaStream_t)stream, d_len);
-  }
-  return attention((const __nv_bfloat16*)d_qkv, (__nv_bfloat16*)d_out, B, T, heads, w, 0, (cudaStream_t)stream, d_len);
+  return qkv_attention(nullptr, (const __nv_bfloat16*)d_qkv, (__nv_bfloat16*)d_out, B, T, heads, w, 0,
+                       (cudaStream_t)stream, d_len);
 }
 
 int b200_encoder_embed_bf16_device(const int64_t* d_ids, const void* d_word, const float* d_tt0, const float* d_pos,

@@ -30,6 +30,16 @@ struct Loader {
   std::map<std::string, const b200_tensor_view*> by_name;
   std::vector<uint16_t> tmp16;
   std::vector<float> tmp32;
+  // Indexes the caller's n views by name (they must outlive the loader); B200_ERR_INVALID for a malformed view.
+  int index(const b200_tensor_view* views, int n) {
+    for (int i = 0; i < n; i++) {
+      B200_CHECK(views[i].name && views[i].data && (views[i].dtype == 0 || views[i].dtype == 1) && views[i].ndim >= 0 &&
+                     views[i].ndim <= 4,
+                 B200_ERR_INVALID, "load_weights: malformed tensor view %d", i);
+      by_name[views[i].name] = &views[i];
+    }
+    return B200_OK;
+  }
   const b200_tensor_view* find(const std::string& name, size_t count) {
     auto it = by_name.find(name);
     if (it == by_name.end()) { set_error("load_weights: tensor '%s' is missing", name.c_str()); return nullptr; }

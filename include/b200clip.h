@@ -306,16 +306,13 @@ int b200_gemm_bf16_device(const void* d_A, const void* d_W, const float* d_bias,
  *   r                                                  (out_group == 0)
  *   (r / out_group) * (out_group + 1) + 1 + r % out_group  (out_group > 0: one cls row skipped per group)
  * and reads residual row r, or res_row_off + r % res_row_mod when res_row_mod > 0.  ld 0 means N.
- * Folded LayerNorm (ln_stats != NULL): A is the raw row x, W carries gamma (W' = W * gamma), bias = d, and the
- * result is rstd * (x W'^T - mean * ln_c) + d, with mean / rstd (eps 1e-5) combined from ln_w / 64 (mean, M2)
- * float2 records per row.  stats_out != NULL: one (mean, M2) float2 record per 64 stored columns of every row
- * (needs N % 64 == 0 and 128-wide column blocks).
- * bn: 0 = the width the library picks (128 whenever stats_out is set), else 32, 64, 128 or 256.  256 is the
- * persistent 128 x 256 kernel of the large-batch shapes: it takes the compile-time epilogue flavours only, and is
- * refused (B200_ERR_INVALID) with force_generic, stats_out or ln_stats.
- * force_generic bit 0 (or any value other than 2): the epilogue flavour that decides every feature at run time,
- * even where a compile-time flavour exists; both store the same bits.  force_generic == 2: with bn = 256, the TMA-store
- * epilogue whatever the grid size (the library takes it from 8 tiles per SM up); the same bits again. */
+ * bn: 0 = the width the library picks, else 32, 64, 128 or 256.  256 is the persistent 128 x 256 kernel of the
+ * large-batch shapes.
+ * flags: 0, or 2 = with bn = 256, the TMA-store epilogue whatever the grid size (the library takes it from 8 tiles
+ * per SM up); it stores the same bits.  Any other bit is refused (B200_ERR_INVALID).
+ * The four reserved members once carried the inputs of a LayerNorm fold that no longer exists.  They keep the
+ * struct's size and layout, so callers that fill it positionally keep working, and must be NULL / 0: anything else
+ * is refused (B200_ERR_INVALID) rather than ignored. */
 typedef struct b200_gemm_epilogue {
   const float* bias;        /* [N] fp32 or NULL */
   const void* residual;     /* bf16, added after the activation, or NULL; may equal the output (in-place update) */
@@ -324,16 +321,13 @@ typedef struct b200_gemm_epilogue {
   int64_t out_ld;
   int32_t out_group;
   int32_t act;              /* 0 none, 1 quick_gelu, 2 gelu(erf) */
-  const void* ln_stats;     /* float2 [M, ln_w / 64] or NULL */
-  const float* ln_c;        /* [N] */
-  int32_t ln_w;
-  void* stats_out;          /* float2 [M, N / 64] or NULL */
+  const void* reserved0;    /* NULL */
+  const void* reserved1;    /* NULL */
+  int32_t reserved2;        /* 0 */
+  const void* reserved3;    /* NULL */
 } b200_gemm_epilogue;
 int b200_gemm_bf16_ex_device(const void* d_A, const void* d_W, void* d_C, int M, int N, int K,
-                             const b200_gemm_epilogue* ep, int bn, int force_generic, int device, void* stream);
-/* The (mean, M2) records of the folded LayerNorm for rows of w bf16 values (w % 64 == 0): d_stats float2
- * [rows, w / 64], record s of a row = mean and sum of squared deviations of its columns 64 s .. 64 s + 63. */
-int b200_row_stats_bf16_device(const void* d_x, int64_t rows, int w, void* d_stats, int device, void* stream);
+                             const b200_gemm_epilogue* ep, int bn, int flags, int device, void* stream);
 
 /* Stand-alone entries of the two other embed kernels, for their parity tests:
  * LayerNorm (eps 1e-5) over rows of `w` bf16 values; multi-head attention over a fused qkv buffer

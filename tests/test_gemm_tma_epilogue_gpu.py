@@ -8,7 +8,7 @@ from test_gemm_gpu import FLAVOURS, _sms, operands, run
 
 pytestmark = pytest.mark.gpu
 
-TMA = 2   # force_generic == 2: the TMA-store epilogue at any grid size (the library takes it from 8 tiles per SM up)
+TMA = 2   # flags == 2: the TMA-store epilogue at any grid size (the library takes it from 8 tiles per SM up)
 
 
 def _nan(rows, cols):
@@ -30,7 +30,7 @@ def test_strided_output_guards_stay_nan(M, N):
     ld = N + 40
     for act, res in FLAVOURS:
         buf = _nan(M + 5, ld)
-        run(A, W, buf, bias=b, residual=R if res else None, out_ld=ld, act=act, bn=256, generic=TMA)
+        run(A, W, buf, bias=b, residual=R if res else None, out_ld=ld, act=act, bn=256, flags=TMA)
         ref = _nan(M, N)
         run(A, W, ref, bias=b, residual=R if res else None, act=act, bn=128)
         what = "M=%d N=%d act=%d res=%d" % (M, N, act, res)
@@ -50,7 +50,7 @@ def test_residual_ld_differs_from_output_ld(M, N, K):
     Rp[:, :N] = R
     for act in (0, 1, 2):
         buf = _nan(M, N + 72)
-        run(A, W, buf, bias=b, residual=Rp, res_ld=N + 16, out_ld=N + 72, act=act, bn=256, generic=TMA)
+        run(A, W, buf, bias=b, residual=Rp, res_ld=N + 16, out_ld=N + 72, act=act, bn=256, flags=TMA)
         ref = _nan(M, N)
         run(A, W, ref, bias=b, residual=R, act=act, bn=128)
         assert torch.equal(buf[:, :N], ref), "act=%d: differs from bn=128" % act
@@ -77,7 +77,7 @@ def test_in_place_residual_across_tile_rounds(extra):
         ref = _nan(M, N)
         run(A, W, ref, bias=b, residual=R, act=act, bn=128)
         inplace = R.clone()
-        run(A, W, inplace, bias=b, residual=inplace, act=act, bn=256, generic=TMA)
+        run(A, W, inplace, bias=b, residual=inplace, act=act, bn=256, flags=TMA)
         assert torch.equal(inplace, ref), "tiles=%d act=%d: in-place residual differs from bn=128" % (tiles, act)
 
 
@@ -100,10 +100,10 @@ def test_row_maps_take_the_register_store_branch(rowmap, grid, width, patch, B):
     for bn in (128, 256):
         if rowmap == "out_group":
             outs[bn] = _nan(B * (gg + 1), width)
-            run(A, W, outs[bn], bias=b, residual=R, out_group=gg, act=1, bn=bn, generic=TMA if bn == 256 else 0)
+            run(A, W, outs[bn], bias=b, residual=R, out_group=gg, act=1, bn=bn, flags=TMA if bn == 256 else 0)
         else:
             outs[bn] = _nan(M, width)
-            run(A, W, outs[bn], bias=b, residual=pos, res_row_mod=gg, res_row_off=1, act=1, bn=bn, generic=TMA if bn == 256 else 0)
+            run(A, W, outs[bn], bias=b, residual=pos, res_row_mod=gg, res_row_off=1, act=1, bn=bn, flags=TMA if bn == 256 else 0)
     if rowmap == "out_group":
         o, o128 = outs[256].view(B, gg + 1, width), outs[128].view(B, gg + 1, width)
         assert bool(torch.isnan(o[:, 0].float()).all()), "a cls row was written"

@@ -172,18 +172,18 @@ def test_wide_vitl14_layer_shapes(shape):
 
 @pytest.mark.timeout(60)
 def test_wide_refusals():
-    """bn = 256 takes the compile-time flavours only: the forced run-time flavour, row statistics and the folded
-    LayerNorm are refused with B200_ERR_INVALID (-1)."""
+    """bn = 256 with an undefined flags bit (bit 0, alone or beside the TMA-store bit) or a non-zero reserved member
+    of the epilogue struct (the removed LayerNorm fold's row statistics and inputs) is refused with B200_ERR_INVALID
+    (-1); without them it runs."""
     import torch
 
     A, W, b, R = operands(128, 256, 64, 1)
     out = torch.empty(128, 256, device="cuda", dtype=torch.bfloat16)
     rec = torch.zeros(128, 4, 2, device="cuda")
-    c = torch.zeros(256, device="cuda")
-    assert gemm(A, W, out, bias=b, bn=256, generic=True) == -1
-    assert gemm(A, W, out, bias=b, residual=R, stats_out=rec, bn=256) == -1
-    xrec = torch.zeros(128, 1, 2, device="cuda")
-    assert gemm(A, W, out, bias=b, ln_stats=xrec, ln_c=c, ln_w=64, bn=256) == -1
+    assert gemm(A, W, out, bias=b, bn=256, flags=1) == -1
+    assert gemm(A, W, out, bias=b, residual=R, bn=256, flags=3) == -1
+    assert gemm(A, W, out, bias=b, residual=R, bn=256, reserved={"reserved3": rec.data_ptr()}) == -1
+    assert gemm(A, W, out, bias=b, bn=256, reserved={"reserved0": rec.data_ptr(), "reserved2": 64}) == -1
     assert gemm(A, W, out, bias=b, bn=256) == 0
     torch.cuda.synchronize()
 

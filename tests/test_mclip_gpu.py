@@ -177,6 +177,43 @@ def test_tiny_encoders_match_golden_and_oracle(name):
     assert torch.equal(f16, emb.half())
 
 
+@pytest.mark.timeout(300)
+def test_concurrent_host_and_device_encodes_share_one_handle_safely():
+    """The query service encodes from Flask threads: host-entry calls (legacy stream) and device-entry calls on a
+    torch stream, from two threads on one handle, must each return what they return alone."""
+    import threading
+
+    import torch
+
+    cfg = mclip_ref.CONFIGS["tiny-xlmr"]
+    sd = mclip_ref.make_state_dict(cfg, seed=0)
+    z = np.load(os.path.join(GOLDEN, "mclip_tiny-xlmr.npz"))
+    ids, lengths = z["ids"], z["lengths"]
+    enc = _encoder(cfg, sd, max_batch=8)
+    want_host = enc.embed_text(ids, lengths)
+    want_dev = enc.embed_text_device(ids, lengths, normalize=False).cpu().numpy()
+    errs = []
+
+    def host_worker():
+        for _ in range(40):
+            if not np.array_equal(enc.embed_text(ids, lengths), want_host):
+                errs.append("host")
+
+    def device_worker():
+        s = torch.cuda.Stream()
+        with torch.cuda.stream(s):
+            for _ in range(40):
+                out = enc.embed_text_device(ids, lengths, normalize=False)
+                s.synchronize()
+                if not np.array_equal(out.cpu().numpy(), want_dev):
+                    errs.append("device")
+
+    ts = [threading.Thread(target=host_worker), threading.Thread(target=device_worker)]
+    [t.start() for t in ts]
+    [t.join() for t in ts]
+    assert not errs, errs[:4]
+
+
 def _padded(ids, pad, T):
     out = np.full((ids.shape[0], T), pad, dtype=np.int64)
     out[:, :ids.shape[1]] = ids

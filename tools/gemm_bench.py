@@ -108,8 +108,7 @@ def ksweep(args, name, power):
             bias = torch.randn(N, device="cuda", generator=g)
             out = torch.randn(M, N, device="cuda", generator=g, dtype=torch.bfloat16)
             for fl, act, res in KSWEEP_FLAVOURS:
-                ep = GemmEpilogueC(bias.data_ptr(), out.data_ptr() if res else None, 0, 0, 0, 0, 0, act, None, None, 0,
-                                   None)
+                ep = GemmEpilogueC(bias.data_ptr(), out.data_ptr() if res else None, 0, 0, 0, 0, 0, act)
 
                 def launch(s, ep=ep):
                     check(lib.b200_gemm_bf16_ex_device(A.data_ptr(), W.data_ptr(), out.data_ptr(), M, N, K, ep, 256, 0,
@@ -171,10 +170,10 @@ def main():
             # patch embedding: product row r -> output row (r / g) (g + 1) + 1 + r % g, positional row 1 + r % g
             out = torch.zeros(M // group * (group + 1), N, device="cuda", dtype=torch.bfloat16)
             pos = torch.randn(group + 1, N, device="cuda", generator=g).bfloat16()
-            ep = GemmEpilogueC(None, pos.data_ptr(), 0, group, 1, 0, group, act, None, None, 0, None)
+            ep = GemmEpilogueC(None, pos.data_ptr(), 0, group, 1, 0, group, act)
         else:
             out = torch.randn(M, N, device="cuda", generator=g).bfloat16()
-            ep = GemmEpilogueC(bias.data_ptr(), out.data_ptr() if res else None, 0, 0, 0, 0, 0, act, None, None, 0, None)
+            ep = GemmEpilogueC(bias.data_ptr(), out.data_ptr() if res else None, 0, 0, 0, 0, 0, act)
         flops = 2.0 * M * N * K
         iters = args.iters if M >= 4096 else args.iters * 20
 

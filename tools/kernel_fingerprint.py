@@ -1,4 +1,4 @@
-"""What the compiler made of the search kernels, in a form two checkouts can be diffed on.  Needs nvcc, no GPU.
+"""What the compiler made of the search and embed kernels, in a form two checkouts can be diffed on.  Needs nvcc, no GPU.
 
     python tools/kernel_fingerprint.py OUT_DIR [CSRC_DIR]
     git worktree add /tmp/parent HEAD~1
@@ -6,7 +6,8 @@
     python tools/kernel_fingerprint.py /tmp/fp_branch
     diff -r /tmp/fp_parent /tmp/fp_branch
 
-Compiles knn_scan / knn_ivf / knn_ivfpq / knn_mma with the flags of build.py plus -Xptxas=-v and writes, per
+Compiles knn_scan / knn_ivf / knn_ivfpq / knn_mma (search) and gemm / attention / attention_wgmma / embed_kernels /
+clip_model / text_encoder (embed path) with the flags of build.py plus -Xptxas=-v and writes, per
 source, `<name>.res` (one line per kernel entry: registers, barriers, shared memory, stack frame, spill bytes) and
 `<name>.sass` (cuobjdump -sass per function, addresses and encodings stripped, functions sorted by name).  A refactor
 that claims to leave a kernel alone shows an empty diff for it; identical SASS settles its speed and its results.
@@ -19,7 +20,8 @@ import sys
 import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SOURCES = ["knn_scan", "knn_ivf", "knn_ivfpq", "knn_mma"]
+SOURCES = ["knn_scan", "knn_ivf", "knn_ivfpq", "knn_mma",
+           "gemm", "attention", "attention_wgmma", "embed_kernels", "clip_model", "text_encoder"]
 
 
 def _build_py():
