@@ -11,7 +11,7 @@ there is no CPU fallback: importing works without a GPU, calling compute without
 from ._lib import lib, B200Error, library_path, launch_count  # noqa: F401
 from .index import B200FlatIndex, B200IVFFlatIndex, B200IVFPQIndex, SynthSpec, load_index, merge_shard_results, merge_packed_results, train_kmeans, build_ivf_index, train_pq, train_ivfpq, build_ivfpq_index, train_opq  # noqa: F401
 from .clip_index import clip_index, build_index, parse_index_key, default_index_key, default_nprobe  # noqa: F401
-from .faiss_io import write_index  # noqa: F401
+from .faiss_io import write_index, index_combiner  # noqa: F401
 
 from .model import B200Clip, ClipArch, Tower, ARCHS, load_clip, synthetic_state_dict, convert_hf_state_dict  # noqa: F401,E402
 from .preprocess import B200Preprocess, to_rgb8  # noqa: F401,E402
@@ -26,6 +26,6 @@ __all__ = [
     "lib", "B200Error", "library_path", "launch_count",
     "B200FlatIndex", "B200IVFFlatIndex", "B200IVFPQIndex", "SynthSpec", "load_index", "merge_shard_results", "train_kmeans", "build_ivf_index",
     "train_pq", "train_ivfpq", "build_ivfpq_index", "train_opq", "clip_index", "build_index", "parse_index_key",
-    "default_index_key", "default_nprobe", "write_index",
+    "default_index_key", "default_nprobe", "write_index", "index_combiner",
     "B200TextEncoder", "EncoderArch", "MCLIP_ARCHS", "MclipTextModel", "load_mclip",
 ]

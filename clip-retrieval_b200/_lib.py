@@ -115,6 +115,10 @@ PROTOTYPES = {
     "b200_index_add_codes": (_i, [_vp, _vp, _i64, _i, _vp]),
     "b200_index_set_pretransform": (_i, [_vp, _i, _vp, _vp]),
     "b200_index_pq_m": (_i, [_vp]),
+    "b200_index_set_host_lists": (_i, [_vp, _i, _vp, _vp, _vp]),
+    "b200_index_set_stream_arena": (_i, [_vp, C.c_size_t]),
+    "b200_index_last_stream_stats": (_i, [_vp, _vp]),
+    "b200_ids_map_device": (_i, [_vp, _i64, _vp, _i64, _vp, _i, _vp]),
     "b200_index_encode_device": (_i, [_vp, _vp, _i64, _vp, _vp, _vp, _vp]),
     "b200_pq_train_f32": (_i, [_vp, _i64, _i, _i, _i, C.c_uint64, _vp, _vp, _i]),
     "b200_opq_train_f32": (_i, [_vp, _i64, _i, _i, _i, _i, _i, _i, C.c_uint64, _vp, _vp, _vp, _i]),

@@ -6,6 +6,8 @@
 #include <mutex>
 #include <vector>
 
+namespace b200 { struct HostLists; }
+
 struct b200_index {
   int d = 0;                // width of the stored space (IVF-PQ: the code space, after any pre-transform)
   int d_in = 0;             // width of a query and of a reconstructed row (== d unless a pre-transform is set)
@@ -48,6 +50,9 @@ struct b200_index {
   float* pt_A = nullptr;            // device [d, d_in] fp32: q' = A q + b; null = no pre-transform
   float* pt_b = nullptr;            // device [d] fp32
   bool pt_orthonormal = false;      // rows of A orthonormal: reconstruct may apply A^T (y - b)
+  // lists in host memory (b200_index_set_host_lists): `rows` stays empty, each query pass stages its probed lists
+  // into a device arena (knn_ivfpq_stream.cu).  null = the resident store above.
+  b200::HostLists* host = nullptr;
 
   // scratch
   void* ws[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // 0: scan internals; 1..3: callers; 4,5: hi-only mode
@@ -163,6 +168,31 @@ int ivf_range_scan(b200_index* idx, const float* d_q, float thresh, unsigned lon
 int grow_pending(b200_index* idx, int64_t need, bool amortised);
 
 // ---- knn_ivfpq.cu ---------------------------------------------------------------------------------------
+struct PqPlan {
+  int cs = 0, mc = 0, warps = 0;
+  size_t smem = 0;
+};
+// What a list scan reads: codes at the index's pitch list after list, list offsets [lists + 1], and the key id of each
+// row (null: the row itself).  The resident store, or a staging arena of host-memory lists.
+struct PqStore {
+  const uint8_t* codes;
+  const uint32_t* row_ids;
+  const int64_t* offsets;
+};
+PqPlan pq_plan(int pitch, int k);
+int pq_coarse_plan(const b200_index* idx, const char* what, int nprobe, SelectPlan* cp);
+size_t pq_w4_bytes(const b200_index* idx, int qb);
+int pq_query_space(b200_index* idx, const float* d_q, int qb, float* w4, const float** q_out, float** tables_out,
+                   cudaStream_t st);
+int pq_probe_step(b200_index* idx, const float* q, int qb, const SelectPlan& cp, unsigned long long* probes, char* w0,
+                  cudaStream_t st);
+int pq_table_step(b200_index* idx, const float* q, int qb, float* tables, cudaStream_t st);
+int pq_launch_scan(b200_index* idx, const PqStore& store, bool range, const PqPlan& pl, int nq, const float* tables,
+                   const unsigned long long* probes, int nprobe, int segs, int cpq, int k, unsigned long long* out,
+                   int64_t out_stride_q, float thresh, unsigned int cap, unsigned int* counter, cudaStream_t st);
+int pq_decode_launch(b200_index* idx, const uint8_t* codes, const int64_t* offsets, int nlists, const int32_t* list_ids,
+                     const uint32_t* id_to_slot, const unsigned long long* keys, const int64_t* ids, int64_t count,
+                     float* d_R, cudaStream_t st);
 int ivfpq_search_keys(b200_index* idx, const float* d_q, int nq, int k, unsigned long long* d_keys, cudaStream_t st);
 // One query (device pointer): (score, slot) keys of every row of the probed lists scoring strictly above `thresh`.
 int ivfpq_range_scan(b200_index* idx, const float* d_q, float thresh, unsigned long long* d_out, unsigned int cap,
@@ -170,6 +200,18 @@ int ivfpq_range_scan(b200_index* idx, const float* d_q, float thresh, unsigned l
 // Rows for keys (search_and_reconstruct) or for ids (reconstruct); exactly one of the two is non-null.
 int ivfpq_decode(b200_index* idx, const unsigned long long* keys, const int64_t* ids, int64_t count, float* d_R,
                  cudaStream_t st);
+
+// ---- knn_ivfpq_stream.cu: IVF-PQ with lists in host memory --------------------------------------------------------
+// search: D, I (the lists' own ids + id_base) into device d_D / d_I, the decoded rows into d_R (or null), each pass
+// decoding from its arena; d_keys [nq, k] is scratch.  Returns with the stream synchronised.
+int ivfpq_stream_search(b200_index* idx, const float* d_q, int nq, int k, unsigned long long* d_keys, float* d_D,
+                        int64_t* d_I, float* d_R, cudaStream_t st);
+// range_search of one query (d_keys [cap] and d_count are scratch): up to `cap` hits into h_D / h_I in ascending
+// list-order slot; *h_count = all hits.
+int ivfpq_stream_range(b200_index* idx, const float* d_q, float thresh, unsigned long long* d_keys, int64_t cap,
+                       unsigned int* d_count, float* h_D, int64_t* h_I, int64_t* h_count, cudaStream_t st);
+int ivfpq_stream_lists(b200_index* idx, int64_t* h_sizes, int64_t* h_ids);
+void host_lists_free(b200_index* idx);
 
 // ---- pq_encode.cu: the PQ pieces OPQ training (opq_train.cu) reuses ---------------------------------------
 // Y [n, d] = X [n, d_in] A^T (+ b): the row pre-transform of encode.

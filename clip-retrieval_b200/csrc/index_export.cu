@@ -38,6 +38,7 @@ int b200_index_get_quantizer(b200_index* idx, float* h_centroids, float* h_codeb
 int b200_index_copy_rows(b200_index* idx, int64_t s0, int64_t n, void* h_rows, int64_t* h_ids) {
   B200_CHECK(idx && s0 >= 0 && n >= 0, B200_ERR_INVALID, "copy_rows: bad argument");
   DeviceGuard g(idx->device);
+  B200_CHECK(!idx->host, B200_ERR_UNSUPPORTED, "copy_rows: the lists are in host memory (the file they came from)");
   if (idx->nlist > 0) B200_TRY(ivf_finalize(idx));
   B200_CHECK(s0 + n <= idx->ntotal, B200_ERR_INVALID, "copy_rows: slots [%lld, %lld) past the %lld stored rows",
              (long long)s0, (long long)(s0 + n), (long long)idx->ntotal);

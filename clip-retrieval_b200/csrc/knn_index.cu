@@ -110,6 +110,15 @@ merge_shards_kernel(const float* __restrict__ Dg, const int64_t* __restrict__ Ig
   }
 }
 
+// out[i] = map[I[i]] (an index file's ids for insertion ids); -1 and ids outside the map stay -1.
+__global__ void ids_map_kernel(const int64_t* __restrict__ I, int64_t n, const int64_t* __restrict__ map, int64_t nmap,
+                               int64_t* __restrict__ out) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int64_t v = I[i];
+  out[i] = (v >= 0 && v < nmap) ? map[v] : -1;
+}
+
 static int ensure_capacity(b200_index* idx, int64_t need) {
   if (need <= idx->capacity) return B200_OK;
   int64_t cap = need;
@@ -140,6 +149,7 @@ static int search_device_impl(b200_index* idx, const float* d_q, int nq, int k, 
   if (idx->pq_M > 0) {
     B200_CHECK(!d_R || !idx->pt_A || idx->pt_orthonormal, B200_ERR_UNSUPPORTED,
                "search_and_reconstruct: the pre-transform matrix is not orthonormal, so rows cannot be mapped back");
+    if (idx->host) return ivfpq_stream_search(idx, d_q, nq, k, keys, d_D, d_I, d_R, st);
     B200_TRY(ivf_finalize(idx));
     B200_TRY(ivfpq_search_keys(idx, d_q, nq, k, keys, st));
   } else if (idx->nlist > 0) {
@@ -386,7 +396,9 @@ static int search_graph(b200_index* idx, const float* d_q, int nq, int k, float*
                         cudaStream_t st) {
   constexpr int GRAPH_MAX_NQ = 4;
   const size_t r_bytes = d_R ? (size_t)nq * k * idx->d_in * 4 : 0;
-  if (!idx->use_graphs || nq < 1 || nq > GRAPH_MAX_NQ || k > 2048 || r_bytes > (8u << 20) || idx->npending > 0) return 0;
+  // lists in host memory: every pass waits on the host for its probes, which a graph cannot replay
+  if (!idx->use_graphs || nq < 1 || nq > GRAPH_MAX_NQ || k > 2048 || r_bytes > (8u << 20) || idx->npending > 0 || idx->host)
+    return 0;
   cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
   B200_CUDA(cudaStreamIsCapturing(st, &cs));
   if (cs != cudaStreamCaptureStatusNone) return 0;
@@ -512,6 +524,11 @@ int b200_index_range_search(b200_index* idx, const float* h_q, float thresh, int
   int64_t* d_I = (int64_t*)((char*)d_D + (((size_t)cap * 4 + 7) & ~(size_t)7));
   B200_TRY(idx->scratch.acquire(0));
   B200_CUDA(cudaMemcpyAsync(d_q, h_q, (size_t)idx->d_in * 4, cudaMemcpyHostToDevice, 0));
+  if (idx->host) {
+    const int rc = ivfpq_stream_range(idx, d_q, thresh, d_keys, cap, d_count, h_D, h_I, h_count, 0);
+    B200_TRY(idx->scratch.release(0));
+    return rc;
+  }
   if (idx->pq_M > 0) {
     B200_TRY(ivf_finalize(idx));
     B200_TRY(ivfpq_range_scan(idx, d_q, thresh, d_keys, (unsigned int)cap, d_count, 0));
@@ -539,6 +556,9 @@ int b200_index_reconstruct_device(b200_index* idx, const int64_t* d_ids, int64_t
   B200_CHECK(idx && d_ids && d_R && n >= 0, B200_ERR_INVALID, "reconstruct: bad argument");
   if (n == 0) return B200_OK;
   DeviceGuard g(idx->device);
+  B200_CHECK(!idx->host, B200_ERR_UNSUPPORTED,
+             "reconstruct: the lists are in host memory and the index keeps no id -> list map (FAISS's on-disk IVF "
+             "without a direct map does not reconstruct either)");
   if (idx->pq_M > 0) {
     std::lock_guard<std::mutex> lock(idx->mu);
     B200_CHECK(!idx->pt_A || idx->pt_orthonormal, B200_ERR_UNSUPPORTED,
@@ -554,6 +574,16 @@ int b200_index_reconstruct_device(b200_index* idx, const int64_t* d_ids, int64_t
   }
   gather_rows_from_slots_kernel<<<(unsigned)((n + 7) / 8), 256, 0, (cudaStream_t)stream>>>(
       idx->rows, idx->d, d_ids, idx->id_base, idx->ntotal, id_to_slot, n, d_R);
+  B200_LAUNCH_OK();
+  return B200_OK;
+}
+
+int b200_ids_map_device(const int64_t* d_I, int64_t n, const int64_t* d_map, int64_t nmap, int64_t* d_out, int device,
+                        void* stream) {
+  B200_CHECK(d_I && d_map && d_out && n >= 0 && nmap >= 0, B200_ERR_INVALID, "ids_map: bad argument");
+  if (n == 0) return B200_OK;
+  DeviceGuard g(device);
+  ids_map_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(d_I, n, d_map, nmap, d_out);
   B200_LAUNCH_OK();
   return B200_OK;
 }

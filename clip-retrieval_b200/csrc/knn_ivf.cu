@@ -247,6 +247,7 @@ void ivf_free(b200_index* idx) {
   if (idx->pq_codebook) cudaFree(idx->pq_codebook);
   if (idx->pt_A) cudaFree(idx->pt_A);
   if (idx->pt_b) cudaFree(idx->pt_b);
+  host_lists_free(idx);
 }
 
 int grow_pending(b200_index* idx, int64_t need, bool amortised) {
@@ -420,6 +421,7 @@ int ivf_add_synthetic(b200_index* idx, int64_t n, int64_t row0, const b200_synth
 }
 
 int ivf_lists(b200_index* idx, int64_t* h_sizes, int64_t* h_ids) {
+  if (idx->host) return ivfpq_stream_lists(idx, h_sizes, h_ids);
   for (int l = 0; l < idx->nlist; l++) h_sizes[l] = idx->h_list_offsets[l + 1] - idx->h_list_offsets[l];
   if (h_ids && idx->ntotal > 0) {
     std::vector<uint32_t> tmp((size_t)idx->ntotal);

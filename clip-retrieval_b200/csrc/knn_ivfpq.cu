@@ -102,6 +102,8 @@ __global__ void pq_tables_kernel(const float* __restrict__ Q, int d, int M, int 
 // nothing else, and inserts.  The leader starts each row's sum at dis0, so with cs = 1 the fp32 sum runs
 // dis0 + T[0] + T[1] + ... in m order.
 // RANGE: no lists; every row scoring strictly above `thresh` is appended as a (score, slot) key.
+// `codes` / `offsets` are the resident list store, or a staging arena of the lists a pass probes (lists in host
+// memory, knn_ivfpq_stream.cu) whose probe keys name arena lists; row_ids == nullptr: a key's id is its row r.
 template <bool RANGE>
 __global__ void __launch_bounds__(PQ_THREADS)
 ivfpq_scan_kernel(const uint8_t* __restrict__ codes, int pitch, const uint32_t* __restrict__ row_ids,
@@ -166,7 +168,7 @@ ivfpq_scan_kernel(const uint8_t* __restrict__ codes, int pitch, const uint32_t* 
       // Only a row scoring at least the worst kept score can enter the list (as in the IVF-Flat scan).
       const bool reach = live && (s == s) && f32_to_ordered(s) >= (uint32_t)(worst >> 32);
       unsigned long long key = 0ull;
-      if (reach) key = make_key(s, __ldg(row_ids + r));
+      if (reach) key = make_key(s, row_ids ? __ldg(row_ids + r) : (uint32_t)r);
       warp_offer(wkeys, k, reach && key > worst, key, &worst, &worst_pos, lane);
     }
   }
@@ -178,9 +180,12 @@ ivfpq_scan_kernel(const uint8_t* __restrict__ codes, int pitch, const uint32_t* 
 // ---- (4) decode: rows for keys (search_and_reconstruct) or ids (reconstruct) ----------------------------
 // One warp per row: y[j] = codebook[m][code_m][t] + centroid_l[j] (fp32 add; no centroid without residuals), then
 // x = A^T (y - b) when a pre-transform is set.  Key 0 / an id outside the shard -> all-ones bits (NaN).
+// A staging arena decodes with id_to_slot == nullptr (a key's id is its arena row) and `list_ids` mapping an arena
+// list to the index's list, whose centroid the row adds; the resident store passes list_ids == nullptr.
 __global__ void pq_decode_kernel(const uint8_t* __restrict__ codes, int pitch, int M, int dsub, int d,
                                  const float* __restrict__ cb, const float* __restrict__ cent, int by_residual,
-                                 const int64_t* __restrict__ offsets, int nlist, const uint32_t* __restrict__ id_to_slot,
+                                 const int64_t* __restrict__ offsets, int nlist, const int32_t* __restrict__ list_ids,
+                                 const uint32_t* __restrict__ id_to_slot,
                                  const unsigned long long* __restrict__ keys, const int64_t* __restrict__ ids,
                                  int64_t id_base, int64_t ntotal, int64_t count, const float* __restrict__ A,
                                  const float* __restrict__ b, int d_in, float* __restrict__ out) {
@@ -199,7 +204,7 @@ __global__ void pq_decode_kernel(const uint8_t* __restrict__ codes, int pitch, i
     for (int j = lane; j < d_in; j += 32) o[j] = __uint_as_float(0xffffffffu);
     return;
   }
-  const int64_t slot = id_to_slot[local];
+  const int64_t slot = id_to_slot ? (int64_t)id_to_slot[local] : local;
   int lo = 0, hi = nlist;   // list of the slot: offsets[l] <= slot < offsets[l + 1]
   while (hi - lo > 1) {
     const int mid = (lo + hi) >> 1;
@@ -210,7 +215,7 @@ __global__ void pq_decode_kernel(const uint8_t* __restrict__ codes, int pitch, i
   for (int j = lane; j < d; j += 32) {
     const int m = j / dsub, t = j - m * dsub;
     const float c = cb[((int64_t)m * PQ_KSUB + row[m]) * dsub + t];
-    y[j] = by_residual ? __fadd_rn(c, cent[(int64_t)lo * d + j]) : c;
+    y[j] = by_residual ? __fadd_rn(c, cent[(int64_t)(list_ids ? list_ids[lo] : lo) * d + j]) : c;
   }
   if (!A) return;
   __syncwarp();
@@ -223,14 +228,10 @@ __global__ void pq_decode_kernel(const uint8_t* __restrict__ codes, int pitch, i
 
 // ---- host side ------------------------------------------------------------------------------------------
 
-struct PqPlan {
-  int cs = 0, mc = 0, warps = 0;
-  size_t smem = 0;
-};
 // The smallest cluster (1, 2, 4 CTAs) whose share of the table plus candidate lists leaves at least 4 warps of
 // lists in the budget; failing that, the most warps.  Depends on (M, k) alone, so every query batch of a shape
 // sums its rows in the same order.
-static PqPlan pq_plan(int pitch, int k) {
+PqPlan pq_plan(int pitch, int k) {
   PqPlan best;
   for (int cs = 1; cs <= 4; cs <<= 1) {
     const int mc = ((pitch + cs - 1) / cs + 15) / 16 * 16;
@@ -246,10 +247,9 @@ static PqPlan pq_plan(int pitch, int k) {
   return best;
 }
 
-static int pq_launch_scan(b200_index* idx, bool range, const PqPlan& pl, int nq, const float* tables,
-                          const unsigned long long* probes, int nprobe, int segs, int cpq, int k,
-                          unsigned long long* out, int64_t out_stride_q, float thresh, unsigned int cap,
-                          unsigned int* counter, cudaStream_t st) {
+int pq_launch_scan(b200_index* idx, const PqStore& store, bool range, const PqPlan& pl, int nq, const float* tables,
+                   const unsigned long long* probes, int nprobe, int segs, int cpq, int k, unsigned long long* out,
+                   int64_t out_stride_q, float thresh, unsigned int cap, unsigned int* counter, cudaStream_t st) {
   const void* fn = range ? (const void*)ivfpq_scan_kernel<true> : (const void*)ivfpq_scan_kernel<false>;
   if (pl.smem > 48 * 1024) B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
   cudaLaunchConfig_t cfg = {};
@@ -264,54 +264,77 @@ static int pq_launch_scan(b200_index* idx, bool range, const PqPlan& pl, int nq,
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pl.cs > 1 ? 1 : 0;
-  const uint8_t* codes = reinterpret_cast<const uint8_t*>(idx->rows);
   const int pitch = idx->row_bytes, by_res = idx->pq_by_residual ? 1 : 0;
   if (range)
-    B200_CUDA(cudaLaunchKernelEx(&cfg, ivfpq_scan_kernel<true>, codes, pitch, (const uint32_t*)idx->row_ids, tables, probes,
-                                 nprobe, segs, cpq, (const int64_t*)idx->list_offsets, by_res, pl.mc, pl.cs, k, out,
-                                 out_stride_q, thresh, cap, counter));
+    B200_CUDA(cudaLaunchKernelEx(&cfg, ivfpq_scan_kernel<true>, store.codes, pitch, store.row_ids, tables, probes, nprobe,
+                                 segs, cpq, store.offsets, by_res, pl.mc, pl.cs, k, out, out_stride_q, thresh, cap, counter));
   else
-    B200_CUDA(cudaLaunchKernelEx(&cfg, ivfpq_scan_kernel<false>, codes, pitch, (const uint32_t*)idx->row_ids, tables, probes,
-                                 nprobe, segs, cpq, (const int64_t*)idx->list_offsets, by_res, pl.mc, pl.cs, k, out,
-                                 out_stride_q, thresh, cap, counter));
+    B200_CUDA(cudaLaunchKernelEx(&cfg, ivfpq_scan_kernel<false>, store.codes, pitch, store.row_ids, tables, probes, nprobe,
+                                 segs, cpq, store.offsets, by_res, pl.mc, pl.cs, k, out, out_stride_q, thresh, cap, counter));
   B200_LAUNCH_OK();
   return B200_OK;
 }
 
 // Select plan of the coarse step: k = nprobe over the nlist scores of a query (two select levels, as the list scan).
-static int pq_coarse_plan(const b200_index* idx, const char* what, int nprobe, SelectPlan* cp) {
+int pq_coarse_plan(const b200_index* idx, const char* what, int nprobe, SelectPlan* cp) {
   B200_CHECK((size_t)select_buffer(nprobe) * 8 <= SELECT_SMEM_MAX, B200_ERR_UNSUPPORTED,
              "ivfpq %s: nprobe=%d exceeds the supported maximum (12800)", what, nprobe);
   return plan_select(idx->nlist, nprobe, cp);
 }
 
-// Steps (0)-(2) for queries [0, qb) of d_q: probes [qb, nprobe] (keys: fp32 coarse score = dis0, list id) and
-// tables [qb, pitch, 256].  `w0` holds the coarse scores, `w4` the transformed queries and the tables.
-static int pq_prepare(b200_index* idx, const float* d_q, int qb, const SelectPlan& cp, unsigned long long* probes, char* w0,
-                      float* w4, float** tables_out, cudaStream_t st) {
-  const int d = idx->d, M = idx->pq_M, pitch = idx->row_bytes, nlist = idx->nlist;
-  const float* q = d_q;
-  float* tables = w4;
+// Step (0) for queries [0, qb) of d_q: the queries in the code space (d_q itself, or A q + b written to `w4`);
+// *tables_out is where the tables of step (2) go in `w4`.
+int pq_query_space(b200_index* idx, const float* d_q, int qb, float* w4, const float** q_out, float** tables_out,
+                   cudaStream_t st) {
+  const int d = idx->d;
+  *q_out = d_q;
+  *tables_out = w4;
   if (idx->pt_A) {
     float* qt = w4;
-    tables = w4 + (((size_t)qb * d + 63) & ~(size_t)63);
+    *tables_out = w4 + (((size_t)qb * d + 63) & ~(size_t)63);
     const int64_t warps = (int64_t)qb * d;
     pq_pretransform_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(d_q, qb, idx->d_in, idx->pt_A, idx->pt_b, d, qt);
     B200_LAUNCH_OK();
-    q = qt;
+    *q_out = qt;
   }
+  return B200_OK;
+}
+
+// Step (1): probes [qb, nprobe] (keys: fp32 coarse score = dis0, list id) of the code-space queries q; `w0` holds the
+// coarse scores.
+int pq_probe_step(b200_index* idx, const float* q, int qb, const SelectPlan& cp, unsigned long long* probes, char* w0,
+                  cudaStream_t st) {
+  const int d = idx->d, nlist = idx->nlist;
   unsigned long long* ck = (unsigned long long*)w0;
   pq_coarse_kernel<<<dim3((nlist + CQ_T - 1) / CQ_T, (qb + CQ_T - 1) / CQ_T), 256, 0, st>>>(q, qb, idx->pq_centroids, nlist,
                                                                                             d, ck);
   B200_LAUNCH_OK();
-  B200_TRY(select_topk(cp, ck, ck + (size_t)qb * nlist, probes, qb, st));
-  pq_tables_kernel<<<dim3(pitch, qb), PQ_KSUB, 0, st>>>(q, d, M, d / M, idx->pq_codebook, tables);
+  return select_topk(cp, ck, ck + (size_t)qb * nlist, probes, qb, st);
+}
+
+// Step (2): tables [qb, pitch, 256] of the code-space queries q.
+int pq_table_step(b200_index* idx, const float* q, int qb, float* tables, cudaStream_t st) {
+  const int d = idx->d, M = idx->pq_M;
+  pq_tables_kernel<<<dim3(idx->row_bytes, qb), PQ_KSUB, 0, st>>>(q, d, M, d / M, idx->pq_codebook, tables);
   B200_LAUNCH_OK();
-  *tables_out = tables;
   return B200_OK;
 }
 
-static size_t pq_w4_bytes(const b200_index* idx, int qb) {
+// Steps (0)-(2) for queries [0, qb) of d_q: probes [qb, nprobe] and tables [qb, pitch, 256].  `w0` holds the coarse
+// scores, `w4` the transformed queries and the tables.
+static int pq_prepare(b200_index* idx, const float* d_q, int qb, const SelectPlan& cp, unsigned long long* probes, char* w0,
+                      float* w4, float** tables_out, cudaStream_t st) {
+  const float* q = nullptr;
+  B200_TRY(pq_query_space(idx, d_q, qb, w4, &q, tables_out, st));
+  B200_TRY(pq_probe_step(idx, q, qb, cp, probes, w0, st));
+  return pq_table_step(idx, q, qb, *tables_out, st);
+}
+
+static PqStore resident_store(const b200_index* idx) {
+  return PqStore{reinterpret_cast<const uint8_t*>(idx->rows), idx->row_ids, idx->list_offsets};
+}
+
+size_t pq_w4_bytes(const b200_index* idx, int qb) {
   return ((((size_t)qb * idx->d + 63) & ~(size_t)63) + (size_t)qb * idx->row_bytes * PQ_KSUB) * 4;
 }
 
@@ -341,7 +364,8 @@ int ivfpq_search_keys(b200_index* idx, const float* d_q, int nq, int k, unsigned
     unsigned long long* k1 = (unsigned long long*)w0;
     unsigned long long* k2 = k1 + (size_t)qb * Mq;
     B200_TRY(scan_timer_begin(idx, st));
-    B200_TRY(pq_launch_scan(idx, false, pl, qb, tables, probes, nprobe, segs, cpq, k, k1, Mq, 0.f, 0, nullptr, st));
+    B200_TRY(pq_launch_scan(idx, resident_store(idx), false, pl, qb, tables, probes, nprobe, segs, cpq, k, k1, Mq, 0.f, 0,
+                            nullptr, st));
     B200_TRY(scan_timer_end(idx, st));
     idx->last_scan_launches++;
     B200_TRY(select_topk(sel, k1, k2, d_keys + (size_t)q0 * k, qb, st));
@@ -371,18 +395,26 @@ int ivfpq_range_scan(b200_index* idx, const float* d_q, float thresh, unsigned l
   const int target = std::max(1, 2 * idx->sms / pl.cs);
   const int segs = list_segments(idx, target, nprobe, PQ_THREADS);
   const int cpq = std::min(nprobe * segs, target);
-  return pq_launch_scan(idx, true, pl, 1, tables, probes, nprobe, segs, cpq, 0, d_out, 0, thresh, cap, d_count, st);
+  return pq_launch_scan(idx, resident_store(idx), true, pl, 1, tables, probes, nprobe, segs, cpq, 0, d_out, 0, thresh, cap,
+                        d_count, st);
 }
 
 int ivfpq_decode(b200_index* idx, const unsigned long long* keys, const int64_t* ids, int64_t count, float* d_R,
                  cudaStream_t st) {
+  return pq_decode_launch(idx, reinterpret_cast<const uint8_t*>(idx->rows), idx->list_offsets, idx->nlist, nullptr,
+                          idx->id_to_slot, keys, ids, count, d_R, st);
+}
+
+int pq_decode_launch(b200_index* idx, const uint8_t* codes, const int64_t* offsets, int nlists, const int32_t* list_ids,
+                     const uint32_t* id_to_slot, const unsigned long long* keys, const int64_t* ids, int64_t count,
+                     float* d_R, cudaStream_t st) {
   if (count == 0) return B200_OK;
   const int warps = 4;
   const size_t smem = idx->pt_A ? (size_t)warps * idx->d * 4 : 0;
   pq_decode_kernel<<<(unsigned)((count + warps - 1) / warps), warps * 32, smem, st>>>(
-      reinterpret_cast<const uint8_t*>(idx->rows), idx->row_bytes, idx->pq_M, idx->d / idx->pq_M, idx->d, idx->pq_codebook,
-      idx->pq_centroids, idx->pq_by_residual ? 1 : 0, idx->list_offsets, idx->nlist, idx->id_to_slot, keys, ids,
-      idx->id_base, idx->ntotal, count, idx->pt_A, idx->pt_b, idx->d_in, d_R);
+      codes, idx->row_bytes, idx->pq_M, idx->d / idx->pq_M, idx->d, idx->pq_codebook, idx->pq_centroids,
+      idx->pq_by_residual ? 1 : 0, offsets, nlists, list_ids, id_to_slot, keys, ids, idx->id_base, idx->ntotal, count,
+      idx->pt_A, idx->pt_b, idx->d_in, d_R);
   B200_LAUNCH_OK();
   return B200_OK;
 }
@@ -425,6 +457,7 @@ int b200_index_create_ivfpq(int d, int nlist, int M, int by_residual, const floa
 int b200_index_add_codes(b200_index* idx, const uint8_t* codes, int64_t n, int codes_on_device, const int32_t* h_lists) {
   B200_CHECK(idx && n >= 0 && (n == 0 || (codes && h_lists)), B200_ERR_INVALID, "add_codes: bad argument");
   B200_CHECK(idx->pq_M > 0, B200_ERR_STATE, "add_codes: not an IVF-PQ index");
+  B200_CHECK(!idx->host, B200_ERR_STATE, "add_codes: the index serves lists in host memory (b200_index_set_host_lists)");
   for (int64_t i = 0; i < n; i++)
     B200_CHECK(h_lists[i] >= 0 && h_lists[i] < idx->nlist, B200_ERR_INVALID, "add_codes: row %lld has list %d of %d",
                (long long)i, h_lists[i], idx->nlist);

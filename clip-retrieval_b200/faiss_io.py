@@ -9,22 +9,36 @@ own writers (`write_index` for a built index, the array writers below for test f
     IxSQ                 IndexScalarQuantizer, QT_fp16  -> rows fp16
     IwFl                 IndexIVFFlat (ArrayInvertedLists)
     IwSq                 IndexIVFScalarQuantizer, QT_fp16, by_residual = false
-    IwPQ                 IndexIVFPQ, 8-bit codes (ArrayInvertedLists)  -> codes uint8 [n, M], served from the codes
+    IwPQ                 IndexIVFPQ, 8-bit codes  -> codes uint8 [n, M], served from the codes
     IHNf                 IndexHNSWFlat as the coarse quantiser of an IVF index: the graph is skipped, its storage
                          rows are the centroids (this engine probes the centroids exactly)
     IxPT                 IndexPreTransform with ONE LinearTransform (LTra: an OPQ matrix; rrot) around an IwPQ
     IxMp / IxM2          IndexIDMap / IDMap2 around one of the above
-That covers what autofaiss writes for large collections, `OPQ{M}_{d},IVF{nlist}_HNSW32,PQ{M}x8`.  Still unsupported,
-with NotImplementedError naming the fourcc: a top-level HNSW index, a flat IndexPQ (IxPq), 4-bit or fast-scan PQ,
-IVF refinement (IwQR), on-disk inverted lists (ilod) and longer transform chains; re-index from the embedding
-shards (`load_index(<folder of .npy>)`) or rebuild as one of the above.
+    ilar                 the inverted lists of an IVF index in the file itself (ArrayInvertedLists)
+    ilod                 OnDiskInvertedLists: the lists in a separate data file (`merged_index.ivfdata` next to
+                         `populated.index`, what `index_combiner` / FAISS's merge_ondisk write; DESIGN §5 (xiv))
+That covers what autofaiss writes for large collections, `OPQ{M}_{d},IVF{nlist}_HNSW32,PQ{M}x8`, and the merged
+on-disk form clip back serves LAION-5B from.  Still unsupported, with NotImplementedError naming the fourcc: a
+top-level HNSW index, a flat IndexPQ (IxPq), 4-bit or fast-scan PQ, IVF refinement (IwQR) and longer transform
+chains; re-index from the embedding shards (`load_index(<folder of .npy>)`) or rebuild as one of the above.
+
+The lists are never copied while parsing: an IVF result holds `invlists`, an `InvLists` of per-list (size, code
+address, id address) into read-only memory maps, and its "codes" / "rows" / "ids" arrays (list after list) are
+built from it only when asked for.
 
 Layout (little endian): fourcc u32; header = d i32, ntotal i64, dummy i64 x2, is_trained u8, metric_type i32
 (0 = inner product, 1 = L2; metric_arg f32 follows when metric_type > 1); vectors are `size u64` + payload.
 The file is parsed through a read-only memory map, so a multi-GB code file is not read into memory before the codes
 are gathered into list order.
+
+OnDiskInvertedLists record (ilod, FAISS OnDiskInvertedListsIOHook): nlist u64, code_size u64, a vector of
+List {size, capacity, offset} (3 x u64), a vector of free Slot {offset, capacity} (2 x u64), the data file name as a
+char vector, totsize u64.  In the data file a list's codes start at `offset` (capacity * code_size bytes) and its
+int64 ids at offset + capacity * code_size.  The directory of the recorded name is always replaced by the index
+file's own (FAISS's IO_FLAG_ONDISK_SAME_DIR): the name was recorded on the machine that ran the merge.
 """
 import mmap
+import os
 import struct
 
 import numpy as np
@@ -42,8 +56,10 @@ def _fourcc_str(v):
 
 
 class _R:
-    def __init__(self, buf):
-        self.b, self.o = memoryview(buf), 0
+    def __init__(self, buf, path=""):
+        self.b, self.o, self.path = memoryview(buf), 0, path
+        self.data = np.frombuffer(self.b, dtype=np.uint8)
+        self.ntotal_at = []                      # offsets of the ntotal fields of the index headers (index_combiner)
 
     def take(self, fmt):
         v = struct.unpack_from("<" + fmt, self.b, self.o)
@@ -85,14 +101,97 @@ def _read_sq(r):
     return d
 
 
+class InvLists:
+    """The inverted lists of an IVF index file, in place: list l holds sizes[l] rows of `d` entries of `dtype`, whose
+    codes start at byte code_off[l] and int64 ids at id_off[l] of `data` (a read-only uint8 view of the index file's
+    or the data file's memory map; the views keep the map open)."""
+
+    def __init__(self, data, sizes, code_off, id_off, dtype, d):
+        self.data, self.dtype, self.d = data, np.dtype(dtype), int(d)
+        self.sizes = np.asarray(sizes, np.int64)
+        self.code_off, self.id_off = np.asarray(code_off, np.int64), np.asarray(id_off, np.int64)
+
+    @property
+    def nlist(self):
+        return self.sizes.size
+
+    @property
+    def ntotal(self):
+        return int(self.sizes.sum())
+
+    def addresses(self):
+        """(code addresses, id addresses) as uint64 [nlist]: what b200_index_set_host_lists takes."""
+        base = np.uint64(self.data.ctypes.data if self.data.size else 0)
+        return base + self.code_off.astype(np.uint64), base + self.id_off.astype(np.uint64)
+
+    def codes(self, l):
+        n, w = int(self.sizes[l]), self.d * self.dtype.itemsize
+        o = int(self.code_off[l])
+        return self.data[o:o + n * w].view(self.dtype).reshape(n, self.d)
+
+    def ids(self, l):
+        n, o = int(self.sizes[l]), int(self.id_off[l])
+        return self.data[o:o + 8 * n].view(np.int64)
+
+    def chunks(self, rows):
+        """(codes [m, d], list of each row [m]) list after list, about `rows` rows at a time (one copy per chunk)."""
+        parts, lists, m = [], [], 0
+        for l in np.nonzero(self.sizes)[0].tolist():
+            parts.append(self.codes(l))
+            lists.append(np.full(int(self.sizes[l]), l, np.int32))
+            m += int(self.sizes[l])
+            if m >= rows:
+                yield np.concatenate(parts), np.concatenate(lists)
+                parts, lists, m = [], [], 0
+        if parts:
+            yield np.concatenate(parts), np.concatenate(lists)
+
+    def all_codes(self):
+        nz = np.nonzero(self.sizes)[0].tolist()
+        return np.concatenate([self.codes(l) for l in nz]) if nz else np.zeros((0, self.d), self.dtype)
+
+    def all_ids(self):
+        nz = np.nonzero(self.sizes)[0].tolist()
+        return np.concatenate([self.ids(l) for l in nz]) if nz else np.zeros(0, np.int64)
+
+
+class _Info(dict):
+    """What read_faiss_index returns.  For an IVF index "rows" / "codes" (the stored rows list after list) and "ids"
+    (their ids, through the id map when there is one) are concatenated from `invlists` on first access."""
+
+    def __missing__(self, key):
+        inv = dict.get(self, "invlists")
+        if inv is None or key not in ("rows", "codes", "ids"):
+            raise KeyError(key)
+        if key == "ids":
+            v = inv.all_ids()
+            if dict.get(self, "id_map") is not None:
+                v = self["id_map"][v]
+        else:
+            v = inv.all_codes()
+        self[key] = v
+        return v
+
+
+def _map_file(path):
+    """A read-only uint8 view of a whole file (empty file: an empty array)."""
+    with open(path, "rb") as f:
+        size = f.seek(0, 2)
+        if size == 0:
+            return np.zeros(0, np.uint8)
+        return np.frombuffer(mmap.mmap(f.fileno(), 0, access=mmap.ACCESS_READ), dtype=np.uint8)
+
+
 def _read_invlists(r, nlist_expected, code_dtype, d):
-    """Inverted lists of `d` entries of `code_dtype` per row: (sizes, rows [n, d] in list order, ids)."""
+    """Inverted lists of `d` entries of `code_dtype` per row, as an InvLists into the memory map(s)."""
     tag = _fourcc_str(r.take("I"))
     if tag == "il00":
         raise ValueError("index has no inverted lists")
+    if tag == "ilod":
+        return _read_ondisk_invlists(r, nlist_expected, code_dtype, d)
     if tag != "ilar":
-        raise NotImplementedError("inverted lists %r: only in-memory ArrayInvertedLists ('ilar') are readable "
-                                  "(on-disk lists keep their codes in a separate .ivfdata file)" % tag)
+        raise NotImplementedError("inverted lists %r: only ArrayInvertedLists ('ilar') and OnDiskInvertedLists "
+                                  "('ilod') are readable" % tag)
     nlist, code_size = r.take("Q"), r.take("Q")
     if nlist != nlist_expected or code_size != d * np.dtype(code_dtype).itemsize:
         raise ValueError("inverted lists: nlist %d (expected %d), code size %d for d=%d" % (nlist, nlist_expected, code_size, d))
@@ -105,14 +204,48 @@ def _read_invlists(r, nlist_expected, code_dtype, d):
         sizes[pairs[:, 0]] = pairs[:, 1]
     else:
         raise ValueError("inverted lists: unknown size encoding %r" % fmt)
-    rows, ids = [], []
-    for n in sizes:
-        if n > 0:
-            rows.append(r.raw(code_dtype, int(n) * d).reshape(int(n), d))
-            ids.append(r.raw(np.int64, int(n)))
-    rows = np.concatenate(rows) if rows else np.zeros((0, d), code_dtype)
-    ids = np.concatenate(ids) if ids else np.zeros(0, np.int64)
-    return sizes, rows, ids
+    # ilar: each non-empty list's codes, then its ids, one list after another
+    per_row = code_size + 8
+    ends = r.o + np.cumsum(sizes * per_row)
+    starts = ends - sizes * per_row
+    if sizes.size and ends[-1] > len(r.b):
+        raise ValueError("%s: the inverted lists run past the end of the file (%d bytes, %d needed)"
+                         % (r.path, len(r.b), int(ends[-1])))
+    r.o = int(ends[-1]) if sizes.size else r.o
+    return InvLists(r.data, sizes, starts, starts + sizes * code_size, code_dtype, d)
+
+
+def _read_ondisk_invlists(r, nlist_expected, code_dtype, d):
+    nlist, code_size = r.take("Q"), r.take("Q")
+    lists = np.array(r.vec(np.uint64, unit_bytes=24)).astype(np.int64).reshape(-1, 3)   # size, capacity, offset
+    slots = r.vec(np.uint64, unit_bytes=16)
+    name = bytes(r.vec(np.uint8)).decode("utf-8", errors="replace")
+    totsize = r.take("Q")
+    del slots                                    # free space inside the data file: nothing to serve
+    width = d * np.dtype(code_dtype).itemsize
+    if nlist != nlist_expected or lists.shape[0] != nlist:
+        raise ValueError("%s: on-disk lists: nlist %d, %d list records (expected %d)"
+                         % (r.path, nlist, lists.shape[0], nlist_expected))
+    if code_size != width:
+        raise ValueError("%s: on-disk lists: code size %d, the index stores %d bytes per row" % (r.path, code_size, width))
+    data_path = os.path.join(os.path.dirname(os.path.abspath(r.path)), os.path.basename(name.replace("\\", "/")))
+    if not os.path.isfile(data_path):
+        raise ValueError("%s: the on-disk lists' data file %s (recorded as %r) is missing" % (r.path, data_path, name))
+    data = _map_file(data_path)
+    if data.size < totsize:
+        raise ValueError("%s: data file %s is short: %d bytes, the index records %d" % (r.path, data_path, data.size, totsize))
+    size, cap, off = lists[:, 0], lists[:, 1], lists[:, 2]
+    bad = np.nonzero(cap < size)[0]
+    if bad.size:
+        l = int(bad[0])
+        raise ValueError("%s: list %d has capacity %d < size %d" % (data_path, l, cap[l], size[l]))
+    end = off + cap * (code_size + 8)
+    bad = np.nonzero((size > 0) & ((off < 0) | (end > data.size)))[0]
+    if bad.size:
+        l = int(bad[0])
+        raise ValueError("%s: list %d (offset %d, capacity %d) runs past the end of the file (%d bytes)"
+                         % (data_path, l, off[l], cap[l], data.size))
+    return InvLists(data, size, off, off + cap * code_size, code_dtype, d)
 
 
 def _read_quantizer(r):
@@ -158,6 +291,7 @@ def _read_index(r):
         codes = r.vec(np.uint8)
         return {"kind": "flat", "d": d, "ntotal": ntotal, "metric": metric, "rows": np.array(codes.view(np.float16).reshape(ntotal, d)), "ids": None}
     if tag in ("IwFl", "IwSq"):
+        r.ntotal_at.append(r.o + 4)
         d, ntotal, _, metric = _header(r)
         nlist, nprobe = r.take("Q"), r.take("Q")
         quant = _read_quantizer(r)
@@ -176,10 +310,13 @@ def _read_index(r):
         else:
             r.take("Q")                  # code_size
             dt = np.float32
-        sizes, rows, ids = _read_invlists(r, nlist, dt, d)
-        return {"kind": "ivfflat", "d": d, "ntotal": ntotal, "metric": metric, "nlist": int(nlist), "nprobe": int(nprobe),
-                "centroids": np.asarray(quant["rows"], dtype=np.float32), "list_sizes": sizes, "rows": rows, "ids": ids}
+        r.invlists_at = r.o
+        inv = _read_invlists(r, nlist, dt, d)
+        return _Info(kind="ivfflat", d=d, ntotal=ntotal, metric=metric, nlist=int(nlist), nprobe=int(nprobe),
+                     centroids=np.asarray(quant["rows"], dtype=np.float32), list_sizes=inv.sizes, invlists=inv,
+                     id_map=None)
     if tag == "IwPQ":
+        r.ntotal_at.append(r.o + 4)
         d, ntotal, _, metric = _header(r)
         nlist, nprobe = r.take("Q"), r.take("Q")
         quant = _read_quantizer(r)
@@ -201,12 +338,14 @@ def _read_index(r):
             raise ValueError("IVF-PQ code size %d for M=%d (8-bit codes take M bytes)" % (code_size, M))
         if codebook.size != M * 256 * (d // M):
             raise ValueError("PQ codebook holds %d floats, expected %d" % (codebook.size, M * 256 * (d // M)))
-        sizes, codes, ids = _read_invlists(r, nlist, np.uint8, M)
-        return {"kind": "ivfpq", "d": d, "ntotal": ntotal, "metric": metric, "nlist": int(nlist), "nprobe": int(nprobe),
-                "M": int(M), "by_residual": by_residual, "centroids": np.array(quant["rows"], dtype=np.float32),
-                "codebook": np.array(codebook).reshape(M, 256, d // M), "list_sizes": sizes, "codes": codes, "ids": ids,
-                "transform": None}
+        r.invlists_at = r.o
+        inv = _read_invlists(r, nlist, np.uint8, M)
+        return _Info(kind="ivfpq", d=d, ntotal=ntotal, metric=metric, nlist=int(nlist), nprobe=int(nprobe), M=int(M),
+                     by_residual=by_residual, centroids=np.array(quant["rows"], dtype=np.float32),
+                     codebook=np.array(codebook).reshape(M, 256, d // M), list_sizes=inv.sizes, invlists=inv,
+                     id_map=None, transform=None)
     if tag == "IxPT":
+        r.ntotal_at.append(r.o + 4)
         _header(r)
         nt = r.take("i")
         if nt != 1:
@@ -227,23 +366,29 @@ def _read_index(r):
         if sub["kind"] == "flat":
             sub["ids"] = np.array(id_map)
         else:
-            sub["ids"] = np.asarray(id_map)[sub["ids"]]
+            sub["id_map"] = np.asarray(id_map)    # the lists' ids index it ("ids" applies it)
         return sub
     raise NotImplementedError(
         "FAISS index type %r is not readable: this engine serves flat, IVF-Flat and IVF-PQ (8-bit codes, flat or HNSW "
-        "coarse quantiser, at most one OPQ / rotation pre-transform) files; a top-level HNSW index, a flat PQ index, "
-        "4-bit / fast-scan PQ, refinement and on-disk lists are not served — rebuild as one of those types, or "
+        "coarse quantiser, at most one OPQ / rotation pre-transform, in-file or on-disk lists) files; a top-level HNSW "
+        "index, a flat PQ index, 4-bit / fast-scan PQ and refinement are not served — rebuild as one of those types, or "
         "re-index from the embedding shards with load_index(<folder of .npy>) or build_ivf_index" % tag)
 
 
-def read_faiss_index(path):
-    """Parse a FAISS index file into plain arrays (see the module docstring for the supported types)."""
+def _parse(path):
     with open(path, "rb") as f:
         if f.seek(0, 2) == 0:
             raise ValueError("%s is empty" % path)
         buf = mmap.mmap(f.fileno(), 0, access=mmap.ACCESS_READ)
-    # every returned array is a copy (the map closes when the last view made while parsing goes away)
-    info = _read_index(_R(buf))
+    r = _R(buf, path)
+    return r, _read_index(r)
+
+
+def read_faiss_index(path):
+    """Parse a FAISS index file into plain arrays (see the module docstring for the supported types).  The quantiser
+    arrays are copies; an IVF index's lists stay in the file's (or its data file's) read-only memory map, which
+    stays open while `invlists` or a view made from it lives."""
+    _, info = _parse(path)
     if info["metric"] != METRIC_INNER_PRODUCT:
         raise NotImplementedError("FAISS index with metric %d: the search path is inner product (cosine on normalised rows)" % info["metric"])
     return info
@@ -418,25 +563,163 @@ def write_ivfpq(path, centroids, codebook, codes, assign, ids=None, nprobe=1, by
     """IndexIVFPQ in the layout read above (test fixtures).  codebook [M, 256, d / M]; codes [n, M] uint8 with list
     `assign[i]`; transform = (A [d, d_in], b or None) wraps it in IxPT (`transform_tag` LTra or rrot); hnsw = an IHNf
     quantiser; id_map wraps everything in IxMp.  nbits / code_size / pq_d override the header fields (refusal tests)."""
-    centroids = np.ascontiguousarray(centroids, dtype=np.float32)
-    codebook = np.ascontiguousarray(codebook, dtype=np.float32)
     codes = np.ascontiguousarray(codes, dtype=np.uint8)
-    nlist, d = centroids.shape
     n, M = codes.shape
     ids = np.arange(n, dtype=np.int64) if ids is None else np.asarray(ids, dtype=np.int64)
     out = []
     if id_map is not None:
         _w_fourcc(out, "IxMp")
-        _w_header(out, transform[0].shape[1] if transform is not None else d, n, METRIC_INNER_PRODUCT)
-    if transform is not None:
-        _w_pretransform(out, transform[0], transform[1], n, transform_tag)
-    _w_ivf_head(out, "IwPQ", d, n, nprobe, centroids, hnsw=hnsw)
-    _w_ivfpq_params(out, d, M, by_residual, codebook, nbits, code_size, pq_d)
+        _w_header(out, transform[0].shape[1] if transform is not None else centroids.shape[1], n, METRIC_INNER_PRODUCT)
+    nlist = _w_ivfpq_head(out, centroids, codebook, n, M, nprobe, by_residual, transform, transform_tag, hnsw, nbits,
+                          code_size, pq_d)
     _w_invlists(out, nlist, M if code_size is None else code_size, codes, ids, assign, sparse_sizes)
     if id_map is not None:
         _w_vec(out, np.asarray(id_map, dtype=np.int64))
     with open(path, "wb") as f:
         f.write(b"".join(out))
+
+
+def _w_ivfpq_head(out, centroids, codebook, n, M, nprobe, by_residual, transform, transform_tag="LTra", hnsw=False,
+                  nbits=8, code_size=None, pq_d=None):
+    """An IVF-PQ index up to its inverted lists (inside IxPT when `transform` is set).  Returns nlist."""
+    centroids = np.ascontiguousarray(centroids, dtype=np.float32)
+    nlist, d = centroids.shape
+    if transform is not None:
+        _w_pretransform(out, transform[0], transform[1], n, transform_tag)
+    _w_ivf_head(out, "IwPQ", d, n, nprobe, centroids, hnsw=hnsw)
+    _w_ivfpq_params(out, d, M, by_residual, np.ascontiguousarray(codebook, dtype=np.float32), nbits, code_size, pq_d)
+    return nlist
+
+
+def _w_ondisk_record(out, nlist, code_size, lists, slots, filename, totsize):
+    """OnDiskInvertedLists (ilod): lists [nlist, 3] (size, capacity, offset), slots [s, 2] (offset, capacity)."""
+    out.append(struct.pack("<I", _fourcc("ilod")))
+    out.append(struct.pack("<QQ", nlist, code_size))
+    lists = np.ascontiguousarray(lists, dtype=np.uint64).reshape(-1, 3)
+    out.append(struct.pack("<Q", lists.shape[0]))
+    out.append(lists.tobytes())
+    slots = np.ascontiguousarray(slots, dtype=np.uint64).reshape(-1, 2)
+    out.append(struct.pack("<Q", slots.shape[0]))
+    out.append(slots.tobytes())
+    name = filename.encode("utf-8")
+    out.append(struct.pack("<Q", len(name)))
+    out.append(name)
+    out.append(struct.pack("<Q", totsize))
+
+
+def write_ivfpq_ondisk(folder, centroids, codebook, codes, assign, ids=None, nprobe=1, by_residual=True, transform=None,
+                       hnsw=False, spare=None, recorded_dir=None, code_size=None, data_bytes=None, lists_override=None):
+    """An on-disk IndexIVFPQ as FAISS's merge_ondisk leaves it (test fixtures): `folder`/populated.index with an ilod
+    record and `folder`/merged_index.ivfdata holding, list after list, each list's codes then its ids.  spare[l]
+    (default 0) rows of unused capacity follow list l's rows (capacity = size + spare: the id address then lies
+    past the spare codes), and one free slot is recorded after the last list.  The record names the data file in
+    `recorded_dir` (default: `folder`), as a merge run elsewhere does.  code_size / data_bytes / lists_override
+    overwrite the record's code size, truncate the data file, or replace the (size, capacity, offset) triples
+    (refusal tests).  Returns the (size, capacity, offset) triples written."""
+    codes = np.ascontiguousarray(codes, dtype=np.uint8)
+    n, M = codes.shape
+    nlist = np.asarray(centroids).shape[0]
+    ids = np.arange(n, dtype=np.int64) if ids is None else np.asarray(ids, dtype=np.int64)
+    assign = np.asarray(assign, dtype=np.int64)
+    spare = np.zeros(nlist, np.int64) if spare is None else np.asarray(spare, np.int64)
+    order = np.argsort(assign, kind="stable")
+    sizes = np.bincount(assign, minlength=nlist).astype(np.int64)
+    os.makedirs(folder, exist_ok=True)
+    data_path = os.path.join(folder, "merged_index.ivfdata")
+    triples = np.zeros((nlist, 3), np.int64)
+    with open(data_path, "wb") as f:
+        off, pos = 0, 0
+        for l in range(nlist):
+            m, cap = int(sizes[l]), int(sizes[l] + spare[l])
+            sel = order[pos:pos + m]
+            pos += m
+            triples[l] = (m, cap, off)
+            f.write(codes[sel].tobytes() + bytes((cap - m) * M))
+            f.write(ids[sel].tobytes() + bytes((cap - m) * 8))
+            off += cap * (M + 8)
+        totsize = off
+        f.write(bytes(64))                       # one free slot past the last list
+    if data_bytes is not None:
+        os.truncate(data_path, data_bytes)
+    if lists_override is not None:
+        triples = np.asarray(lists_override, np.int64)
+    out = []
+    _w_ivfpq_head(out, centroids, codebook, n, M, nprobe, by_residual, transform, hnsw=hnsw)
+    name = os.path.join(recorded_dir if recorded_dir is not None else os.path.abspath(folder), "merged_index.ivfdata")
+    _w_ondisk_record(out, nlist, M if code_size is None else code_size, triples, np.array([[totsize, 64]]), name,
+                     totsize + 64)
+    with open(os.path.join(folder, "populated.index"), "wb") as f:
+        f.write(b"".join(out))
+    return triples
+
+
+def index_combiner(input_folder, output_folder):
+    """clip_retrieval.clip_back_prepro.index_combiner on the host: merge the IVF index parts under `input_folder`
+    (the files whose name contains "index", in sorted order) into `output_folder`/merged_index.ivfdata and
+    `output_folder`/populated.index, what FAISS's merge_ondisk(shift_ids=False) writes and `load_index(output_folder)`
+    serves.  The data file holds one list after another, each the parts' rows of that list in file order (codes,
+    then ids), capacity = size, ids kept as stored; populated.index is the first part's header with ntotal = the sum
+    and an ilod record.  Works list by list from the parts' memory maps, so host memory stays bounded by one list.
+    Refuses parts whose nlist, d, M, by_residual, centroids, codebook or pre-transform differ from the first part's
+    (merging them would silently mix incompatible codes), and parts inside an id map (IxMp: the merge moves list ids,
+    not the map)."""
+    names = sorted(f for f in os.listdir(input_folder) if "index" in f)
+    files = [os.path.join(input_folder, f) for f in names if os.path.isfile(os.path.join(input_folder, f))]
+    if not files:
+        raise ValueError("index_combiner: no file whose name contains 'index' under %s" % input_folder)
+    parts = []
+    for p in files:
+        r, info = _parse(p)
+        if info["kind"] == "flat":
+            raise ValueError("index_combiner: %s is a flat index; only IVF indices have lists to merge" % p)
+        if info.get("id_map") is not None:
+            raise ValueError("index_combiner: %s is wrapped in an id map (IxMp); merging lists would detach the ids "
+                             "from the map" % p)
+        parts.append((p, r, info))
+    p0, r0, i0 = parts[0]
+
+    def fields(info):
+        t = info.get("transform")
+        return {"kind": info["kind"], "nlist": info["nlist"], "d": info["d"], "M": info.get("M"),
+                "by_residual": info.get("by_residual"), "centroids": info["centroids"].tobytes(),
+                "codebook": None if info.get("codebook") is None else info["codebook"].tobytes(),
+                "pre-transform": None if t is None else (t[0].tobytes(), None if t[1] is None else t[1].tobytes())}
+
+    f0 = fields(i0)
+    for p, _, info in parts[1:]:
+        f = fields(info)
+        for key in f0:
+            if f[key] != f0[key]:
+                raise ValueError("index_combiner: %s differs from %s in its %s; parts must share one trained quantiser"
+                                 % (p, p0, key))
+    nlist, inv0 = i0["nlist"], i0["invlists"]
+    width = inv0.d * inv0.dtype.itemsize
+    os.makedirs(output_folder, exist_ok=True)
+    data_path = os.path.abspath(os.path.join(output_folder, "merged_index.ivfdata"))
+    triples = np.zeros((nlist, 3), np.int64)
+    off = 0
+    with open(data_path, "wb") as f:
+        for l in range(nlist):
+            invs = [info["invlists"] for _, _, info in parts]
+            m = sum(int(inv.sizes[l]) for inv in invs)
+            triples[l] = (m, m, off)
+            if m:
+                for inv in invs:
+                    if inv.sizes[l]:
+                        f.write(inv.codes(l).data)
+                for inv in invs:
+                    if inv.sizes[l]:
+                        f.write(inv.ids(l).data)
+            off += m * (width + 8)
+    total = int(triples[:, 0].sum())
+    head = bytearray(r0.b[:r0.invlists_at])
+    for at in r0.ntotal_at:
+        struct.pack_into("<q", head, at, total)
+    out = [bytes(head)]
+    _w_ondisk_record(out, nlist, width, triples, np.zeros((0, 2)), data_path, off)
+    with open(os.path.join(output_folder, "populated.index"), "wb") as f:
+        f.write(b"".join(out))
+    return os.path.join(output_folder, "populated.index")
 
 
 class _StoreReader:

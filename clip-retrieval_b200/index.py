@@ -211,12 +211,16 @@ class _IndexBase:
                     break
                 cap = int(cnt.value)
             n = int(cnt.value)
-            order = np.argsort(I[:n], kind="stable")
+            order = self._range_order(I[:n])
             Ds.append(D[:n][order])
             Is.append(I[:n][order])
             lims.append(lims[-1] + n)
         return (np.asarray(lims, dtype=np.uint64), np.concatenate(Ds) if Ds else np.empty(0, np.float32),
                 np.concatenate(Is) if Is else np.empty(0, np.int64))
+
+    def _range_order(self, I):
+        """Order of one query's range hits: by id."""
+        return np.argsort(I, kind="stable")
 
     def reconstruct(self, key):
         torch = _torch()
@@ -389,6 +393,50 @@ class B200IVFPQIndex(_IVFBase):
             raise ValueError("add_codes: expected codes [n, %d] and lists [n]" % M)
         check(lib.b200_index_add_codes(self._h, codes.ctypes.data, codes.shape[0], 0, lists.ctypes.data), "add_codes")
 
+    # ---- lists in host memory (an on-disk index's memory map) ----
+    @property
+    def streamed(self):
+        """True when the lists are served from host memory (`set_host_lists`), False when they are in HBM."""
+        return getattr(self, "_host_lists", None) is not None
+
+    def set_host_lists(self, invlists):
+        """Serve the lists from host memory: `invlists` is a faiss_io.InvLists (list l: sizes[l] code rows of M bytes
+        and their int64 ids, in a read-only memory map) and must describe this index's nlist lists of M-byte codes.
+        Nothing is copied; the index keeps `invlists` (hence the map) alive.  Each search pass stages its probed
+        lists into a device arena (C ABI `b200_index_set_host_lists`); results carry the lists' own ids and equal a
+        resident load of the same lists bit for bit.  The index must hold no rows."""
+        if invlists.nlist != self.nlist or invlists.d != self.M or invlists.dtype != np.uint8:
+            raise ValueError("set_host_lists: %d lists of %d-byte codes for an index of nlist=%d, M=%d"
+                             % (invlists.nlist, invlists.d, self.nlist, self.M))
+        sizes = np.ascontiguousarray(invlists.sizes, np.int64)
+        code_addr, id_addr = invlists.addresses()
+        check(lib.b200_index_set_host_lists(self._h, self.nlist, sizes.ctypes.data, code_addr.ctypes.data,
+                                            id_addr.ctypes.data), "set_host_lists")
+        self._host_lists = invlists
+
+    def set_stream_arena(self, nbytes):
+        """Bytes per device arena of a streamed index (two arenas and as much pinned host staging); never less than
+        nprobe x the largest list, which `0` selects.  Default 256 MiB."""
+        check(lib.b200_index_set_stream_arena(self._h, C.c_size_t(int(nbytes))), "set_stream_arena")
+
+    def last_stream_stats(self):
+        """Streamed index, last search: {gather_ms, copy_ms, staged_bytes, passes} (host gather time, device time of
+        the host-to-device copies, code bytes moved, query passes)."""
+        s = np.zeros(4, np.float64)
+        check(lib.b200_index_last_stream_stats(self._h, s.ctypes.data), "last_stream_stats")
+        return {"gather_ms": float(s[0]), "copy_ms": float(s[1]), "staged_bytes": int(s[2]), "passes": int(s[3])}
+
+    def _range_order(self, I):
+        # a streamed index returns range hits in list-order slot, the insertion order of a resident load of its file
+        return np.arange(I.size) if self.streamed else np.argsort(I, kind="stable")
+
+    def reconstruct(self, key):
+        if self.streamed:
+            raise NotImplementedError("reconstruct: the lists are served from host memory and the index keeps no id -> "
+                                      "list map (as FAISS's on-disk IVF without a direct map); use "
+                                      "search_and_reconstruct, which decodes the rows it returns")
+        return super().reconstruct(key)
+
     def set_pretransform(self, A, b=None):
         """Queries become A q (+ b), A [d, d_in] fp32; `d` then reports d_in (the width a caller passes)."""
         A = np.ascontiguousarray(A, dtype=np.float32)
@@ -413,7 +461,7 @@ def list_embedding_shards(path):
     return files
 
 
-def load_index(path, enable_faiss_memory_mapping=False, device=0):
+def load_index(path, enable_faiss_memory_mapping=False, device=0, max_device_bytes=None):
     """Counterpart of clip_back.load_index (clip_back.py:589-596) for fp16 embedding shards.
 
     `path` is a `.npy` file or a folder of `.npy` shards in the layout the reference writer
@@ -423,8 +471,16 @@ def load_index(path, enable_faiss_memory_mapping=False, device=0):
     A FAISS index file (what the reference passes: `image.index`, or a folder holding `populated.index`) is read by
     faiss_io.read_faiss_index when it is a flat / fp16 / IVF-Flat inner-product index, or an IVF-PQ one (8-bit codes,
     flat or HNSW coarse quantiser, optionally behind one OPQ / rotation pre-transform and an id map: what autofaiss
-    writes for large collections) served from its codes; the file's nprobe is kept.  Other types raise
-    NotImplementedError naming what is missing.
+    writes for large collections) served from its codes; the file's nprobe is kept.  The lists may be in the file
+    (ilar) or, for the folder `index_combiner` / FAISS merge_ondisk writes, in `merged_index.ivfdata` beside
+    `populated.index` (ilod).  Other types raise NotImplementedError naming what is missing.
+
+    Residency (IVF-PQ, either list format): the codes go to HBM when ntotal x the padded code pitch fits within
+    `max_device_bytes`; otherwise the lists stay in the file's memory map and every search streams the probed ones
+    (`B200IVFPQIndex.set_host_lists`).  The default budget is the free device memory at load time less the search
+    scratch the index needs, so any file that fits is resident; an explicit budget lets the indices and the model of
+    one ClipResource share a card, and 0 always streams.  Flat and IVF-Flat indices are always resident.  Either way
+    results carry the file's ids.
     """
     del enable_faiss_memory_mapping
     from . import faiss_io
@@ -433,7 +489,7 @@ def load_index(path, enable_faiss_memory_mapping=False, device=0):
     if os.path.isdir(path) and os.path.exists(os.path.join(path, "populated.index")):
         target = os.path.join(path, "populated.index")          # clip_back.py:591-592
     if os.path.isfile(target) and not target.endswith(".npy") and faiss_io.looks_like_faiss_index(target):
-        return index_from_faiss(faiss_io.read_faiss_index(target), device=device)
+        return index_from_faiss(faiss_io.read_faiss_index(target), device=device, max_device_bytes=max_device_bytes)
     files = list_embedding_shards(path)
     first = np.load(files[0], mmap_mode="r")
     index = B200FlatIndex(first.shape[1], device=device)
@@ -703,10 +759,56 @@ class _IdMapped:
         lims, D, I = self._index.range_search(x, thresh)
         return lims, D, self._m(I)
 
+    def search_device(self, q, k, reconstruct=False, out=None):
+        """The inner index's search_device with I mapped to the file's ids on the device (C ABI b200_ids_map_device),
+        in place in the returned (or the caller's `out`) I tensor."""
+        torch = _torch()
+        res = self._index.search_device(q, k, reconstruct=reconstruct, out=out)
+        I = res[1]
+        dm = getattr(self, "_dmap", None)
+        if dm is None or dm.device != I.device:
+            dm = self._dmap = torch.from_numpy(self._map).to(I.device)
+        st = torch.cuda.current_stream(I.device).cuda_stream
+        check(lib.b200_ids_map_device(I.data_ptr(), I.numel(), dm.data_ptr(), dm.numel(), I.data_ptr(),
+                                      I.device.index or 0, st), "ids_map")
+        return res
 
-def index_from_faiss(info, device=0):
-    """Index from the arrays faiss_io.read_faiss_index returns."""
-    d, ids = info["d"], info["ids"]
+
+STREAM_SCRATCH_BYTES = 256 << 20   # search workspace a resident IVF-PQ index keeps beside its codes (default budget)
+
+
+def _resident_budget(info, device):
+    """Device bytes an IVF-PQ index's codes may take by default: the free memory now, less the search scratch and the
+    8 bytes per row of slot ids and their inverse that a resident index keeps."""
+    torch = _torch()
+    free, _ = torch.cuda.mem_get_info(device)
+    return free - STREAM_SCRATCH_BYTES - 8 * int(info["ntotal"])
+
+
+def index_from_faiss(info, device=0, max_device_bytes=None):
+    """Index from the arrays faiss_io.read_faiss_index returns (see load_index for the residency rule)."""
+    d = info["d"]
+    if info["kind"] == "ivfpq":
+        inv = info["invlists"]
+        pitch = (info["M"] + 15) // 16 * 16
+        budget = _resident_budget(info, device) if max_device_bytes is None else int(max_device_bytes)
+        index = B200IVFPQIndex(d, info["nlist"], info["M"], info["centroids"], info["codebook"],
+                               by_residual=info["by_residual"], device=device)
+        if info.get("transform") is not None:
+            A, b = info["transform"]
+            index.set_pretransform(A, b)
+        index.nprobe = max(1, info["nprobe"])
+        if inv.ntotal * pitch > budget:
+            index.set_host_lists(inv)        # ids come straight from the lists
+            return index if info.get("id_map") is None else _IdMapped(index, info["id_map"])
+        for codes, lists in inv.chunks(1 << 22):   # rows per host-to-device chunk: the map may be a multi-GB file
+            index.add_codes(codes, lists)
+        index.finalize()
+        ids = info["ids"]
+        if not np.array_equal(ids, np.arange(len(ids), dtype=np.int64)):
+            return _IdMapped(index, ids)
+        return index
+    ids = info["ids"]
     if info["kind"] == "flat":
         index = B200FlatIndex(d, device=device)
         index.reserve(info["ntotal"])
@@ -714,19 +816,6 @@ def index_from_faiss(info, device=0):
         step = 1 << 20
         for s in range(0, rows.shape[0], step):
             index.add(np.ascontiguousarray(rows[s:s + step]))
-    elif info["kind"] == "ivfpq":
-        index = B200IVFPQIndex(d, info["nlist"], info["M"], info["centroids"], info["codebook"],
-                               by_residual=info["by_residual"], device=device)
-        if info.get("transform") is not None:
-            A, b = info["transform"]
-            index.set_pretransform(A, b)
-        lists = np.repeat(np.arange(info["nlist"], dtype=np.int32), info["list_sizes"])
-        codes = info["codes"]
-        step = 1 << 22   # rows per host-to-device chunk: the codes may be a memory map of a multi-GB file
-        for s in range(0, codes.shape[0], step):
-            index.add_codes(np.ascontiguousarray(codes[s:s + step]), lists[s:s + step])
-        index.nprobe = max(1, info["nprobe"])
-        index.finalize()
     else:
         index = B200IVFFlatIndex(d, info["nlist"], info["centroids"], device=device)
         lists = np.repeat(np.arange(info["nlist"], dtype=np.int32), info["list_sizes"])

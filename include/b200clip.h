@@ -91,6 +91,24 @@ int b200_index_add_codes(b200_index* idx, const uint8_t* codes, int64_t n, int c
  * A^T (y - b), which needs orthonormal rows of A (checked here within 4e-5, as FAISS does); otherwise reconstruct and
  * search with rows return B200_ERR_UNSUPPORTED while search itself works.  b200_index_d reports d_in afterwards. */
 int b200_index_set_pretransform(b200_index* idx, int d_in, const float* h_A, const float* h_b);
+/* IVF-PQ only, on an index holding no rows: serve the lists from HOST memory (an on-disk index's memory map) instead
+ * of HBM.  List l has h_sizes[l] rows; its M-byte code rows start at address h_code_addr[l] and its int64 ids at
+ * h_id_addr[l].  The memory must stay mapped, unchanged, for the life of the handle; nothing is copied here.
+ * Centroids, codebook and pre-transform stay on the device.  Each search pass copies the probes to the host, gathers
+ * the probed lists (ascending list id, file order inside a list) into pinned staging, copies them to a device arena on
+ * a copy stream and scans them there; two arenas overlap the gather and copy of one pass with the scan of the one
+ * before.  Search, search_device, range_search, ivf_lists and ntotal keep their contracts; ids are the lists' own
+ * (+ id_base), equal scores rank in list-order slot as in a resident load of the same lists, and every result equals
+ * that resident load's bit for bit.  Searches are never captured in CUDA graphs and return with the stream
+ * synchronised; reconstruct, add_codes and copy_rows return an error.  May be called again to re-point the lists. */
+int b200_index_set_host_lists(b200_index* idx, int nlist, const int64_t* h_sizes, const uint64_t* h_code_addr,
+                              const uint64_t* h_id_addr);
+/* Lists in host memory: bytes per device arena (two are allocated, plus as much pinned staging).  An arena is never
+ * smaller than nprobe x the largest list, so one query always fits; 0 = that least size.  Default 256 MiB. */
+int b200_index_set_stream_arena(b200_index* idx, size_t bytes);
+/* Lists in host memory, the last search or range_search: h_stats[4] = {host gather ms, copy ms (device events around
+ * each pass's host-to-device copies), code bytes staged, passes}. */
+int b200_index_last_stream_stats(const b200_index* idx, double* h_stats);
 /* M of an IVF-PQ index; 0 for the other kinds. */
 int b200_index_pq_m(const b200_index* idx);
 /* IVF-PQ only: encode n fp32 rows d_x [n, width] (width = d_in when a pre-transform is set, else d; 16-byte aligned
@@ -205,6 +223,10 @@ int b200_index_range_search(b200_index* idx, const float* h_q, float thresh, int
 /* reconstruct(id) for a batch of ids (device buffers): d_R [n, d] fp32; id -1 -> NaN row.  Flat and IVF (the IVF
  * store is in list order; an id -> slot map is built on first use). */
 int b200_index_reconstruct_device(b200_index* idx, const int64_t* d_ids, int64_t n, float* d_R, void* stream);
+/* d_out[i] = d_map[d_I[i]] for 0 <= d_I[i] < nmap, else -1 (device buffers, asynchronous on `stream`; d_out may be
+ * d_I): an index file's own ids for the insertion ids a search returns. */
+int b200_ids_map_device(const int64_t* d_I, int64_t n, const int64_t* d_map, int64_t nmap, int64_t* d_out, int device,
+                        void* stream);
 /* Merge G sorted candidate lists per query into one top-k (the step after the all-gather of
  * per-shard candidates, SURVEY.md §8e): d_Dg/d_Ig are [G, nq, k]; outputs [nq, k]. */
 int b200_topk_merge_device(const float* d_Dg, const int64_t* d_Ig, int G, int nq, int k,
