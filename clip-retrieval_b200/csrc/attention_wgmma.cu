@@ -11,10 +11,14 @@
 //
 // Per key block j of a query tile: S = Q K^T (4 x wgmma m64nNk16, both operands in shared memory), online softmax in
 // fp32 registers, then O += P V (wgmma m64n64k16 with P as the register A operand -- the S accumulator fragment packed
-// to bf16 is exactly the A fragment -- and V as the MN-major B operand straight from its TMA tile).  S_{j+1} is issued
-// before the softmax of block j, so the tensor cores work on it while the warpgroup computes exponentials.  Only the
-// last key block of a tile (the end of the sequence, or the causal diagonal) is masked, and it is computed on
-// N = 16 * ceil(keys / 16) columns and as many k16 steps of P V.
+// to bf16 is exactly the A fragment -- and V as the MN-major B operand straight from its TMA tile).  P_j V_j and
+// S_{j+1} are issued back to back after the softmax of block j, and the warpgroup waits for both before the next
+// softmax: inside one warpgroup the exponentials never overlap its own wgmmas, only those of the other warpgroups on the
+// SM (two CTAs of two).  Only the last key block of a tile (the end of the sequence, or the causal diagonal) is masked,
+// and it is computed on N = 16 * ceil(keys / 16) columns, its softmax on those columns and as many k16 steps of P V.
+//
+// The exponentials are ex2.approx.ftz: the same MUFU result as exp2f except that results below 2^-126 are flushed to
+// zero, which saves the range test and rescale exp2f wraps around every score.
 //
 // With per-sample key lengths (len[b] in 1..T, the key-padding mask of a bidirectional encoder) a sample sees keys
 // < len[b] only: the key blocks at or past len[b] are not loaded, the query tiles wholly past it are not computed, and
@@ -69,14 +73,18 @@ struct AttwRow {
   float m_lo, m_hi, l_lo, l_hi;
 };
 
-// Online softmax of one score block (in place: s becomes P, unnormalised) and the matching rescale of O.
+// Online softmax of one score block (in place: s becomes P, unnormalised), the matching rescale of O, and P packed to
+// bf16 as the A operand of P V (k-slice kk covers accumulator column blocks 2kk, 2kk+1).  Only the first NREG
+// registers (NREG / 2 columns) are computed: the last block of a tile is narrowed to 16 * ceil(keys / 16) columns, and
+// the registers past them would only be masked to -inf, giving P = 0 that no k16 step of P V reads.  Leaving them out
+// changes no maximum and no sum.
 // accumulator fragment: register i holds row 16*warp + lane/4 + 8*((i/2)%2), column 8*(i/4) + 2*(lane%4) + i%2
-template <bool MASK>
-__device__ __forceinline__ void attw_softmax(float (&s)[32], float (&o)[32], AttwRow& r, int lane, int key0, int kend,
-                                             int r_lo, int causal, float scale_log2e) {
+template <bool MASK, int NREG>
+__device__ __forceinline__ void attw_softmax(float (&s)[32], float (&o)[32], uint32_t (&pa)[4][4], AttwRow& r,
+                                             int lane, int key0, int kend, int r_lo, int causal, float scale_log2e) {
   float bm_lo = -INFINITY, bm_hi = -INFINITY;
 #pragma unroll
-  for (int i = 0; i < 32; i++) {
+  for (int i = 0; i < NREG; i++) {
     if (MASK) {
       const int key = key0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
       const int row = r_lo + 8 * ((i >> 1) & 1);
@@ -92,7 +100,7 @@ __device__ __forceinline__ void attw_softmax(float (&s)[32], float (&o)[32], Att
   const float mn_lo = fmaxf(r.m_lo, bm_lo), mn_hi = fmaxf(r.m_hi, bm_hi);
   // rows that have seen no live key yet keep m = -inf; avoid (-inf) - (-inf)
   const float ms_lo = mn_lo == -INFINITY ? 0.f : mn_lo, ms_hi = mn_hi == -INFINITY ? 0.f : mn_hi;
-  const float a_lo = exp2f((r.m_lo - ms_lo) * scale_log2e), a_hi = exp2f((r.m_hi - ms_hi) * scale_log2e);
+  const float a_lo = ptx::ex2_ftz((r.m_lo - ms_lo) * scale_log2e), a_hi = ptx::ex2_ftz((r.m_hi - ms_hi) * scale_log2e);
   r.m_lo = mn_lo;
   r.m_hi = mn_hi;
   r.l_lo *= a_lo;
@@ -101,11 +109,19 @@ __device__ __forceinline__ void attw_softmax(float (&s)[32], float (&o)[32], Att
   for (int i = 0; i < 32; i++) {
     const bool hi = (i >> 1) & 1;
     o[i] *= hi ? a_hi : a_lo;
+    if (i >= NREG) continue;
     // (s - m) * scale rounded as written, not fused into one fma: P, and so every embedding, stays bit for bit what
     // the earlier one-tile-per-CTA kernel computed
-    s[i] = exp2f((s[i] - (hi ? ms_hi : ms_lo)) * scale_log2e);
+    s[i] = ptx::ex2_ftz((s[i] - (hi ? ms_hi : ms_lo)) * scale_log2e);
     if (hi) r.l_hi += s[i];
     else r.l_lo += s[i];
+  }
+#pragma unroll
+  for (int kk = 0; kk < 4; kk++) {
+    pa[kk][0] = kk < NREG / 8 ? attw_pack(s[8 * kk + 0], s[8 * kk + 1]) : 0u;
+    pa[kk][1] = kk < NREG / 8 ? attw_pack(s[8 * kk + 2], s[8 * kk + 3]) : 0u;
+    pa[kk][2] = kk < NREG / 8 ? attw_pack(s[8 * kk + 4], s[8 * kk + 5]) : 0u;
+    pa[kk][3] = kk < NREG / 8 ? attw_pack(s[8 * kk + 6], s[8 * kk + 7]) : 0u;
   }
 }
 
@@ -145,7 +161,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16*
   // the warpgroup index through a shuffle: the compiler then knows it is uniform across the warp, and so is every
   // branch around a wgmma that depends on it (else it serialises the wgmmas)
   const int wg = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 7, 0);
-  const int tid = threadIdx.x & 127, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x & 127, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
   const int cq = h * ATTW_HD, ck = w + h * ATTW_HD, cv = 2 * w + h * ATTW_HD;
   // query tile t: warpgroup t % 2, its (t / 2)-th tile, in slot 2 (t % 2) + (t / 2) % 2, phase (t / 4) % 2
   auto load_q = [&](int t) {
@@ -180,6 +196,9 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16*
     const int nkt = (kend + ATTW_BK - 1) / ATTW_BK;
     const int last_cols = 16 * ((kend - (nkt - 1) * ATTW_BK + 15) / 16);
     const int r_lo = q0 + 16 * warp + (lane >> 2);
+    // a warp whose 16 rows all lie at or past the sample's keys (warps 1-3 of the last tile at T = 257) has no output
+    // to compute: it skips the softmax and the stores, and takes part in every wgmma of its warpgroup with P = 0
+    const bool live = q0 + 16 * warp < L;
     ptx::mbar_wait(barQ + slot, (t >> 2) & 1);
     const uint64_t dq = ptx::wgmma_desc_k_sw128(ptx::smem_u32(sQ + slot * ATTW_TILE));
 
@@ -206,18 +225,18 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16*
         // the tile's last Q K^T is done: once every warp of the warpgroup is here, the Q slot can be refilled
         ptx::named_barrier_sync(1 + wg, 128);
         if (tid == 0 && t + ATTW_QSLOTS < nlb) load_q(t + ATTW_QSLOTS);
-        attw_softmax<true>(s, o, r, lane, j * ATTW_BK, kend, r_lo, causal, scale_log2e);
-      } else {
-        attw_softmax<false>(s, o, r, lane, j * ATTW_BK, kend, r_lo, causal, scale_log2e);
       }
-      // P as the A operand: k-slice kk covers accumulator column blocks 2kk, 2kk+1
       uint32_t pa[4][4];
+      if (live) {
+        const int key0 = j * ATTW_BK;
+        if (!last) attw_softmax<false, 32>(s, o, pa, r, lane, key0, kend, r_lo, causal, scale_log2e);
+        else if (last_cols == 16) attw_softmax<true, 8>(s, o, pa, r, lane, key0, kend, r_lo, causal, scale_log2e);
+        else if (last_cols == 32) attw_softmax<true, 16>(s, o, pa, r, lane, key0, kend, r_lo, causal, scale_log2e);
+        else if (last_cols == 48) attw_softmax<true, 24>(s, o, pa, r, lane, key0, kend, r_lo, causal, scale_log2e);
+        else attw_softmax<true, 32>(s, o, pa, r, lane, key0, kend, r_lo, causal, scale_log2e);
+      } else {
 #pragma unroll
-      for (int kk = 0; kk < 4; kk++) {
-        pa[kk][0] = attw_pack(s[8 * kk + 0], s[8 * kk + 1]);
-        pa[kk][1] = attw_pack(s[8 * kk + 2], s[8 * kk + 3]);
-        pa[kk][2] = attw_pack(s[8 * kk + 4], s[8 * kk + 5]);
-        pa[kk][3] = attw_pack(s[8 * kk + 6], s[8 * kk + 7]);
+        for (int kk = 0; kk < 4; kk++) pa[kk][0] = pa[kk][1] = pa[kk][2] = pa[kk][3] = 0u;
       }
       const int ksteps = last ? last_cols / 16 : 4;
       ptx::mbar_wait(barV + j, 0);
@@ -236,6 +255,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16*
     for (int j = 0; j < nkt; j++) block(j);
     ptx::wgmma_wait<0>();
     ptx::fence_regs(o);
+    if (!live) continue;
 
     float l_lo = r.l_lo, l_hi = r.l_hi;
     l_lo += __shfl_xor_sync(0xffffffffu, l_lo, 1);
@@ -262,8 +282,8 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16*
       }
     }
   }
-  // rows of the query tiles past the sample's keys (none without lengths): 8 x 16-byte stores per row of the head
-  for (int i = nlb * ATTW_BQ * 8 + (int)threadIdx.x; i < T * 8; i += ATTW_THREADS)
+  // rows of the warps past the sample's keys (none without lengths): 8 x 16-byte stores per row of the head
+  for (int i = 16 * ((L + 15) / 16) * 8 + (int)threadIdx.x; i < T * 8; i += ATTW_THREADS)
     *reinterpret_cast<uint4*>(ob + (int64_t)(i >> 3) * w + 8 * (i & 7)) = make_uint4(0u, 0u, 0u, 0u);
 }
 
