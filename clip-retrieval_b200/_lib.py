@@ -185,6 +185,7 @@ PROTOTYPES = {
     "b200_mlp_load_layer": (_i, [_vp, _i, _vp, _vp]),
     "b200_mlp_forward_device": (_i, [_vp, _vp, _i, _vp, _vp]),
     "b200_text_encoder_create": (_i, [C.POINTER(TextEncoderConfigC), _i, C.POINTER(_vp)]),
+    "b200_text_encoder_create_mlp": (_i, [C.POINTER(TextEncoderConfigC), _i, _i, C.POINTER(_vp)]),
     "b200_text_encoder_destroy": (_i, [_vp]),
     "b200_text_encoder_load_weights": (_i, [_vp, C.POINTER(TensorViewC), _i]),
     "b200_text_encoder_encode_device": (_i, [_vp, _vp, _vp, _i, _i, _vp, _i, _i, _vp]),
@@ -193,6 +194,8 @@ PROTOTYPES = {
     "b200_text_encoder_set_profiling": (_i, [_vp, _i]),
     "b200_layernorm_eps_bf16_device": (_i, [_vp, _vp, _vp, _vp, _i64, _i, C.c_float, _i, _vp]),
     "b200_attention_len_bf16_device": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "b200_text_lengths_device": (_i, [_vp, _i, _i, _i64, _vp, _vp]),
+    "b200_mean_mlp_head_device": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "b200_encoder_embed_bf16_device": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, C.c_float, _vp, _i, _i, _i, _i, _i, _vp]),
 }
 

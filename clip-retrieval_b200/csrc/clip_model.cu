@@ -49,6 +49,7 @@ struct b200_clip {
   b200_clip_config cfg;
   int device = 0, sms = 132;
   bool loaded = false;
+  bool has_text = true;       // false: an image-only handle (all-zero text tower config), no text weights or buffers
   b200::Tower vis, txt;
   // vision front end
   int grid = 0, Kp = 0;
@@ -204,8 +205,9 @@ extern "C" {
 
 int b200_clip_create(const b200_clip_config* cfg, int device, b200_clip** out) {
   B200_CHECK(cfg && out, B200_ERR_INVALID, "clip_create: null argument");
+  const bool has_text = cfg->text.width != 0 || cfg->text.layers != 0 || cfg->text.heads != 0 || cfg->text.mlp != 0;
   B200_CHECK(cfg->max_batch >= 1 && cfg->embed_dim >= 8 && cfg->patch >= 1 && cfg->image_size >= cfg->patch &&
-                 cfg->context_length >= 1 && cfg->vocab_size >= 2,
+                 (!has_text || (cfg->context_length >= 1 && cfg->vocab_size >= 2)),
              B200_ERR_INVALID, "clip_create: bad config");
   int ndev = 0;
   B200_CUDA(cudaGetDeviceCount(&ndev));
@@ -216,6 +218,7 @@ int b200_clip_create(const b200_clip_config* cfg, int device, b200_clip** out) {
   m->cfg = *cfg;
   m->device = device;
   m->sms = sm_count(device);
+  m->has_text = has_text;
   if (const char* g = getenv("B200_GRAPHS")) m->use_graphs = atoi(g) != 0;
   m->grid = cfg->image_size / cfg->patch;
   const int k_raw = 3 * cfg->patch * cfg->patch;
@@ -224,7 +227,7 @@ int b200_clip_create(const b200_clip_config* cfg, int device, b200_clip** out) {
   int rc = B200_OK;
   auto build = [&]() -> int {
     B200_TRY(make_tower(m, &m->vis, cfg->vision, T, cfg->embed_dim));
-    B200_TRY(make_tower(m, &m->txt, cfg->text, cfg->context_length, cfg->embed_dim));
+    if (has_text) B200_TRY(make_tower(m, &m->txt, cfg->text, cfg->context_length, cfg->embed_dim));
     DeviceAllocs& al = m->allocs;
     B200_TRY(make_linear(al, &m->conv, cfg->vision.width, m->Kp, false));
     const size_t prow = (size_t)cfg->max_batch * m->grid * m->grid;
@@ -235,16 +238,19 @@ int b200_clip_create(const b200_clip_config* cfg, int device, b200_clip** out) {
     B200_TRY(al.alloc(&m->cls_pos0, (size_t)cfg->vision.width));
     B200_TRY(al.alloc(&m->lnpre_g, (size_t)cfg->vision.width));
     B200_TRY(al.alloc(&m->lnpre_b, (size_t)cfg->vision.width));
-    B200_TRY(al.alloc(&m->tok_emb, (size_t)cfg->vocab_size * cfg->text.width));
-    B200_TRY(al.alloc(&m->tpos, (size_t)cfg->context_length * cfg->text.width));
-    B200_TRY(al.alloc(&m->pool_idx, (size_t)cfg->max_batch));
+    if (has_text) {
+      B200_TRY(al.alloc(&m->tok_emb, (size_t)cfg->vocab_size * cfg->text.width));
+      B200_TRY(al.alloc(&m->tpos, (size_t)cfg->context_length * cfg->text.width));
+      B200_TRY(al.alloc(&m->pool_idx, (size_t)cfg->max_batch));
+    }
+    const size_t tok_bytes = has_text ? (size_t)cfg->context_length * 8 : 0;
     B200_TRY(al.alloc(&m->feat, (size_t)cfg->max_batch * cfg->embed_dim));
     const size_t in_bytes = std::max((size_t)cfg->max_batch * 3 * cfg->image_size * cfg->image_size * 4,
-                                     (size_t)cfg->max_batch * cfg->context_length * 8);
+                                     (size_t)cfg->max_batch * tok_bytes);
     B200_TRY(al.alloc(&m->stage_in, in_bytes));
     B200_TRY(al.alloc(&m->stage_out, (size_t)cfg->max_batch * cfg->embed_dim * 4));
     const int gb = std::min(GRAPH_MAX_B, cfg->max_batch);
-    B200_TRY(al.alloc(&m->g_in, std::max((size_t)gb * 3 * cfg->image_size * cfg->image_size * 4, (size_t)gb * cfg->context_length * 8)));
+    B200_TRY(al.alloc(&m->g_in, std::max((size_t)gb * 3 * cfg->image_size * cfg->image_size * 4, (size_t)gb * tok_bytes)));
     B200_TRY(al.alloc(&m->g_out, (size_t)gb * cfg->embed_dim * 4));
     return B200_OK;
   };
@@ -296,12 +302,14 @@ int b200_clip_load_weights(b200_clip* m, const b200_tensor_view* tensors, int n)
   B200_TRY(ld.put_f32("visual.ln_post.weight", m->vis.lnf_g, vw));
   B200_TRY(ld.put_f32("visual.ln_post.bias", m->vis.lnf_b, vw));
   B200_TRY(ld.put_bf16("visual.proj", m->vis.proj, vw, D, D));
-  B200_TRY(ld.put_bf16("token_embedding.weight", m->tok_emb, (size_t)c.vocab_size, tw, tw));
-  B200_TRY(ld.put_f32("positional_embedding", m->tpos, (size_t)c.context_length * tw));
-  B200_TRY(load_tower(ld, m->txt, ""));
-  B200_TRY(ld.put_f32("ln_final.weight", m->txt.lnf_g, tw));
-  B200_TRY(ld.put_f32("ln_final.bias", m->txt.lnf_b, tw));
-  B200_TRY(ld.put_bf16("text_projection", m->txt.proj, tw, D, D));
+  if (m->has_text) {
+    B200_TRY(ld.put_bf16("token_embedding.weight", m->tok_emb, (size_t)c.vocab_size, tw, tw));
+    B200_TRY(ld.put_f32("positional_embedding", m->tpos, (size_t)c.context_length * tw));
+    B200_TRY(load_tower(ld, m->txt, ""));
+    B200_TRY(ld.put_f32("ln_final.weight", m->txt.lnf_g, tw));
+    B200_TRY(ld.put_f32("ln_final.bias", m->txt.lnf_b, tw));
+    B200_TRY(ld.put_bf16("text_projection", m->txt.proj, tw, D, D));
+  }
   B200_CUDA(cudaDeviceSynchronize());
   m->loaded = true;
   return B200_OK;
@@ -311,6 +319,7 @@ static int encode_device(b200_clip* m, const void* d_in, int B, void* d_out, int
                          cudaStream_t st) {
   B200_CHECK(m && (B == 0 || (d_in && d_out)) && B >= 0, B200_ERR_INVALID, "encode: bad argument");
   B200_CHECK(m->loaded, B200_ERR_STATE, "encode: weights not loaded");
+  B200_CHECK(image || m->has_text, B200_ERR_UNSUPPORTED, "encode_text: this handle has no text tower");
   B200_CHECK(out_dtype == B200_OUT_F16 || out_dtype == B200_OUT_F32, B200_ERR_INVALID, "encode: out_dtype %d", out_dtype);
   DeviceGuard g(m->device);
   m->timer.launches = 0;
@@ -393,6 +402,7 @@ int b200_clip_encode_text_device(b200_clip* m, const int64_t* d_tokens, int B, v
 static int encode_host(b200_clip* m, const void* h_in, int B, void* h_out, int out_dtype, int normalize, bool image) {
   B200_CHECK(m && (B == 0 || (h_in && h_out)) && B >= 0, B200_ERR_INVALID, "encode: bad argument");
   B200_CHECK(m->loaded, B200_ERR_STATE, "encode: weights not loaded");
+  B200_CHECK(image || m->has_text, B200_ERR_UNSUPPORTED, "encode_text: this handle has no text tower");
   std::lock_guard<std::mutex> lock(m->mu);
   DeviceGuard g(m->device);
   if (!m->s_copy) {

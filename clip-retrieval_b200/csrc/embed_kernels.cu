@@ -427,6 +427,41 @@ int encoder_embed(const int64_t* ids, const __nv_bfloat16* word, const float* tt
   return B200_OK;
 }
 
+// The pieces of the masked-mean heads below.  s_row[j] = (sum over t < L, ascending, of x[b*T + t, j] in fp32) / L
+// with L = len[b] clamped to 1..T: one thread per column.
+__device__ __forceinline__ void masked_mean_row(const __nv_bfloat16* __restrict__ x, int T, int w,
+                                                const int* __restrict__ len, int b, float* s_row) {
+  const int L = min(max(len[b], 1), T);
+  const __nv_bfloat16* src = x + (size_t)b * T * w;
+  for (int j = threadIdx.x; j < w; j += blockDim.x) {
+    float acc = 0.f;
+    for (int t = 0; t < L; t++) acc += __bfloat162float(src[(size_t)t * w + j]);
+    s_row[j] = acc / (float)L;
+  }
+}
+
+// Column j0 + (threadIdx.x & 63) of s_row [K] @ WT [K, N] for a block of 256 threads: the reduction dimension is split
+// over 4 quarters, each summed in two interleaved fma chains, and the quarters are added in a fixed order.  Every
+// thread of the block must call it (it synchronises); the value is meaningful in threads 0..63 with column < N.
+__device__ __forceinline__ float split_column_dot(const float* s_row, int K, const float* __restrict__ WT, int N,
+                                                  int j0, float* s_part) {
+  const int jj = threadIdx.x & 63, quarter = threadIdx.x >> 6;
+  const int j = j0 + jj;
+  const int per = (K + 3) / 4, i0 = quarter * per, i1 = min(K, i0 + per);
+  float acc0 = 0.f, acc1 = 0.f;
+  if (j < N) {
+    int i = i0;
+    for (; i + 1 < i1; i += 2) {
+      acc0 = fmaf(s_row[i], WT[(size_t)i * N + j], acc0);
+      acc1 = fmaf(s_row[i + 1], WT[(size_t)(i + 1) * N + j], acc1);
+    }
+    if (i < i1) acc0 = fmaf(s_row[i], WT[(size_t)i * N + j], acc0);
+  }
+  s_part[quarter * 64 + jj] = acc0 + acc1;
+  __syncthreads();
+  return (s_part[jj] + s_part[64 + jj]) + (s_part[128 + jj] + s_part[192 + jj]);
+}
+
 // Masked mean + projection, split like pool_proj_split_kernel: a block owns 64 output columns of one sample, forms
 // the mean row itself (one thread per column, tokens in ascending order) and splits the projection over 4 quarters
 // of the reduction dimension.
@@ -438,32 +473,53 @@ masked_mean_proj_kernel(const __nv_bfloat16* __restrict__ x, int T, int w, const
   float* s_row = sm;                // [w]
   float* s_part = sm + w;           // [4][64]
   const int b = blockIdx.y, j0 = blockIdx.x * 64;
-  const int L = min(max(len[b], 1), T);
-  const __nv_bfloat16* src = x + (size_t)b * T * w;
-  for (int j = threadIdx.x; j < w; j += blockDim.x) {
-    float acc = 0.f;
-    for (int t = 0; t < L; t++) acc += __bfloat162float(src[(size_t)t * w + j]);
-    s_row[j] = acc / (float)L;
-  }
+  masked_mean_row(x, T, w, len, b, s_row);
   __syncthreads();
-  const int jj = threadIdx.x & 63, quarter = threadIdx.x >> 6;
-  const int j = j0 + jj;
-  const int per = (w + 3) / 4, i0 = quarter * per, i1 = min(w, i0 + per);
-  float acc0 = 0.f, acc1 = 0.f;
-  if (j < D) {
-    int i = i0;
-    for (; i + 1 < i1; i += 2) {
-      acc0 = fmaf(s_row[i], projT[(size_t)i * D + j], acc0);
-      acc1 = fmaf(s_row[i + 1], projT[(size_t)(i + 1) * D + j], acc1);
-    }
-    if (i < i1) acc0 = fmaf(s_row[i], projT[(size_t)i * D + j], acc0);
-  }
-  s_part[quarter * 64 + jj] = acc0 + acc1;
+  const float f = split_column_dot(s_row, w, projT, D, j0, s_part);
+  const int j = j0 + threadIdx.x;
+  if (threadIdx.x < 64 && j < D) feat[(size_t)b * D + j] = bias != nullptr ? f + bias[j] : f;
+}
+
+// open_clip's MLP text head (proj "mlp": Linear(w, h, bias=False), GELU, Linear(h, D, bias=False)) on the masked
+// mean, in two launches so that each layer is spread over (columns / 64) x B blocks.  Layer 1: every block forms the
+// mean row of its sample, then hid[b, j] = gelu_erf(mean . W1T[:, j]) for its 64 columns j.
+__global__ void __launch_bounds__(256)
+masked_mean_mlp1_kernel(const __nv_bfloat16* __restrict__ x, int T, int w, const int* __restrict__ len,
+                        const float* __restrict__ w1T, int h, float* __restrict__ hid) {
+  extern __shared__ float sm[];
+  float* s_row = sm;                // [w]
+  float* s_part = sm + w;           // [4][64]
+  const int b = blockIdx.y, j0 = blockIdx.x * 64;
+  masked_mean_row(x, T, w, len, b, s_row);
   __syncthreads();
-  if (quarter == 0 && j < D) {
-    const float f = (s_part[jj] + s_part[64 + jj]) + (s_part[128 + jj] + s_part[192 + jj]);
-    feat[(size_t)b * D + j] = bias != nullptr ? f + bias[j] : f;
-  }
+  const float y = split_column_dot(s_row, w, w1T, h, j0, s_part);
+  const int j = j0 + threadIdx.x;
+  if (threadIdx.x < 64 && j < h) hid[(size_t)b * h + j] = 0.5f * y * (1.0f + erff(y * 0.70710678118654752f));
+}
+
+// Layer 2: feat[b, j] = hid[b, :] . W2T[:, j] for the block's 64 columns j.
+__global__ void __launch_bounds__(256)
+mlp2_kernel(const float* __restrict__ hid, int h, const float* __restrict__ w2T, int D, float* __restrict__ feat) {
+  extern __shared__ float sm[];
+  float* s_row = sm;                // [h]
+  float* s_part = sm + h;           // [4][64]
+  const int b = blockIdx.y, j0 = blockIdx.x * 64;
+  for (int i = threadIdx.x; i < h; i += blockDim.x) s_row[i] = hid[(size_t)b * h + i];
+  __syncthreads();
+  const float f = split_column_dot(s_row, h, w2T, D, j0, s_part);
+  const int j = j0 + threadIdx.x;
+  if (threadIdx.x < 64 && j < D) feat[(size_t)b * D + j] = f;
+}
+
+// len[b] = the first t with ids[b, t] == pad_id, or T when the row has none (right-padded rows: the token count).
+__global__ void token_lengths_kernel(const int64_t* __restrict__ ids, int B, int T, int64_t pad_id,
+                                     int* __restrict__ len) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const int64_t* row = ids + (size_t)b * T;
+  int t = 0;
+  while (t < T && row[t] != pad_id) t++;
+  len[b] = t;
 }
 
 // clip_back.py normalized(): a / |a|, with |a| == 0 replaced by 1 (a zero row stays zero, never NaN).
@@ -493,6 +549,29 @@ int masked_mean_proj_norm(const __nv_bfloat16* x, int T, int w, const int* len, 
   masked_mean_proj_kernel<<<dim3((D + 63) / 64, B), 256, smem, st>>>(x, T, w, len, projT, bias, D, feat);
   B200_LAUNCH_OK();
   feat_normalized_cast_kernel<<<B, 256, 0, st>>>(feat, D, out, out_f16, normalize);
+  B200_LAUNCH_OK();
+  return B200_OK;
+}
+
+int masked_mean_mlp_norm(const __nv_bfloat16* x, int T, int w, const int* len, const float* w1T, int h,
+                         const float* w2T, int D, float* hid, float* feat, void* out, int out_f16, int normalize, int B,
+                         cudaStream_t st) {
+  if (B == 0) return B200_OK;
+  const size_t smem = (size_t)(std::max(w, h) + 256) * sizeof(float);
+  B200_CHECK(smem <= 48 * 1024, B200_ERR_UNSUPPORTED, "masked_mean_mlp: width %d / hidden %d too large", w, h);
+  masked_mean_mlp1_kernel<<<dim3((h + 63) / 64, B), 256, (size_t)(w + 256) * sizeof(float), st>>>(x, T, w, len, w1T, h,
+                                                                                                   hid);
+  B200_LAUNCH_OK();
+  mlp2_kernel<<<dim3((D + 63) / 64, B), 256, (size_t)(h + 256) * sizeof(float), st>>>(hid, h, w2T, D, feat);
+  B200_LAUNCH_OK();
+  feat_normalized_cast_kernel<<<B, 256, 0, st>>>(feat, D, out, out_f16, normalize);
+  B200_LAUNCH_OK();
+  return B200_OK;
+}
+
+int token_lengths(const int64_t* ids, int B, int T, int64_t pad_id, int* len, cudaStream_t st) {
+  if (B == 0) return B200_OK;
+  token_lengths_kernel<<<(B + 127) / 128, 128, 0, st>>>(ids, B, T, pad_id, len);
   B200_LAUNCH_OK();
   return B200_OK;
 }

@@ -48,6 +48,14 @@ int encoder_embed(const int64_t* ids, const __nv_bfloat16* word, const float* tt
 // sample); out = f / (normalize ? (|f| == 0 ? 1 : |f|) : 1) as fp16 or fp32 (clip_back.py normalized()).
 int masked_mean_proj_norm(const __nv_bfloat16* x, int T, int w, const int* len, const float* projT, const float* bias,
                           int D, float* feat, void* out, int out_f16, int normalize, int B, cudaStream_t st);
+// open_clip's MLP text head on the masked mean m of masked_mean_proj_norm: hid = gelu_erf(m @ w1T [w, h]) into hid
+// fp32 [B, h], f = hid @ w2T [h, D] into feat fp32 [B, D], all in fp32 (each layer in blocks of 64 output columns
+// per sample); out as masked_mean_proj_norm writes it.
+int masked_mean_mlp_norm(const __nv_bfloat16* x, int T, int w, const int* len, const float* w1T, int h,
+                         const float* w2T, int D, float* hid, float* feat, void* out, int out_f16, int normalize, int B,
+                         cudaStream_t st);
+// len[b] = index of the first pad_id in row b of ids [B, T], T when there is none (0 for a row of padding only).
+int token_lengths(const int64_t* ids, int B, int T, int64_t pad_id, int* len, cudaStream_t st);
 // argmax(tokens, dim=-1) (first maximum) -> pool_idx[b]
 int token_argmax(const int64_t* tokens, int* pool_idx, int B, int T, cudaStream_t st);
 

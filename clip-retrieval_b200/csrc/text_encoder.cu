@@ -6,6 +6,8 @@
 //   per layer (post-LN):  x = LN1(x + Wo · attn(Wqkv · x + b, keys < len[b]) + bo)
 //                         x = LN2(x + W2 · gelu_erf(W1 · x + b1) + b2)
 //   out = normalized(mean over t < len[b] of x, @ projection (+ bias))
+//   or, with the MLP head of open_clip's HF text towers (b200_text_encoder_create_mlp):
+//   out = normalized(W2 · gelu_erf(W1 · mean over t < len[b] of x)), no biases, all in fp32
 // Weights bf16 [N, K] for the GEMMs (q, k, v concatenated into one [3w, w] in-projection at load time), LayerNorm
 // affine, biases, position / token-type tables and the projection fp32.  Activations bf16 [rows, width] sized for
 // max_batch x max_tokens rows, so the GEMM operand maps are built once; the 3-D map of the wgmma attention depends
@@ -45,8 +47,11 @@ struct b200_text_encoder {
   float* pos = nullptr;            // [positions, w]
   float *emb_g = nullptr, *emb_b = nullptr;
   std::vector<b200::EncLayer> L;
-  float* projT = nullptr;          // [w, D]
+  float* projT = nullptr;          // [w, D] (linear head)
   float* proj_b = nullptr;         // [D] or null
+  int hidden = 0;                  // > 0: the MLP head, w -> hidden -> D
+  float *w1T = nullptr, *w2T = nullptr;   // [w, hidden], [hidden, D]
+  float* hid = nullptr;            // [max_batch, hidden]
   // activations
   __nv_bfloat16 *x = nullptr, *qkv = nullptr, *a = nullptr, *f = nullptr;
   CUtensorMap tm_x, tm_a, tm_f;
@@ -108,6 +113,11 @@ int enc_forward(b200_text_encoder* m, const int64_t* d_ids, const int* d_len, in
     B200_TRY(enc_gemm(m, m->tm_f, L.fc2, M, e4, st));
     B200_TRY(enc_ln(m, L.ln2_g, L.ln2_b, M, st));
   }
+  if (m->hidden > 0) {
+    TimedSpan sp(m->timer, ENC_OTHER, st, 3);
+    return masked_mean_mlp_norm(m->x, T, w, d_len, m->w1T, m->hidden, m->w2T, c.out_dim, m->hid, m->feat, d_out, out_f16,
+                                normalize, B, st);
+  }
   TimedSpan sp(m->timer, ENC_OTHER, st, 2);
   return masked_mean_proj_norm(m->x, T, w, d_len, m->projT, m->proj_b, c.out_dim, m->feat, d_out, out_f16, normalize,
                                B, st);
@@ -137,9 +147,11 @@ int enc_encode(b200_text_encoder* m, const int64_t* d_ids, const int* d_len, int
 
 using namespace b200;
 
-extern "C" {
+namespace b200 {
+namespace {
 
-int b200_text_encoder_create(const b200_text_encoder_config* cfg, int device, b200_text_encoder** out) {
+// hidden == 0: the linear projection head; > 0: the MLP head (cfg->proj_bias must be 0).
+int text_encoder_create(const b200_text_encoder_config* cfg, int hidden, int device, b200_text_encoder** out) {
   B200_CHECK(cfg && out, B200_ERR_INVALID, "text_encoder_create: null argument");
   const b200_text_encoder_config& c = *cfg;
   B200_CHECK(c.layers >= 1 && c.heads >= 1 && c.width == 64 * c.heads && c.width <= 2048 && c.ffn >= 64 &&
@@ -158,6 +170,7 @@ int b200_text_encoder_create(const b200_text_encoder_config* cfg, int device, b2
   m->cfg = c;
   m->device = device;
   m->sms = sm_count(device);
+  m->hidden = hidden;
   auto build = [&]() -> int {
     const int w = c.width;
     const size_t rows = (size_t)c.max_batch * c.max_tokens;
@@ -176,8 +189,14 @@ int b200_text_encoder_create(const b200_text_encoder_config* cfg, int device, b2
       B200_TRY(al.alloc(&L.ln1_g, (size_t)w)); B200_TRY(al.alloc(&L.ln1_b, (size_t)w));
       B200_TRY(al.alloc(&L.ln2_g, (size_t)w)); B200_TRY(al.alloc(&L.ln2_b, (size_t)w));
     }
-    B200_TRY(al.alloc(&m->projT, (size_t)w * c.out_dim));
-    if (c.proj_bias) B200_TRY(al.alloc(&m->proj_b, (size_t)c.out_dim));
+    if (hidden > 0) {
+      B200_TRY(al.alloc(&m->w1T, (size_t)w * hidden));
+      B200_TRY(al.alloc(&m->w2T, (size_t)hidden * c.out_dim));
+      B200_TRY(al.alloc(&m->hid, (size_t)c.max_batch * hidden));
+    } else {
+      B200_TRY(al.alloc(&m->projT, (size_t)w * c.out_dim));
+      if (c.proj_bias) B200_TRY(al.alloc(&m->proj_b, (size_t)c.out_dim));
+    }
     B200_TRY(al.alloc(&m->x, rows * w));
     B200_TRY(al.alloc(&m->qkv, rows * 3 * w));
     B200_TRY(al.alloc(&m->a, rows * w));
@@ -198,6 +217,22 @@ int b200_text_encoder_create(const b200_text_encoder_config* cfg, int device, b2
   }
   *out = m;
   return B200_OK;
+}
+
+}  // namespace
+
+}  // namespace b200
+
+extern "C" {
+
+int b200_text_encoder_create(const b200_text_encoder_config* cfg, int device, b200_text_encoder** out) {
+  return text_encoder_create(cfg, 0, device, out);
+}
+
+int b200_text_encoder_create_mlp(const b200_text_encoder_config* cfg, int hidden, int device, b200_text_encoder** out) {
+  B200_CHECK(cfg && hidden >= 1 && hidden <= 12 * 1024 - 256 && cfg->proj_bias == 0, B200_ERR_INVALID,
+             "text_encoder_create_mlp: hidden %d (1..%d) and proj_bias 0 required", hidden, 12 * 1024 - 256);
+  return text_encoder_create(cfg, hidden, device, out);
 }
 
 int b200_text_encoder_destroy(b200_text_encoder* m) {
@@ -247,15 +282,22 @@ int b200_text_encoder_load_weights(b200_text_encoder* m, const b200_tensor_view*
     B200_TRY(ld.put_f32(p + "output.LayerNorm.weight", L.ln2_g, w));
     B200_TRY(ld.put_f32(p + "output.LayerNorm.bias", L.ln2_b, w));
   }
-  {
-    // nn.Linear weight [D, w] -> fp32 [w, D]: a projection thread reads one output column, consecutive threads
-    // consecutive columns
-    const b200_tensor_view* pw = ld.find("projection.weight", D * w);
+  // nn.Linear weight [N, K] -> fp32 [K, N]: a projection thread reads one output column, consecutive threads
+  // consecutive columns
+  auto put_transposed = [&](const char* name, float* dst, size_t N, size_t K) -> int {
+    const b200_tensor_view* pw = ld.find(name, N * K);
     if (!pw) return B200_ERR_INVALID;
-    std::vector<float> t(w * D);
-    for (size_t d = 0; d < D; d++)
-      for (size_t k = 0; k < w; k++) t[k * D + d] = view_get(*pw, d * w + k);
-    B200_CUDA(cudaMemcpy(m->projT, t.data(), t.size() * 4, cudaMemcpyHostToDevice));
+    std::vector<float> t(K * N);
+    for (size_t d = 0; d < N; d++)
+      for (size_t k = 0; k < K; k++) t[k * N + d] = view_get(*pw, d * K + k);
+    B200_CUDA(cudaMemcpy(dst, t.data(), t.size() * 4, cudaMemcpyHostToDevice));
+    return B200_OK;
+  };
+  if (m->hidden > 0) {
+    B200_TRY(put_transposed("projection.0.weight", m->w1T, (size_t)m->hidden, w));
+    B200_TRY(put_transposed("projection.2.weight", m->w2T, D, (size_t)m->hidden));
+  } else {
+    B200_TRY(put_transposed("projection.weight", m->projT, D, w));
   }
   if (c.proj_bias) B200_TRY(ld.put_f32("projection.bias", m->proj_b, D));
   B200_CUDA(cudaDeviceSynchronize());
@@ -330,6 +372,23 @@ int b200_attention_len_bf16_device(const void* d_qkv, const int32_t* d_len, void
   DeviceGuard g(device);
   return qkv_attention(nullptr, (const __nv_bfloat16*)d_qkv, (__nv_bfloat16*)d_out, B, T, heads, w, 0,
                        (cudaStream_t)stream, d_len);
+}
+
+int b200_text_lengths_device(const int64_t* d_ids, int B, int T, int64_t pad_id, int32_t* d_len, void* stream) {
+  B200_CHECK(B >= 0 && T >= 1 && (B == 0 || (d_ids && d_len)), B200_ERR_INVALID, "text_lengths: bad argument");
+  return token_lengths(d_ids, B, T, pad_id, d_len, (cudaStream_t)stream);
+}
+
+int b200_mean_mlp_head_device(const void* d_x, int B, int T, int w, const int32_t* d_len, const float* d_w1T,
+                              int hidden, const float* d_w2T, int D, float* d_hid, float* d_feat, void* d_out,
+                              int out_dtype, int normalize, int device, void* stream) {
+  B200_CHECK(B >= 0 && T >= 1 && w >= 1 && hidden >= 1 && D >= 1 &&
+                 (B == 0 || (d_x && d_len && d_w1T && d_w2T && d_hid && d_feat && d_out)) &&
+                 (out_dtype == B200_OUT_F16 || out_dtype == B200_OUT_F32),
+             B200_ERR_INVALID, "mean_mlp_head: bad argument");
+  DeviceGuard g(device);
+  return masked_mean_mlp_norm((const __nv_bfloat16*)d_x, T, w, d_len, d_w1T, hidden, d_w2T, D, d_hid, d_feat, d_out,
+                              out_dtype == B200_OUT_F16, normalize, B, (cudaStream_t)stream);
 }
 
 int b200_encoder_embed_bf16_device(const int64_t* d_ids, const void* d_word, const float* d_tt0, const float* d_pos,

@@ -306,10 +306,13 @@ class _MissingTokenizer:
 
 class B200TextEncoder:
     """A BERT-family text encoder on one GPU (b200_text_encoder_*).  Inputs are right-padded ids [B, T] and the
-    per-sample token counts; padding never changes a sample's result."""
+    per-sample token counts; padding never changes a sample's result.  `mlp_hidden` > 0 selects open_clip's MLP head
+    (width -> mlp_hidden -> out_dim, GELU between, no biases; weights projection.0.weight / projection.2.weight)
+    instead of the linear projection."""
 
-    def __init__(self, arch, device=0, max_batch=64, max_tokens=None):
+    def __init__(self, arch, device=0, max_batch=64, max_tokens=None, mlp_hidden=0):
         self.arch = arch
+        self.mlp_hidden = int(mlp_hidden)
         self.device_index = int(device)
         self.max_batch = int(max_batch)
         self.max_tokens = int(max_tokens or arch.max_tokens)
@@ -319,7 +322,11 @@ class B200TextEncoder:
                                       arch.max_positions, arch.type_vocab_size, arch.position_offset,
                                       arch.layer_norm_eps, arch.out_dim, 1 if arch.proj_bias else 0,
                                       self.max_batch, self.max_tokens)
-        check(lib.b200_text_encoder_create(C.byref(cfg), self.device_index, C.byref(self._h)), "text_encoder_create")
+        if self.mlp_hidden:
+            check(lib.b200_text_encoder_create_mlp(C.byref(cfg), self.mlp_hidden, self.device_index, C.byref(self._h)),
+                  "text_encoder_create_mlp")
+        else:
+            check(lib.b200_text_encoder_create(C.byref(cfg), self.device_index, C.byref(self._h)), "text_encoder_create")
 
     def __del__(self):
         try:
@@ -360,15 +367,17 @@ class B200TextEncoder:
                   "text_encoder_encode")
         return out
 
-    def embed_text(self, ids, lengths, normalize=True):
-        """Host arrays in, np.float32 [B, out_dim] out (H2D, forward, D2H in one library call)."""
+    def embed_text(self, ids, lengths, normalize=True, dtype=np.float32):
+        """Host arrays in, np.float32 (or `dtype` np.float16) [B, out_dim] out (H2D, forward, D2H in one library
+        call)."""
         ids = np.ascontiguousarray(ids, dtype=np.int64)
         lengths = np.ascontiguousarray(lengths, dtype=np.int32)
         if ids.ndim != 2 or lengths.shape != (ids.shape[0],):
             raise ValueError("embed_text: ids [B, T] and lengths [B], got %r and %r" % (ids.shape, lengths.shape))
-        out = np.empty((ids.shape[0], self.arch.out_dim), dtype=np.float32)
+        out = np.empty((ids.shape[0], self.arch.out_dim), dtype=dtype)
         check(lib.b200_text_encoder_encode(self._h, ids.ctypes.data, lengths.ctypes.data, ids.shape[0], ids.shape[1],
-                                           out.ctypes.data, 0, 1 if normalize else 0), "text_encoder_encode")
+                                           out.ctypes.data, 1 if out.dtype == np.float16 else 0, 1 if normalize else 0),
+              "text_encoder_encode")
         return out
 
     def set_profiling(self, on):

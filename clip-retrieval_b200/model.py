@@ -540,11 +540,16 @@ def load_clip(clip_model="ViT-B/32", use_jit=True, warmup_batch_size=1, clip_cac
     Returns (model, preprocess, tokenizer).  Weights come from `<clip_cache_path>/<model>.pt` (a
     state_dict in the OpenAI/open_clip key layout, or a HuggingFace CLIPModel state_dict); the name
     prefix `synthetic:` selects seeded random weights of that architecture (benchmarks; no network).
+    `open_clip:xlm-roberta-base-ViT-B-32` / `open_clip:xlm-roberta-large-ViT-H-14` give a `B200XLMRClip`
+    (xlmr_clip.py) and the XLM-R tokenizer of `<clip_cache_path>/xlm-roberta-{base,large}/tokenizer.json`.
     `use_jit` is accepted and ignored (there is no TorchScript path).  Cached per argument tuple like
     the upstream loader, so reader and mapper builders share one model."""
     del use_jit
+    from .xlmr_clip import load_xlmr_clip, resolve_xlmr_clip
+
     torch = _torch()
-    arch, key = resolve_arch(clip_model)
+    xlmr = resolve_xlmr_clip(clip_model)
+    arch, key = xlmr if xlmr is not None else resolve_arch(clip_model)
     if device is None:
         dev_index = torch.cuda.current_device() if torch.cuda.is_available() else 0
     else:
@@ -553,6 +558,9 @@ def load_clip(clip_model="ViT-B/32", use_jit=True, warmup_batch_size=1, clip_cac
             raise RuntimeError("b200clip has no CPU path: device=%r" % (device,))
         dev_index = d.index if d.index is not None else torch.cuda.current_device()
     mb = max_batch or max(int(warmup_batch_size), 1)
+    if xlmr is not None:
+        # open_clip's XLM-RoBERTa CLIPs: an image-only CLIP handle and the text encoder with the MLP head
+        return load_xlmr_clip(clip_model, arch, key, warmup_batch_size, clip_cache_path, dev_index, mb)
     model = B200Clip(arch, device=dev_index, max_batch=mb)
     if clip_model.startswith("synthetic:"):
         model.load_state_dict(synthetic_state_dict(arch, seed=0))

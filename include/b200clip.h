@@ -294,6 +294,10 @@ typedef struct b200_tensor_view {
 #define B200_OUT_F16 1
 #define B200_OUT_F32 0
 
+/* A `text` tower config of all zeros makes an image-only handle (the image tower of a CLIP whose text tower runs
+ * elsewhere, e.g. open_clip's XLM-RoBERTa models on a b200_text_encoder): no text weights or activations are
+ * allocated, context_length and vocab_size are not read, load_weights needs only the visual.* tensors, and the
+ * encode_text entries return B200_ERR_UNSUPPORTED. */
 int b200_clip_create(const b200_clip_config* cfg, int device, b200_clip** out);
 int b200_clip_destroy(b200_clip* m);
 /* Upload weights given as a state_dict in the open_clip/OpenAI key layout; converts to the
@@ -381,6 +385,11 @@ typedef struct b200_text_encoder_config {
 } b200_text_encoder_config;
 
 int b200_text_encoder_create(const b200_text_encoder_config* cfg, int device, b200_text_encoder** out);
+/* The same encoder with the MLP head of open_clip's HuggingFace text towers (proj "mlp", mean pooler):
+ * out = normalized(W2 · gelu_erf(W1 · mean)), W1 [hidden, width], W2 [out_dim, hidden], no biases, fp32 throughout.
+ * cfg->proj_bias must be 0; load_weights then takes projection.0.weight and projection.2.weight instead of
+ * projection.weight. */
+int b200_text_encoder_create_mlp(const b200_text_encoder_config* cfg, int hidden, int device, b200_text_encoder** out);
 int b200_text_encoder_destroy(b200_text_encoder* m);
 /* Weights in the HuggingFace BERT / XLM-RoBERTa key layout without a model prefix:
  * embeddings.{word,position,token_type}_embeddings.weight, embeddings.LayerNorm.{weight,bias},
@@ -410,6 +419,16 @@ int b200_layernorm_eps_bf16_device(const void* d_in, void* d_out, const float* d
                                    int64_t rows, int w, float eps, int device, void* stream);
 int b200_attention_len_bf16_device(const void* d_qkv, const int32_t* d_len, void* d_out, int B, int T, int heads,
                                    int w, int device, void* stream);
+/* d_len[b] = index of the first pad_id in row b of d_ids [B, T] (int64), T when the row has none: the token count
+ * of a right-padded row, computed on the device (a row of padding only gives 0, which the encoder reads as 1).
+ * Asynchronous on `stream`, on the current device. */
+int b200_text_lengths_device(const int64_t* d_ids, int B, int T, int64_t pad_id, int32_t* d_len, void* stream);
+/* The MLP head alone: masked mean of d_x bf16 [B*T, w] over t < d_len[b], d_hid [B, hidden] = gelu_erf(mean @ d_w1T),
+ * d_feat [B, D] = d_hid @ d_w2T (d_w1T fp32 [w, hidden], d_w2T fp32 [hidden, D]: the nn.Linear weights transposed),
+ * d_out [B, D] as the encoder writes it. */
+int b200_mean_mlp_head_device(const void* d_x, int B, int T, int w, const int32_t* d_len, const float* d_w1T,
+                              int hidden, const float* d_w2T, int D, float* d_hid, float* d_feat, void* d_out,
+                              int out_dtype, int normalize, int device, void* stream);
 int b200_encoder_embed_bf16_device(const int64_t* d_ids, const void* d_word, const float* d_tt0, const float* d_pos,
                                    int position_offset, const float* d_gamma, const float* d_beta, float eps,
                                    void* d_out, int B, int T, int w, int vocab, int device, void* stream);
