@@ -168,6 +168,7 @@ int ivf_range_scan(b200_index* idx, const float* d_q, float thresh, unsigned lon
 int grow_pending(b200_index* idx, int64_t need, bool amortised);
 
 // ---- knn_ivfpq.cu ---------------------------------------------------------------------------------------
+constexpr int PQ_QB = 256;   // queries per batch or streamed pass at most (bounds the tables scratch)
 struct PqPlan {
   int cs = 0, mc = 0, warps = 0;
   size_t smem = 0;
@@ -179,17 +180,32 @@ struct PqStore {
   const uint32_t* row_ids;
   const int64_t* offsets;
 };
-PqPlan pq_plan(int pitch, int k);
-int pq_coarse_plan(const b200_index* idx, const char* what, int nprobe, SelectPlan* cp);
-size_t pq_w4_bytes(const b200_index* idx, int qb);
-int pq_query_space(b200_index* idx, const float* d_q, int qb, float* w4, const float** q_out, float** tables_out,
-                   cudaStream_t st);
-int pq_probe_step(b200_index* idx, const float* q, int qb, const SelectPlan& cp, unsigned long long* probes, char* w0,
-                  cudaStream_t st);
-int pq_table_step(b200_index* idx, const float* q, int qb, float* tables, cudaStream_t st);
-int pq_launch_scan(b200_index* idx, const PqStore& store, bool range, const PqPlan& pl, int nq, const float* tables,
-                   const unsigned long long* probes, int nprobe, int segs, int cpq, int k, unsigned long long* out,
-                   int64_t out_stride_q, float thresh, unsigned int cap, unsigned int* counter, cudaStream_t st);
+// Everything an IVF-PQ search decides before its first launch, whether its lists sit in HBM or in host memory: the
+// coarse select `cp`, the list-scan plan `pl`, `segs` segments per probed list, `cpq` clusters per query, Mq candidates
+// per query and their select `sel`, for batches of at most qmax queries; and the scratch: w0 the coarse scores and the
+// candidates, `probes` [qmax, nprobe], w4 the code-space queries and the tables.
+struct PqSearch {
+  int nprobe = 0, k = 0, qmax = 0, segs = 0, cpq = 0;
+  int64_t Mq = 0;
+  SelectPlan cp, sel;
+  PqPlan pl;
+  unsigned long long* w0 = nullptr;
+  unsigned long long* probes = nullptr;
+  float* w4 = nullptr;
+};
+// Top-k search of nq queries; a range search plans one query with k = 0 (no candidates, an empty select).
+int pq_search_plan(b200_index* idx, int nq, int k, PqSearch* s);
+// Steps (0)-(2) for queries [0, qb) of d_q: the code-space queries, then when `probes` is set their probes into s.probes,
+// then when `tables` is non-null their tables [qb, pitch, 256] into scratch at *tables.
+int pq_prepare(b200_index* idx, const PqSearch& s, const float* d_q, int qb, bool probes, float** tables, cudaStream_t st);
+// The list scan of qb queries' `probes` [qb, nprobe] over `store` (timed, counted, its plan recorded), then the select of
+// each query's k best into out [qb, k].
+int pq_scan_select(b200_index* idx, const PqSearch& s, const PqStore& store, int qb, const float* tables,
+                   const unsigned long long* probes, unsigned long long* out, cudaStream_t st);
+// The range scan of one query: *counter = 0, then every row above `thresh` appended to out (up to `cap` keys).
+int pq_scan_range(b200_index* idx, const PqSearch& s, const PqStore& store, const float* tables,
+                  const unsigned long long* probes, float thresh, unsigned long long* out, unsigned int cap,
+                  unsigned int* counter, cudaStream_t st);
 int pq_decode_launch(b200_index* idx, const uint8_t* codes, const int64_t* offsets, int nlists, const int32_t* list_ids,
                      const uint32_t* id_to_slot, const unsigned long long* keys, const int64_t* ids, int64_t count,
                      float* d_R, cudaStream_t st);

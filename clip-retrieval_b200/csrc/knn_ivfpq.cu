@@ -24,7 +24,6 @@ namespace b200 {
 constexpr int PQ_KSUB = 256;
 constexpr int PQ_THREADS = 256;                 // list-scan CTA: 8 warps at most, one code row per thread
 constexpr size_t PQ_SMEM_BUDGET = 200 * 1024;   // shared memory one list-scan CTA may take
-constexpr int PQ_QB = 256;                      // queries per batch (bounds the scratch)
 
 static int pq_pitch(int M) { return (M + 15) / 16 * 16; }
 
@@ -231,7 +230,7 @@ __global__ void pq_decode_kernel(const uint8_t* __restrict__ codes, int pitch, i
 // The smallest cluster (1, 2, 4 CTAs) whose share of the table plus candidate lists leaves at least 4 warps of
 // lists in the budget; failing that, the most warps.  Depends on (M, k) alone, so every query batch of a shape
 // sums its rows in the same order.
-PqPlan pq_plan(int pitch, int k) {
+static PqPlan pq_plan(int pitch, int k) {
   PqPlan best;
   for (int cs = 1; cs <= 4; cs <<= 1) {
     const int mc = ((pitch + cs - 1) / cs + 15) / 16 * 16;
@@ -247,13 +246,14 @@ PqPlan pq_plan(int pitch, int k) {
   return best;
 }
 
-int pq_launch_scan(b200_index* idx, const PqStore& store, bool range, const PqPlan& pl, int nq, const float* tables,
-                   const unsigned long long* probes, int nprobe, int segs, int cpq, int k, unsigned long long* out,
-                   int64_t out_stride_q, float thresh, unsigned int cap, unsigned int* counter, cudaStream_t st) {
+static int pq_launch_scan(b200_index* idx, const PqSearch& s, const PqStore& store, bool range, int nq,
+                          const float* tables, const unsigned long long* probes, unsigned long long* out, float thresh,
+                          unsigned int cap, unsigned int* counter, cudaStream_t st) {
+  const PqPlan& pl = s.pl;
   const void* fn = range ? (const void*)ivfpq_scan_kernel<true> : (const void*)ivfpq_scan_kernel<false>;
   if (pl.smem > 48 * 1024) B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)((int64_t)nq * cpq * pl.cs));
+  cfg.gridDim = dim3((unsigned)((int64_t)nq * s.cpq * pl.cs));
   cfg.blockDim = dim3(range ? PQ_THREADS : pl.warps * 32);
   cfg.dynamicSmemBytes = pl.smem;
   cfg.stream = st;
@@ -266,137 +266,107 @@ int pq_launch_scan(b200_index* idx, const PqStore& store, bool range, const PqPl
   cfg.numAttrs = pl.cs > 1 ? 1 : 0;
   const int pitch = idx->row_bytes, by_res = idx->pq_by_residual ? 1 : 0;
   if (range)
-    B200_CUDA(cudaLaunchKernelEx(&cfg, ivfpq_scan_kernel<true>, store.codes, pitch, store.row_ids, tables, probes, nprobe,
-                                 segs, cpq, store.offsets, by_res, pl.mc, pl.cs, k, out, out_stride_q, thresh, cap, counter));
+    B200_CUDA(cudaLaunchKernelEx(&cfg, ivfpq_scan_kernel<true>, store.codes, pitch, store.row_ids, tables, probes, s.nprobe,
+                                 s.segs, s.cpq, store.offsets, by_res, pl.mc, pl.cs, s.k, out, s.Mq, thresh, cap, counter));
   else
-    B200_CUDA(cudaLaunchKernelEx(&cfg, ivfpq_scan_kernel<false>, store.codes, pitch, store.row_ids, tables, probes, nprobe,
-                                 segs, cpq, store.offsets, by_res, pl.mc, pl.cs, k, out, out_stride_q, thresh, cap, counter));
+    B200_CUDA(cudaLaunchKernelEx(&cfg, ivfpq_scan_kernel<false>, store.codes, pitch, store.row_ids, tables, probes, s.nprobe,
+                                 s.segs, s.cpq, store.offsets, by_res, pl.mc, pl.cs, s.k, out, s.Mq, thresh, cap, counter));
   B200_LAUNCH_OK();
   return B200_OK;
 }
 
-// Select plan of the coarse step: k = nprobe over the nlist scores of a query (two select levels, as the list scan).
-int pq_coarse_plan(const b200_index* idx, const char* what, int nprobe, SelectPlan* cp) {
-  B200_CHECK((size_t)select_buffer(nprobe) * 8 <= SELECT_SMEM_MAX, B200_ERR_UNSUPPORTED,
-             "ivfpq %s: nprobe=%d exceeds the supported maximum (12800)", what, nprobe);
-  return plan_select(idx->nlist, nprobe, cp);
+int pq_search_plan(b200_index* idx, int nq, int k, PqSearch* s) {
+  s->nprobe = std::min(idx->nprobe, idx->nlist);
+  s->k = k;
+  // select plan of the coarse step: k = nprobe over the nlist scores of a query (two select levels, as the list scan)
+  B200_CHECK((size_t)select_buffer(s->nprobe) * 8 <= SELECT_SMEM_MAX, B200_ERR_UNSUPPORTED,
+             "ivfpq %s: nprobe=%d exceeds the supported maximum (12800)", k ? "search" : "range_search", s->nprobe);
+  B200_TRY(plan_select(idx->nlist, s->nprobe, &s->cp));
+  s->pl = pq_plan(idx->row_bytes, k);
+  B200_CHECK(s->pl.warps >= 1, B200_ERR_UNSUPPORTED, "search: k=%d exceeds the supported maximum (8192)", k);
+  s->qmax = std::min(PQ_QB, nq);
+  // clusters per query: enough to fill the chip twice; segments of at least ~PQ_THREADS rows
+  const int target = std::max(1, 2 * idx->sms / s->pl.cs);
+  s->segs = list_segments(idx, target, (int64_t)s->qmax * s->nprobe, PQ_THREADS);
+  s->cpq = (int)std::min<int64_t>((int64_t)s->nprobe * s->segs, std::max<int64_t>(1, (target + s->qmax - 1) / s->qmax));
+  s->Mq = (int64_t)s->cpq * s->pl.warps * k;   // candidates per query
+  B200_TRY(plan_select(s->Mq, k, &s->sel));
+  const size_t w4 = ((((size_t)s->qmax * idx->d + 63) & ~(size_t)63) + (size_t)s->qmax * idx->row_bytes * PQ_KSUB) * 4;
+  B200_TRY(index_ws(idx, 0, std::max(s->cp.keys(s->qmax), s->sel.keys(s->qmax)) * 8, (void**)&s->w0));
+  B200_TRY(index_ws(idx, 3, (size_t)s->qmax * s->nprobe * 8, (void**)&s->probes));
+  return index_ws(idx, 4, w4, (void**)&s->w4);
 }
 
-// Step (0) for queries [0, qb) of d_q: the queries in the code space (d_q itself, or A q + b written to `w4`);
-// *tables_out is where the tables of step (2) go in `w4`.
-int pq_query_space(b200_index* idx, const float* d_q, int qb, float* w4, const float** q_out, float** tables_out,
-                   cudaStream_t st) {
-  const int d = idx->d;
-  *q_out = d_q;
-  *tables_out = w4;
-  if (idx->pt_A) {
-    float* qt = w4;
-    *tables_out = w4 + (((size_t)qb * d + 63) & ~(size_t)63);
-    const int64_t warps = (int64_t)qb * d;
-    pq_pretransform_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(d_q, qb, idx->d_in, idx->pt_A, idx->pt_b, d, qt);
-    B200_LAUNCH_OK();
-    *q_out = qt;
-  }
-  return B200_OK;
-}
-
-// Step (1): probes [qb, nprobe] (keys: fp32 coarse score = dis0, list id) of the code-space queries q; `w0` holds the
-// coarse scores.
-int pq_probe_step(b200_index* idx, const float* q, int qb, const SelectPlan& cp, unsigned long long* probes, char* w0,
-                  cudaStream_t st) {
+int pq_prepare(b200_index* idx, const PqSearch& s, const float* d_q, int qb, bool probes, float** tables, cudaStream_t st) {
   const int d = idx->d, nlist = idx->nlist;
-  unsigned long long* ck = (unsigned long long*)w0;
-  pq_coarse_kernel<<<dim3((nlist + CQ_T - 1) / CQ_T, (qb + CQ_T - 1) / CQ_T), 256, 0, st>>>(q, qb, idx->pq_centroids, nlist,
-                                                                                            d, ck);
-  B200_LAUNCH_OK();
-  return select_topk(cp, ck, ck + (size_t)qb * nlist, probes, qb, st);
-}
-
-// Step (2): tables [qb, pitch, 256] of the code-space queries q.
-int pq_table_step(b200_index* idx, const float* q, int qb, float* tables, cudaStream_t st) {
-  const int d = idx->d, M = idx->pq_M;
-  pq_tables_kernel<<<dim3(idx->row_bytes, qb), PQ_KSUB, 0, st>>>(q, d, M, d / M, idx->pq_codebook, tables);
+  const float* q = d_q;
+  float* t = s.w4;
+  if (idx->pt_A) {   // (0) q' = A q + b at the start of w4, the tables after it
+    t = s.w4 + (((size_t)qb * d + 63) & ~(size_t)63);
+    const int64_t warps = (int64_t)qb * d;
+    pq_pretransform_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(d_q, qb, idx->d_in, idx->pt_A, idx->pt_b, d, s.w4);
+    B200_LAUNCH_OK();
+    q = s.w4;
+  }
+  if (probes) {   // (1) probe keys: fp32 coarse score = dis0, list id
+    pq_coarse_kernel<<<dim3((nlist + CQ_T - 1) / CQ_T, (qb + CQ_T - 1) / CQ_T), 256, 0, st>>>(q, qb, idx->pq_centroids,
+                                                                                            nlist, d, s.w0);
+    B200_LAUNCH_OK();
+    B200_TRY(select_topk(s.cp, s.w0, s.w0 + (size_t)qb * nlist, s.probes, qb, st));
+  }
+  if (!tables) return B200_OK;
+  *tables = t;   // (2)
+  pq_tables_kernel<<<dim3(idx->row_bytes, qb), PQ_KSUB, 0, st>>>(q, d, idx->pq_M, d / idx->pq_M, idx->pq_codebook, t);
   B200_LAUNCH_OK();
   return B200_OK;
 }
 
-// Steps (0)-(2) for queries [0, qb) of d_q: probes [qb, nprobe] and tables [qb, pitch, 256].  `w0` holds the coarse
-// scores, `w4` the transformed queries and the tables.
-static int pq_prepare(b200_index* idx, const float* d_q, int qb, const SelectPlan& cp, unsigned long long* probes, char* w0,
-                      float* w4, float** tables_out, cudaStream_t st) {
-  const float* q = nullptr;
-  B200_TRY(pq_query_space(idx, d_q, qb, w4, &q, tables_out, st));
-  B200_TRY(pq_probe_step(idx, q, qb, cp, probes, w0, st));
-  return pq_table_step(idx, q, qb, *tables_out, st);
+int pq_scan_select(b200_index* idx, const PqSearch& s, const PqStore& store, int qb, const float* tables,
+                   const unsigned long long* probes, unsigned long long* out, cudaStream_t st) {
+  B200_TRY(scan_timer_begin(idx, st));
+  B200_TRY(pq_launch_scan(idx, s, store, false, qb, tables, probes, s.w0, 0.f, 0, nullptr, st));
+  B200_TRY(scan_timer_end(idx, st));
+  idx->last_scan_launches++;
+  B200_TRY(select_topk(s.sel, s.w0, s.w0 + (size_t)qb * s.Mq, out, qb, st));
+  idx->last_scan_plan[0] = 4;
+  idx->last_scan_plan[1] = s.pl.mc;
+  idx->last_scan_plan[2] = s.pl.cs;
+  idx->last_scan_plan[3] = s.pl.warps;
+  return B200_OK;
+}
+
+int pq_scan_range(b200_index* idx, const PqSearch& s, const PqStore& store, const float* tables,
+                  const unsigned long long* probes, float thresh, unsigned long long* out, unsigned int cap,
+                  unsigned int* counter, cudaStream_t st) {
+  B200_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned int), st));
+  return pq_launch_scan(idx, s, store, true, 1, tables, probes, out, thresh, cap, counter, st);
 }
 
 static PqStore resident_store(const b200_index* idx) {
   return PqStore{reinterpret_cast<const uint8_t*>(idx->rows), idx->row_ids, idx->list_offsets};
 }
 
-size_t pq_w4_bytes(const b200_index* idx, int qb) {
-  return ((((size_t)qb * idx->d + 63) & ~(size_t)63) + (size_t)qb * idx->row_bytes * PQ_KSUB) * 4;
-}
-
 int ivfpq_search_keys(b200_index* idx, const float* d_q, int nq, int k, unsigned long long* d_keys, cudaStream_t st) {
-  const int nprobe = std::min(idx->nprobe, idx->nlist);
-  SelectPlan cp, sel;
-  B200_TRY(pq_coarse_plan(idx, "search", nprobe, &cp));
-  const PqPlan pl = pq_plan(idx->row_bytes, k);
-  B200_CHECK(pl.warps >= 1, B200_ERR_UNSUPPORTED, "search: k=%d exceeds the supported maximum (8192)", k);
-  const int qmax = std::min(PQ_QB, nq);
-  // clusters per query: enough to fill the chip twice; segments of at least ~PQ_THREADS rows
-  const int target = std::max(1, 2 * idx->sms / pl.cs);
-  const int segs = list_segments(idx, target, (int64_t)qmax * nprobe, PQ_THREADS);
-  const int cpq = (int)std::min<int64_t>((int64_t)nprobe * segs, std::max<int64_t>(1, (target + qmax - 1) / qmax));
-  const int64_t Mq = (int64_t)cpq * pl.warps * k;   // candidates per query
-  B200_TRY(plan_select(Mq, k, &sel));
-  void *w0 = nullptr, *w3 = nullptr, *w4 = nullptr;
-  B200_TRY(index_ws(idx, 0, std::max(cp.keys(qmax), sel.keys(qmax)) * 8, &w0));
-  B200_TRY(index_ws(idx, 3, (size_t)qmax * nprobe * 8, &w3));
-  B200_TRY(index_ws(idx, 4, pq_w4_bytes(idx, qmax), &w4));
-  unsigned long long* probes = (unsigned long long*)w3;
+  PqSearch s;
+  B200_TRY(pq_search_plan(idx, nq, k, &s));
   idx->ev_used = 0;
   for (int q0 = 0; q0 < nq; q0 += PQ_QB) {
     const int qb = std::min(PQ_QB, nq - q0);
     float* tables = nullptr;
-    B200_TRY(pq_prepare(idx, d_q + (size_t)q0 * idx->d_in, qb, cp, probes, (char*)w0, (float*)w4, &tables, st));
-    unsigned long long* k1 = (unsigned long long*)w0;
-    unsigned long long* k2 = k1 + (size_t)qb * Mq;
-    B200_TRY(scan_timer_begin(idx, st));
-    B200_TRY(pq_launch_scan(idx, resident_store(idx), false, pl, qb, tables, probes, nprobe, segs, cpq, k, k1, Mq, 0.f, 0,
-                            nullptr, st));
-    B200_TRY(scan_timer_end(idx, st));
-    idx->last_scan_launches++;
-    B200_TRY(select_topk(sel, k1, k2, d_keys + (size_t)q0 * k, qb, st));
+    B200_TRY(pq_prepare(idx, s, d_q + (size_t)q0 * idx->d_in, qb, true, &tables, st));
+    B200_TRY(pq_scan_select(idx, s, resident_store(idx), qb, tables, s.probes, d_keys + (size_t)q0 * k, st));
   }
-  idx->last_scan_plan[0] = 4;
-  idx->last_scan_plan[1] = pl.mc;
-  idx->last_scan_plan[2] = pl.cs;
-  idx->last_scan_plan[3] = pl.warps;
   return B200_OK;
 }
 
 // One query (device pointer): (score, slot) keys of every row of the probed lists scoring strictly above `thresh`.
 int ivfpq_range_scan(b200_index* idx, const float* d_q, float thresh, unsigned long long* d_out, unsigned int cap,
                      unsigned int* d_count, cudaStream_t st) {
-  const int nprobe = std::min(idx->nprobe, idx->nlist);
-  SelectPlan cp;
-  B200_TRY(pq_coarse_plan(idx, "range_search", nprobe, &cp));
-  const PqPlan pl = pq_plan(idx->row_bytes, 0);
-  void *w0 = nullptr, *w3 = nullptr, *w4 = nullptr;
-  B200_TRY(index_ws(idx, 0, cp.keys(1) * 8, &w0));
-  B200_TRY(index_ws(idx, 3, (size_t)nprobe * 8, &w3));
-  B200_TRY(index_ws(idx, 4, pq_w4_bytes(idx, 1), &w4));
-  unsigned long long* probes = (unsigned long long*)w3;
+  PqSearch s;
+  B200_TRY(pq_search_plan(idx, 1, 0, &s));
   float* tables = nullptr;
-  B200_TRY(pq_prepare(idx, d_q, 1, cp, probes, (char*)w0, (float*)w4, &tables, st));
-  B200_CUDA(cudaMemsetAsync(d_count, 0, sizeof(unsigned int), st));
-  const int target = std::max(1, 2 * idx->sms / pl.cs);
-  const int segs = list_segments(idx, target, nprobe, PQ_THREADS);
-  const int cpq = std::min(nprobe * segs, target);
-  return pq_launch_scan(idx, resident_store(idx), true, pl, 1, tables, probes, nprobe, segs, cpq, 0, d_out, 0, thresh, cap,
-                        d_count, st);
+  B200_TRY(pq_prepare(idx, s, d_q, 1, true, &tables, st));
+  return pq_scan_range(idx, s, resident_store(idx), tables, s.probes, thresh, d_out, cap, d_count, st);
 }
 
 int ivfpq_decode(b200_index* idx, const unsigned long long* keys, const int64_t* ids, int64_t count, float* d_R,

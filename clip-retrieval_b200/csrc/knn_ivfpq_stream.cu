@@ -1,7 +1,7 @@
 // IVF-PQ with its lists in host memory: the on-disk index (`populated.index` + `merged_index.ivfdata`) served from
 // the caller's read-only memory map, for collections whose codes do not fit in HBM.  Centroids, codebook and
 // pre-transform stay on the device as for a resident index (knn_ivfpq.cu); the lists do not.  A search:
-//   A. coarse step of every query on the GPU (pq_probe_step), the probes [nq, nprobe] copied to the host;
+//   A. coarse step of every query on the GPU (pq_prepare), the probes [nq, nprobe] copied to the host;
 //   B. passes: the host takes queries in order while the union of their probed lists fits the arena, numbers those
 //      lists in ascending list id (arena list i), gathers their code rows from the map into pinned staging at the
 //      store's pitch, and rewrites each probe key's list id into its arena list; a copy stream moves staging, arena
@@ -22,7 +22,6 @@
 
 namespace b200 {
 
-constexpr int STREAM_QB = 256;                      // queries per pass at most (the tables scratch of a pass)
 constexpr size_t STREAM_ARENA_DEFAULT = 256u << 20;  // bytes per arena unless b200_index_set_stream_arena says otherwise
 
 struct StreamBuf {
@@ -32,9 +31,9 @@ struct StreamBuf {
   int64_t* d_off = nullptr;
   int32_t* h_lid = nullptr;                   // pinned [nlist]: arena list -> list id
   int32_t* d_lid = nullptr;
-  unsigned long long* h_probes = nullptr;     // pinned [STREAM_QB, nprobe]: probe keys naming arena lists
+  unsigned long long* h_probes = nullptr;     // pinned [PQ_QB, nprobe]: probe keys naming arena lists
   unsigned long long* d_probes = nullptr;
-  unsigned long long* h_keys = nullptr;       // pinned [STREAM_QB, k]: the pass's selected keys
+  unsigned long long* h_keys = nullptr;       // pinned [PQ_QB, k]: the pass's selected keys
   cudaEvent_t copy_beg = nullptr, copy_end = nullptr, done = nullptr;
   int q0 = 0, qb = 0, nl = 0;                 // the pass it holds
   bool pending = false;
@@ -91,13 +90,24 @@ void host_lists_free(b200_index* idx) {
   idx->host = nullptr;
 }
 
+// Frees the device (or pinned) buffer *p and clears the pointer, then allocates `bytes` of it unless 0: a failed call
+// leaves null, never a freed address.
+template <typename T>
+static int regrow(T** p, size_t bytes, bool pinned) {
+  const cudaError_t e = *p ? (pinned ? cudaFreeHost(*p) : cudaFree(*p)) : cudaSuccess;
+  *p = nullptr;
+  B200_CUDA(e);
+  if (bytes) B200_CUDA(pinned ? cudaHostAlloc((void**)p, bytes, cudaHostAllocDefault) : cudaMalloc((void**)p, bytes));
+  return B200_OK;
+}
+
 // Arenas of max(arena_bytes / pitch, nprobe x the largest list) rows, so that one query always fits; probe and key
-// staging for a pass of STREAM_QB queries.
+// staging for a pass of PQ_QB queries.
 static int ensure_bufs(b200_index* idx, int nprobe, int k) {
   HostLists* H = idx->host;
   const int64_t pitch = idx->row_bytes;
   const int64_t rows = std::max<int64_t>({(int64_t)(H->arena_bytes / (size_t)pitch), (int64_t)nprobe * idx->max_list, 1});
-  const size_t pcap = (size_t)STREAM_QB * nprobe, kcap = (size_t)STREAM_QB * k;
+  const size_t pcap = (size_t)PQ_QB * nprobe, kcap = (size_t)PQ_QB * k;
   if (!H->copy_st) B200_CUDA(cudaStreamCreateWithFlags(&H->copy_st, cudaStreamNonBlocking));
   for (StreamBuf& b : H->buf) {
     if (!b.done) {
@@ -110,24 +120,15 @@ static int ensure_bufs(b200_index* idx, int nprobe, int k) {
       B200_CUDA(cudaMalloc((void**)&b.d_lid, (size_t)idx->nlist * 4));
     }
     if (rows > H->arena_rows) {
-      if (b.d_arena) B200_CUDA(cudaFree(b.d_arena));
-      if (b.h_stage) B200_CUDA(cudaFreeHost(b.h_stage));
-      b.d_arena = nullptr;
-      b.h_stage = nullptr;
-      B200_CUDA(cudaMalloc((void**)&b.d_arena, (size_t)rows * pitch));
-      B200_CUDA(cudaHostAlloc((void**)&b.h_stage, (size_t)rows * pitch, cudaHostAllocDefault));
+      B200_TRY(regrow(&b.d_arena, (size_t)rows * pitch, false));
+      B200_TRY(regrow(&b.h_stage, (size_t)rows * pitch, true));
       memset(b.h_stage, 0, (size_t)rows * pitch);
     }
     if (pcap > H->probe_cap) {
-      if (b.h_probes) B200_CUDA(cudaFreeHost(b.h_probes));
-      if (b.d_probes) B200_CUDA(cudaFree(b.d_probes));
-      B200_CUDA(cudaHostAlloc((void**)&b.h_probes, pcap * 8, cudaHostAllocDefault));
-      B200_CUDA(cudaMalloc((void**)&b.d_probes, pcap * 8));
+      B200_TRY(regrow(&b.h_probes, pcap * 8, true));
+      B200_TRY(regrow(&b.d_probes, pcap * 8, false));
     }
-    if (kcap > H->key_cap) {
-      if (b.h_keys) B200_CUDA(cudaFreeHost(b.h_keys));
-      B200_CUDA(cudaHostAlloc((void**)&b.h_keys, kcap * 8, cudaHostAllocDefault));
-    }
+    if (kcap > H->key_cap) B200_TRY(regrow(&b.h_keys, kcap * 8, true));
   }
   H->arena_rows = std::max(H->arena_rows, rows);
   H->probe_cap = std::max(H->probe_cap, pcap);
@@ -135,7 +136,7 @@ static int ensure_bufs(b200_index* idx, int nprobe, int k) {
   return B200_OK;
 }
 
-// Queries [a, *b) whose probed lists together fit the arena (at least query a; at most STREAM_QB): their lists in
+// Queries [a, *b) whose probed lists together fit the arena (at least query a; at most PQ_QB): their lists in
 // ascending id become the arena lists of `B` (offsets, list ids), and their probe keys name arena lists.
 static int plan_pass(b200_index* idx, StreamBuf& B, int nprobe, int a, int nq, int* b, int64_t* rows_out) {
   HostLists* H = idx->host;
@@ -143,7 +144,7 @@ static int plan_pass(b200_index* idx, StreamBuf& B, int nprobe, int a, int nq, i
   L.clear();
   int64_t rows = 0;
   int q = a;
-  for (; q < nq && q - a < STREAM_QB; q++) {
+  for (; q < nq && q - a < PQ_QB; q++) {
     const size_t mark0 = L.size();
     int64_t add = 0;
     for (int p = 0; p < nprobe; p++) {
@@ -224,6 +225,12 @@ static void gather(b200_index* idx, StreamBuf& B, int64_t rows) {
   for (auto& x : th) x.join();
 }
 
+// Arena row r of B -> (the index's list, position in that list).
+static std::pair<int32_t, int64_t> arena_row(const StreamBuf& B, int64_t r) {
+  const int a = (int)(std::upper_bound(B.h_off, B.h_off + B.nl + 1, r) - B.h_off) - 1;
+  return {B.h_lid[a], r - B.h_off[a]};
+}
+
 // Keys of a finished pass -> D and the lists' own ids (+ id_base).
 static int finish_pass(b200_index* idx, StreamBuf& B, int k) {
   HostLists* H = idx->host;
@@ -231,7 +238,6 @@ static int finish_pass(b200_index* idx, StreamBuf& B, int k) {
   float ms = 0.f;
   B200_CUDA(cudaEventElapsedTime(&ms, B.copy_beg, B.copy_end));
   H->copy_ms += ms;
-  const int64_t* off = B.h_off;
   for (int64_t i = 0; i < (int64_t)B.qb * k; i++) {
     const unsigned long long key = B.h_keys[i];
     const int64_t o = (int64_t)B.q0 * k + i;
@@ -240,10 +246,9 @@ static int finish_pass(b200_index* idx, StreamBuf& B, int k) {
       H->out_I[o] = -1;
       continue;
     }
-    const int64_t r = host_key_id(key);
-    const int a = (int)(std::upper_bound(off, off + B.nl + 1, r) - off) - 1;
+    const auto [l, pos] = arena_row(B, host_key_id(key));
     H->out_D[o] = host_key_score(key);
-    H->out_I[o] = idx->id_base + H->ids[B.h_lid[a]][r - off[a]];
+    H->out_I[o] = idx->id_base + H->ids[l][pos];
   }
   B.pending = false;
   return B200_OK;
@@ -269,17 +274,13 @@ static int stage_pass(b200_index* idx, StreamBuf& B, int64_t rows, int nprobe, c
 }
 
 // Step A: probes of queries [0, nq) into H->probes.
-static int all_probes(b200_index* idx, const float* d_q, int nq, int nprobe, const SelectPlan& cp, char* w0,
-                      unsigned long long* w3, float* w4, cudaStream_t st) {
+static int all_probes(b200_index* idx, const PqSearch& s, const float* d_q, int nq, cudaStream_t st) {
   HostLists* H = idx->host;
-  H->probes.resize((size_t)nq * nprobe);
-  for (int b0 = 0; b0 < nq; b0 += STREAM_QB) {
-    const int bq = std::min(STREAM_QB, nq - b0);
-    const float* q = nullptr;
-    float* tables = nullptr;
-    B200_TRY(pq_query_space(idx, d_q + (size_t)b0 * idx->d_in, bq, w4, &q, &tables, st));
-    B200_TRY(pq_probe_step(idx, q, bq, cp, w3, w0, st));
-    B200_CUDA(cudaMemcpyAsync(H->probes.data() + (size_t)b0 * nprobe, w3, (size_t)bq * nprobe * 8,
+  H->probes.resize((size_t)nq * s.nprobe);
+  for (int b0 = 0; b0 < nq; b0 += PQ_QB) {
+    const int bq = std::min(PQ_QB, nq - b0);
+    B200_TRY(pq_prepare(idx, s, d_q + (size_t)b0 * idx->d_in, bq, true, nullptr, st));
+    B200_CUDA(cudaMemcpyAsync(H->probes.data() + (size_t)b0 * s.nprobe, s.probes, (size_t)bq * s.nprobe * 8,
                               cudaMemcpyDeviceToHost, st));
     B200_CUDA(cudaStreamSynchronize(st));
   }
@@ -295,49 +296,26 @@ static void reset_stats(HostLists* H) {
 int ivfpq_stream_search(b200_index* idx, const float* d_q, int nq, int k, unsigned long long* d_keys, float* d_D,
                         int64_t* d_I, float* d_R, cudaStream_t st) {
   HostLists* H = idx->host;
-  const int nprobe = std::min(idx->nprobe, idx->nlist);
-  SelectPlan cp, sel;
-  B200_TRY(pq_coarse_plan(idx, "search", nprobe, &cp));
-  const PqPlan pl = pq_plan(idx->row_bytes, k);
-  B200_CHECK(pl.warps >= 1, B200_ERR_UNSUPPORTED, "search: k=%d exceeds the supported maximum (8192)", k);
-  B200_TRY(ensure_bufs(idx, nprobe, k));
-  const int qmax = std::min(STREAM_QB, nq);
-  // the resident search's launch shape (knn_ivfpq.cu): it changes how work is split, never a result
-  const int target = std::max(1, 2 * idx->sms / pl.cs);
-  const int segs = list_segments(idx, target, (int64_t)qmax * nprobe, 256);
-  const int cpq = (int)std::min<int64_t>((int64_t)nprobe * segs, std::max<int64_t>(1, (target + qmax - 1) / qmax));
-  const int64_t Mq = (int64_t)cpq * pl.warps * k;
-  B200_TRY(plan_select(Mq, k, &sel));
-  void *w0 = nullptr, *w3 = nullptr, *w4 = nullptr;
-  B200_TRY(index_ws(idx, 0, std::max(cp.keys(qmax), sel.keys(qmax)) * 8, &w0));
-  B200_TRY(index_ws(idx, 3, (size_t)qmax * nprobe * 8, &w3));
-  B200_TRY(index_ws(idx, 4, pq_w4_bytes(idx, qmax), &w4));
+  PqSearch s;
+  B200_TRY(pq_search_plan(idx, nq, k, &s));
+  B200_TRY(ensure_bufs(idx, s.nprobe, k));
   reset_stats(H);
   H->out_D.resize((size_t)nq * k);
   H->out_I.resize((size_t)nq * k);
-  B200_TRY(all_probes(idx, d_q, nq, nprobe, cp, (char*)w0, (unsigned long long*)w3, (float*)w4, st));
+  B200_TRY(all_probes(idx, s, d_q, nq, st));
   int p = 0;
   for (int a = 0; a < nq; p++) {
     StreamBuf& B = H->buf[p & 1];
     if (B.pending) B200_TRY(finish_pass(idx, B, k));   // pass p - 2: its arena and staging are free again
     int b = a;
     int64_t rows = 0;
-    B200_TRY(plan_pass(idx, B, nprobe, a, nq, &b, &rows));
-    B200_TRY(stage_pass(idx, B, rows, nprobe, H->copy_st));
-    const float* q = nullptr;
+    B200_TRY(plan_pass(idx, B, s.nprobe, a, nq, &b, &rows));
+    B200_TRY(stage_pass(idx, B, rows, s.nprobe, H->copy_st));
     float* tables = nullptr;
-    B200_TRY(pq_query_space(idx, d_q + (size_t)a * idx->d_in, B.qb, (float*)w4, &q, &tables, st));
-    B200_TRY(pq_table_step(idx, q, B.qb, tables, st));
+    B200_TRY(pq_prepare(idx, s, d_q + (size_t)a * idx->d_in, B.qb, false, &tables, st));
     B200_CUDA(cudaStreamWaitEvent(st, B.copy_end, 0));
-    unsigned long long* k1 = (unsigned long long*)w0;
-    unsigned long long* k2 = k1 + (size_t)B.qb * Mq;
-    B200_TRY(scan_timer_begin(idx, st));
-    B200_TRY(pq_launch_scan(idx, PqStore{B.d_arena, nullptr, B.d_off}, false, pl, B.qb, tables, B.d_probes, nprobe, segs,
-                            cpq, k, k1, Mq, 0.f, 0, nullptr, st));
-    B200_TRY(scan_timer_end(idx, st));
-    idx->last_scan_launches++;
     unsigned long long* keys = d_keys + (size_t)a * k;
-    B200_TRY(select_topk(sel, k1, k2, keys, B.qb, st));
+    B200_TRY(pq_scan_select(idx, s, PqStore{B.d_arena, nullptr, B.d_off}, B.qb, tables, B.d_probes, keys, st));
     if (d_R)
       B200_TRY(pq_decode_launch(idx, B.d_arena, B.d_off, B.nl, B.d_lid, nullptr, keys, nullptr, (int64_t)B.qb * k,
                                 d_R + (size_t)a * k * idx->d_in, st));
@@ -353,42 +331,26 @@ int ivfpq_stream_search(b200_index* idx, const float* d_q, int nq, int k, unsign
   B200_CUDA(cudaMemcpyAsync(d_D, H->out_D.data(), (size_t)nq * k * 4, cudaMemcpyHostToDevice, st));
   B200_CUDA(cudaMemcpyAsync(d_I, H->out_I.data(), (size_t)nq * k * 8, cudaMemcpyHostToDevice, st));
   B200_CUDA(cudaStreamSynchronize(st));
-  idx->last_scan_plan[0] = 4;
-  idx->last_scan_plan[1] = pl.mc;
-  idx->last_scan_plan[2] = pl.cs;
-  idx->last_scan_plan[3] = pl.warps;
   return B200_OK;
 }
 
 int ivfpq_stream_range(b200_index* idx, const float* d_q, float thresh, unsigned long long* d_keys, int64_t cap,
                        unsigned int* d_count, float* h_D, int64_t* h_I, int64_t* h_count, cudaStream_t st) {
   HostLists* H = idx->host;
-  const int nprobe = std::min(idx->nprobe, idx->nlist);
-  SelectPlan cp;
-  B200_TRY(pq_coarse_plan(idx, "range_search", nprobe, &cp));
-  const PqPlan pl = pq_plan(idx->row_bytes, 0);
-  B200_TRY(ensure_bufs(idx, nprobe, 1));
-  void *w0 = nullptr, *w3 = nullptr, *w4 = nullptr;
-  B200_TRY(index_ws(idx, 0, cp.keys(1) * 8, &w0));
-  B200_TRY(index_ws(idx, 3, (size_t)nprobe * 8, &w3));
-  B200_TRY(index_ws(idx, 4, pq_w4_bytes(idx, 1), &w4));
+  PqSearch s;
+  B200_TRY(pq_search_plan(idx, 1, 0, &s));
+  B200_TRY(ensure_bufs(idx, s.nprobe, 1));
   reset_stats(H);
-  B200_TRY(all_probes(idx, d_q, 1, nprobe, cp, (char*)w0, (unsigned long long*)w3, (float*)w4, st));
+  B200_TRY(all_probes(idx, s, d_q, 1, st));
   StreamBuf& B = H->buf[0];
   int b = 0;
   int64_t rows = 0;
-  B200_TRY(plan_pass(idx, B, nprobe, 0, 1, &b, &rows));
-  B200_TRY(stage_pass(idx, B, rows, nprobe, st));
-  const float* q = nullptr;
+  B200_TRY(plan_pass(idx, B, s.nprobe, 0, 1, &b, &rows));
+  B200_TRY(stage_pass(idx, B, rows, s.nprobe, st));
   float* tables = nullptr;
-  B200_TRY(pq_query_space(idx, d_q, 1, (float*)w4, &q, &tables, st));
-  B200_TRY(pq_table_step(idx, q, 1, tables, st));
-  B200_CUDA(cudaMemsetAsync(d_count, 0, sizeof(unsigned int), st));
-  const int target = std::max(1, 2 * idx->sms / pl.cs);
-  const int segs = list_segments(idx, target, nprobe, 256);
-  const int cpq = std::min(nprobe * segs, target);
-  B200_TRY(pq_launch_scan(idx, PqStore{B.d_arena, nullptr, B.d_off}, true, pl, 1, tables, B.d_probes, nprobe, segs, cpq,
-                          0, d_keys, 0, thresh, (unsigned int)cap, d_count, st));
+  B200_TRY(pq_prepare(idx, s, d_q, 1, false, &tables, st));
+  B200_TRY(pq_scan_range(idx, s, PqStore{B.d_arena, nullptr, B.d_off}, tables, B.d_probes, thresh, d_keys,
+                         (unsigned int)cap, d_count, st));
   unsigned int cnt = 0;
   B200_CUDA(cudaMemcpyAsync(&cnt, d_count, 4, cudaMemcpyDeviceToHost, st));
   B200_CUDA(cudaStreamSynchronize(st));
@@ -404,10 +366,7 @@ int ivfpq_stream_range(b200_index* idx, const float* d_q, float thresh, unsigned
   struct Hit { int64_t slot; float D; int64_t I; };
   std::vector<Hit> hits((size_t)m);
   for (int64_t i = 0; i < m; i++) {
-    const int64_t r = host_key_id(keys[i]);
-    const int a = (int)(std::upper_bound(B.h_off, B.h_off + B.nl + 1, r) - B.h_off) - 1;
-    const int32_t l = B.h_lid[a];
-    const int64_t pos = r - B.h_off[a];
+    const auto [l, pos] = arena_row(B, host_key_id(keys[i]));
     hits[i] = Hit{H->starts[l] + pos, host_key_score(keys[i]), idx->id_base + H->ids[l][pos]};
   }
   std::sort(hits.begin(), hits.end(), [](const Hit& x, const Hit& y) { return x.slot < y.slot; });
@@ -476,13 +435,11 @@ int b200_index_set_stream_arena(b200_index* idx, size_t bytes) {
   DeviceGuard g(idx->device);
   idx->host->arena_bytes = bytes;
   // shrink: drop the arenas, the next search allocates what it needs
-  for (StreamBuf& b : idx->host->buf) {
-    if (b.d_arena) B200_CUDA(cudaFree(b.d_arena));
-    if (b.h_stage) B200_CUDA(cudaFreeHost(b.h_stage));
-    b.d_arena = nullptr;
-    b.h_stage = nullptr;
-  }
   idx->host->arena_rows = 0;
+  for (StreamBuf& b : idx->host->buf) {
+    B200_TRY(regrow(&b.d_arena, 0, false));
+    B200_TRY(regrow(&b.h_stage, 0, true));
+  }
   return B200_OK;
 }
 

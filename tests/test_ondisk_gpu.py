@@ -83,6 +83,8 @@ def test_streamed_equals_resident(tmp_path, d, M, by_residual):
         for nq in (1, 7):
             D, I = _same(res, st, Q[:nq], k, nprobe, ranges=(k == 40))
             assert (I[I >= 0] >= (5 << 32)).all()
+            plan = _inner(res).last_scan_plan()   # both residencies launch the same list scan
+            assert plan[0] == 4 and _inner(st).last_scan_plan() == plan, (plan, _inner(st).last_scan_plan())
     _same(res, st, Q, 40, 7, device=False, ranges=False)         # 300 queries: beyond one pass
     # an arena of the least size: passes alternate between the two arenas
     _inner(st).set_stream_arena(0)
