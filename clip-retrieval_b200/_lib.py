@@ -174,6 +174,7 @@ PROTOTYPES = {
     "b200_dedup_device": (_i, [_vp, _i, _i, C.c_float, _vp, _vp, _vp, C.c_size_t, _i, _vp]),
     "b200_prompt_argmax_device": (_i, [_vp, _i, _i, _vp, _i, _i, _vp, _i, _vp]),
     "b200_preproc_create": (_i, [_i, C.POINTER(C.c_float), C.POINTER(C.c_float), _i, C.POINTER(_vp)]),
+    "b200_preproc_create_mode": (_i, [_i, C.POINTER(C.c_float), C.POINTER(C.c_float), _i, _i, C.POINTER(_vp)]),
     "b200_preproc_destroy": (_i, [_vp]),
     "b200_preproc_run": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp]),
     "b200_jpeg_create": (_i, [_i, C.POINTER(_vp)]),

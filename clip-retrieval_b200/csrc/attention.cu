@@ -5,7 +5,9 @@
 // First version on mma.sync.m16n8k16 (bf16 in, fp32 accumulate); 4% of the forward's flops.
 // Per-sample key lengths (len[b] in 1..T) as in attention_wgmma.cu: keys >= len[b] are staged as zeros and masked,
 // the key loop stops at the 32-key block holding len[b] - 1, and rows >= len[b] are written as zeros.
+// Shapes whose whole-head K + V would pass 200 KB run on attention_stream_kernel below, with the same per-block step.
 #include "embed_kernels.cuh"
+#include "ptx.cuh"
 
 namespace b200 {
 
@@ -32,6 +34,128 @@ __device__ __forceinline__ uint32_t pack2(float lo, float hi) {
 }
 
 constexpr int ATT_KB = 32;  // keys per inner block
+
+// Q fragments of rows r0 / r1 straight from global (rows >= T read as zeros):
+// a[ks] = {Q[r0][k0..], Q[r1][k0..], Q[r0][k0+8..], Q[r1][k0+8..]}
+template <int HD>
+__device__ __forceinline__ void load_q_frags(const __nv_bfloat16* base, size_t ld, int r0, int r1, int T, int lane,
+                                             uint32_t (&qa)[HD / 16][4]) {
+#pragma unroll
+  for (int ks = 0; ks < HD / 16; ks++) {
+    const int k0 = ks * 16 + (lane & 3) * 2;
+    qa[ks][0] = r0 < T ? *reinterpret_cast<const uint32_t*>(base + (size_t)r0 * ld + k0) : 0u;
+    qa[ks][1] = r1 < T ? *reinterpret_cast<const uint32_t*>(base + (size_t)r1 * ld + k0) : 0u;
+    qa[ks][2] = r0 < T ? *reinterpret_cast<const uint32_t*>(base + (size_t)r0 * ld + k0 + 8) : 0u;
+    qa[ks][3] = r1 < T ? *reinterpret_cast<const uint32_t*>(base + (size_t)r1 * ld + k0 + 8) : 0u;
+  }
+}
+
+// o / l of rows r0 / r1 into ob (the head's column block of the sample's output rows): rows >= L as zeros, rows >= T
+// not written.
+template <int HD>
+__device__ __forceinline__ void store_rows(__nv_bfloat16* ob, int w, int r0, int r1, int T, int L,
+                                           const float (&o)[HD / 8][4], float l0, float l1, int lane) {
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  const float i0 = 1.0f / l0, i1 = 1.0f / l1;
+#pragma unroll
+  for (int i = 0; i < HD / 8; i++) {
+    const int col = i * 8 + (lane & 3) * 2;
+    if (r0 < T) *reinterpret_cast<uint32_t*>(ob + (size_t)r0 * w + col) = r0 < L ? pack2(o[i][0] * i0, o[i][1] * i0) : 0u;
+    if (r1 < T) *reinterpret_cast<uint32_t*>(ob + (size_t)r1 * w + col) = r1 < L ? pack2(o[i][2] * i1, o[i][3] * i1) : 0u;
+  }
+}
+
+// One 32-key block kb of a warp's 16 query rows (r0 = its row of lane / 4, r1 = r0 + 8): S = Q K^T on mma.sync, the
+// mask (keys >= L, and keys > row when causal), the fp32 online softmax update of (m, l, o), then O += P V with P in
+// bf16.  sK_u / sV_u address key kb at sK_u + kb * LDS * 2: both kernels call this, the whole-K/V kernel with its
+// buffer's base, the streaming kernel with a ring stage's base shifted back by the stage's first key.
+template <int HD>
+__device__ __forceinline__ void attention_block_step(uint32_t sK_u, uint32_t sV_u, int kb, const uint32_t (&qa)[HD / 16][4],
+                                                     float (&o)[HD / 8][4], float& m0, float& m1, float& l0, float& l1,
+                                                     int r0, int r1, int L, int causal, float scale_log2e, int lane) {
+  constexpr int LDS = HD + 8;
+  float s[ATT_KB / 8][4];
+#pragma unroll
+  for (int nt = 0; nt < ATT_KB / 8; nt++) {
+    s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
+#pragma unroll
+    for (int kp = 0; kp < HD / 32; kp++) {
+      // four 8x8 blocks of K: keys kb+nt*8.., d = kp*32 + {0,8,16,24}
+      uint32_t b0, b1, b2, b3;
+      const uint32_t addr = sK_u + (uint32_t)(((kb + nt * 8 + (lane & 7)) * LDS + kp * 32 + (lane >> 3) * 8) * 2);
+      ldmatrix_x4(b0, b1, b2, b3, addr);
+      mma_bf16_16816(s[nt], qa[kp * 2], b0, b1);
+      mma_bf16_16816(s[nt], qa[kp * 2 + 1], b2, b3);
+    }
+    if constexpr (HD % 32 != 0) {
+      // tail k-step (HD = 80): d = HD-16 .. HD-1; only matrices 0,1 are meaningful
+      uint32_t b0, b1, b2, b3;
+      const int dcol = (HD / 32) * 32 + ((lane >> 3) & 1) * 8;
+      const uint32_t addr = sK_u + (uint32_t)(((kb + nt * 8 + (lane & 7)) * LDS + dcol) * 2);
+      ldmatrix_x4(b0, b1, b2, b3, addr);
+      mma_bf16_16816(s[nt], qa[HD / 16 - 1], b0, b1);
+    }
+  }
+  // mask + block row max (scores stay unscaled; the scale folds into the exp2 argument)
+  float bm0 = -INFINITY, bm1 = -INFINITY;
+#pragma unroll
+  for (int nt = 0; nt < ATT_KB / 8; nt++) {
+    const int key = kb + nt * 8 + (lane & 3) * 2;
+#pragma unroll
+    for (int e = 0; e < 2; e++) {
+      const int kk = key + e;
+      const bool dead0 = kk >= L || (causal && kk > r0);
+      const bool dead1 = kk >= L || (causal && kk > r1);
+      if (dead0) s[nt][e] = -INFINITY;
+      if (dead1) s[nt][2 + e] = -INFINITY;
+      bm0 = fmaxf(bm0, s[nt][e]);
+      bm1 = fmaxf(bm1, s[nt][2 + e]);
+    }
+  }
+  bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 1));
+  bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 2));
+  bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 1));
+  bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 2));
+  const float mn0 = fmaxf(m0, bm0), mn1 = fmaxf(m1, bm1);
+  // rows that have seen no live key yet keep m = -inf; avoid (-inf) - (-inf)
+  const float ms0 = mn0 == -INFINITY ? 0.f : mn0, ms1 = mn1 == -INFINITY ? 0.f : mn1;
+  const float a0 = exp2f((m0 - ms0) * scale_log2e), a1 = exp2f((m1 - ms1) * scale_log2e);
+  m0 = mn0;
+  m1 = mn1;
+  l0 *= a0;
+  l1 *= a1;
+#pragma unroll
+  for (int i = 0; i < HD / 8; i++) {
+    o[i][0] *= a0; o[i][1] *= a0;
+    o[i][2] *= a1; o[i][3] *= a1;
+  }
+  uint32_t pa[ATT_KB / 16][4];
+#pragma unroll
+  for (int nt = 0; nt < ATT_KB / 8; nt++) {
+    const float p0 = exp2f((s[nt][0] - ms0) * scale_log2e), p1 = exp2f((s[nt][1] - ms0) * scale_log2e);
+    const float p2 = exp2f((s[nt][2] - ms1) * scale_log2e), p3 = exp2f((s[nt][3] - ms1) * scale_log2e);
+    l0 += p0 + p1;
+    l1 += p2 + p3;
+    pa[nt >> 1][(nt & 1) * 2 + 0] = pack2(p0, p1);
+    pa[nt >> 1][(nt & 1) * 2 + 1] = pack2(p2, p3);
+  }
+  // O += P V : V^T fragments through ldmatrix.trans
+#pragma unroll
+  for (int kk = 0; kk < ATT_KB / 16; kk++) {
+#pragma unroll
+    for (int dp = 0; dp < HD / 16; dp++) {
+      uint32_t b0, b1, b2, b3;
+      const int key = kb + kk * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
+      const int dcol = dp * 16 + (lane >> 4) * 8;
+      ldmatrix_x4_trans(b0, b1, b2, b3, sV_u + (uint32_t)((key * LDS + dcol) * 2));
+      mma_bf16_16816(o[dp * 2], pa[kk], b0, b1);
+      mma_bf16_16816(o[dp * 2 + 1], pa[kk], b2, b3);
+    }
+  }
+}
 
 template <int HD>
 __global__ void __launch_bounds__(256)
@@ -70,16 +194,8 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
 
   for (int qb = warp; qb < qblocks; qb += nwarps) {
     const int r0 = qb * 16 + (lane >> 2), r1 = r0 + 8;
-    // Q fragments straight from global: a[ks] = {Q[r0][k0..], Q[r1][k0..], Q[r0][k0+8..], Q[r1][k0+8..]}
     uint32_t qa[HD / 16][4];
-#pragma unroll
-    for (int ks = 0; ks < HD / 16; ks++) {
-      const int k0 = ks * 16 + (lane & 3) * 2;
-      qa[ks][0] = r0 < T ? *reinterpret_cast<const uint32_t*>(base + (size_t)r0 * ld + k0) : 0u;
-      qa[ks][1] = r1 < T ? *reinterpret_cast<const uint32_t*>(base + (size_t)r1 * ld + k0) : 0u;
-      qa[ks][2] = r0 < T ? *reinterpret_cast<const uint32_t*>(base + (size_t)r0 * ld + k0 + 8) : 0u;
-      qa[ks][3] = r1 < T ? *reinterpret_cast<const uint32_t*>(base + (size_t)r1 * ld + k0 + 8) : 0u;
-    }
+    load_q_frags<HD>(base, ld, r0, r1, T, lane, qa);
     float o[HD / 8][4];
 #pragma unroll
     for (int i = 0; i < HD / 8; i++) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
@@ -87,97 +203,9 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
 
     const int kend = causal ? min(Lp, (qb * 16 + 16 + ATT_KB - 1) / ATT_KB * ATT_KB) : Lp;
     for (int kb = 0; kb < kend; kb += ATT_KB) {
-      float s[ATT_KB / 8][4];
-#pragma unroll
-      for (int nt = 0; nt < ATT_KB / 8; nt++) {
-        s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
-#pragma unroll
-        for (int kp = 0; kp < HD / 32; kp++) {
-          // four 8x8 blocks of K: keys kb+nt*8.., d = kp*32 + {0,8,16,24}
-          uint32_t b0, b1, b2, b3;
-          const uint32_t addr = sK_u + (uint32_t)(((kb + nt * 8 + (lane & 7)) * LDS + kp * 32 + (lane >> 3) * 8) * 2);
-          ldmatrix_x4(b0, b1, b2, b3, addr);
-          mma_bf16_16816(s[nt], qa[kp * 2], b0, b1);
-          mma_bf16_16816(s[nt], qa[kp * 2 + 1], b2, b3);
-        }
-        if constexpr (HD % 32 != 0) {
-          // tail k-step (HD = 80): d = HD-16 .. HD-1; only matrices 0,1 are meaningful
-          uint32_t b0, b1, b2, b3;
-          const int dcol = (HD / 32) * 32 + ((lane >> 3) & 1) * 8;
-          const uint32_t addr = sK_u + (uint32_t)(((kb + nt * 8 + (lane & 7)) * LDS + dcol) * 2);
-          ldmatrix_x4(b0, b1, b2, b3, addr);
-          mma_bf16_16816(s[nt], qa[HD / 16 - 1], b0, b1);
-        }
-      }
-      // mask + block row max (scores stay unscaled; the scale folds into the exp2 argument)
-      float bm0 = -INFINITY, bm1 = -INFINITY;
-#pragma unroll
-      for (int nt = 0; nt < ATT_KB / 8; nt++) {
-        const int key = kb + nt * 8 + (lane & 3) * 2;
-#pragma unroll
-        for (int e = 0; e < 2; e++) {
-          const int kk = key + e;
-          const bool dead0 = kk >= L || (causal && kk > r0);
-          const bool dead1 = kk >= L || (causal && kk > r1);
-          if (dead0) s[nt][e] = -INFINITY;
-          if (dead1) s[nt][2 + e] = -INFINITY;
-          bm0 = fmaxf(bm0, s[nt][e]);
-          bm1 = fmaxf(bm1, s[nt][2 + e]);
-        }
-      }
-      bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 1));
-      bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 2));
-      bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 1));
-      bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 2));
-      const float mn0 = fmaxf(m0, bm0), mn1 = fmaxf(m1, bm1);
-      // rows that have seen no live key yet keep m = -inf; avoid (-inf) - (-inf)
-      const float ms0 = mn0 == -INFINITY ? 0.f : mn0, ms1 = mn1 == -INFINITY ? 0.f : mn1;
-      const float a0 = exp2f((m0 - ms0) * scale_log2e), a1 = exp2f((m1 - ms1) * scale_log2e);
-      m0 = mn0;
-      m1 = mn1;
-      l0 *= a0;
-      l1 *= a1;
-#pragma unroll
-      for (int i = 0; i < HD / 8; i++) {
-        o[i][0] *= a0; o[i][1] *= a0;
-        o[i][2] *= a1; o[i][3] *= a1;
-      }
-      uint32_t pa[ATT_KB / 16][4];
-#pragma unroll
-      for (int nt = 0; nt < ATT_KB / 8; nt++) {
-        const float p0 = exp2f((s[nt][0] - ms0) * scale_log2e), p1 = exp2f((s[nt][1] - ms0) * scale_log2e);
-        const float p2 = exp2f((s[nt][2] - ms1) * scale_log2e), p3 = exp2f((s[nt][3] - ms1) * scale_log2e);
-        l0 += p0 + p1;
-        l1 += p2 + p3;
-        pa[nt >> 1][(nt & 1) * 2 + 0] = pack2(p0, p1);
-        pa[nt >> 1][(nt & 1) * 2 + 1] = pack2(p2, p3);
-      }
-      // O += P V : V^T fragments through ldmatrix.trans
-#pragma unroll
-      for (int kk = 0; kk < ATT_KB / 16; kk++) {
-#pragma unroll
-        for (int dp = 0; dp < HD / 16; dp++) {
-          uint32_t b0, b1, b2, b3;
-          const int key = kb + kk * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
-          const int dcol = dp * 16 + (lane >> 4) * 8;
-          ldmatrix_x4_trans(b0, b1, b2, b3, sV_u + (uint32_t)((key * LDS + dcol) * 2));
-          mma_bf16_16816(o[dp * 2], pa[kk], b0, b1);
-          mma_bf16_16816(o[dp * 2 + 1], pa[kk], b2, b3);
-        }
-      }
+      attention_block_step<HD>(sK_u, sV_u, kb, qa, o, m0, m1, l0, l1, r0, r1, L, causal, scale_log2e, lane);
     }
-    l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
-    l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
-    l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
-    l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-    const float i0 = 1.0f / l0, i1 = 1.0f / l1;
-    __nv_bfloat16* ob = out + (size_t)b * T * w + (size_t)h * HD;
-#pragma unroll
-    for (int i = 0; i < HD / 8; i++) {
-      const int col = i * 8 + (lane & 3) * 2;
-      if (r0 < T) *reinterpret_cast<uint32_t*>(ob + (size_t)r0 * w + col) = r0 < L ? pack2(o[i][0] * i0, o[i][1] * i0) : 0u;
-      if (r1 < T) *reinterpret_cast<uint32_t*>(ob + (size_t)r1 * w + col) = r1 < L ? pack2(o[i][2] * i1, o[i][3] * i1) : 0u;
-    }
+    store_rows<HD>(out + (size_t)b * T * w + (size_t)h * HD, w, r0, r1, T, L, o, l0, l1, lane);
   }
   // rows of the 16-row query blocks past the sample's keys (none without lengths)
   __nv_bfloat16* ob = out + (size_t)b * T * w + (size_t)h * HD;
@@ -185,12 +213,141 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
     *reinterpret_cast<uint4*>(ob + (size_t)(i / CPR) * w + (i % CPR) * 8) = make_uint4(0u, 0u, 0u, 0u);
 }
 
+// Longer sequences (whole-head K + V past 200 KB of shared memory: T > 704 / 576 / 480 / 352 at head dim 64 / 80 /
+// 96 / 128): one CTA per (128-row query chunk, head, sample), chunk fastest so that the chunks of a head read its K/V
+// from L2.  Eight warps own 16 query rows each; K and V pass through a ring of ATS_STAGES blocks of 64 keys, filled
+// by warp 0 with one bulk copy per row (rows padded to HD + 8 elements as above) and handed over by full / empty
+// mbarriers, so shared memory no longer grows with T.  The arithmetic per 32-key block is attention_block_step.
+// A chunk loads keys < len[b] only, and with causal only keys up to its last row; a chunk wholly at or past len[b]
+// writes zeros and loads nothing.
+constexpr int ATS_ROWS = 128;    // query rows per CTA (8 warps x 16)
+constexpr int ATS_KEYS = 64;     // keys per ring stage
+constexpr int ATS_STAGES = 3;
+
+template <int HD>
+constexpr size_t attention_stream_smem() {
+  return (size_t)ATS_STAGES * 2 * ATS_KEYS * (HD + 8) * sizeof(__nv_bfloat16) + 2 * ATS_STAGES * sizeof(uint64_t);
+}
+
+template <int HD>
+__global__ void __launch_bounds__(256, HD <= 96 ? 2 : 1)
+attention_stream_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ out, int T, int w,
+                        float scale_log2e, int causal, const int* __restrict__ len) {
+  constexpr int LDS = HD + 8;
+  constexpr int CPR = HD / 8;                                    // 16-byte chunks per row
+  constexpr uint32_t MAT = ATS_KEYS * LDS * sizeof(__nv_bfloat16);   // one stage's K (or V) block, bytes
+  constexpr uint32_t STAGE = 2 * MAT;
+  extern __shared__ __align__(16) unsigned char att_smem[];
+  uint64_t* full = reinterpret_cast<uint64_t*>(att_smem + ATS_STAGES * STAGE);
+  uint64_t* empty = full + ATS_STAGES;
+
+  const int chunk = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int L = len != nullptr ? min(max(len[b], 1), T) : T;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const size_t ld = (size_t)3 * w;
+  const __nv_bfloat16* base = qkv + (size_t)b * T * ld + (size_t)h * HD;
+  __nv_bfloat16* ob = out + (size_t)b * T * w + (size_t)h * HD;
+  const int row0 = chunk * ATS_ROWS;
+  if (row0 >= L) {
+    for (int i = threadIdx.x; i < min(ATS_ROWS, T - row0) * CPR; i += blockDim.x)
+      *reinterpret_cast<uint4*>(ob + (size_t)(row0 + i / CPR) * w + (i % CPR) * 8) = make_uint4(0u, 0u, 0u, 0u);
+    return;
+  }
+  const int nkeys = causal ? min(L, row0 + ATS_ROWS) : L;       // keys this chunk reads: rows < nkeys of the sample
+  const int nblk = (nkeys + ATS_KEYS - 1) / ATS_KEYS;
+  const int nlive = min(ATS_ROWS / 16, (L - row0 + 15) / 16);   // warps with a row < L; they alone take part
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < ATS_STAGES; s++) {
+      ptx::mbar_init(&full[s], 1);
+      ptx::mbar_init(&empty[s], nlive);
+    }
+    ptx::fence_barrier_init();
+  }
+  // The last block's rows >= nkeys are never loaded but are read by its 32-key steps (masked: P = 0).  Zero them in
+  // the stage it lands in, so that P . V never meets uninitialised shared memory; an earlier block of the same stage
+  // leaves finite K/V rows there instead.
+  {
+    const int rem = nkeys - (nblk - 1) * ATS_KEYS;
+    unsigned char* st = att_smem + ((nblk - 1) % ATS_STAGES) * STAGE;
+    for (int i = threadIdx.x; i < (ATS_KEYS - rem) * CPR * 2; i += blockDim.x) {
+      const int r = rem + i / (2 * CPR), c = i % (2 * CPR);
+      *reinterpret_cast<uint4*>(st + (c / CPR) * MAT + (size_t)r * LDS * 2 + (c % CPR) * 16) = make_uint4(0u, 0u, 0u, 0u);
+    }
+    ptx::fence_proxy_async();
+  }
+  __syncthreads();
+
+  const uint32_t ring = ptx::smem_u32(att_smem);
+  // warp 0: K and V rows of key block j into stage j % ATS_STAGES
+  auto load_block = [&](int j) {
+    const int s = j % ATS_STAGES, k0 = j * ATS_KEYS, n = min(ATS_KEYS, nkeys - k0);
+    if (lane == 0) ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)n * 2 * HD * sizeof(__nv_bfloat16));
+    __syncwarp();
+    for (int r = lane; r < n; r += 32) {
+      const __nv_bfloat16* src = base + (size_t)(k0 + r) * ld + w;
+      const uint32_t dst = ring + s * STAGE + r * LDS * sizeof(__nv_bfloat16);
+      ptx::bulk_load(dst, src, HD * sizeof(__nv_bfloat16), &full[s]);
+      ptx::bulk_load(dst + MAT, src + w, HD * sizeof(__nv_bfloat16), &full[s]);
+    }
+  };
+  if (warp == 0)
+    for (int j = 0; j < min(ATS_STAGES - 1, nblk); j++) load_block(j);
+
+  const int qb = chunk * (ATS_ROWS / 16) + warp;
+  if (warp < nlive) {
+    const int r0 = qb * 16 + (lane >> 2), r1 = r0 + 8;
+    uint32_t qa[HD / 16][4];
+    load_q_frags<HD>(base, ld, r0, r1, T, lane, qa);
+    float o[HD / 8][4];
+#pragma unroll
+    for (int i = 0; i < HD / 8; i++) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
+    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+    const int Lp = (L + ATT_KB - 1) / ATT_KB * ATT_KB;
+    const int kend = causal ? min(Lp, (qb * 16 + 16 + ATT_KB - 1) / ATT_KB * ATT_KB) : Lp;
+    for (int j = 0; j < nblk; j++) {
+      // refill the stage block j - 1 used, once every live warp is done with it
+      if (warp == 0 && j + ATS_STAGES - 1 < nblk) {
+        if (j > 0) ptx::mbar_wait(&empty[(j - 1) % ATS_STAGES], ((j - 1) / ATS_STAGES) & 1);
+        load_block(j + ATS_STAGES - 1);
+      }
+      const int s = j % ATS_STAGES;
+      ptx::mbar_wait(&full[s], (j / ATS_STAGES) & 1);
+      // key kb of block j sits at row kb - j * ATS_KEYS of the stage
+      const uint32_t sK_u = ring + s * STAGE - (uint32_t)(j * ATS_KEYS * LDS * sizeof(__nv_bfloat16));
+      for (int kb = j * ATS_KEYS; kb < min(kend, (j + 1) * ATS_KEYS); kb += ATT_KB)
+        attention_block_step<HD>(sK_u, sK_u + MAT, kb, qa, o, m0, m1, l0, l1, r0, r1, L, causal, scale_log2e, lane);
+      __syncwarp();
+      if (lane == 0) ptx::mbar_arrive(&empty[s]);
+    }
+    store_rows<HD>(ob, w, r0, r1, T, L, o, l0, l1, lane);
+  } else {
+    // rows of this warp lie at or past len[b]
+    for (int i = lane; i < max(0, min(16, T - qb * 16)) * CPR; i += 32)
+      *reinterpret_cast<uint4*>(ob + (size_t)(qb * 16 + i / CPR) * w + (i % CPR) * 8) = make_uint4(0u, 0u, 0u, 0u);
+  }
+}
+
+template <int HD>
+static int launch_attention_stream(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int heads, int w,
+                                   int causal, cudaStream_t st, const int* len) {
+  B200_CHECK(B <= 65535 && heads <= 65535, B200_ERR_UNSUPPORTED,
+             "attention: %d samples x %d heads at sequence length %d: the streaming kernel takes at most 65535 of each",
+             B, heads, T);
+  constexpr size_t smem = attention_stream_smem<HD>();
+  auto kern = attention_stream_kernel<HD>;
+  B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const float scale_log2e = (1.0f / sqrtf((float)HD)) * 1.4426950408889634f;
+  kern<<<dim3((T + ATS_ROWS - 1) / ATS_ROWS, heads, B), 256, smem, st>>>(qkv, out, T, w, scale_log2e, causal, len);
+  B200_LAUNCH_OK();
+  return B200_OK;
+}
+
 template <int HD>
 static int launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int heads, int w, int causal,
                             cudaStream_t st, const int* len) {
   const int Tp = (T + ATT_KB - 1) / ATT_KB * ATT_KB;
   const size_t smem = (size_t)2 * Tp * (HD + 8) * sizeof(__nv_bfloat16);
-  B200_CHECK(smem <= 200 * 1024, B200_ERR_UNSUPPORTED, "attention: sequence length %d too long for the small-T kernel", T);
+  if (smem > 200 * 1024) return launch_attention_stream<HD>(qkv, out, B, T, heads, w, causal, st, len);
   auto kern = attention_kernel<HD>;
   if (smem > 48 * 1024) B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const float scale_log2e = (1.0f / sqrtf((float)HD)) * 1.4426950408889634f;

@@ -189,6 +189,7 @@ __global__ void __launch_bounds__(256) resize_v_norm_kernel(const ImgDesc* __res
 
 struct b200_preproc {
   int device = 0, n_px = 224;
+  int resize_mode = B200_RESIZE_SHORTEST;
   float mean[3], stdv[3];
   std::mutex mu;                       // one batch at a time per handle (workspaces are shared)
   void* ws[4] = {nullptr, nullptr, nullptr, nullptr};   // descs, coefs, tmp, staged pixels
@@ -218,14 +219,21 @@ static int crop_origin(int new_size, int n_px) { return (int)nearbyint((double)(
 extern "C" {
 
 int b200_preproc_create(int n_px, const float* mean3, const float* std3, int device, b200_preproc** out) {
+  return b200_preproc_create_mode(n_px, mean3, std3, B200_RESIZE_SHORTEST, device, out);
+}
+
+int b200_preproc_create_mode(int n_px, const float* mean3, const float* std3, int resize_mode, int device,
+                             b200_preproc** out) {
   B200_CHECK(out && mean3 && std3, B200_ERR_INVALID, "preproc_create: null argument");
+  B200_CHECK(resize_mode == B200_RESIZE_SHORTEST || resize_mode == B200_RESIZE_SQUASH, B200_ERR_INVALID,
+             "preproc_create: resize mode %d (0 shortest side + centre crop, 1 squash)", resize_mode);
   B200_CHECK(n_px >= 1 && n_px <= 4096, B200_ERR_INVALID, "preproc_create: n_px %d out of range", n_px);
   int ndev = 0;
   B200_CUDA(cudaGetDeviceCount(&ndev));
   B200_CHECK(device >= 0 && device < ndev, B200_ERR_INVALID, "preproc_create: device %d of %d", device, ndev);
   b200_preproc* p = new (std::nothrow) b200_preproc();
   B200_CHECK(p != nullptr, B200_ERR_OOM, "preproc_create: host allocation failed");
-  p->device = device; p->n_px = n_px;
+  p->device = device; p->n_px = n_px; p->resize_mode = resize_mode;
   for (int c = 0; c < 3; c++) { p->mean[c] = mean3[c]; p->stdv[c] = std3[c]; }
   *out = p;
   return B200_OK;
@@ -258,8 +266,13 @@ int b200_preproc_run(b200_preproc* p, const uint8_t* pixels, int pixels_on_devic
     d.h = h_heights[i]; d.w = h_widths[i]; d.pix_off = h_offsets[i];
     B200_CHECK(d.h >= 1 && d.w >= 1 && d.h <= 65536 && d.w <= 65536 && d.pix_off >= 0, B200_ERR_INVALID,
                "preproc_run: image %d has size %dx%d offset %lld", i, d.h, d.w, (long long)d.pix_off);
-    resized_shape(d.h, d.w, n_px, &d.new_h, &d.new_w);
-    d.top = crop_origin(d.new_h, n_px); d.left = crop_origin(d.new_w, n_px);
+    if (p->resize_mode == B200_RESIZE_SQUASH) {   // Resize((n_px, n_px)): both sides to n_px, nothing cropped
+      d.new_h = d.new_w = n_px;
+      d.top = d.left = 0;
+    } else {
+      resized_shape(d.h, d.w, n_px, &d.new_h, &d.new_w);
+      d.top = crop_origin(d.new_h, n_px); d.left = crop_origin(d.new_w, n_px);
+    }
     const Axis ah = axis_params(d.w, d.new_w), av = axis_params(d.h, d.new_h);
     d.ksize_h = d.w == d.new_w ? 1 : ah.ksize;
     d.ksize_v = d.h == d.new_h ? 1 : av.ksize;

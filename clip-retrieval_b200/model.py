@@ -51,6 +51,9 @@ _L14 = (768, 224, 14, Tower(1024, 24, 16, 4096), Tower(768, 12, 12, 3072))
 _L14_336 = (768, 336, 14, Tower(1024, 24, 16, 4096), Tower(768, 12, 12, 3072))
 _H14 = (1024, 224, 14, Tower(1280, 32, 16, 5120), Tower(1024, 24, 16, 4096))
 _B32_256 = (512, 256, 32, Tower(768, 12, 12, 3072), Tower(512, 12, 8, 2048))
+# ViT-H/14 at 378 px (Apple's DFN5B weights, `ViT-H-14-378-quickgelu`): the H/14 towers with T = 27^2 + 1 = 730 image
+# tokens.  Config recalled from open_clip's model config, not read from its source (DESIGN.md §5 (xvi)).
+_H14_378 = (1024, 378, 14, Tower(1280, 32, 16, 5120), Tower(1024, 24, 16, 4096))
 
 ARCHS = {
     # bare names -> OpenAI clip.load (QuickGELU)
@@ -65,6 +68,7 @@ ARCHS = {
     "open_clip:ViT-L-14": ClipArch(*_L14, quick_gelu=False),
     "open_clip:ViT-L-14-336": ClipArch(*_L14_336, quick_gelu=False),
     "open_clip:ViT-H-14": ClipArch(*_H14, quick_gelu=False),
+    "open_clip:ViT-H-14-378": ClipArch(*_H14_378, quick_gelu=False),
 }
 ARCHS["ViT-H/14"] = ARCHS["open_clip:ViT-H-14"]
 
@@ -367,14 +371,36 @@ def _tensor_views(sd):
 
 # ---- preprocess / tokenizer (returned by load_clip for signature parity; reader-side, CPU) ----------
 
-def make_preprocess(n_px):
+# open_clip pretrained tags whose transform squashes the image to n_px x n_px instead of resizing the shorter side
+# and cropping (resize_mode="squash" in open_clip's pretrained config, as recalled: DESIGN.md §5 (xvi)).
+_SQUASH_TAGS = {"open_clip:ViT-H-14-378": ("dfn5b",)}
+
+
+def preprocess_mode(clip_model):
+    """"squash" or "shortest": the resize step of the transform `load_clip` returns for this name (and that
+    `ClipMapper` runs on the GPU for `image_rgb8` batches)."""
+    name = clip_model[len("synthetic:"):] if clip_model.startswith("synthetic:") else clip_model
+    if name.startswith("open_clip:"):
+        arch_name, _, pretrained = name.partition("/")
+        if arch_name.endswith("-quickgelu"):
+            arch_name = arch_name[: -len("-quickgelu")]
+        if pretrained in _SQUASH_TAGS.get(arch_name, ()):
+            return "squash"
+    return "shortest"
+
+
+def make_preprocess(n_px, resize_mode="shortest"):
     """torchvision Compose[Resize(n_px, BICUBIC), CenterCrop, RGB, ToTensor, Normalize(OpenAI mean/std)] —
-    the transform SURVEY.md §4 verified bit-exactly against the reference's test_tensors fixtures."""
+    the transform SURVEY.md §4 verified bit-exactly against the reference's test_tensors fixtures.  With
+    resize_mode "squash", Resize((n_px, n_px), BICUBIC) and no crop."""
     from torchvision import transforms as T
     from torchvision.transforms import InterpolationMode
 
+    if resize_mode not in ("shortest", "squash"):
+        raise ValueError("resize_mode %r: 'shortest' or 'squash'" % (resize_mode,))
+    size = (n_px, n_px) if resize_mode == "squash" else n_px
     return T.Compose([
-        T.Resize(n_px, interpolation=InterpolationMode.BICUBIC),
+        T.Resize(size, interpolation=InterpolationMode.BICUBIC),
         T.CenterCrop(n_px),
         lambda im: im.convert("RGB"),
         T.ToTensor(),
@@ -574,7 +600,7 @@ def load_clip(clip_model="ViT-B/32", use_jit=True, warmup_batch_size=1, clip_cac
                 "no checkpoint for %r under clip_cache_path=%r (no network here); use 'synthetic:%s' for "
                 "seeded random weights" % (clip_model, clip_cache_path, clip_model))
         model.load_state_dict(read_checkpoint(ckpt, arch))
-    preprocess = make_preprocess(arch.image_size)
+    preprocess = make_preprocess(arch.image_size, preprocess_mode(clip_model))
     bpe = os.path.join(clip_cache_path, "bpe_simple_vocab_16e6.txt.gz") if clip_cache_path else None
     if bpe and os.path.exists(bpe):
         tokenizer = SimpleTokenizer(bpe, arch.context_length)

@@ -5,6 +5,8 @@
 returns the float32 `[n, 3, n_px, n_px]` batch on the device that `ClipMapper` / `encode_image`
 consume — bit-identical to torchvision's Compose[Resize(bicubic), CenterCrop, ToTensor, Normalize]
 on the host (tests/test_preprocess_gpu.py; pinned on the reference's own test_tensors fixtures).
+`resize_mode="squash"` resizes both sides to n_px with no crop instead (Resize((n_px, n_px)), open_clip's
+"squash"), the transform of the checkpoints that `model.preprocess_mode` names.
 `B200Preprocess.from_jpeg_bytes(list_of_bytes)` additionally decodes on the GPU (nvJPEG): what crosses PCIe is the
 compressed file.  Streams nvJPEG cannot parse fall back to PIL on the host, as the reference decodes every image."""
 import ctypes as C
@@ -16,6 +18,7 @@ from ._lib import lib, check
 
 OPENAI_MEAN = (0.48145466, 0.4578275, 0.40821073)
 OPENAI_STD = (0.26862954, 0.26130258, 0.27577711)
+RESIZE_MODES = {"shortest": 0, "squash": 1}   # B200_RESIZE_SHORTEST / B200_RESIZE_SQUASH
 
 
 def to_rgb8(image):
@@ -49,15 +52,19 @@ def pack_images(images):
 
 
 class B200Preprocess:
-    def __init__(self, n_px=224, mean=OPENAI_MEAN, std=OPENAI_STD, device=None):
+    def __init__(self, n_px=224, mean=OPENAI_MEAN, std=OPENAI_STD, device=None, resize_mode="shortest"):
+        if resize_mode not in RESIZE_MODES:
+            raise ValueError("resize_mode %r: one of %s" % (resize_mode, ", ".join(RESIZE_MODES)))
         if device is None:
             device = torch.cuda.current_device() if torch.cuda.is_available() else 0
         self.device = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
         self.n_px = int(n_px)
+        self.resize_mode = resize_mode
         m = (C.c_float * 3)(*mean)
         s = (C.c_float * 3)(*std)
         h = C.c_void_p()
-        check(lib.b200_preproc_create(self.n_px, m, s, self.device.index or 0, C.byref(h)))
+        check(lib.b200_preproc_create_mode(self.n_px, m, s, RESIZE_MODES[resize_mode], self.device.index or 0,
+                                           C.byref(h)))
         self._h = h
 
     def __del__(self):

@@ -444,6 +444,13 @@ int b200_encoder_embed_bf16_device(const int64_t* d_ids, const void* d_word, con
  * takes.  One batch at a time per handle; returns after the batch has been produced on `stream`. */
 typedef struct b200_preproc b200_preproc;
 int b200_preproc_create(int n_px, const float* mean3, const float* std3, int device, b200_preproc** out);
+/* The same with the resize step chosen: B200_RESIZE_SHORTEST is the transform above (b200_preproc_create's);
+ * B200_RESIZE_SQUASH is Resize((n_px, n_px), BICUBIC) with no crop — both sides scaled to n_px whatever the aspect
+ * ratio (open_clip's resize_mode "squash"). */
+#define B200_RESIZE_SHORTEST 0
+#define B200_RESIZE_SQUASH 1
+int b200_preproc_create_mode(int n_px, const float* mean3, const float* std3, int resize_mode, int device,
+                             b200_preproc** out);
 int b200_preproc_destroy(b200_preproc* p);
 int b200_preproc_run(b200_preproc* p, const uint8_t* pixels, int pixels_on_device, const int64_t* h_offsets,
                      const int32_t* h_heights, const int32_t* h_widths, int n, float* d_out, void* stream);
