@@ -166,6 +166,10 @@ PROTOTYPES = {
     "b200_clip_set_profiling": (_i, [_vp, _i]),
     "b200_layernorm_bf16_device": (_i, [_vp, _vp, _vp, _vp, _i64, _i, _i, _vp]),
     "b200_attention_bf16_device": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "b200_vision_front_bf16_device": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _i, _i, _vp, _i, _vp]),
+    "b200_text_embed_bf16_device": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "b200_token_argmax_device": (_i, [_vp, _i, _i, _vp, _i, _vp]),
+    "b200_pool_ln_proj_device": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp]),
     "b200_gemm_bf16_device": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "b200_gemm_bf16_ex_device": (_i, [_vp, _vp, _vp, _i, _i, _i, C.POINTER(GemmEpilogueC), _i, _i, _i, _vp]),
     "b200_index_last_hi_only_fallbacks": (_i, [_vp]),
@@ -197,6 +201,7 @@ PROTOTYPES = {
     "b200_attention_len_bf16_device": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "b200_text_lengths_device": (_i, [_vp, _i, _i, _i64, _vp, _vp]),
     "b200_mean_mlp_head_device": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "b200_mean_proj_head_device": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp]),
     "b200_encoder_embed_bf16_device": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, C.c_float, _vp, _i, _i, _i, _i, _i, _vp]),
 }
 

@@ -159,7 +159,7 @@ static int encode_image_chunk(b200_clip* m, const float* d_px, int B, void* d_ou
     B200_TRY(layernorm_rows(t.x, w, t.x, w, m->lnpre_g, m->lnpre_b, (int64_t)B * T, w, st)); }
   B200_TRY(run_blocks(m, t, B, 0, st));
   { TimedSpan sp(m->timer, CLS_OTHER, st, 1);
-    B200_TRY(pool_ln_proj_norm(t.x, T, w, nullptr, t.lnf_g, t.lnf_b, t.proj, m->cfg.embed_dim, d_out, out_f16, normalize, B, st, m->feat)); }
+    B200_TRY(pool_ln_proj_norm(t.x, T, w, nullptr, t.lnf_g, t.lnf_b, t.proj, m->cfg.embed_dim, m->feat, d_out, out_f16, normalize, B, st)); }
   return B200_OK;
 }
 
@@ -172,7 +172,7 @@ static int encode_text_chunk(b200_clip* m, const int64_t* d_tok, int B, void* d_
     B200_TRY(token_argmax(d_tok, m->pool_idx, B, T, st)); }
   B200_TRY(run_blocks(m, t, B, 1, st));
   { TimedSpan sp(m->timer, CLS_OTHER, st, 1);
-    B200_TRY(pool_ln_proj_norm(t.x, T, w, m->pool_idx, t.lnf_g, t.lnf_b, t.proj, m->cfg.embed_dim, d_out, out_f16, normalize, B, st, m->feat)); }
+    B200_TRY(pool_ln_proj_norm(t.x, T, w, m->pool_idx, t.lnf_g, t.lnf_b, t.proj, m->cfg.embed_dim, m->feat, d_out, out_f16, normalize, B, st)); }
   return B200_OK;
 }
 
@@ -467,6 +467,42 @@ int b200_attention_bf16_device(const void* d_qkv, void* d_out, int B, int T, int
   DeviceGuard g(device);
   return qkv_attention(nullptr, (const __nv_bfloat16*)d_qkv, (__nv_bfloat16*)d_out, B, T, heads, w, causal,
                        (cudaStream_t)stream);
+}
+int b200_vision_front_bf16_device(const float* d_pixels, int B, int S, int p, int Kp, void* d_cols, const float* d_cls,
+                                  int T, int w, void* d_x, int device, void* stream) {
+  B200_CHECK(B >= 0 && p >= 1 && S >= p && Kp >= 3 * p * p && (B == 0 || (d_pixels && d_cols)) &&
+                 (d_x == nullptr || (d_cls && T >= 1 && w >= 1)),
+             B200_ERR_INVALID, "vision_front: bad argument");
+  if (B == 0) return B200_OK;
+  DeviceGuard g(device);
+  B200_TRY(im2col_patches(d_pixels, (__nv_bfloat16*)d_cols, B, S, p, Kp, (cudaStream_t)stream));
+  if (d_x) B200_TRY(write_cls_rows((__nv_bfloat16*)d_x, d_cls, B, T, w, (cudaStream_t)stream));
+  return B200_OK;
+}
+int b200_text_embed_bf16_device(const int64_t* d_tokens, const void* d_tok_emb, const float* d_pos, void* d_x, int B,
+                                int T, int w, int vocab, int device, void* stream) {
+  B200_CHECK(B >= 0 && T >= 1 && w >= 8 && w % 8 == 0 && vocab >= 1 && (B == 0 || (d_tokens && d_tok_emb && d_pos && d_x)),
+             B200_ERR_INVALID, "text_embed: bad argument");
+  if (B == 0) return B200_OK;
+  DeviceGuard g(device);
+  return text_embed(d_tokens, (const __nv_bfloat16*)d_tok_emb, d_pos, (__nv_bfloat16*)d_x, B, T, w, vocab,
+                    (cudaStream_t)stream);
+}
+int b200_token_argmax_device(const int64_t* d_tokens, int B, int T, int32_t* d_idx, int device, void* stream) {
+  B200_CHECK(B >= 0 && T >= 1 && (B == 0 || (d_tokens && d_idx)), B200_ERR_INVALID, "token_argmax: bad argument");
+  if (B == 0) return B200_OK;
+  DeviceGuard g(device);
+  return token_argmax(d_tokens, d_idx, B, T, (cudaStream_t)stream);
+}
+int b200_pool_ln_proj_device(const void* d_x, int B, int T, int w, const int32_t* d_pool_idx, const float* d_gamma,
+                             const float* d_beta, const void* d_proj, int D, float* d_feat, void* d_out, int out_dtype,
+                             int normalize, int device, void* stream) {
+  B200_CHECK(B >= 0 && T >= 1 && w >= 1 && D >= 1 && (B == 0 || (d_x && d_gamma && d_beta && d_proj && d_feat && d_out)) &&
+                 (out_dtype == B200_OUT_F16 || out_dtype == B200_OUT_F32),
+             B200_ERR_INVALID, "pool_ln_proj: bad argument");
+  DeviceGuard g(device);
+  return pool_ln_proj_norm((const __nv_bfloat16*)d_x, T, w, d_pool_idx, d_gamma, d_beta, (const __nv_bfloat16*)d_proj,
+                           D, d_feat, d_out, out_dtype == B200_OUT_F16, normalize, B, (cudaStream_t)stream);
 }
 
 int b200_clip_set_profiling(b200_clip* m, int on) {

@@ -236,52 +236,10 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
   return t;
 }
 
-__global__ void __launch_bounds__(256)
-pool_proj_kernel(const __nv_bfloat16* __restrict__ x, int T, int w, const int* __restrict__ pool_idx,
-                 const float* __restrict__ gamma, const float* __restrict__ beta,
-                 const __nv_bfloat16* __restrict__ proj, int D, void* __restrict__ out, int out_f16, int normalize) {
-  extern __shared__ float sm[];
-  float* s_row = sm;          // [w]
-  float* s_out = sm + w;      // [D]
-  __shared__ float red[8];
-  const int b = blockIdx.x;
-  const int t = pool_idx ? pool_idx[b] : 0;
-  const __nv_bfloat16* src = x + ((size_t)b * T + t) * w;
-  float part = 0.f;
-  for (int j = threadIdx.x; j < w; j += blockDim.x) {
-    const float f = __bfloat162float(src[j]);
-    s_row[j] = f;
-    part += f;
-  }
-  const float mean = block_sum(part, red) / (float)w;
-  part = 0.f;
-  for (int j = threadIdx.x; j < w; j += blockDim.x) {
-    const float dlt = s_row[j] - mean;
-    part += dlt * dlt;
-  }
-  const float rstd = rsqrtf(block_sum(part, red) / (float)w + 1e-5f);
-  for (int j = threadIdx.x; j < w; j += blockDim.x) s_row[j] = (s_row[j] - mean) * rstd * gamma[j] + beta[j];
-  __syncthreads();
-  part = 0.f;
-  for (int j = threadIdx.x; j < D; j += blockDim.x) {
-    float acc = 0.f;
-    for (int i = 0; i < w; i++) acc = fmaf(s_row[i], __bfloat162float(proj[(size_t)i * D + j]), acc);
-    s_out[j] = acc;
-    part += acc * acc;
-  }
-  const float ss = block_sum(part, red);
-  // reference: `features /= features.norm(dim=-1, keepdim=True)` — no epsilon (mapper.py:58,66)
-  const float inv = normalize ? 1.0f / sqrtf(ss) : 1.0f;
-  for (int j = threadIdx.x; j < D; j += blockDim.x) {
-    const float v = s_out[j] * inv;
-    if (out_f16) reinterpret_cast<__half*>(out)[(size_t)b * D + j] = __float2half_rn(v);
-    else reinterpret_cast<float*>(out)[(size_t)b * D + j] = v;
-  }
-}
-// One block per sample leaves the projection to a w-long dependent loop per thread on a single SM at batch 1
-// (clip_back.py:226-246's shape).  Here a
-// block owns 64 output columns of one sample: the pooled row is normalised redundantly per block (w values), the projection is split over
-// 64 columns x 4 quarters of the reduction dimension, raw features go to `feat` and a second tiny kernel normalises.
+// A block owns 64 output columns of one sample, so that batch 1 (clip_back.py:226-246's shape) still spreads the
+// projection over D / 64 SMs instead of a w-long dependent loop per thread on one: the pooled row is normalised
+// redundantly per block (w values), the projection is split over 64 columns x 4 quarters of the reduction dimension,
+// raw features go to `feat` and a second tiny kernel normalises.
 __global__ void __launch_bounds__(256)
 pool_proj_split_kernel(const __nv_bfloat16* __restrict__ x, int T, int w, const int* __restrict__ pool_idx,
                        const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -311,8 +269,8 @@ pool_proj_split_kernel(const __nv_bfloat16* __restrict__ x, int T, int w, const 
   const int jj = threadIdx.x & 63, quarter = threadIdx.x >> 6;
   const int j = j0 + jj;
   const int per = (w + 3) / 4, i0 = quarter * per, i1 = min(w, i0 + per);
-  float acc0 = 0.f, acc1 = 0.f;   // same summation order as the one-block kernel would need a single chain; two chains
-  if (j < D) {                     // halve the latency and the result is still deterministic
+  float acc0 = 0.f, acc1 = 0.f;   // two interleaved chains halve the latency; the order is fixed, so deterministic
+  if (j < D) {
     int i = i0;
     for (; i + 1 < i1; i += 2) {
       acc0 = fmaf(s_row[i], __bfloat162float(proj[(size_t)i * D + j]), acc0);
@@ -345,21 +303,14 @@ feat_norm_cast_kernel(const float* __restrict__ feat, int D, void* __restrict__ 
 }
 
 int pool_ln_proj_norm(const __nv_bfloat16* x, int T, int w, const int* pool_idx, const float* gamma, const float* beta,
-                      const __nv_bfloat16* proj, int D, void* out, int out_f16, int normalize, int B, cudaStream_t st,
-                      float* feat_scratch) {
+                      const __nv_bfloat16* proj, int D, float* feat, void* out, int out_f16, int normalize, int B,
+                      cudaStream_t st) {
   if (B == 0) return B200_OK;
-  if (feat_scratch != nullptr) {
-    const size_t smem2 = (size_t)(w + 256) * sizeof(float);
-    B200_CHECK(smem2 <= 48 * 1024, B200_ERR_UNSUPPORTED, "pool_proj: width too large");
-    pool_proj_split_kernel<<<dim3((D + 63) / 64, B), 256, smem2, st>>>(x, T, w, pool_idx, gamma, beta, proj, D, feat_scratch);
-    B200_LAUNCH_OK();
-    feat_norm_cast_kernel<<<B, 256, 0, st>>>(feat_scratch, D, out, out_f16, normalize);
-    B200_LAUNCH_OK();
-    return B200_OK;
-  }
-  const size_t smem = (size_t)(w + D) * sizeof(float);
-  B200_CHECK(smem <= 48 * 1024, B200_ERR_UNSUPPORTED, "pool_proj: width+embed_dim too large");
-  pool_proj_kernel<<<B, 256, smem, st>>>(x, T, w, pool_idx, gamma, beta, proj, D, out, out_f16, normalize);
+  const size_t smem = (size_t)(w + 256) * sizeof(float);
+  B200_CHECK(smem <= 48 * 1024, B200_ERR_UNSUPPORTED, "pool_proj: width %d too large", w);
+  pool_proj_split_kernel<<<dim3((D + 63) / 64, B), 256, smem, st>>>(x, T, w, pool_idx, gamma, beta, proj, D, feat);
+  B200_LAUNCH_OK();
+  feat_norm_cast_kernel<<<B, 256, 0, st>>>(feat, D, out, out_f16, normalize);
   B200_LAUNCH_OK();
   return B200_OK;
 }

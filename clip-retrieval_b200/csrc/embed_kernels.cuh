@@ -33,11 +33,12 @@ int attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int he
 bool attention_wgmma_supported(int T, int heads, int w);
 int attention_wgmma(const CUtensorMap& tmQKV, __nv_bfloat16* out, int B, int T, int heads, int w, int causal,
                     cudaStream_t st, const int* len = nullptr);
-// K8/K10/K11: pooled row (x[b*T + pool_index(b)]) -> LN -> @ proj [w, D] -> optional L2 normalise
-// -> fp16 or fp32.  pool_idx == nullptr pools token 0 (vision); else row pool_idx[b] (text EOT).
+// K8/K10/K11: pooled row (x[b*T + pool_index(b)]) -> LN -> @ proj [w, D] into feat fp32 [B, D] (blocks of 64 output
+// columns per sample) -> optional L2 normalise -> fp16 or fp32.  pool_idx == nullptr pools token 0 (vision); else row
+// pool_idx[b] (text EOT).
 int pool_ln_proj_norm(const __nv_bfloat16* x, int T, int w, const int* pool_idx, const float* gamma, const float* beta,
-                      const __nv_bfloat16* proj, int D, void* out, int out_f16, int normalize, int B, cudaStream_t st,
-                      float* feat_scratch = nullptr);   // fp32 [B, D]: when given, the projection is split over D / 64 blocks per sample
+                      const __nv_bfloat16* proj, int D, float* feat, void* out, int out_f16, int normalize, int B,
+                      cudaStream_t st);
 // BERT-family embedding: x[b*T + t, :] = LN_eps((word[ids[b,t]] + tt0) + pos[pos_off + t]) in fp32, stored bf16
 // (HF's order of additions; tt0 = token-type row 0, or nullptr when the model has no token types).  word bf16
 // [vocab, w]; tt0, pos, gamma, beta fp32.  Ids outside [0, vocab) are clamped.

@@ -391,6 +391,17 @@ int b200_mean_mlp_head_device(const void* d_x, int B, int T, int w, const int32_
                               out_dtype == B200_OUT_F16, normalize, B, (cudaStream_t)stream);
 }
 
+int b200_mean_proj_head_device(const void* d_x, int B, int T, int w, const int32_t* d_len, const float* d_projT,
+                               const float* d_bias, int D, float* d_feat, void* d_out, int out_dtype, int normalize,
+                               int device, void* stream) {
+  B200_CHECK(B >= 0 && T >= 1 && w >= 1 && D >= 1 && (B == 0 || (d_x && d_len && d_projT && d_feat && d_out)) &&
+                 (out_dtype == B200_OUT_F16 || out_dtype == B200_OUT_F32),
+             B200_ERR_INVALID, "mean_proj_head: bad argument");
+  DeviceGuard g(device);
+  return masked_mean_proj_norm((const __nv_bfloat16*)d_x, T, w, d_len, d_projT, d_bias, D, d_feat, d_out,
+                               out_dtype == B200_OUT_F16, normalize, B, (cudaStream_t)stream);
+}
+
 int b200_encoder_embed_bf16_device(const int64_t* d_ids, const void* d_word, const float* d_tt0, const float* d_pos,
                                    int position_offset, const float* d_gamma, const float* d_beta, float eps,
                                    void* d_out, int B, int T, int w, int vocab, int device, void* stream) {

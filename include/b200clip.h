@@ -362,6 +362,25 @@ int b200_layernorm_bf16_device(const void* d_in, void* d_out, const float* d_gam
                                int64_t rows, int w, int device, void* stream);
 int b200_attention_bf16_device(const void* d_qkv, void* d_out, int B, int T, int heads, int w, int causal,
                                int device, void* stream);
+/* The ends of the two towers, for their parity tests.
+ * Vision front: d_pixels fp32 NCHW [B, 3, S, S] -> d_cols bf16 [B * g * g, Kp] (g = S / p, Kp >= 3 p^2): row
+ * b * g * g + py * g + px, column c * p * p + i * p + j holds pixel (c, py * p + i, px * p + j) rounded to bf16, and
+ * columns >= 3 p^2 are not written.  With d_x non-NULL, row b * T of d_x bf16 [B * T, w] becomes d_cls (fp32 [w])
+ * rounded to bf16 for every b (the class-token rows) and no other row is written.
+ * Text front: d_x bf16 [B * T, w] row b * T + t = bf16(d_tok_emb[clamp(d_tokens[b, t], 0, vocab - 1)] + d_pos[t])
+ * (d_tokens int64 [B, T], d_tok_emb bf16 [vocab, w], d_pos fp32 [T, w], w a multiple of 8); the EOT index
+ * d_idx int32 [B] = the first t of the largest token of row b.
+ * Tower end: d_out [B, D] = normalise(LN(x[b * T + t_b]) @ d_proj) with t_b = d_pool_idx[b] (int32), or 0 when
+ * d_pool_idx is NULL; LN eps 1e-5 with fp32 d_gamma, d_beta [w]; d_proj bf16 [w, D]; d_feat fp32 [B, D] receives the
+ * raw projected features; normalise is `/ |f|` with no epsilon when `normalize` (a zero row gives NaN), else none. */
+int b200_vision_front_bf16_device(const float* d_pixels, int B, int S, int p, int Kp, void* d_cols, const float* d_cls,
+                                  int T, int w, void* d_x, int device, void* stream);
+int b200_text_embed_bf16_device(const int64_t* d_tokens, const void* d_tok_emb, const float* d_pos, void* d_x, int B,
+                                int T, int w, int vocab, int device, void* stream);
+int b200_token_argmax_device(const int64_t* d_tokens, int B, int T, int32_t* d_idx, int device, void* stream);
+int b200_pool_ln_proj_device(const void* d_x, int B, int T, int w, const int32_t* d_pool_idx, const float* d_gamma,
+                             const float* d_beta, const void* d_proj, int D, float* d_feat, void* d_out, int out_dtype,
+                             int normalize, int device, void* stream);
 /* ------------------------------------------------------------------------------------------
  * Multilingual text towers (use_mclip).  Replaces the M-CLIP text model of the query service
  * (clip_back.py:222-224,836-859: XLM-RoBERTa-Large + mean pool + LinearTransformation) and the
@@ -432,6 +451,12 @@ int b200_mean_mlp_head_device(const void* d_x, int B, int T, int w, const int32_
 int b200_encoder_embed_bf16_device(const int64_t* d_ids, const void* d_word, const float* d_tt0, const float* d_pos,
                                    int position_offset, const float* d_gamma, const float* d_beta, float eps,
                                    void* d_out, int B, int T, int w, int vocab, int device, void* stream);
+/* The linear head alone: masked mean of d_x bf16 [B*T, w] over t < d_len[b] (clamped to 1..T), d_feat [B, D] =
+ * mean @ d_projT (+ d_bias) (d_projT fp32 [w, D]: the nn.Linear weight transposed; d_bias fp32 [D] or NULL), d_out
+ * [B, D] as the encoder writes it. */
+int b200_mean_proj_head_device(const void* d_x, int B, int T, int w, const int32_t* d_len, const float* d_projT,
+                               const float* d_bias, int D, float* d_feat, void* d_out, int out_dtype, int normalize,
+                               int device, void* stream);
 
 /* ---- image transform in front of the embed path (SURVEY §8(f) row 1) ----------------------------
  * Replaces `preprocess(PIL.Image)` as the reference calls it per image on the host

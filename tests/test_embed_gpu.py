@@ -33,20 +33,12 @@ def _model(name, max_batch):
 
 @pytest.mark.timeout(120)
 def test_layernorm_matches_fp32_reference():
-    import torch
-    from clip_retrieval_b200._lib import lib, check
+    """The fixed-epsilon LayerNorm entry under the float64 bound of test_embed_kernels_gpu.check_layernorm, at a few
+    tower widths (every row class, in place included)."""
+    from test_embed_kernels_gpu import check_layernorm
 
     for rows, w in ((1, 64), (77, 512), (1000, 768), (515, 1024), (33, 1280)):
-        g = torch.Generator(device="cuda").manual_seed(rows + w)
-        x = (torch.randn(rows, w, device="cuda", generator=g) * 3 + 0.5).bfloat16()
-        ga = torch.randn(w, device="cuda", generator=g)
-        be = torch.randn(w, device="cuda", generator=g)
-        out = torch.empty_like(x)
-        check(lib.b200_layernorm_bf16_device(x.data_ptr(), out.data_ptr(), ga.data_ptr(), be.data_ptr(), rows, w, 0,
-                                             torch.cuda.current_stream().cuda_stream), "ln")
-        ref = torch.nn.functional.layer_norm(x.float(), (w,), ga, be, 1e-5)
-        err = (out.float() - ref).abs()
-        assert bool((err <= ref.abs() * 2 ** -7 + 1e-2).all()), "rows=%d w=%d max err %g" % (rows, w, err.max().item())
+        check_layernorm(w, rows, ((1e-5, None),))
 
 
 def attention_ref64(qkv, B, T, heads, hd, causal):

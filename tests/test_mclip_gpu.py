@@ -1,6 +1,6 @@
-"""The multilingual text towers on the GPU (use_mclip): key-length attention, LayerNorm with an epsilon and the
-encoder embedding at kernel level; the whole encoder against the HuggingFace goldens and the fp32 oracle, at the
-real XLM-R-Large and DistilBERT-multilingual sizes too; padding invariance; the mapper and the query service.
+"""The multilingual text towers on the GPU (use_mclip): key-length attention and the encoder embedding at kernel level
+(LayerNorm with an epsilon and the linear head are in test_embed_kernels_gpu.py); the whole encoder against the
+HuggingFace goldens and the fp32 oracle, at the real XLM-R-Large and DistilBERT-multilingual sizes too; padding invariance; the mapper and the query service.
 Ids come from the goldens or are synthetic: no test here needs the `tokenizers` package."""
 import os
 from dataclasses import replace
@@ -105,22 +105,12 @@ def test_key_length_one_hot_v_probes(T):
 @pytest.mark.timeout(120)
 @pytest.mark.parametrize("eps", [1e-12, 1e-5])
 def test_layernorm_eps_matches_float64(eps):
-    import torch
-    from clip_retrieval_b200._lib import lib, check
+    """The LayerNorm entry with an epsilon under the float64 bound of test_embed_kernels_gpu.check_layernorm, at the
+    encoder widths; its rows include variances comparable to either epsilon."""
+    from test_embed_kernels_gpu import check_layernorm
 
     for rows, w in ((1, 64), (77, 768), (515, 1024)):
-        g = torch.Generator(device="cuda").manual_seed(rows + w)
-        x = (torch.randn(rows, w, device="cuda", generator=g) * 3 + 0.5).bfloat16()
-        x[0, :] = 0.25                               # a constant row: variance 0, the epsilon alone
-        ga = torch.randn(w, device="cuda", generator=g)
-        be = torch.randn(w, device="cuda", generator=g)
-        out = torch.empty_like(x)
-        check(lib.b200_layernorm_eps_bf16_device(x.data_ptr(), out.data_ptr(), ga.data_ptr(), be.data_ptr(), rows, w,
-                                                 eps, 0, torch.cuda.current_stream().cuda_stream), "ln")
-        ref = torch.nn.functional.layer_norm(x.double(), (w,), ga.double(), be.double(), eps)
-        err = (out.double() - ref).abs()
-        assert bool((err <= ref.abs() * 2 ** -7 + 1e-2).all()), "rows=%d w=%d eps=%g max err %g" % (
-            rows, w, eps, err.max().item())
+        check_layernorm(w, rows, ((eps, eps),))
 
 
 @pytest.mark.timeout(120)
