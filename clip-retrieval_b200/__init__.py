@@ -14,7 +14,7 @@ from .index import B200FlatIndex, B200IVFFlatIndex, B200IVFPQIndex, SynthSpec, l
 from .clip_index import clip_index, build_index, parse_index_key, default_index_key, default_nprobe  # noqa: F401
 from .faiss_io import write_index, index_combiner  # noqa: F401
 
-from .model import B200Clip, ClipArch, Tower, ARCHS, load_clip, synthetic_state_dict, convert_hf_state_dict  # noqa: F401,E402
+from .model import B200Clip, ClipArch, Tower, ARCHS, G14_ARCHS, load_clip, synthetic_state_dict, convert_hf_state_dict  # noqa: F401,E402
 from .preprocess import B200Preprocess, to_rgb8  # noqa: F401,E402
 from .mclip import B200TextEncoder, EncoderArch, MCLIP_ARCHS, MclipTextModel, load_mclip  # noqa: F401,E402
 from .xlmr_clip import B200XLMRClip, XLMRClipArch, XLMR_CLIP_ARCHS  # noqa: F401,E402
@@ -24,7 +24,7 @@ from .service import B200KnnService, ClipResource, MicroBatcher  # noqa: F401,E4
 from .sharded import ShardedIndex, B200ShardedIndex, shard_range  # noqa: F401,E402
 
 __all__ = [
-    "B200Clip", "ClipArch", "Tower", "ARCHS", "load_clip", "synthetic_state_dict", "convert_hf_state_dict", "ClipMapper", "get_non_uniques", "get_violent_items", "dedup_mask", "H14NsfwDetector", "get_unsafe_items", "B200Preprocess", "to_rgb8", "B200KnnService", "ClipResource", "MicroBatcher", "ShardedIndex", "B200ShardedIndex", "shard_range",
+    "B200Clip", "ClipArch", "Tower", "ARCHS", "G14_ARCHS", "load_clip", "synthetic_state_dict", "convert_hf_state_dict", "ClipMapper", "get_non_uniques", "get_violent_items", "dedup_mask", "H14NsfwDetector", "get_unsafe_items", "B200Preprocess", "to_rgb8", "B200KnnService", "ClipResource", "MicroBatcher", "ShardedIndex", "B200ShardedIndex", "shard_range",
     "lib", "B200Error", "library_path", "launch_count",
     "B200FlatIndex", "B200IVFFlatIndex", "B200IVFPQIndex", "SynthSpec", "load_index", "merge_shard_results", "train_kmeans", "build_ivf_index",
     "train_pq", "train_ivfpq", "build_ivfpq_index", "train_opq", "clip_index", "build_index", "parse_index_key",

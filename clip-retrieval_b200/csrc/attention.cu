@@ -6,6 +6,9 @@
 // Per-sample key lengths (len[b] in 1..T) as in attention_wgmma.cu: keys >= len[b] are staged as zeros and masked,
 // the key loop stops at the 32-key block holding len[b] - 1, and rows >= len[b] are written as zeros.
 // Shapes whose whole-head K + V would pass 200 KB run on attention_stream_kernel below, with the same per-block step.
+// Head dims 88 and 104 (ViT-g-14, ViT-bigG-14: HD % 16 == 8) take the same kernels with an 8-wide tail at every step:
+// the last Q fragment's upper half is zero registers (columns HD.. of the qkv row are the next head's Q, or K), QK^T
+// ends with one 8-dim k-step, P.V with one unpaired n8 tile, and the K/V rows are padded to HD + 16 (att_lds).
 #include "embed_kernels.cuh"
 #include "ptx.cuh"
 
@@ -35,11 +38,19 @@ __device__ __forceinline__ uint32_t pack2(float lo, float hi) {
 
 constexpr int ATT_KB = 32;  // keys per inner block
 
+// Padded K/V row in shared memory (elements): an odd number of 16-byte chunks, so that the 8 rows of an ldmatrix
+// 8x8 block fall in distinct bank groups.  HD + 8 for HD % 16 == 0 (144 B / 176 B / 208 B / 272 B rows at 64 / 80 / 96
+// / 128), HD + 16 for HD % 16 == 8 (208 B / 240 B at 88 / 104; HD + 8 would give an even 12 / 14 chunks).
+__host__ __device__ constexpr int att_lds(int hd) { return hd % 16 == 0 ? hd + 8 : hd + 16; }
+// k16 Q fragments per row pair: the last one of HD % 16 == 8 holds dims HD-8..HD-1 and zero registers above.
+__host__ __device__ constexpr int att_qfrags(int hd) { return (hd + 15) / 16; }
+
 // Q fragments of rows r0 / r1 straight from global (rows >= T read as zeros):
-// a[ks] = {Q[r0][k0..], Q[r1][k0..], Q[r0][k0+8..], Q[r1][k0+8..]}
+// a[ks] = {Q[r0][k0..], Q[r1][k0..], Q[r0][k0+8..], Q[r1][k0+8..]}; for HD % 16 == 8 the last fragment's upper half
+// (dims HD..HD+7, which belong to the next head) is zero and is not loaded.
 template <int HD>
 __device__ __forceinline__ void load_q_frags(const __nv_bfloat16* base, size_t ld, int r0, int r1, int T, int lane,
-                                             uint32_t (&qa)[HD / 16][4]) {
+                                             uint32_t (&qa)[att_qfrags(HD)][4]) {
 #pragma unroll
   for (int ks = 0; ks < HD / 16; ks++) {
     const int k0 = ks * 16 + (lane & 3) * 2;
@@ -47,6 +58,13 @@ __device__ __forceinline__ void load_q_frags(const __nv_bfloat16* base, size_t l
     qa[ks][1] = r1 < T ? *reinterpret_cast<const uint32_t*>(base + (size_t)r1 * ld + k0) : 0u;
     qa[ks][2] = r0 < T ? *reinterpret_cast<const uint32_t*>(base + (size_t)r0 * ld + k0 + 8) : 0u;
     qa[ks][3] = r1 < T ? *reinterpret_cast<const uint32_t*>(base + (size_t)r1 * ld + k0 + 8) : 0u;
+  }
+  if constexpr (HD % 16 == 8) {
+    const int k0 = HD - 8 + (lane & 3) * 2;
+    qa[HD / 16][0] = r0 < T ? *reinterpret_cast<const uint32_t*>(base + (size_t)r0 * ld + k0) : 0u;
+    qa[HD / 16][1] = r1 < T ? *reinterpret_cast<const uint32_t*>(base + (size_t)r1 * ld + k0) : 0u;
+    qa[HD / 16][2] = 0u;
+    qa[HD / 16][3] = 0u;
   }
 }
 
@@ -73,11 +91,16 @@ __device__ __forceinline__ void store_rows(__nv_bfloat16* ob, int w, int r0, int
 // bf16.  sK_u / sV_u address key kb at sK_u + kb * LDS * 2: both kernels call this, the whole-K/V kernel with its
 // buffer's base, the streaming kernel with a ring stage's base shifted back by the stage's first key.
 template <int HD>
-__device__ __forceinline__ void attention_block_step(uint32_t sK_u, uint32_t sV_u, int kb, const uint32_t (&qa)[HD / 16][4],
-                                                     float (&o)[HD / 8][4], float& m0, float& m1, float& l0, float& l1,
-                                                     int r0, int r1, int L, int causal, float scale_log2e, int lane) {
-  constexpr int LDS = HD + 8;
+__device__ __forceinline__ void attention_block_step(uint32_t sK_u, uint32_t sV_u, int kb,
+                                                     const uint32_t (&qa)[att_qfrags(HD)][4], float (&o)[HD / 8][4],
+                                                     float& m0, float& m1, float& l0, float& l1, int r0, int r1, int L,
+                                                     int causal, float scale_log2e, int lane) {
+  constexpr int LDS = att_lds(HD);
   float s[ATT_KB / 8][4];
+  // HD % 16 == 8: K dims HD-8..HD-1 of the block's 32 keys, one 8x8 matrix per 8 keys (matrix nt = keys kb + nt*8..)
+  uint32_t kt[4] = {0u, 0u, 0u, 0u};
+  if constexpr (HD % 16 == 8)
+    ldmatrix_x4(kt[0], kt[1], kt[2], kt[3], sK_u + (uint32_t)(((kb + lane) * LDS + HD - 8) * 2));
 #pragma unroll
   for (int nt = 0; nt < ATT_KB / 8; nt++) {
     s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
@@ -90,13 +113,18 @@ __device__ __forceinline__ void attention_block_step(uint32_t sK_u, uint32_t sV_
       mma_bf16_16816(s[nt], qa[kp * 2], b0, b1);
       mma_bf16_16816(s[nt], qa[kp * 2 + 1], b2, b3);
     }
-    if constexpr (HD % 32 != 0) {
-      // tail k-step (HD = 80): d = HD-16 .. HD-1; only matrices 0,1 are meaningful
+    if constexpr (HD % 32 >= 16) {
+      // 16-wide tail k-step (HD = 80, 88): d = (HD/32)*32 .. +15; only matrices 0,1 are meaningful
       uint32_t b0, b1, b2, b3;
       const int dcol = (HD / 32) * 32 + ((lane >> 3) & 1) * 8;
       const uint32_t addr = sK_u + (uint32_t)(((kb + nt * 8 + (lane & 7)) * LDS + dcol) * 2);
       ldmatrix_x4(b0, b1, b2, b3, addr);
-      mma_bf16_16816(s[nt], qa[HD / 16 - 1], b0, b1);
+      mma_bf16_16816(s[nt], qa[(HD / 32) * 2], b0, b1);
+    }
+    if constexpr (HD % 16 == 8) {
+      // 8-wide tail k-step (HD = 88, 104): d = HD-8 .. HD-1 against the zero-topped last Q fragment; the K operand's
+      // upper half is a zero register too, so the shared-memory padding never enters the sum
+      mma_bf16_16816(s[nt], qa[HD / 16], kt[nt], 0u);
     }
   }
   // mask + block row max (scores stay unscaled; the scale folds into the exp2 argument)
@@ -155,13 +183,21 @@ __device__ __forceinline__ void attention_block_step(uint32_t sK_u, uint32_t sV_
       mma_bf16_16816(o[dp * 2 + 1], pa[kk], b2, b3);
     }
   }
+  if constexpr (HD % 16 == 8) {
+    // the unpaired last n8 tile (d = HD-8 .. HD-1): V^T of keys kb + 8j.. as matrix j, so {b0, b1} / {b2, b3} are
+    // the k16 halves of keys kb.. / kb+16..
+    uint32_t b0, b1, b2, b3;
+    ldmatrix_x4_trans(b0, b1, b2, b3, sV_u + (uint32_t)(((kb + lane) * LDS + HD - 8) * 2));
+    mma_bf16_16816(o[HD / 8 - 1], pa[0], b0, b1);
+    mma_bf16_16816(o[HD / 8 - 1], pa[1], b2, b3);
+  }
 }
 
 template <int HD>
 __global__ void __launch_bounds__(256)
 attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ out, int T, int w, float scale_log2e,
                  int causal, const int* __restrict__ len) {
-  constexpr int LDS = HD + 8;  // padded row (elements): 144 B / 176 B rows -> conflict-free ldmatrix
+  constexpr int LDS = att_lds(HD);  // padded row (elements) -> conflict-free ldmatrix
   extern __shared__ __align__(16) unsigned char att_smem[];
   __nv_bfloat16* sK = reinterpret_cast<__nv_bfloat16*>(att_smem);
   const int Tp = (T + ATT_KB - 1) / ATT_KB * ATT_KB;
@@ -194,7 +230,7 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
 
   for (int qb = warp; qb < qblocks; qb += nwarps) {
     const int r0 = qb * 16 + (lane >> 2), r1 = r0 + 8;
-    uint32_t qa[HD / 16][4];
+    uint32_t qa[att_qfrags(HD)][4];
     load_q_frags<HD>(base, ld, r0, r1, T, lane, qa);
     float o[HD / 8][4];
 #pragma unroll
@@ -216,7 +252,7 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
 // Longer sequences (whole-head K + V past 200 KB of shared memory: T > 704 / 576 / 480 / 352 at head dim 64 / 80 /
 // 96 / 128): one CTA per (128-row query chunk, head, sample), chunk fastest so that the chunks of a head read its K/V
 // from L2.  Eight warps own 16 query rows each; K and V pass through a ring of ATS_STAGES blocks of 64 keys, filled
-// by warp 0 with one bulk copy per row (rows padded to HD + 8 elements as above) and handed over by full / empty
+// by warp 0 with one bulk copy per row (rows padded to att_lds(HD) elements as above) and handed over by full / empty
 // mbarriers, so shared memory no longer grows with T.  The arithmetic per 32-key block is attention_block_step.
 // A chunk loads keys < len[b] only, and with causal only keys up to its last row; a chunk wholly at or past len[b]
 // writes zeros and loads nothing.
@@ -226,14 +262,14 @@ constexpr int ATS_STAGES = 3;
 
 template <int HD>
 constexpr size_t attention_stream_smem() {
-  return (size_t)ATS_STAGES * 2 * ATS_KEYS * (HD + 8) * sizeof(__nv_bfloat16) + 2 * ATS_STAGES * sizeof(uint64_t);
+  return (size_t)ATS_STAGES * 2 * ATS_KEYS * att_lds(HD) * sizeof(__nv_bfloat16) + 2 * ATS_STAGES * sizeof(uint64_t);
 }
 
 template <int HD>
 __global__ void __launch_bounds__(256, HD <= 96 ? 2 : 1)
 attention_stream_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ out, int T, int w,
                         float scale_log2e, int causal, const int* __restrict__ len) {
-  constexpr int LDS = HD + 8;
+  constexpr int LDS = att_lds(HD);
   constexpr int CPR = HD / 8;                                    // 16-byte chunks per row
   constexpr uint32_t MAT = ATS_KEYS * LDS * sizeof(__nv_bfloat16);   // one stage's K (or V) block, bytes
   constexpr uint32_t STAGE = 2 * MAT;
@@ -296,7 +332,7 @@ attention_stream_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __
   const int qb = chunk * (ATS_ROWS / 16) + warp;
   if (warp < nlive) {
     const int r0 = qb * 16 + (lane >> 2), r1 = r0 + 8;
-    uint32_t qa[HD / 16][4];
+    uint32_t qa[att_qfrags(HD)][4];
     load_q_frags<HD>(base, ld, r0, r1, T, lane, qa);
     float o[HD / 8][4];
 #pragma unroll
@@ -346,7 +382,7 @@ template <int HD>
 static int launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int heads, int w, int causal,
                             cudaStream_t st, const int* len) {
   const int Tp = (T + ATT_KB - 1) / ATT_KB * ATT_KB;
-  const size_t smem = (size_t)2 * Tp * (HD + 8) * sizeof(__nv_bfloat16);
+  const size_t smem = (size_t)2 * Tp * att_lds(HD) * sizeof(__nv_bfloat16);
   if (smem > 200 * 1024) return launch_attention_stream<HD>(qkv, out, B, T, heads, w, causal, st, len);
   auto kern = attention_kernel<HD>;
   if (smem > 48 * 1024) B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -365,9 +401,11 @@ int attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int he
   const int hd = w / heads;
   if (hd == 64) return launch_attention<64>(qkv, out, B, T, heads, w, causal, st, len);
   if (hd == 80) return launch_attention<80>(qkv, out, B, T, heads, w, causal, st, len);
+  if (hd == 88) return launch_attention<88>(qkv, out, B, T, heads, w, causal, st, len);
   if (hd == 96) return launch_attention<96>(qkv, out, B, T, heads, w, causal, st, len);
+  if (hd == 104) return launch_attention<104>(qkv, out, B, T, heads, w, causal, st, len);
   if (hd == 128) return launch_attention<128>(qkv, out, B, T, heads, w, causal, st, len);
-  set_error("attention: head dimension %d not supported (64, 80, 96, 128)", hd);
+  set_error("attention: head dimension %d not supported (64, 80, 88, 96, 104, 128)", hd);
   return B200_ERR_UNSUPPORTED;
 }
 

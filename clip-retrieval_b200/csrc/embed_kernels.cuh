@@ -21,7 +21,8 @@ int layernorm_rows(const __nv_bfloat16* in, int64_t in_ld, __nv_bfloat16* out, i
 int layernorm_rows_eps(const __nv_bfloat16* in, int64_t in_ld, __nv_bfloat16* out, int64_t out_ld, const float* gamma,
                        const float* beta, int64_t rows, int w, float eps, cudaStream_t st);
 // K4: multi-head attention over the fused qkv buffer [B*T, 3w] -> out [B*T, w]; causal for text.  mma.sync kernels
-// (attention.cu) for the head dimensions the wgmma kernel does not take (80, 96, 128) and for head dim 64 past T = 320:
+// (attention.cu) for the head dimensions the wgmma kernel does not take (80, 88, 96, 104, 128) and for head dim 64 past
+// T = 320:
 // whole K/V of a head in shared memory while it fits in 200 KB, K/V streamed through a ring of 64-key stages beyond.
 // len (device int32 [B], values 1..T, or nullptr = T): sample b attends to its keys < len[b], and its rows >= len[b]
 // of `out` are zeros — the key-padding mask of a bidirectional encoder (both kernels).

@@ -72,6 +72,19 @@ ARCHS = {
 }
 ARCHS["ViT-H/14"] = ARCHS["open_clip:ViT-H-14"]
 
+# The two largest LAION CLIPs, whose image towers have head dims 88 (g) and 104 (bigG): 224 px, patch 14 (T = 257),
+# context 77, erf GELU.  Configs recalled from open_clip's model configs (head_width 88 / 104, mlp_ratio 4.3637 / 4.9231
+# -> int(width * ratio)) and the laion/CLIP-ViT-{g,bigG}-14 HuggingFace configs, not read from either (DESIGN.md §5
+# (xvii)).  Kept apart from ARCHS, whose entries all have head dims in (64, 80, 96, 128); resolve_arch reads both.
+_G14 = (1024, 224, 14, Tower(1408, 40, 16, 6144), Tower(1024, 24, 16, 4096))
+_BIGG14 = (1280, 224, 14, Tower(1664, 48, 16, 8192), Tower(1280, 32, 20, 5120))
+G14_ARCHS = {
+    "open_clip:ViT-g-14": ClipArch(*_G14, quick_gelu=False),          # laion2b_s12b_b42k, laion2b_s34b_b88k
+    "open_clip:ViT-bigG-14": ClipArch(*_BIGG14, quick_gelu=False),    # laion2b_s39b_b160k
+}
+# Every architecture a `clip_model` name can resolve to.
+KNOWN_ARCHS = {**ARCHS, **G14_ARCHS}
+
 # `hf_clip:<repo>` names -> (architecture key, quick_gelu): HuggingFace CLIPModel checkpoints of the same towers.
 HF_REPOS = {
     "openai/clip-vit-base-patch32": ("open_clip:ViT-B-32", True),
@@ -82,6 +95,9 @@ HF_REPOS = {
     "laion/CLIP-ViT-B-32-laion2B-s34B-b79K": ("open_clip:ViT-B-32", False),
     "laion/CLIP-ViT-L-14-laion2B-s32B-b82K": ("open_clip:ViT-L-14", False),
     "laion/CLIP-ViT-H-14-laion2B-s32B-b79K": ("open_clip:ViT-H-14", False),
+    "laion/CLIP-ViT-g-14-laion2B-s12B-b42K": ("open_clip:ViT-g-14", False),
+    "laion/CLIP-ViT-g-14-laion2B-s34B-b88K": ("open_clip:ViT-g-14", False),
+    "laion/CLIP-ViT-bigG-14-laion2B-39B-b160k": ("open_clip:ViT-bigG-14", False),
 }
 # `nm:<repo>` (DeepSparse, README.md:201) names quantised ONNX exports of these open_clip towers.
 NM_REPOS = {
@@ -128,9 +144,9 @@ def resolve_arch(clip_model):
         if pretrained == "openai":
             quick = True
         key = "open_clip:" + arch_name
-        if key not in ARCHS:
-            raise ValueError("unknown clip_model %r; known: %s" % (clip_model, ", ".join(sorted(ARCHS))))
-        return replace(ARCHS[key], quick_gelu=quick), key + ("-quickgelu" if quick else "")
+        if key not in KNOWN_ARCHS:
+            raise ValueError("unknown clip_model %r; known: %s" % (clip_model, ", ".join(sorted(KNOWN_ARCHS))))
+        return replace(KNOWN_ARCHS[key], quick_gelu=quick), key + ("-quickgelu" if quick else "")
     for prefix, table in (("hf_clip:", HF_REPOS), ("nm:", NM_REPOS)):
         if name.startswith(prefix):
             repo = name[len(prefix):]
@@ -138,10 +154,10 @@ def resolve_arch(clip_model):
                 raise ValueError("unknown %s repository %r; known: %s (or load a state_dict with "
                                  "B200Clip(arch_from_hf_config(config)))" % (prefix, repo, ", ".join(sorted(table))))
             key, quick = table[repo]
-            return replace(ARCHS[key], quick_gelu=quick), name
-    if name not in ARCHS:
-        raise ValueError("unknown clip_model %r; known: %s" % (clip_model, ", ".join(sorted(ARCHS))))
-    return ARCHS[name], name
+            return replace(KNOWN_ARCHS[key], quick_gelu=quick), name
+    if name not in KNOWN_ARCHS:
+        raise ValueError("unknown clip_model %r; known: %s" % (clip_model, ", ".join(sorted(KNOWN_ARCHS))))
+    return KNOWN_ARCHS[name], name
 
 
 def synthetic_state_dict(arch, seed=0):
@@ -518,19 +534,26 @@ class _MissingTokenizer:
         raise RuntimeError(self.why)
 
 
+# The weight files of a HuggingFace snapshot folder, in the order they are looked for: one file, or the index of a
+# sharded snapshot (its "weight_map" names the shard of every tensor), as `save_pretrained` writes large models.
+HF_SNAPSHOT_FILES = ("pytorch_model.bin", "model.safetensors", "pytorch_model.bin.index.json",
+                     "model.safetensors.index.json")
+
+
 def _find_checkpoint(key, clip_cache_path):
     """`<clip_cache_path>/<name>.{pt,pth,bin}` with `/`, `@`, `:` of the model name turned into `-`
-    (e.g. `ViT-L-14.pt`, `hf_clip-patrickjohncyh-fashion-clip.bin`), or a HuggingFace snapshot folder
-    `<clip_cache_path>/<repo>/pytorch_model.bin` for `hf_clip:` names."""
+    (e.g. `ViT-L-14.pt`, `ViT-bigG-14.pt`, `hf_clip-patrickjohncyh-fashion-clip.bin`), or for `hf_clip:` names the
+    first of HF_SNAPSHOT_FILES in a HuggingFace snapshot folder `<clip_cache_path>/<repo>/`."""
     if not clip_cache_path:
         return None
     stems = [key.replace("open_clip:", "").replace("/", "-").replace("@", "-").replace(":", "-")]
     if key.startswith("hf_clip:"):
         repo = key[len("hf_clip:"):]
         stems.append(repo.replace("/", "-"))
-        p = os.path.join(clip_cache_path, repo, "pytorch_model.bin")
-        if os.path.exists(p):
-            return p
+        for f in HF_SNAPSHOT_FILES:
+            p = os.path.join(clip_cache_path, repo, f)
+            if os.path.exists(p):
+                return p
     for stem in stems:
         for ext in (".pt", ".pth", ".bin"):
             p = os.path.join(clip_cache_path, stem + ext)
@@ -539,15 +562,39 @@ def _find_checkpoint(key, clip_cache_path):
     return None
 
 
+def _read_tensor_file(path):
+    """One weight file: a `.safetensors` file, or anything torch.load / torch.jit.load reads."""
+    torch = _torch()
+    if path.endswith(".safetensors"):
+        from safetensors.torch import load_file
+
+        return load_file(path, device="cpu")
+    try:
+        return torch.load(path, map_location="cpu", weights_only=False)
+    except RuntimeError:
+        return torch.jit.load(path, map_location="cpu")
+
+
+def _read_sharded(index_path):
+    """The state_dict of a sharded HuggingFace snapshot: every shard the index's weight_map names, each read once."""
+    import json
+
+    with open(index_path) as f:
+        weight_map = json.load(f)["weight_map"]
+    folder = os.path.dirname(index_path)
+    sd = {}
+    for shard in sorted(set(weight_map.values())):
+        part = _read_tensor_file(os.path.join(folder, shard))
+        sd.update((k, part[k]) for k, s in weight_map.items() if s == shard)
+    return sd
+
+
 def read_checkpoint(path, arch):
     """Load a checkpoint file into the OpenAI/open_clip state_dict key layout `load_state_dict` takes.
     Accepted: a plain state_dict, a training checkpoint `{"state_dict": ...}` (optionally with `module.`
-    prefixes), a TorchScript archive (OpenAI's released `.pt` files), a HuggingFace CLIPModel state_dict."""
-    torch = _torch()
-    try:
-        obj = torch.load(path, map_location="cpu", weights_only=False)
-    except RuntimeError:
-        obj = torch.jit.load(path, map_location="cpu")
+    prefixes), a TorchScript archive (OpenAI's released `.pt` files), a HuggingFace CLIPModel state_dict, as one
+    `.bin` / `.safetensors` file or as the `*.index.json` of a sharded snapshot."""
+    obj = _read_sharded(path) if path.endswith(".index.json") else _read_tensor_file(path)
     sd = obj if isinstance(obj, dict) else obj.state_dict()
     if "state_dict" in sd and isinstance(sd["state_dict"], dict):
         sd = sd["state_dict"]
