@@ -55,6 +55,10 @@ class ClipConfigC(C.Structure):
     ]
 
 
+class ResNetConfigC(C.Structure):
+    _fields_ = [("layers", C.c_int32 * 4), ("width", C.c_int32), ("heads", C.c_int32)]
+
+
 class TextEncoderConfigC(C.Structure):
     _fields_ = [
         ("layers", C.c_int32),
@@ -156,6 +160,7 @@ PROTOTYPES = {
     "b200_nccl_comm_init_all": (_i, [_i, C.POINTER(C.c_int), C.POINTER(_vp)]),
     "b200_nccl_comm_destroy": (_i, [_vp]),
     "b200_clip_create": (_i, [C.POINTER(ClipConfigC), _i, C.POINTER(_vp)]),
+    "b200_clip_create_resnet": (_i, [C.POINTER(ClipConfigC), C.POINTER(ResNetConfigC), _i, C.POINTER(_vp)]),
     "b200_clip_destroy": (_i, [_vp]),
     "b200_clip_load_weights": (_i, [_vp, C.POINTER(TensorViewC), _i]),
     "b200_clip_encode_image_device": (_i, [_vp, _vp, _i, _vp, _i, _i, _vp]),
@@ -172,6 +177,10 @@ PROTOTYPES = {
     "b200_pool_ln_proj_device": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp]),
     "b200_gemm_bf16_device": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "b200_gemm_bf16_ex_device": (_i, [_vp, _vp, _vp, _i, _i, _i, C.POINTER(GemmEpilogueC), _i, _i, _i, _vp]),
+    "b200_conv_bf16_device": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, C.POINTER(GemmEpilogueC), _i, _i, _vp]),
+    "b200_stem_gather_device": (_i, [_vp, _i, _i, _vp, _i, _vp]),
+    "b200_avgpool_bf16_device": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _i, _vp]),
+    "b200_attnpool_tokens_device": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp]),
     "b200_index_last_hi_only_fallbacks": (_i, [_vp]),
     "b200_index_last_scan_plan": (_i, [_vp, _vp]),
     "b200_kmeans_train_f16": (_i, [_vp, _i64, _i, _i, _i, C.c_uint64, _i, _vp, _vp, _i]),

@@ -11,6 +11,7 @@
 #include "embed_kernels.cuh"
 #include "gemm.cuh"
 #include "layers.cuh"
+#include "resnet.cuh"
 #include "weights.cuh"
 #include <map>
 #include <mutex>
@@ -51,6 +52,7 @@ struct b200_clip {
   bool loaded = false;
   bool has_text = true;       // false: an image-only handle (all-zero text tower config), no text weights or buffers
   b200::Tower vis, txt;
+  b200::ResNetTower* rn = nullptr;   // the ResNet image tower (b200_clip_create_resnet) in place of vis and its front
   // vision front end
   int grid = 0, Kp = 0;
   b200::Linear conv;          // [w, Kp]
@@ -146,6 +148,9 @@ static int run_blocks(b200_clip* m, Tower& t, int B, int causal, cudaStream_t st
 
 static int encode_image_chunk(b200_clip* m, const float* d_px, int B, void* d_out, int out_f16, int normalize,
                               cudaStream_t st) {
+  if (m->rn)
+    return resnet_encode(*m->rn, m->timer, CLS_GEMM, CLS_ATTN, CLS_OTHER, m->sms, d_px, B, m->feat, d_out, out_f16,
+                         normalize, st);
   Tower& t = m->vis;
   const int g = m->grid, w = t.width, T = t.T;
   { TimedSpan sp(m->timer, CLS_OTHER, st, 2);
@@ -197,6 +202,53 @@ static int load_tower(Loader& ld, Tower& t, const std::string& prefix) {
   return B200_OK;
 }
 
+// What both image towers share: the text tower and its front, the projected features, and the staging buffers of the
+// host and graph entries.
+static int make_text_and_staging(b200_clip* m) {
+  const b200_clip_config* cfg = &m->cfg;
+  DeviceAllocs& al = m->allocs;
+  if (m->has_text) {
+    B200_TRY(make_tower(m, &m->txt, cfg->text, cfg->context_length, cfg->embed_dim));
+    B200_TRY(al.alloc(&m->tok_emb, (size_t)cfg->vocab_size * cfg->text.width));
+    B200_TRY(al.alloc(&m->tpos, (size_t)cfg->context_length * cfg->text.width));
+    B200_TRY(al.alloc(&m->pool_idx, (size_t)cfg->max_batch));
+  }
+  const size_t tok_bytes = m->has_text ? (size_t)cfg->context_length * 8 : 0;
+  B200_TRY(al.alloc(&m->feat, (size_t)cfg->max_batch * cfg->embed_dim));
+  const size_t in_bytes = std::max((size_t)cfg->max_batch * 3 * cfg->image_size * cfg->image_size * 4,
+                                   (size_t)cfg->max_batch * tok_bytes);
+  B200_TRY(al.alloc(&m->stage_in, in_bytes));
+  B200_TRY(al.alloc(&m->stage_out, (size_t)cfg->max_batch * cfg->embed_dim * 4));
+  const int gb = std::min(GRAPH_MAX_B, cfg->max_batch);
+  B200_TRY(al.alloc(&m->g_in, std::max((size_t)gb * 3 * cfg->image_size * cfg->image_size * 4, (size_t)gb * tok_bytes)));
+  B200_TRY(al.alloc(&m->g_out, (size_t)gb * cfg->embed_dim * 4));
+  return B200_OK;
+}
+
+// The ViT image tower's visual.* tensors.
+static int load_vit(b200_clip* m, Loader& ld) {
+  const b200_clip_config& c = m->cfg;
+  const size_t vw = c.vision.width, D = c.embed_dim;
+  const size_t T = (size_t)m->grid * m->grid + 1, kraw = (size_t)3 * c.patch * c.patch;
+  B200_TRY(ld.put_bf16("visual.conv1.weight", m->conv.w, vw, kraw, m->Kp));
+  B200_TRY(ld.put_bf16("visual.positional_embedding", m->vpos, T, vw, vw));
+  {
+    const b200_tensor_view* cls = ld.find("visual.class_embedding", vw);
+    const b200_tensor_view* pos = ld.find("visual.positional_embedding", T * vw);
+    if (!cls || !pos) return B200_ERR_INVALID;
+    std::vector<float> v(vw);
+    for (size_t j = 0; j < vw; j++) v[j] = view_get(*cls, j) + view_get(*pos, j);
+    B200_CUDA(cudaMemcpy(m->cls_pos0, v.data(), vw * 4, cudaMemcpyHostToDevice));
+  }
+  B200_TRY(ld.put_f32("visual.ln_pre.weight", m->lnpre_g, vw));
+  B200_TRY(ld.put_f32("visual.ln_pre.bias", m->lnpre_b, vw));
+  B200_TRY(load_tower(ld, m->vis, "visual."));
+  B200_TRY(ld.put_f32("visual.ln_post.weight", m->vis.lnf_g, vw));
+  B200_TRY(ld.put_f32("visual.ln_post.bias", m->vis.lnf_b, vw));
+  B200_TRY(ld.put_bf16("visual.proj", m->vis.proj, vw, D, D));
+  return B200_OK;
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -227,7 +279,6 @@ int b200_clip_create(const b200_clip_config* cfg, int device, b200_clip** out) {
   int rc = B200_OK;
   auto build = [&]() -> int {
     B200_TRY(make_tower(m, &m->vis, cfg->vision, T, cfg->embed_dim));
-    if (has_text) B200_TRY(make_tower(m, &m->txt, cfg->text, cfg->context_length, cfg->embed_dim));
     DeviceAllocs& al = m->allocs;
     B200_TRY(make_linear(al, &m->conv, cfg->vision.width, m->Kp, false));
     const size_t prow = (size_t)cfg->max_batch * m->grid * m->grid;
@@ -238,21 +289,7 @@ int b200_clip_create(const b200_clip_config* cfg, int device, b200_clip** out) {
     B200_TRY(al.alloc(&m->cls_pos0, (size_t)cfg->vision.width));
     B200_TRY(al.alloc(&m->lnpre_g, (size_t)cfg->vision.width));
     B200_TRY(al.alloc(&m->lnpre_b, (size_t)cfg->vision.width));
-    if (has_text) {
-      B200_TRY(al.alloc(&m->tok_emb, (size_t)cfg->vocab_size * cfg->text.width));
-      B200_TRY(al.alloc(&m->tpos, (size_t)cfg->context_length * cfg->text.width));
-      B200_TRY(al.alloc(&m->pool_idx, (size_t)cfg->max_batch));
-    }
-    const size_t tok_bytes = has_text ? (size_t)cfg->context_length * 8 : 0;
-    B200_TRY(al.alloc(&m->feat, (size_t)cfg->max_batch * cfg->embed_dim));
-    const size_t in_bytes = std::max((size_t)cfg->max_batch * 3 * cfg->image_size * cfg->image_size * 4,
-                                     (size_t)cfg->max_batch * tok_bytes);
-    B200_TRY(al.alloc(&m->stage_in, in_bytes));
-    B200_TRY(al.alloc(&m->stage_out, (size_t)cfg->max_batch * cfg->embed_dim * 4));
-    const int gb = std::min(GRAPH_MAX_B, cfg->max_batch);
-    B200_TRY(al.alloc(&m->g_in, std::max((size_t)gb * 3 * cfg->image_size * cfg->image_size * 4, (size_t)gb * tok_bytes)));
-    B200_TRY(al.alloc(&m->g_out, (size_t)gb * cfg->embed_dim * 4));
-    return B200_OK;
+    return make_text_and_staging(m);
   };
   rc = build();
   if (rc != B200_OK) {
@@ -263,11 +300,44 @@ int b200_clip_create(const b200_clip_config* cfg, int device, b200_clip** out) {
   return B200_OK;
 }
 
+// The ResNet image tower (resnet.cuh) with the same text tower, staging, graphs and entries as b200_clip_create.
+int b200_clip_create_resnet(const b200_clip_config* cfg, const b200_resnet_config* rc, int device, b200_clip** out) {
+  B200_CHECK(cfg && rc && out, B200_ERR_INVALID, "clip_create_resnet: null argument");
+  const bool has_text = cfg->text.width != 0 || cfg->text.layers != 0 || cfg->text.heads != 0 || cfg->text.mlp != 0;
+  const bool no_vit = cfg->patch == 0 && cfg->vision.width == 0 && cfg->vision.layers == 0 && cfg->vision.heads == 0 &&
+                      cfg->vision.mlp == 0;
+  B200_CHECK(no_vit && cfg->max_batch >= 1 && cfg->embed_dim >= 8 && cfg->image_size >= 32 && cfg->image_size % 32 == 0 &&
+                 (!has_text || (cfg->context_length >= 1 && cfg->vocab_size >= 2)),
+             B200_ERR_INVALID, "clip_create_resnet: bad config (vision and patch must be zero, image_size a multiple of 32)");
+  int ndev = 0;
+  B200_CUDA(cudaGetDeviceCount(&ndev));
+  B200_CHECK(device >= 0 && device < ndev, B200_ERR_INVALID, "clip_create_resnet: device %d of %d", device, ndev);
+  DeviceGuard g(device);
+  b200_clip* m = new (std::nothrow) b200_clip();
+  B200_CHECK(m != nullptr, B200_ERR_OOM, "clip_create_resnet: host allocation failed");
+  m->cfg = *cfg;
+  m->device = device;
+  m->sms = sm_count(device);
+  m->has_text = has_text;
+  if (const char* e = getenv("B200_GRAPHS")) m->use_graphs = atoi(e) != 0;
+  m->rn = new (std::nothrow) ResNetTower();
+  int rc_ = m->rn == nullptr ? B200_ERR_OOM : B200_OK;
+  if (rc_ == B200_OK) rc_ = resnet_create(m->allocs, m->rn, *rc, cfg->image_size, cfg->embed_dim, cfg->max_batch);
+  if (rc_ == B200_OK) rc_ = make_text_and_staging(m);
+  if (rc_ != B200_OK) {
+    b200_clip_destroy(m);
+    return rc_;
+  }
+  *out = m;
+  return B200_OK;
+}
+
 int b200_clip_destroy(b200_clip* m) {
   if (!m) return B200_OK;
   DeviceGuard g(m->device);
   cudaDeviceSynchronize();
   m->allocs.free_all();
+  delete m->rn;
   for (auto& kv : m->graphs) if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
   if (m->cap_stream) cudaStreamDestroy(m->cap_stream);
   if (m->s_copy) {
@@ -284,24 +354,9 @@ int b200_clip_load_weights(b200_clip* m, const b200_tensor_view* tensors, int n)
   Loader ld;
   B200_TRY(ld.index(tensors, n));
   const b200_clip_config& c = m->cfg;
-  const size_t vw = c.vision.width, tw = c.text.width, D = c.embed_dim;
-  const size_t T = (size_t)m->grid * m->grid + 1, kraw = (size_t)3 * c.patch * c.patch;
-  B200_TRY(ld.put_bf16("visual.conv1.weight", m->conv.w, vw, kraw, m->Kp));
-  B200_TRY(ld.put_bf16("visual.positional_embedding", m->vpos, T, vw, vw));
-  {
-    const b200_tensor_view* cls = ld.find("visual.class_embedding", vw);
-    const b200_tensor_view* pos = ld.find("visual.positional_embedding", T * vw);
-    if (!cls || !pos) return B200_ERR_INVALID;
-    std::vector<float> v(vw);
-    for (size_t j = 0; j < vw; j++) v[j] = view_get(*cls, j) + view_get(*pos, j);
-    B200_CUDA(cudaMemcpy(m->cls_pos0, v.data(), vw * 4, cudaMemcpyHostToDevice));
-  }
-  B200_TRY(ld.put_f32("visual.ln_pre.weight", m->lnpre_g, vw));
-  B200_TRY(ld.put_f32("visual.ln_pre.bias", m->lnpre_b, vw));
-  B200_TRY(load_tower(ld, m->vis, "visual."));
-  B200_TRY(ld.put_f32("visual.ln_post.weight", m->vis.lnf_g, vw));
-  B200_TRY(ld.put_f32("visual.ln_post.bias", m->vis.lnf_b, vw));
-  B200_TRY(ld.put_bf16("visual.proj", m->vis.proj, vw, D, D));
+  const size_t tw = c.text.width, D = c.embed_dim;
+  if (m->rn) B200_TRY(resnet_load(ld, *m->rn));
+  else B200_TRY(load_vit(m, ld));
   if (m->has_text) {
     B200_TRY(ld.put_bf16("token_embedding.weight", m->tok_emb, (size_t)c.vocab_size, tw, tw));
     B200_TRY(ld.put_f32("positional_embedding", m->tpos, (size_t)c.context_length * tw));

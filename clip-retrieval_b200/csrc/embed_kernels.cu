@@ -243,7 +243,8 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
 __global__ void __launch_bounds__(256)
 pool_proj_split_kernel(const __nv_bfloat16* __restrict__ x, int T, int w, const int* __restrict__ pool_idx,
                        const float* __restrict__ gamma, const float* __restrict__ beta,
-                       const __nv_bfloat16* __restrict__ proj, int D, float* __restrict__ feat) {
+                       const __nv_bfloat16* __restrict__ proj, int D, const float* __restrict__ bias,
+                       float* __restrict__ feat) {
   extern __shared__ float sm[];
   float* s_row = sm;                // [w]
   float* s_part = sm + w;           // [4][64]
@@ -257,14 +258,16 @@ pool_proj_split_kernel(const __nv_bfloat16* __restrict__ x, int T, int w, const 
     s_row[j] = f;
     part += f;
   }
-  const float mean = block_sum(part, red) / (float)w;
-  part = 0.f;
-  for (int j = threadIdx.x; j < w; j += blockDim.x) {
-    const float dlt = s_row[j] - mean;
-    part += dlt * dlt;
+  if (gamma != nullptr) {   // null: the ResNet attention pool's c_proj, no LayerNorm
+    const float mean = block_sum(part, red) / (float)w;
+    part = 0.f;
+    for (int j = threadIdx.x; j < w; j += blockDim.x) {
+      const float dlt = s_row[j] - mean;
+      part += dlt * dlt;
+    }
+    const float rstd = rsqrtf(block_sum(part, red) / (float)w + 1e-5f);
+    for (int j = threadIdx.x; j < w; j += blockDim.x) s_row[j] = (s_row[j] - mean) * rstd * gamma[j] + beta[j];
   }
-  const float rstd = rsqrtf(block_sum(part, red) / (float)w + 1e-5f);
-  for (int j = threadIdx.x; j < w; j += blockDim.x) s_row[j] = (s_row[j] - mean) * rstd * gamma[j] + beta[j];
   __syncthreads();
   const int jj = threadIdx.x & 63, quarter = threadIdx.x >> 6;
   const int j = j0 + jj;
@@ -280,7 +283,10 @@ pool_proj_split_kernel(const __nv_bfloat16* __restrict__ x, int T, int w, const 
   }
   s_part[quarter * 64 + jj] = acc0 + acc1;
   __syncthreads();
-  if (quarter == 0 && j < D) feat[(size_t)b * D + j] = (s_part[jj] + s_part[64 + jj]) + (s_part[128 + jj] + s_part[192 + jj]);
+  if (quarter == 0 && j < D) {
+    const float f = (s_part[jj] + s_part[64 + jj]) + (s_part[128 + jj] + s_part[192 + jj]);
+    feat[(size_t)b * D + j] = bias != nullptr ? f + bias[j] : f;
+  }
 }
 
 __global__ void __launch_bounds__(256)
@@ -308,7 +314,21 @@ int pool_ln_proj_norm(const __nv_bfloat16* x, int T, int w, const int* pool_idx,
   if (B == 0) return B200_OK;
   const size_t smem = (size_t)(w + 256) * sizeof(float);
   B200_CHECK(smem <= 48 * 1024, B200_ERR_UNSUPPORTED, "pool_proj: width %d too large", w);
-  pool_proj_split_kernel<<<dim3((D + 63) / 64, B), 256, smem, st>>>(x, T, w, pool_idx, gamma, beta, proj, D, feat);
+  pool_proj_split_kernel<<<dim3((D + 63) / 64, B), 256, smem, st>>>(x, T, w, pool_idx, gamma, beta, proj, D, nullptr,
+                                                                     feat);
+  B200_LAUNCH_OK();
+  feat_norm_cast_kernel<<<B, 256, 0, st>>>(feat, D, out, out_f16, normalize);
+  B200_LAUNCH_OK();
+  return B200_OK;
+}
+
+int pool_proj_bias_norm(const __nv_bfloat16* x, int T, int w, const __nv_bfloat16* proj, const float* bias, int D,
+                        float* feat, void* out, int out_f16, int normalize, int B, cudaStream_t st) {
+  if (B == 0) return B200_OK;
+  const size_t smem = (size_t)(w + 256) * sizeof(float);
+  B200_CHECK(smem <= 48 * 1024, B200_ERR_UNSUPPORTED, "pool_proj: width %d too large", w);
+  pool_proj_split_kernel<<<dim3((D + 63) / 64, B), 256, smem, st>>>(x, T, w, nullptr, nullptr, nullptr, proj, D, bias,
+                                                                     feat);
   B200_LAUNCH_OK();
   feat_norm_cast_kernel<<<B, 256, 0, st>>>(feat, D, out, out_f16, normalize);
   B200_LAUNCH_OK();

@@ -40,6 +40,19 @@ int attention_wgmma(const CUtensorMap& tmQKV, __nv_bfloat16* out, int B, int T, 
 int pool_ln_proj_norm(const __nv_bfloat16* x, int T, int w, const int* pool_idx, const float* gamma, const float* beta,
                       const __nv_bfloat16* proj, int D, float* feat, void* out, int out_f16, int normalize, int B,
                       cudaStream_t st);
+// The same tail with the LayerNorm skipped and a bias added (the ResNet attention pool's c_proj on token 0):
+// feat[b] = x[b * T] @ proj [w, D] + bias[D], then normalise and cast as pool_ln_proj_norm does.
+int pool_proj_bias_norm(const __nv_bfloat16* x, int T, int w, const __nv_bfloat16* proj, const float* bias, int D,
+                        float* feat, void* out, int out_f16, int normalize, int B, cudaStream_t st);
+// ResNet image tower (conv.cu).  Stem gather: pixels fp32 NCHW [B, 3, S, S] -> bf16 [B * (S/2)^2, Kp], column
+// c * 9 + r * 3 + s = pixel (c, 2 oy - 1 + r, 2 ox - 1 + s) (zero outside the image), columns >= 27 not written.
+int stem_gather(const float* px, __nv_bfloat16* cols, int B, int S, int Kp, cudaStream_t st);
+// AvgPool2d(k) (floor mode) of NHWC bf16 [B, H, W, C] -> [B, H / k, W / k, C], fp32 sums; C a multiple of 8.
+int avgpool_nhwc(const __nv_bfloat16* in, __nv_bfloat16* out, int B, int H, int W, int C, int k, cudaStream_t st);
+// Attention-pool tokens: x [B * HW, C] -> out [B * (HW + 1), C]: token 0 the fp32 spatial mean, token t pixel t - 1,
+// each + pos[t] (fp32 [HW + 1, C]), rounded to bf16.
+int attnpool_tokens(const __nv_bfloat16* x, int B, int HW, int C, const float* pos, __nv_bfloat16* out,
+                    cudaStream_t st);
 // BERT-family embedding: x[b*T + t, :] = LN_eps((word[ids[b,t]] + tt0) + pos[pos_off + t]) in fp32, stored bf16
 // (HF's order of additions; tt0 = token-type row 0, or nullptr when the model has no token types).  word bf16
 // [vocab, w]; tt0, pos, gamma, beta fp32.  Ids outside [0, vocab) are clamped.

@@ -102,7 +102,7 @@ static int launch_bn_spec(const CUtensorMap& tmA, const CUtensorMap& tmB, int M,
   return B200_OK;
 }
 
-// the epilogue flavour (activation | residual << 2) fixed at compile time; gemm_bf16_launch has checked ep.act
+// the epilogue flavour (activation | residual << 2) fixed at compile time; gemm_bf16_launch has checked ep.act (0..3)
 template <int BN>
 static int launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, const GemmEpilogue& ep,
                      cudaStream_t st) {
@@ -110,9 +110,11 @@ static int launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int 
     case 0: return launch_bn_spec<BN, 0>(tmA, tmB, M, N, K, ep, st);
     case 1: return launch_bn_spec<BN, 1>(tmA, tmB, M, N, K, ep, st);
     case 2: return launch_bn_spec<BN, 2>(tmA, tmB, M, N, K, ep, st);
+    case 3: return launch_bn_spec<BN, 3>(tmA, tmB, M, N, K, ep, st);
     case 4: return launch_bn_spec<BN, 4>(tmA, tmB, M, N, K, ep, st);
     case 5: return launch_bn_spec<BN, 5>(tmA, tmB, M, N, K, ep, st);
-    default: return launch_bn_spec<BN, 6>(tmA, tmB, M, N, K, ep, st);
+    case 6: return launch_bn_spec<BN, 6>(tmA, tmB, M, N, K, ep, st);
+    default: return launch_bn_spec<BN, 7>(tmA, tmB, M, N, K, ep, st);
   }
 }
 
@@ -170,9 +172,11 @@ static int launch_wide(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, in
     case 0: return launch_wide_spec<0>(tmA, tmB, M, N, K, ep, st, force_tma);
     case 1: return launch_wide_spec<1>(tmA, tmB, M, N, K, ep, st, force_tma);
     case 2: return launch_wide_spec<2>(tmA, tmB, M, N, K, ep, st, force_tma);
+    case 3: return launch_wide_spec<3>(tmA, tmB, M, N, K, ep, st, force_tma);
     case 4: return launch_wide_spec<4>(tmA, tmB, M, N, K, ep, st, force_tma);
     case 5: return launch_wide_spec<5>(tmA, tmB, M, N, K, ep, st, force_tma);
-    default: return launch_wide_spec<6>(tmA, tmB, M, N, K, ep, st, force_tma);
+    case 6: return launch_wide_spec<6>(tmA, tmB, M, N, K, ep, st, force_tma);
+    default: return launch_wide_spec<7>(tmA, tmB, M, N, K, ep, st, force_tma);
   }
 }
 
@@ -184,7 +188,7 @@ int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int
              "gemm: output must be 16-byte aligned with ld %% 8 == 0");
   B200_CHECK(ep.residual == nullptr || (ep.res_ld % 8 == 0 && ((uintptr_t)ep.residual & 15) == 0), B200_ERR_INVALID,
              "gemm: residual must be 16-byte aligned with ld %% 8 == 0");
-  B200_CHECK(ep.act >= 0 && ep.act <= 2, B200_ERR_INVALID, "gemm: act=%d", ep.act);
+  B200_CHECK(ep.act >= 0 && ep.act <= ACT_RELU, B200_ERR_INVALID, "gemm: act=%d", ep.act);
   if (bn == GEMM_WIDE_BN) return launch_wide(tmA, tmB, M, N, K, ep, st, force_tma_epilogue);
   if (bn == 128) return launch_bn<128>(tmA, tmB, M, N, K, ep, st);
   if (bn == 64) return launch_bn<64>(tmA, tmB, M, N, K, ep, st);
@@ -199,9 +203,11 @@ using namespace b200;
 
 // The stand-alone entries: A [M, K] and W [N, K] contiguous, everything else as the epilogue says.  bn = 0 takes
 // gemm_pick_bn's width.
+// The public entries take activations 0..2: ACT_RELU is internal to the ResNet tower and its convolution entry.
 static int gemm_entry(const void* d_A, const void* d_W, int M, int N, int K, const GemmEpilogue& ep, int bn, int device,
                       void* stream, bool force_tma_epilogue = false) {
   B200_CHECK(d_A && d_W && ep.out, B200_ERR_INVALID, "gemm: null operand");
+  B200_CHECK(ep.act >= 0 && ep.act <= 2, B200_ERR_INVALID, "gemm: act=%d", ep.act);
   B200_CHECK(bn == 0 || bn == 32 || bn == 64 || bn == 128 || bn == GEMM_WIDE_BN, B200_ERR_INVALID, "gemm: unsupported column block %d", bn);
   DeviceGuard g(device);
   if (bn == 0) bn = gemm_pick_bn(M, N, sm_count(device));

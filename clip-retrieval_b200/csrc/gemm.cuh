@@ -26,11 +26,13 @@ constexpr int GEMM_THREADS = 288;  // warps 0..7: two consumer warpgroups (64 ro
 constexpr int GEMM_GROUP_M = 16;
 constexpr int GEMM_WARP_TMA = 8;
 
-enum { ACT_NONE = 0, ACT_QUICK_GELU = 1, ACT_GELU = 2 };
+// ACT_RELU is internal (the ResNet image tower): relu(acc + bias + residual), the residual added *before* the
+// activation.  The public GEMM entries accept 0..2 only.
+enum { ACT_NONE = 0, ACT_QUICK_GELU = 1, ACT_GELU = 2, ACT_RELU = 3 };
 
 struct GemmEpilogue {
   const float* bias = nullptr;              // [N] fp32 or null
-  const __nv_bfloat16* residual = nullptr;  // added after the activation, or null
+  const __nv_bfloat16* residual = nullptr;  // added after the activation (before it for ACT_RELU), or null
   int64_t res_ld = 0;                       // residual leading dimension (elements)
   int res_row_mod = 0;                      // > 0: residual row = res_row_off + row % res_row_mod
   int res_row_off = 0;
@@ -106,7 +108,9 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
 // act(pre) + residual, pre = accumulator + bias: the per-element arithmetic of every epilogue, rounded to bf16 by the
 // caller (pack_bf16x2).  __fadd_rn: never contracted with the activation's last multiply into an FMA — every epilogue
 // (either kernel, register or TMA store) rounds the same way and stays bit-identical to the others.
+// ACT_RELU: relu(pre + residual), the bottleneck block's `out += identity; out = relu(out)`.
 __device__ __forceinline__ float epi_apply(float pre, int act, bool has_res, float res) {
+  if (act == ACT_RELU) return fmaxf(has_res ? __fadd_rn(pre, res) : pre, 0.0f);
   const float v = act_apply(pre, act);
   return has_res ? __fadd_rn(v, res) : v;
 }
@@ -144,10 +148,17 @@ __device__ __forceinline__ void epi_chunk(const EpiRow& er, const uint32_t* r, c
   }
 }
 
-template <int BN, int SPEC>
-__global__ void __launch_bounds__(GEMM_THREADS, 2)
-gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N,
-                       int K, GemmEpilogue ep) {
+// Geometry of an implicit 3x3 stride-1 pad-1 convolution (conv.cu): the A operand is the NHWC activation [B, H, W, C]
+// read through an im2col tensor map, K = 9 * cb * 64 with k-block kbi = tap * cb + channel slice, tap = 3 r + s.
+struct ConvGeom {
+  int H = 0, W = 0, cb = 0;   // cb = ceil(C / 64)
+};
+
+// The 128-row tile of one CTA.  CONV: the producer's A box is one im2col load (128 output pixels x 64 channels of one
+// tap, borders and channels >= C zero-filled by TMA) instead of a 128 x 64 tile of A; everything else is shared.
+template <int BN, int SPEC, bool CONV>
+__device__ __forceinline__ void gemm_bf16_wgmma_tile(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K,
+                                                     const GemmEpilogue& ep, const ConvGeom& cg) {
   using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
@@ -185,7 +196,17 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
         const int stage = kbi % STAGES;
         if (kbi >= STAGES) ptx::mbar_wait(&empty[stage], ((kbi / STAGES) - 1) & 1);
         ptx::mbar_arrive_expect_tx(&full[stage], Cfg::STAGE_BYTES);
-        ptx::tma_load_2d(sA + stage * Cfg::A_BYTES, &tmA, &full[stage], kbi * GEMM_BK, m_blk * GEMM_BM);
+        if constexpr (CONV) {
+          // output pixel m_blk * 128 = (n, h, w): the box starts at input pixel (h - 1, w - 1) of image n, the tap's
+          // (r, s) offset is added to every pixel of it; rows run on across image rows and images
+          const int tap = kbi / cg.cb, cs = kbi - tap * cg.cb;
+          const int m0 = m_blk * GEMM_BM, hw = cg.H * cg.W;
+          const int n = m0 / hw, rem = m0 - n * hw, h = rem / cg.W, w = rem - h * cg.W;
+          ptx::tma_load_im2col_4d(sA + stage * Cfg::A_BYTES, &tmA, &full[stage], cs * GEMM_BK, w - 1, h - 1, n,
+                                  (uint16_t)(tap % 3), (uint16_t)(tap / 3));
+        } else {
+          ptx::tma_load_2d(sA + stage * Cfg::A_BYTES, &tmA, &full[stage], kbi * GEMM_BK, m_blk * GEMM_BM);
+        }
         ptx::tma_load_2d(sB + stage * Cfg::B_BYTES, &tmB, &full[stage], kbi * GEMM_BK, n0);
       }
     }
@@ -260,6 +281,22 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     }
     epi_chunk<SPEC>(er, r, s_bias, c, n0, N, res[ci]);
   }
+}
+
+template <int BN, int SPEC>
+__global__ void __launch_bounds__(GEMM_THREADS, 2)
+gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N,
+                       int K, GemmEpilogue ep) {
+  gemm_bf16_wgmma_tile<BN, SPEC, false>(tmA, tmB, M, N, K, ep, ConvGeom());
+}
+
+// Implicit-GEMM 3x3 convolution (stride 1, pad 1): out[B*H*W, N] = epilogue(im2col(x) · W^T), W packed [N, 9 * cb * 64]
+// (conv.cu).  tmA is an im2col map over x [B, H, W, C] (make_tmap_im2col_3x3).
+template <int BN, int SPEC>
+__global__ void __launch_bounds__(GEMM_THREADS, 2)
+conv3x3_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N,
+                          int K, GemmEpilogue ep, ConvGeom cg) {
+  gemm_bf16_wgmma_tile<BN, SPEC, true>(tmA, tmB, M, N, K, ep, cg);
 }
 
 // ---- persistent 128 x 256 tiles for the large-batch shapes ----------------------------------------------------
@@ -565,13 +602,22 @@ int make_tmap_2d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t row
                  uint32_t box_rows, uint32_t box_cols);
 int make_tmap_3d(CUtensorMap* out, const void* ptr, int dtype_bf16, uint64_t planes, uint64_t rows, uint64_t cols,
                  uint64_t ld_row, uint64_t ld_plane, uint32_t box_rows, uint32_t box_cols);
+// [B, H, W, C] bf16 NHWC activations (C a multiple of 8) seen through an im2col map for the 3x3 pad-1 convolution:
+// boxes of 128 pixels x 64 channels, 128B swizzle (the layout of a 128 x 64 tiled A box), zero fill outside.
+int make_tmap_im2col_3x3(CUtensorMap* out, const void* ptr, int B, int H, int W, int C);
 // tmB must have boxes of bn rows x 64 columns (128 rows for bn = 256).  The epilogue flavour (activation | residual
-// << 2) is a template argument of the kernel: ep.act outside 0..2 is B200_ERR_INVALID.  bn = 256 (the persistent
+// << 2) is a template argument of the kernel: ep.act outside 0..3 is B200_ERR_INVALID (the public entries take 0..2).  bn = 256 (the persistent
 // kernel) stores by TMA from 8 tiles per CTA up (or with force_tma_epilogue), else from registers.
 int gemm_bf16_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int M, int N, int K,
                      const GemmEpilogue& ep, cudaStream_t st, bool force_tma_epilogue = false);
 // Pick the column-block width for a GEMM with N output columns: 256 (persistent kernel) for large grids, else 128,
 // or 64 / 32 when the grid would be under-filled.
 int gemm_pick_bn(int M, int N, int sms);
+// The implicit 3x3 convolution: tmA from make_tmap_im2col_3x3 over [>= B, H, W, C], tmB over W [N, 9 * cb * 64] with
+// boxes of bn rows x 64 columns (bn 32, 64 or 128), M = B * H * W.
+int conv3x3_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, int M, int N, const ConvGeom& cg,
+                   const GemmEpilogue& ep, cudaStream_t st);
+// Column-block width of the convolution: 128, or 64 / 32 when the grid would be under-filled.
+int conv_pick_bn(int M, int N, int sms);
 
 }  // namespace b200

@@ -68,6 +68,18 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// 4-D im2col load (tensor map from cuTensorMapEncodeIm2col over [N, H, W, C]): coordinates (c, w, h, n) of the first
+// pixel of the box, then pixels in the map's bounding box in (w, h, n) order; the offsets (ow, oh) are added to every
+// pixel's (w, h).  Pixels and channels outside the tensor are written as zeros.
+__device__ __forceinline__ void tma_load_im2col_4d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int32_t c,
+                                                   int32_t w, int32_t h, int32_t n, uint16_t ow, uint16_t oh) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
+      "[%2], {%7, %8};"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c), "r"(w), "r"(h), "r"(n),
+      "h"(ow), "h"(oh)
+      : "memory");
+}
 // 1-D bulk copy of `bytes` (a multiple of 16; both addresses 16-byte aligned) from global to shared memory, counted
 // against `bar`'s transaction bytes.
 __device__ __forceinline__ void bulk_load(uint32_t smem_dst, const void* src, uint32_t bytes, uint64_t* bar) {

@@ -82,8 +82,45 @@ G14_ARCHS = {
     "open_clip:ViT-g-14": ClipArch(*_G14, quick_gelu=False),          # laion2b_s12b_b42k, laion2b_s34b_b88k
     "open_clip:ViT-bigG-14": ClipArch(*_BIGG14, quick_gelu=False),    # laion2b_s39b_b160k
 }
+
+
+@dataclass(frozen=True)
+class ResNetArch:
+    """OpenAI's ModifiedResNet image tower (include/b200clip.h b200_clip_create_resnet) with the CLIP text tower:
+    `layers` Bottleneck blocks per stage, stem width `width` (stage i has planes width * 2^i), and an attention pool of
+    32 * width channels in heads of 64."""
+    embed_dim: int
+    image_size: int
+    layers: tuple
+    width: int
+    text: Tower
+    context_length: int = 77
+    vocab_size: int = 49408
+    quick_gelu: bool = True
+
+    @property
+    def heads(self):
+        return 32 * self.width // 64
+
+
+# OpenAI's five ResNet CLIPs (clip.load names; open_clip serves the same towers as `open_clip:RN50[-quickgelu]/{openai,
+# yfcc15m,cc12m}`, `open_clip:RN101[-quickgelu]/{openai,yfcc15m}`, `open_clip:RN50x{4,16,64}/openai`).  Configs recalled
+# from OpenAI's and open_clip's model configs, not read from either (DESIGN.md §5 (xviii)).  Kept apart from ARCHS and
+# G14_ARCHS, whose entries are ViTs; resolve_arch reads all three.
+_RN = {
+    "RN50": (1024, 224, (3, 4, 6, 3), 64, Tower(512, 12, 8, 2048)),
+    "RN101": (512, 224, (3, 4, 23, 3), 64, Tower(512, 12, 8, 2048)),
+    "RN50x4": (640, 288, (4, 6, 10, 6), 80, Tower(640, 12, 10, 2560)),
+    "RN50x16": (768, 384, (6, 8, 18, 8), 96, Tower(768, 12, 12, 3072)),
+    "RN50x64": (1024, 448, (3, 15, 36, 10), 128, Tower(1024, 12, 16, 4096)),
+}
+RESNET_ARCHS = {}
+for _k, _a in _RN.items():
+    RESNET_ARCHS[_k] = ResNetArch(*_a, quick_gelu=True)                   # bare names -> OpenAI clip.load
+    RESNET_ARCHS["open_clip:" + _k] = ResNetArch(*_a, quick_gelu=False)   # QuickGELU with `-quickgelu` / `openai`
+
 # Every architecture a `clip_model` name can resolve to.
-KNOWN_ARCHS = {**ARCHS, **G14_ARCHS}
+KNOWN_ARCHS = {**ARCHS, **G14_ARCHS, **RESNET_ARCHS}
 
 # `hf_clip:<repo>` names -> (architecture key, quick_gelu): HuggingFace CLIPModel checkpoints of the same towers.
 HF_REPOS = {
@@ -170,6 +207,8 @@ def synthetic_state_dict(arch, seed=0):
         return torch.randn(*shape, generator=g, dtype=torch.float32) * std
 
     sd = {}
+    if isinstance(arch, ResNetArch):
+        _resnet_visual(sd, arch, rn, g)
 
     def tower(prefix, t):
         w, L = t.width, t.layers
@@ -188,17 +227,19 @@ def synthetic_state_dict(arch, seed=0):
             sd[p + "mlp.c_proj.weight"] = rn(w, t.mlp, std=(w ** -0.5) * ((2 * L) ** -0.5))
             sd[p + "mlp.c_proj.bias"] = rn(w, std=0.02)
 
-    v, t = arch.vision, arch.text
-    grid = arch.image_size // arch.patch
-    sd["visual.conv1.weight"] = rn(v.width, 3, arch.patch, arch.patch, std=(3 * arch.patch ** 2) ** -0.5)
-    sd["visual.class_embedding"] = rn(v.width, std=v.width ** -0.5)
-    sd["visual.positional_embedding"] = rn(grid * grid + 1, v.width, std=v.width ** -0.5)
-    sd["visual.ln_pre.weight"] = 1.0 + rn(v.width, std=0.1)
-    sd["visual.ln_pre.bias"] = rn(v.width, std=0.05)
-    tower("visual.", v)
-    sd["visual.ln_post.weight"] = 1.0 + rn(v.width, std=0.1)
-    sd["visual.ln_post.bias"] = rn(v.width, std=0.05)
-    sd["visual.proj"] = rn(v.width, arch.embed_dim, std=v.width ** -0.5)
+    t = arch.text
+    if not isinstance(arch, ResNetArch):
+        v = arch.vision
+        grid = arch.image_size // arch.patch
+        sd["visual.conv1.weight"] = rn(v.width, 3, arch.patch, arch.patch, std=(3 * arch.patch ** 2) ** -0.5)
+        sd["visual.class_embedding"] = rn(v.width, std=v.width ** -0.5)
+        sd["visual.positional_embedding"] = rn(grid * grid + 1, v.width, std=v.width ** -0.5)
+        sd["visual.ln_pre.weight"] = 1.0 + rn(v.width, std=0.1)
+        sd["visual.ln_pre.bias"] = rn(v.width, std=0.05)
+        tower("visual.", v)
+        sd["visual.ln_post.weight"] = 1.0 + rn(v.width, std=0.1)
+        sd["visual.ln_post.bias"] = rn(v.width, std=0.05)
+        sd["visual.proj"] = rn(v.width, arch.embed_dim, std=v.width ** -0.5)
     sd["token_embedding.weight"] = rn(arch.vocab_size, t.width, std=0.02)
     sd["positional_embedding"] = rn(arch.context_length, t.width, std=0.01)
     tower("", t)
@@ -206,6 +247,54 @@ def synthetic_state_dict(arch, seed=0):
     sd["ln_final.bias"] = rn(t.width, std=0.05)
     sd["text_projection"] = rn(t.width, arch.embed_dim, std=t.width ** -0.5)
     return sd
+
+
+def _resnet_visual(sd, arch, rn, g):
+    """visual.* of a ResNetArch in OpenAI's key layout: He-scaled convolutions, and BatchNorm layers with non-trivial
+    affine and running statistics (so a forward that skips or misplaces the fold is visibly wrong).  bn3 of each block
+    is scaled down (OpenAI zero-initialises it) so that the residual stream stays O(1) at depth."""
+    torch = _torch()
+    w = arch.width
+
+    def conv(name, cout, cin, k):
+        sd[name + ".weight"] = rn(cout, cin, k, k, std=(2.0 / (cin * k * k)) ** 0.5)
+
+    def bn(name, n, gain=1.0):
+        sd[name + ".weight"] = gain * (1.0 + rn(n, std=0.2))
+        sd[name + ".bias"] = rn(n, std=0.1)
+        sd[name + ".running_mean"] = rn(n, std=0.2)
+        sd[name + ".running_var"] = 0.5 + torch.rand(n, generator=g)
+        sd[name + ".num_batches_tracked"] = torch.tensor(1000, dtype=torch.int64)
+
+    conv("visual.conv1", w // 2, 3, 3)
+    bn("visual.bn1", w // 2)
+    conv("visual.conv2", w // 2, w // 2, 3)
+    bn("visual.bn2", w // 2)
+    conv("visual.conv3", w, w // 2, 3)
+    bn("visual.bn3", w)
+    cin = w
+    for s, n in enumerate(arch.layers):
+        planes = w << s
+        for j in range(n):
+            p = "visual.layer%d.%d." % (s + 1, j)
+            conv(p + "conv1", planes, cin, 1)
+            bn(p + "bn1", planes)
+            conv(p + "conv2", planes, planes, 3)
+            bn(p + "bn2", planes)
+            conv(p + "conv3", 4 * planes, planes, 1)
+            bn(p + "bn3", 4 * planes, gain=0.3)
+            if (j == 0 and s > 0) or cin != 4 * planes:
+                conv(p + "downsample.0", 4 * planes, cin, 1)
+                bn(p + "downsample.1", 4 * planes)
+            cin = 4 * planes
+    C, T = 32 * w, (arch.image_size // 32) ** 2 + 1
+    a = "visual.attnpool."
+    sd[a + "positional_embedding"] = rn(T, C, std=C ** -0.5)
+    for n in ("q", "k", "v"):
+        sd[a + n + "_proj.weight"] = rn(C, C, std=C ** -0.5)
+        sd[a + n + "_proj.bias"] = rn(C, std=0.02)
+    sd[a + "c_proj.weight"] = rn(arch.embed_dim, C, std=C ** -0.5)
+    sd[a + "c_proj.bias"] = rn(arch.embed_dim, std=0.02)
 
 
 def convert_hf_state_dict(sd, arch):
@@ -252,6 +341,16 @@ class B200Clip:
         self.max_batch = int(max_batch)
         self._h = C.c_void_p()
         self._lock = threading.Lock()
+        if isinstance(arch, ResNetArch):
+            cfg = _lib.ClipConfigC(
+                arch.embed_dim, arch.image_size, 0, _lib.TowerConfigC(0, 0, 0, 0), arch.context_length, arch.vocab_size,
+                _lib.TowerConfigC(arch.text.width, arch.text.layers, arch.text.heads, arch.text.mlp),
+                1 if arch.quick_gelu else 0, self.max_batch,
+            )
+            rc = _lib.ResNetConfigC((C.c_int32 * 4)(*arch.layers), arch.width, arch.heads)
+            check(lib.b200_clip_create_resnet(C.byref(cfg), C.byref(rc), self.device_index, C.byref(self._h)),
+                  "clip_create_resnet")
+            return
         cfg = _lib.ClipConfigC(
             arch.embed_dim, arch.image_size, arch.patch,
             _lib.TowerConfigC(arch.vision.width, arch.vision.layers, arch.vision.heads, arch.vision.mlp),

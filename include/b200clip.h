@@ -299,6 +299,19 @@ typedef struct b200_tensor_view {
  * allocated, context_length and vocab_size are not read, load_weights needs only the visual.* tensors, and the
  * encode_text entries return B200_ERR_UNSUPPORTED. */
 int b200_clip_create(const b200_clip_config* cfg, int device, b200_clip** out);
+/* OpenAI's ResNet CLIPs (RN50, RN101, RN50x4, RN50x16, RN50x64; ModifiedResNet): the image tower is a stem of three
+ * 3x3 convolutions and an average pool, four stages of Bottleneck blocks (layers[i] blocks, planes width * 2^i, stride
+ * 1, 2, 2, 2 taken by average pools), and an attention pool of `heads` heads of 64 over the (S/32)^2 pixels plus their
+ * mean.  `cfg` supplies the text tower, embed_dim, image_size (a multiple of 32), quick_gelu and max_batch; its
+ * `vision` and `patch` must be zero.  load_weights reads the visual.* keys of OpenAI's state_dict (BatchNorm running
+ * statistics folded into the convolutions in fp64, eps 1e-5; num_batches_tracked is ignored).  Every other
+ * b200_clip_* entry works on the handle unchanged. */
+typedef struct b200_resnet_config {
+  int32_t layers[4];   /* Bottleneck blocks per stage */
+  int32_t width;       /* stem width w: planes of stage i are w * 2^i, the attention pool has 32 w channels */
+  int32_t heads;       /* attention-pool heads: 32 w / 64 */
+} b200_resnet_config;
+int b200_clip_create_resnet(const b200_clip_config* cfg, const b200_resnet_config* rc, int device, b200_clip** out);
 int b200_clip_destroy(b200_clip* m);
 /* Upload weights given as a state_dict in the open_clip/OpenAI key layout; converts to the
  * packed bf16 device layout.  Missing or mis-shaped tensors are an error. */
@@ -381,6 +394,28 @@ int b200_token_argmax_device(const int64_t* d_tokens, int B, int T, int32_t* d_i
 int b200_pool_ln_proj_device(const void* d_x, int B, int T, int w, const int32_t* d_pool_idx, const float* d_gamma,
                              const float* d_beta, const void* d_proj, int D, float* d_feat, void* d_out, int out_dtype,
                              int normalize, int device, void* stream);
+/* The kernels of the ResNet image tower, for their parity tests.
+ * Convolution: d_x NHWC bf16 [B, H, W, C] (C a multiple of 8) -> d_out [B * H * W, N] rows (ld ep->out_ld, 0 = N):
+ *   ksize 3: stride 1, pad 1, as an implicit GEMM (im2col TMA loads, no im2col buffer); d_w bf16 [N, 9 * C64] with
+ *            C64 = ceil(C / 64) * 64, column (3 r + s) * C64 + c = weight[n, c, r, s], zero in the padding columns;
+ *            bn 0 (the library's pick), 32, 64 or 128.
+ *   ksize 1: the GEMM of the rows, d_w [N, C]; bn as for b200_gemm_bf16_ex_device (256: the persistent kernel).
+ *   The epilogue is b200_gemm_epilogue without row maps (out_group and res_row_mod 0); act 0 none or 3 relu, which
+ *   computes relu(acc + bias + residual) with the residual added before the activation (ksize 1 also takes 1, 2).
+ *   The kernel is conv3x3_bf16_wgmma_kernel.
+ * Stem gather: d_pixels fp32 NCHW [B, 3, S, S] (S even) -> d_cols bf16 [B * (S/2)^2, 64], row b (S/2)^2 + oy S/2 + ox,
+ *   column c * 9 + r * 3 + s = pixel (c, 2 oy - 1 + r, 2 ox - 1 + s), zero outside the image; columns 27..63 are not
+ *   written.
+ * Average pool: NHWC bf16 [B, H, W, C] -> [B, H / k, W / k, C] (floor), fp32 sum of each k x k window / k^2, C a
+ *   multiple of 8.
+ * Attention-pool tokens: d_x bf16 [B * HW, C] -> d_out bf16 [B * (HW + 1), C]: row b (HW + 1) = fp32 mean of the HW
+ *   rows of sample b + d_pos[0], row b (HW + 1) + t = row b HW + t - 1 + d_pos[t] (d_pos fp32 [HW + 1, C]). */
+int b200_conv_bf16_device(const void* d_x, int B, int H, int W, int C, const void* d_w, int N, int ksize, void* d_out,
+                          const b200_gemm_epilogue* ep, int bn, int device, void* stream);
+int b200_stem_gather_device(const float* d_pixels, int B, int S, void* d_cols, int device, void* stream);
+int b200_avgpool_bf16_device(const void* d_in, int B, int H, int W, int C, int k, void* d_out, int device, void* stream);
+int b200_attnpool_tokens_device(const void* d_x, int B, int HW, int C, const float* d_pos, void* d_out, int device,
+                                void* stream);
 /* ------------------------------------------------------------------------------------------
  * Multilingual text towers (use_mclip).  Replaces the M-CLIP text model of the query service
  * (clip_back.py:222-224,836-859: XLM-RoBERTa-Large + mean pool + LinearTransformation) and the
