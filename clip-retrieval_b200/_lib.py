@@ -161,6 +161,7 @@ PROTOTYPES = {
     "b200_nccl_comm_destroy": (_i, [_vp]),
     "b200_clip_create": (_i, [C.POINTER(ClipConfigC), _i, C.POINTER(_vp)]),
     "b200_clip_create_resnet": (_i, [C.POINTER(ClipConfigC), C.POINTER(ResNetConfigC), _i, C.POINTER(_vp)]),
+    "b200_clip_create_siglip": (_i, [C.POINTER(ClipConfigC), _i, C.POINTER(_vp)]),
     "b200_clip_destroy": (_i, [_vp]),
     "b200_clip_load_weights": (_i, [_vp, C.POINTER(TensorViewC), _i]),
     "b200_clip_encode_image_device": (_i, [_vp, _vp, _i, _vp, _i, _i, _vp]),
@@ -181,6 +182,9 @@ PROTOTYPES = {
     "b200_stem_gather_device": (_i, [_vp, _i, _i, _vp, _i, _vp]),
     "b200_avgpool_bf16_device": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     "b200_attnpool_tokens_device": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp]),
+    "b200_latent_pool_attention_device": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _i, _vp]),
+    "b200_pool_last_ln_proj_bias_device": (_i, [_vp, _i, _i, _i, _vp, _vp, C.c_float, _vp, _vp, _i, _vp, _vp, _i, _i, _i,
+                                                _vp]),
     "b200_index_last_hi_only_fallbacks": (_i, [_vp]),
     "b200_index_last_scan_plan": (_i, [_vp, _vp]),
     "b200_kmeans_train_f16": (_i, [_vp, _i64, _i, _i, _i, C.c_uint64, _i, _vp, _vp, _i]),

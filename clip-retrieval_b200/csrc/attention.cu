@@ -6,9 +6,10 @@
 // Per-sample key lengths (len[b] in 1..T) as in attention_wgmma.cu: keys >= len[b] are staged as zeros and masked,
 // the key loop stops at the 32-key block holding len[b] - 1, and rows >= len[b] are written as zeros.
 // Shapes whose whole-head K + V would pass 200 KB run on attention_stream_kernel below, with the same per-block step.
-// Head dims 88 and 104 (ViT-g-14, ViT-bigG-14: HD % 16 == 8) take the same kernels with an 8-wide tail at every step:
-// the last Q fragment's upper half is zero registers (columns HD.. of the qkv row are the next head's Q, or K), QK^T
-// ends with one 8-dim k-step, P.V with one unpaired n8 tile, and the K/V rows are padded to HD + 16 (att_lds).
+// Head dims 72, 88 and 104 (SigLIP-SO400M, ViT-g-14, ViT-bigG-14: HD % 16 == 8) take the same kernels with an 8-wide
+// tail at every step: the last Q fragment's upper half is zero registers (columns HD.. of the qkv row are the next
+// head's Q, or K), QK^T ends with one 8-dim k-step, P.V with one unpaired n8 tile, and the K/V rows are padded to
+// HD + 16 (att_lds).
 #include "embed_kernels.cuh"
 #include "ptx.cuh"
 
@@ -40,7 +41,8 @@ constexpr int ATT_KB = 32;  // keys per inner block
 
 // Padded K/V row in shared memory (elements): an odd number of 16-byte chunks, so that the 8 rows of an ldmatrix
 // 8x8 block fall in distinct bank groups.  HD + 8 for HD % 16 == 0 (144 B / 176 B / 208 B / 272 B rows at 64 / 80 / 96
-// / 128), HD + 16 for HD % 16 == 8 (208 B / 240 B at 88 / 104; HD + 8 would give an even 12 / 14 chunks).
+// / 128), HD + 16 for HD % 16 == 8 (176 B / 208 B / 240 B at 72 / 88 / 104; HD + 8 would give an even 10 / 12 / 14
+// chunks).
 __host__ __device__ constexpr int att_lds(int hd) { return hd % 16 == 0 ? hd + 8 : hd + 16; }
 // k16 Q fragments per row pair: the last one of HD % 16 == 8 holds dims HD-8..HD-1 and zero registers above.
 __host__ __device__ constexpr int att_qfrags(int hd) { return (hd + 15) / 16; }
@@ -122,7 +124,7 @@ __device__ __forceinline__ void attention_block_step(uint32_t sK_u, uint32_t sV_
       mma_bf16_16816(s[nt], qa[(HD / 32) * 2], b0, b1);
     }
     if constexpr (HD % 16 == 8) {
-      // 8-wide tail k-step (HD = 88, 104): d = HD-8 .. HD-1 against the zero-topped last Q fragment; the K operand's
+      // 8-wide tail k-step (HD = 72, 88, 104): d = HD-8 .. HD-1 against the zero-topped last Q fragment; the K operand's
       // upper half is a zero register too, so the shared-memory padding never enters the sum
       mma_bf16_16816(s[nt], qa[HD / 16], kt[nt], 0u);
     }
@@ -249,8 +251,8 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
     *reinterpret_cast<uint4*>(ob + (size_t)(i / CPR) * w + (i % CPR) * 8) = make_uint4(0u, 0u, 0u, 0u);
 }
 
-// Longer sequences (whole-head K + V past 200 KB of shared memory: T > 704 / 576 / 480 / 352 at head dim 64 / 80 /
-// 96 / 128): one CTA per (128-row query chunk, head, sample), chunk fastest so that the chunks of a head read its K/V
+// Longer sequences (whole-head K + V past 200 KB of shared memory: T > 704 / 576 / 576 / 480 / 352 at head dim 64 / 72 /
+// 80 / 96 / 128): one CTA per (128-row query chunk, head, sample), chunk fastest so that the chunks of a head read its K/V
 // from L2.  Eight warps own 16 query rows each; K and V pass through a ring of ATS_STAGES blocks of 64 keys, filled
 // by warp 0 with one bulk copy per row (rows padded to att_lds(HD) elements as above) and handed over by full / empty
 // mbarriers, so shared memory no longer grows with T.  The arithmetic per 32-key block is attention_block_step.
@@ -400,12 +402,13 @@ int attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int T, int he
   if (B == 0) return B200_OK;
   const int hd = w / heads;
   if (hd == 64) return launch_attention<64>(qkv, out, B, T, heads, w, causal, st, len);
+  if (hd == 72) return launch_attention<72>(qkv, out, B, T, heads, w, causal, st, len);
   if (hd == 80) return launch_attention<80>(qkv, out, B, T, heads, w, causal, st, len);
   if (hd == 88) return launch_attention<88>(qkv, out, B, T, heads, w, causal, st, len);
   if (hd == 96) return launch_attention<96>(qkv, out, B, T, heads, w, causal, st, len);
   if (hd == 104) return launch_attention<104>(qkv, out, B, T, heads, w, causal, st, len);
   if (hd == 128) return launch_attention<128>(qkv, out, B, T, heads, w, causal, st, len);
-  set_error("attention: head dimension %d not supported (64, 80, 88, 96, 104, 128)", hd);
+  set_error("attention: head dimension %d not supported (64, 72, 80, 88, 96, 104, 128)", hd);
   return B200_ERR_UNSUPPORTED;
 }
 

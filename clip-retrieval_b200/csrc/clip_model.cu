@@ -28,8 +28,19 @@ struct Layer {
   Linear qkv, out, fc, proj;
 };
 
+// How a tower turns its last residual stream into features.
+enum Pool {
+  POOL_FIRST = 0,    // LN(row 0) @ proj (CLIP image tower: the class token)
+  POOL_EOT = 1,      // LN(row argmax(tokens)) @ proj (CLIP text tower)
+  POOL_LAST = 2,     // LN(row T - 1) @ proj + proj_b (SigLIP text tower)
+  POOL_LATENT = 3,   // LN over every row, then the latent-query attention-pool head (SigLIP image tower)
+};
+
 struct Tower {
   int width = 0, layers = 0, heads = 0, mlp = 0, T = 0;
+  float ln_eps = 1e-5f;        // every LayerNorm of the tower, its final one included
+  int causal = 0;
+  int pool = POOL_FIRST;
   std::vector<Layer> L;
   // activations
   __nv_bfloat16 *x = nullptr, *h = nullptr, *qkv = nullptr, *a = nullptr, *f = nullptr;
@@ -37,6 +48,15 @@ struct Tower {
   CUtensorMap tm_qkv;          // make_qkv_map over max_batch samples, built when the wgmma attention takes the tower
   float *lnf_g = nullptr, *lnf_b = nullptr;  // ln_post / ln_final
   __nv_bfloat16* proj = nullptr;             // [width, D]
+  float* proj_b = nullptr;                   // [D] (POOL_LAST) or null
+};
+
+// SigLIP's image head (timm AttentionPoolLatent): out = y + fc2(gelu(fc1(LN(y)))) with y = proj(attn(q, kv(LN(x)))),
+// where q = q_proj(latent) is input-independent and computed once at load time.
+struct LatentHead {
+  Linear kv, proj, fc1, fc2;   // [2w, w], [w, w], [mlp, w], [w, mlp], all with biases
+  float* q = nullptr;          // [w] fp32
+  float *ln_g = nullptr, *ln_b = nullptr;
 };
 
 constexpr int GRAPH_MAX_B = 8;   // forwards of at most this many samples are replayed from a captured graph
@@ -53,13 +73,15 @@ struct b200_clip {
   bool has_text = true;       // false: an image-only handle (all-zero text tower config), no text weights or buffers
   b200::Tower vis, txt;
   b200::ResNetTower* rn = nullptr;   // the ResNet image tower (b200_clip_create_resnet) in place of vis and its front
+  bool siglip = false;               // b200_clip_create_siglip: timm/open_clip SigLIP towers
+  b200::LatentHead head;             // SigLIP's image head
   // vision front end
   int grid = 0, Kp = 0;
   b200::Linear conv;          // [w, Kp]
   __nv_bfloat16* cols = nullptr;  // [max_batch*g*g, Kp]
   CUtensorMap tm_cols;
   __nv_bfloat16* vpos = nullptr;  // positional_embedding bf16 [T, w] (residual operand of the patch GEMM)
-  float* cls_pos0 = nullptr;      // class_embedding + positional_embedding[0]
+  float* cls_pos0 = nullptr;      // class_embedding + positional_embedding[0] (not SigLIP)
   float *lnpre_g = nullptr, *lnpre_b = nullptr;
   // text front end
   __nv_bfloat16* tok_emb = nullptr;  // [vocab, w]
@@ -123,21 +145,21 @@ static int run_linear(b200_clip* m, const CUtensorMap& tmA, const Linear& l, int
   return linear_gemm(l, tmA, M, ep, m->sms, st);
 }
 
-static int run_blocks(b200_clip* m, Tower& t, int B, int causal, cudaStream_t st) {
+static int run_blocks(b200_clip* m, Tower& t, int B, cudaStream_t st) {
   const int w = t.width;
   const int M = B * t.T;
   const int act = m->cfg.quick_gelu ? ACT_QUICK_GELU : ACT_GELU;
   for (auto& L : t.L) {
     { TimedSpan sp(m->timer, CLS_LN, st, 1);
-      B200_TRY(layernorm_rows(t.x, w, t.h, w, L.ln1_g, L.ln1_b, M, w, st)); }
+      B200_TRY(layernorm_rows_eps(t.x, w, t.h, w, L.ln1_g, L.ln1_b, M, w, t.ln_eps, st)); }
     GemmEpilogue e1; e1.out = t.qkv; e1.out_ld = 3 * w;
     B200_TRY(run_linear(m, t.tm_h, L.qkv, M, e1, st, CLS_G_QKV));
     { TimedSpan sp(m->timer, CLS_ATTN, st, 1);
-      B200_TRY(qkv_attention(&t.tm_qkv, t.qkv, t.a, B, t.T, t.heads, w, causal, st)); }
+      B200_TRY(qkv_attention(&t.tm_qkv, t.qkv, t.a, B, t.T, t.heads, w, t.causal, st)); }
     GemmEpilogue e2; e2.out = t.x; e2.out_ld = w; e2.residual = t.x; e2.res_ld = w;
     B200_TRY(run_linear(m, t.tm_a, L.out, M, e2, st, CLS_G_OUT));
     { TimedSpan sp(m->timer, CLS_LN, st, 1);
-      B200_TRY(layernorm_rows(t.x, w, t.h, w, L.ln2_g, L.ln2_b, M, w, st)); }
+      B200_TRY(layernorm_rows_eps(t.x, w, t.h, w, L.ln2_g, L.ln2_b, M, w, t.ln_eps, st)); }
     GemmEpilogue e3; e3.out = t.f; e3.out_ld = t.mlp; e3.act = act;
     B200_TRY(run_linear(m, t.tm_h, L.fc, M, e3, st, CLS_G_FC));
     GemmEpilogue e4; e4.out = t.x; e4.out_ld = w; e4.residual = t.x; e4.res_ld = w;
@@ -146,11 +168,44 @@ static int run_blocks(b200_clip* m, Tower& t, int B, int causal, cudaStream_t st
   return B200_OK;
 }
 
+// SigLIP image tower: patch GEMM with its bias and the positional rows as the residual (no class row, no ln_pre),
+// the blocks, LN of every row, then the latent attention-pool head on M = B rows.
+static int encode_image_chunk_siglip(b200_clip* m, const float* d_px, int B, void* d_out, int out_f16, int normalize,
+                                     cudaStream_t st) {
+  Tower& t = m->vis;
+  LatentHead& hd = m->head;
+  const int g = m->grid, w = t.width, T = t.T;
+  { TimedSpan sp(m->timer, CLS_OTHER, st, 1);
+    B200_TRY(im2col_patches(d_px, m->cols, B, m->cfg.image_size, m->cfg.patch, m->Kp, st)); }
+  GemmEpilogue ep; ep.out = t.x; ep.out_ld = w;
+  ep.residual = m->vpos; ep.res_ld = w; ep.res_row_mod = g * g; ep.res_row_off = 0;
+  B200_TRY(run_linear(m, m->tm_cols, m->conv, B * T, ep, st, CLS_GEMM));
+  B200_TRY(run_blocks(m, t, B, st));
+  { TimedSpan sp(m->timer, CLS_LN, st, 1);
+    B200_TRY(layernorm_rows_eps(t.x, w, t.h, w, t.lnf_g, t.lnf_b, (int64_t)B * T, w, t.ln_eps, st)); }
+  GemmEpilogue e1; e1.out = t.qkv; e1.out_ld = 2 * w;
+  B200_TRY(run_linear(m, t.tm_h, hd.kv, B * T, e1, st, CLS_GEMM));
+  { TimedSpan sp(m->timer, CLS_ATTN, st, 1);
+    B200_TRY(latent_pool_attention(t.qkv, hd.q, t.a, B, T, t.heads, w, st)); }
+  GemmEpilogue e2; e2.out = t.x; e2.out_ld = w;
+  B200_TRY(run_linear(m, t.tm_a, hd.proj, B, e2, st, CLS_GEMM));
+  { TimedSpan sp(m->timer, CLS_LN, st, 1);
+    B200_TRY(layernorm_rows_eps(t.x, w, t.h, w, hd.ln_g, hd.ln_b, B, w, t.ln_eps, st)); }
+  GemmEpilogue e3; e3.out = t.f; e3.out_ld = t.mlp; e3.act = ACT_GELU;
+  B200_TRY(run_linear(m, t.tm_h, hd.fc1, B, e3, st, CLS_GEMM));
+  GemmEpilogue e4; e4.out = t.x; e4.out_ld = w; e4.residual = t.x; e4.res_ld = w;
+  B200_TRY(run_linear(m, t.tm_f, hd.fc2, B, e4, st, CLS_GEMM));
+  { TimedSpan sp(m->timer, CLS_OTHER, st, 1);
+    B200_TRY(rows_feat_norm_cast(t.x, w, m->feat, d_out, out_f16, normalize, B, st)); }
+  return B200_OK;
+}
+
 static int encode_image_chunk(b200_clip* m, const float* d_px, int B, void* d_out, int out_f16, int normalize,
                               cudaStream_t st) {
   if (m->rn)
     return resnet_encode(*m->rn, m->timer, CLS_GEMM, CLS_ATTN, CLS_OTHER, m->sms, d_px, B, m->feat, d_out, out_f16,
                          normalize, st);
+  if (m->siglip) return encode_image_chunk_siglip(m, d_px, B, d_out, out_f16, normalize, st);
   Tower& t = m->vis;
   const int g = m->grid, w = t.width, T = t.T;
   { TimedSpan sp(m->timer, CLS_OTHER, st, 2);
@@ -162,7 +217,7 @@ static int encode_image_chunk(b200_clip* m, const float* d_px, int B, void* d_ou
   B200_TRY(run_linear(m, m->tm_cols, m->conv, B * g * g, ep, st, CLS_GEMM));
   { TimedSpan sp(m->timer, CLS_LN, st, 1);
     B200_TRY(layernorm_rows(t.x, w, t.x, w, m->lnpre_g, m->lnpre_b, (int64_t)B * T, w, st)); }
-  B200_TRY(run_blocks(m, t, B, 0, st));
+  B200_TRY(run_blocks(m, t, B, st));
   { TimedSpan sp(m->timer, CLS_OTHER, st, 1);
     B200_TRY(pool_ln_proj_norm(t.x, T, w, nullptr, t.lnf_g, t.lnf_b, t.proj, m->cfg.embed_dim, m->feat, d_out, out_f16, normalize, B, st)); }
   return B200_OK;
@@ -172,10 +227,18 @@ static int encode_text_chunk(b200_clip* m, const int64_t* d_tok, int B, void* d_
                              cudaStream_t st) {
   Tower& t = m->txt;
   const int w = t.width, T = t.T;
+  if (t.pool == POOL_LAST) {
+    { TimedSpan sp(m->timer, CLS_OTHER, st, 1);
+      B200_TRY(text_embed(d_tok, m->tok_emb, m->tpos, t.x, B, T, w, m->cfg.vocab_size, st)); }
+    B200_TRY(run_blocks(m, t, B, st));
+    TimedSpan sp(m->timer, CLS_OTHER, st, 2);
+    return pool_last_ln_proj_bias_norm(t.x, T, w, t.lnf_g, t.lnf_b, t.ln_eps, t.proj, t.proj_b, m->cfg.embed_dim,
+                                       m->feat, d_out, out_f16, normalize, B, st);
+  }
   { TimedSpan sp(m->timer, CLS_OTHER, st, 2);
     B200_TRY(text_embed(d_tok, m->tok_emb, m->tpos, t.x, B, T, w, m->cfg.vocab_size, st));
     B200_TRY(token_argmax(d_tok, m->pool_idx, B, T, st)); }
-  B200_TRY(run_blocks(m, t, B, 1, st));
+  B200_TRY(run_blocks(m, t, B, st));
   { TimedSpan sp(m->timer, CLS_OTHER, st, 1);
     B200_TRY(pool_ln_proj_norm(t.x, T, w, m->pool_idx, t.lnf_g, t.lnf_b, t.proj, m->cfg.embed_dim, m->feat, d_out, out_f16, normalize, B, st)); }
   return B200_OK;
@@ -209,6 +272,8 @@ static int make_text_and_staging(b200_clip* m) {
   DeviceAllocs& al = m->allocs;
   if (m->has_text) {
     B200_TRY(make_tower(m, &m->txt, cfg->text, cfg->context_length, cfg->embed_dim));
+    m->txt.causal = 1;
+    m->txt.pool = POOL_EOT;
     B200_TRY(al.alloc(&m->tok_emb, (size_t)cfg->vocab_size * cfg->text.width));
     B200_TRY(al.alloc(&m->tpos, (size_t)cfg->context_length * cfg->text.width));
     B200_TRY(al.alloc(&m->pool_idx, (size_t)cfg->max_batch));
@@ -246,6 +311,71 @@ static int load_vit(b200_clip* m, Loader& ld) {
   B200_TRY(ld.put_f32("visual.ln_post.weight", m->vis.lnf_g, vw));
   B200_TRY(ld.put_f32("visual.ln_post.bias", m->vis.lnf_b, vw));
   B200_TRY(ld.put_bf16("visual.proj", m->vis.proj, vw, D, D));
+  return B200_OK;
+}
+
+// SigLIP's tensors in open_clip's layout: the timm trunk under visual.trunk.*, the text tower under text.*.
+static int load_siglip(b200_clip* m, Loader& ld) {
+  const b200_clip_config& c = m->cfg;
+  const size_t w = c.vision.width, mlp = c.vision.mlp, T = m->vis.T, kraw = (size_t)3 * c.patch * c.patch;
+  const std::string v = "visual.trunk.";
+  B200_TRY(ld.put_bf16(v + "patch_embed.proj.weight", m->conv.w, w, kraw, m->Kp));
+  B200_TRY(ld.put_f32(v + "patch_embed.proj.bias", m->conv.b, w));
+  B200_TRY(ld.put_bf16(v + "pos_embed", m->vpos, T, w, w));
+  for (int i = 0; i < m->vis.layers; i++) {
+    Layer& L = m->vis.L[i];
+    const std::string p = v + "blocks." + std::to_string(i) + ".";
+    B200_TRY(ld.put_f32(p + "norm1.weight", L.ln1_g, w));
+    B200_TRY(ld.put_f32(p + "norm1.bias", L.ln1_b, w));
+    B200_TRY(ld.put_bf16(p + "attn.qkv.weight", L.qkv.w, 3 * w, w, w));
+    B200_TRY(ld.put_f32(p + "attn.qkv.bias", L.qkv.b, 3 * w));
+    B200_TRY(ld.put_bf16(p + "attn.proj.weight", L.out.w, w, w, w));
+    B200_TRY(ld.put_f32(p + "attn.proj.bias", L.out.b, w));
+    B200_TRY(ld.put_f32(p + "norm2.weight", L.ln2_g, w));
+    B200_TRY(ld.put_f32(p + "norm2.bias", L.ln2_b, w));
+    B200_TRY(ld.put_bf16(p + "mlp.fc1.weight", L.fc.w, mlp, w, w));
+    B200_TRY(ld.put_f32(p + "mlp.fc1.bias", L.fc.b, mlp));
+    B200_TRY(ld.put_bf16(p + "mlp.fc2.weight", L.proj.w, w, mlp, mlp));
+    B200_TRY(ld.put_f32(p + "mlp.fc2.bias", L.proj.b, w));
+  }
+  B200_TRY(ld.put_f32(v + "norm.weight", m->vis.lnf_g, w));
+  B200_TRY(ld.put_f32(v + "norm.bias", m->vis.lnf_b, w));
+  const std::string a = v + "attn_pool.";
+  LatentHead& hd = m->head;
+  {
+    // q = q_proj(latent) in fp64 from the checkpoint's values, stored fp32
+    const b200_tensor_view* lat = ld.find(a + "latent", w);
+    const b200_tensor_view* qw = ld.find(a + "q.weight", w * w);
+    const b200_tensor_view* qb = ld.find(a + "q.bias", w);
+    if (!lat || !qw || !qb) return B200_ERR_INVALID;
+    std::vector<float> q(w);
+    for (size_t i = 0; i < w; i++) {
+      double acc = view_get(*qb, i);
+      for (size_t j = 0; j < w; j++) acc += (double)view_get(*qw, i * w + j) * (double)view_get(*lat, j);
+      q[i] = (float)acc;
+    }
+    B200_CUDA(cudaMemcpy(hd.q, q.data(), w * 4, cudaMemcpyHostToDevice));
+  }
+  B200_TRY(ld.put_bf16(a + "kv.weight", hd.kv.w, 2 * w, w, w));
+  B200_TRY(ld.put_f32(a + "kv.bias", hd.kv.b, 2 * w));
+  B200_TRY(ld.put_bf16(a + "proj.weight", hd.proj.w, w, w, w));
+  B200_TRY(ld.put_f32(a + "proj.bias", hd.proj.b, w));
+  B200_TRY(ld.put_f32(a + "norm.weight", hd.ln_g, w));
+  B200_TRY(ld.put_f32(a + "norm.bias", hd.ln_b, w));
+  B200_TRY(ld.put_bf16(a + "mlp.fc1.weight", hd.fc1.w, mlp, w, w));
+  B200_TRY(ld.put_f32(a + "mlp.fc1.bias", hd.fc1.b, mlp));
+  B200_TRY(ld.put_bf16(a + "mlp.fc2.weight", hd.fc2.w, w, mlp, mlp));
+  B200_TRY(ld.put_f32(a + "mlp.fc2.bias", hd.fc2.b, w));
+  if (m->has_text) {
+    const size_t tw = c.text.width, D = c.embed_dim;
+    B200_TRY(ld.put_bf16("text.token_embedding.weight", m->tok_emb, (size_t)c.vocab_size, tw, tw));
+    B200_TRY(ld.put_f32("text.positional_embedding", m->tpos, (size_t)c.context_length * tw));
+    B200_TRY(load_tower(ld, m->txt, "text."));
+    B200_TRY(ld.put_f32("text.ln_final.weight", m->txt.lnf_g, tw));
+    B200_TRY(ld.put_f32("text.ln_final.bias", m->txt.lnf_b, tw));
+    B200_TRY(ld.put_bf16_t("text.text_projection.weight", m->txt.proj, D, tw));
+    B200_TRY(ld.put_f32("text.text_projection.bias", m->txt.proj_b, D));
+  }
   return B200_OK;
 }
 
@@ -332,6 +462,69 @@ int b200_clip_create_resnet(const b200_clip_config* cfg, const b200_resnet_confi
   return B200_OK;
 }
 
+// SigLIP (open_clip's timm-trunk configs): the ViT handle with no class row and no ln_pre, a patch bias, the latent
+// attention-pool head, a bidirectional text tower pooled at its last position with a biased projection, and LayerNorm
+// eps 1e-6 everywhere.
+int b200_clip_create_siglip(const b200_clip_config* cfg, int device, b200_clip** out) {
+  B200_CHECK(cfg && out, B200_ERR_INVALID, "clip_create_siglip: null argument");
+  const bool has_text = cfg->text.width != 0 || cfg->text.layers != 0 || cfg->text.heads != 0 || cfg->text.mlp != 0;
+  B200_CHECK(cfg->max_batch >= 1 && cfg->patch >= 1 && cfg->image_size >= cfg->patch && cfg->vision.heads >= 1 &&
+                 cfg->embed_dim == cfg->vision.width && cfg->quick_gelu == 0 &&
+                 (!has_text || (cfg->context_length >= 1 && cfg->vocab_size >= 2)),
+             B200_ERR_INVALID, "clip_create_siglip: bad config (embed_dim must equal the vision width, quick_gelu 0)");
+  int ndev = 0;
+  B200_CUDA(cudaGetDeviceCount(&ndev));
+  B200_CHECK(device >= 0 && device < ndev, B200_ERR_INVALID, "clip_create_siglip: device %d of %d", device, ndev);
+  DeviceGuard g(device);
+  b200_clip* m = new (std::nothrow) b200_clip();
+  B200_CHECK(m != nullptr, B200_ERR_OOM, "clip_create_siglip: host allocation failed");
+  m->cfg = *cfg;
+  m->device = device;
+  m->sms = sm_count(device);
+  m->has_text = has_text;
+  m->siglip = true;
+  if (const char* e = getenv("B200_GRAPHS")) m->use_graphs = atoi(e) != 0;
+  m->grid = cfg->image_size / cfg->patch;
+  m->Kp = (3 * cfg->patch * cfg->patch + 63) / 64 * 64;
+  const int T = m->grid * m->grid;
+  auto build = [&]() -> int {
+    const int w = cfg->vision.width;
+    B200_TRY(make_tower(m, &m->vis, cfg->vision, T, cfg->embed_dim));
+    m->vis.ln_eps = 1e-6f;
+    m->vis.pool = POOL_LATENT;
+    DeviceAllocs& al = m->allocs;
+    B200_TRY(make_linear(al, &m->conv, w, m->Kp, true));
+    const size_t prow = (size_t)cfg->max_batch * T;
+    B200_TRY(al.alloc(&m->cols, prow * m->Kp));
+    B200_CUDA(cudaMemset(m->cols, 0, prow * m->Kp * 2));
+    B200_TRY(make_tmap_2d(&m->tm_cols, m->cols, 1, prow, m->Kp, m->Kp, GEMM_BM, GEMM_BK));
+    B200_TRY(al.alloc(&m->vpos, (size_t)T * w));
+    LatentHead& hd = m->head;
+    B200_TRY(make_linear(al, &hd.kv, 2 * w, w, true));
+    B200_TRY(make_linear(al, &hd.proj, w, w, true));
+    B200_TRY(make_linear(al, &hd.fc1, cfg->vision.mlp, w, true));
+    B200_TRY(make_linear(al, &hd.fc2, w, cfg->vision.mlp, true));
+    B200_TRY(al.alloc(&hd.q, (size_t)w));
+    B200_TRY(al.alloc(&hd.ln_g, (size_t)w));
+    B200_TRY(al.alloc(&hd.ln_b, (size_t)w));
+    B200_TRY(make_text_and_staging(m));
+    if (has_text) {
+      m->txt.ln_eps = 1e-6f;
+      m->txt.causal = 0;
+      m->txt.pool = POOL_LAST;
+      B200_TRY(al.alloc(&m->txt.proj_b, (size_t)cfg->embed_dim));
+    }
+    return B200_OK;
+  };
+  const int rc = build();
+  if (rc != B200_OK) {
+    b200_clip_destroy(m);
+    return rc;
+  }
+  *out = m;
+  return B200_OK;
+}
+
 int b200_clip_destroy(b200_clip* m) {
   if (!m) return B200_OK;
   DeviceGuard g(m->device);
@@ -355,6 +548,12 @@ int b200_clip_load_weights(b200_clip* m, const b200_tensor_view* tensors, int n)
   B200_TRY(ld.index(tensors, n));
   const b200_clip_config& c = m->cfg;
   const size_t tw = c.text.width, D = c.embed_dim;
+  if (m->siglip) {
+    B200_TRY(load_siglip(m, ld));
+    B200_CUDA(cudaDeviceSynchronize());
+    m->loaded = true;
+    return B200_OK;
+  }
   if (m->rn) B200_TRY(resnet_load(ld, *m->rn));
   else B200_TRY(load_vit(m, ld));
   if (m->has_text) {
@@ -558,6 +757,26 @@ int b200_pool_ln_proj_device(const void* d_x, int B, int T, int w, const int32_t
   DeviceGuard g(device);
   return pool_ln_proj_norm((const __nv_bfloat16*)d_x, T, w, d_pool_idx, d_gamma, d_beta, (const __nv_bfloat16*)d_proj,
                            D, d_feat, d_out, out_dtype == B200_OUT_F16, normalize, B, (cudaStream_t)stream);
+}
+
+int b200_latent_pool_attention_device(const void* d_kv, int B, int T, int heads, int w, const float* d_q, void* d_out,
+                                      int device, void* stream) {
+  B200_CHECK(B >= 0 && T >= 1 && (B == 0 || (d_kv && d_q && d_out)), B200_ERR_INVALID, "latent_pool: bad argument");
+  DeviceGuard g(device);
+  return latent_pool_attention((const __nv_bfloat16*)d_kv, d_q, (__nv_bfloat16*)d_out, B, T, heads, w,
+                               (cudaStream_t)stream);
+}
+int b200_pool_last_ln_proj_bias_device(const void* d_x, int B, int T, int w, const float* d_gamma, const float* d_beta,
+                                       float eps, const void* d_proj, const float* d_bias, int D, float* d_feat,
+                                       void* d_out, int out_dtype, int normalize, int device, void* stream) {
+  B200_CHECK(B >= 0 && T >= 1 && w >= 1 && D >= 1 && eps > 0.f &&
+                 (B == 0 || (d_x && d_gamma && d_beta && d_proj && d_bias && d_feat && d_out)) &&
+                 (out_dtype == B200_OUT_F16 || out_dtype == B200_OUT_F32),
+             B200_ERR_INVALID, "pool_last_ln_proj_bias: bad argument");
+  DeviceGuard g(device);
+  return pool_last_ln_proj_bias_norm((const __nv_bfloat16*)d_x, T, w, d_gamma, d_beta, eps,
+                                     (const __nv_bfloat16*)d_proj, d_bias, D, d_feat, d_out,
+                                     out_dtype == B200_OUT_F16, normalize, B, (cudaStream_t)stream);
 }
 
 int b200_clip_set_profiling(b200_clip* m, int on) {

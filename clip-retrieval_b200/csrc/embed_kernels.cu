@@ -289,6 +289,51 @@ pool_proj_split_kernel(const __nv_bfloat16* __restrict__ x, int T, int w, const 
   }
 }
 
+// SigLIP's text tail, pool_proj_split_kernel's arithmetic on the last row of each sample (the tower attends
+// bidirectionally over every position, pads included, and pools position T - 1), with LayerNorm at `eps` and a bias.
+__global__ void __launch_bounds__(256)
+pool_last_proj_split_kernel(const __nv_bfloat16* __restrict__ x, int T, int w, const float* __restrict__ gamma,
+                            const float* __restrict__ beta, float eps, const __nv_bfloat16* __restrict__ proj, int D,
+                            const float* __restrict__ bias, float* __restrict__ feat) {
+  extern __shared__ float sm[];
+  float* s_row = sm;                // [w]
+  float* s_part = sm + w;           // [4][64]
+  __shared__ float red[8];
+  const int b = blockIdx.y, j0 = blockIdx.x * 64;
+  const __nv_bfloat16* src = x + ((size_t)b * T + T - 1) * w;
+  float part = 0.f;
+  for (int j = threadIdx.x; j < w; j += blockDim.x) {
+    const float f = __bfloat162float(src[j]);
+    s_row[j] = f;
+    part += f;
+  }
+  const float mean = block_sum(part, red) / (float)w;
+  part = 0.f;
+  for (int j = threadIdx.x; j < w; j += blockDim.x) {
+    const float dlt = s_row[j] - mean;
+    part += dlt * dlt;
+  }
+  const float rstd = rsqrtf(block_sum(part, red) / (float)w + eps);
+  for (int j = threadIdx.x; j < w; j += blockDim.x) s_row[j] = (s_row[j] - mean) * rstd * gamma[j] + beta[j];
+  __syncthreads();
+  const int jj = threadIdx.x & 63, quarter = threadIdx.x >> 6;
+  const int j = j0 + jj;
+  const int per = (w + 3) / 4, i0 = quarter * per, i1 = min(w, i0 + per);
+  float acc0 = 0.f, acc1 = 0.f;
+  if (j < D) {
+    int i = i0;
+    for (; i + 1 < i1; i += 2) {
+      acc0 = fmaf(s_row[i], __bfloat162float(proj[(size_t)i * D + j]), acc0);
+      acc1 = fmaf(s_row[i + 1], __bfloat162float(proj[(size_t)(i + 1) * D + j]), acc1);
+    }
+    if (i < i1) acc0 = fmaf(s_row[i], __bfloat162float(proj[(size_t)i * D + j]), acc0);
+  }
+  s_part[quarter * 64 + jj] = acc0 + acc1;
+  __syncthreads();
+  if (quarter == 0 && j < D)
+    feat[(size_t)b * D + j] = ((s_part[jj] + s_part[64 + jj]) + (s_part[128 + jj] + s_part[192 + jj])) + bias[j];
+}
+
 __global__ void __launch_bounds__(256)
 feat_norm_cast_kernel(const float* __restrict__ feat, int D, void* __restrict__ out, int out_f16, int normalize) {
   __shared__ float red[8];
@@ -318,6 +363,49 @@ int pool_ln_proj_norm(const __nv_bfloat16* x, int T, int w, const int* pool_idx,
                                                                      feat);
   B200_LAUNCH_OK();
   feat_norm_cast_kernel<<<B, 256, 0, st>>>(feat, D, out, out_f16, normalize);
+  B200_LAUNCH_OK();
+  return B200_OK;
+}
+
+int pool_last_ln_proj_bias_norm(const __nv_bfloat16* x, int T, int w, const float* gamma, const float* beta, float eps,
+                                const __nv_bfloat16* proj, const float* bias, int D, float* feat, void* out, int out_f16,
+                                int normalize, int B, cudaStream_t st) {
+  if (B == 0) return B200_OK;
+  const size_t smem = (size_t)(w + 256) * sizeof(float);
+  B200_CHECK(smem <= 48 * 1024, B200_ERR_UNSUPPORTED, "pool_proj: width %d too large", w);
+  pool_last_proj_split_kernel<<<dim3((D + 63) / 64, B), 256, smem, st>>>(x, T, w, gamma, beta, eps, proj, D, bias,
+                                                                          feat);
+  B200_LAUNCH_OK();
+  feat_norm_cast_kernel<<<B, 256, 0, st>>>(feat, D, out, out_f16, normalize);
+  B200_LAUNCH_OK();
+  return B200_OK;
+}
+
+// feat[b] = x[b] (bf16 -> fp32), then normalised and cast as feat_norm_cast_kernel does.
+__global__ void __launch_bounds__(256)
+rows_feat_norm_cast_kernel(const __nv_bfloat16* __restrict__ x, int D, float* __restrict__ feat,
+                           void* __restrict__ out, int out_f16, int normalize) {
+  __shared__ float red[8];
+  const int b = blockIdx.x;
+  float part = 0.f;
+  for (int j = threadIdx.x; j < D; j += blockDim.x) {
+    const float v = __bfloat162float(x[(size_t)b * D + j]);
+    feat[(size_t)b * D + j] = v;
+    part += v * v;
+  }
+  const float ss = block_sum(part, red);
+  const float inv = normalize ? 1.0f / sqrtf(ss) : 1.0f;
+  for (int j = threadIdx.x; j < D; j += blockDim.x) {
+    const float v = __bfloat162float(x[(size_t)b * D + j]) * inv;
+    if (out_f16) reinterpret_cast<__half*>(out)[(size_t)b * D + j] = __float2half_rn(v);
+    else reinterpret_cast<float*>(out)[(size_t)b * D + j] = v;
+  }
+}
+
+int rows_feat_norm_cast(const __nv_bfloat16* x, int D, float* feat, void* out, int out_f16, int normalize, int B,
+                        cudaStream_t st) {
+  if (B == 0) return B200_OK;
+  rows_feat_norm_cast_kernel<<<B, 256, 0, st>>>(x, D, feat, out, out_f16, normalize);
   B200_LAUNCH_OK();
   return B200_OK;
 }

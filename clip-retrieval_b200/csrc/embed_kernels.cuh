@@ -21,7 +21,7 @@ int layernorm_rows(const __nv_bfloat16* in, int64_t in_ld, __nv_bfloat16* out, i
 int layernorm_rows_eps(const __nv_bfloat16* in, int64_t in_ld, __nv_bfloat16* out, int64_t out_ld, const float* gamma,
                        const float* beta, int64_t rows, int w, float eps, cudaStream_t st);
 // K4: multi-head attention over the fused qkv buffer [B*T, 3w] -> out [B*T, w]; causal for text.  mma.sync kernels
-// (attention.cu) for the head dimensions the wgmma kernel does not take (80, 88, 96, 104, 128) and for head dim 64 past
+// (attention.cu) for the head dimensions the wgmma kernel does not take (72, 80, 88, 96, 104, 128) and for head dim 64 past
 // T = 320:
 // whole K/V of a head in shared memory while it fits in 200 KB, K/V streamed through a ring of 64-key stages beyond.
 // len (device int32 [B], values 1..T, or nullptr = T): sample b attends to its keys < len[b], and its rows >= len[b]
@@ -44,6 +44,20 @@ int pool_ln_proj_norm(const __nv_bfloat16* x, int T, int w, const int* pool_idx,
 // feat[b] = x[b * T] @ proj [w, D] + bias[D], then normalise and cast as pool_ln_proj_norm does.
 int pool_proj_bias_norm(const __nv_bfloat16* x, int T, int w, const __nv_bfloat16* proj, const float* bias, int D,
                         float* feat, void* out, int out_f16, int normalize, int B, cudaStream_t st);
+// SigLIP's text tail: feat[b] = LN_eps(x[b * T + T - 1]) @ proj [w, D] + bias[D], then normalise and cast as
+// pool_ln_proj_norm does.
+int pool_last_ln_proj_bias_norm(const __nv_bfloat16* x, int T, int w, const float* gamma, const float* beta, float eps,
+                                const __nv_bfloat16* proj, const float* bias, int D, float* feat, void* out, int out_f16,
+                                int normalize, int B, cudaStream_t st);
+// feat fp32 [B, D] = x bf16 [B, D], then normalise and cast as pool_ln_proj_norm does (the SigLIP image tower, whose
+// attention-pool head ends in a GEMM).
+int rows_feat_norm_cast(const __nv_bfloat16* x, int D, float* feat, void* out, int out_f16, int normalize, int B,
+                        cudaStream_t st);
+// SigLIP's latent-query attention pool (latent_pool.cu): kv bf16 [B * T, 2w] (k | v, heads of hd = w / heads),
+// q fp32 [w] -> out bf16 [B, w] with out[b, h hd + j] = sum_t softmax_t(q_h . k_{b,t,h} hd^-0.5) v_{b,t,h,j}; scores,
+// softmax and sums in fp32.  hd a multiple of 8, at most 128.
+int latent_pool_attention(const __nv_bfloat16* kv, const float* q, __nv_bfloat16* out, int B, int T, int heads, int w,
+                          cudaStream_t st);
 // ResNet image tower (conv.cu).  Stem gather: pixels fp32 NCHW [B, 3, S, S] -> bf16 [B * (S/2)^2, Kp], column
 // c * 9 + r * 3 + s = pixel (c, 2 oy - 1 + r, 2 ox - 1 + s) (zero outside the image), columns >= 27 not written.
 int stem_gather(const float* px, __nv_bfloat16* cols, int B, int S, int Kp, cudaStream_t st);

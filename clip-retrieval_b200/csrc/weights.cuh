@@ -59,6 +59,16 @@ struct Loader {
     B200_CUDA(cudaMemcpy(dst, tmp16.data(), tmp16.size() * 2, cudaMemcpyHostToDevice));
     return B200_OK;
   }
+  // dst bf16 [rows, cols] <- the transpose of src [cols, rows] (a Linear weight into the [in, out] layout)
+  int put_bf16_t(const std::string& name, __nv_bfloat16* dst, size_t src_rows, size_t src_cols) {
+    const b200_tensor_view* v = find(name, src_rows * src_cols);
+    if (!v) return B200_ERR_INVALID;
+    tmp16.assign(src_rows * src_cols, 0);
+    for (size_t r = 0; r < src_rows; r++)
+      for (size_t c = 0; c < src_cols; c++) tmp16[c * src_rows + r] = f32_to_bf16_rn(view_get(*v, r * src_cols + c));
+    B200_CUDA(cudaMemcpy(dst, tmp16.data(), tmp16.size() * 2, cudaMemcpyHostToDevice));
+    return B200_OK;
+  }
   int put_f32(const std::string& name, float* dst, size_t count) {
     const b200_tensor_view* v = find(name, count);
     if (!v) return B200_ERR_INVALID;

@@ -12,11 +12,11 @@ With `use_mclip=True` the captions go through the multilingual encoder of `mclip
 Extension (SURVEY §8(f) row 1): when the batch carries `image_rgb8` (a list of decoded uint8 HWC
 images of any size — what a reader yields if its `preprocess` is `to_rgb8` instead of the torchvision
 transform) instead of `image_tensor`, Resize/CenterCrop/ToTensor/Normalize run on the GPU
-(`B200Preprocess`, bit-exact with the host transform, including its resize mode: `model.preprocess_mode`) and
-feed the image tower in place.
+(`B200Preprocess`, bit-exact with the host transform, including its resize mode, mean and std:
+`model.preprocess_params`) and feed the image tower in place.
 """
 from .mclip import build_mclip
-from .model import load_clip, preprocess_mode
+from .model import load_clip, preprocess_params
 from .preprocess import B200Preprocess
 
 
@@ -53,7 +53,7 @@ class ClipMapper:
             clip_cache_path=clip_cache_path,
         )
         self.model = model
-        self._resize_mode = preprocess_mode(clip_model)
+        self._resize_mode, self._mean, self._std = preprocess_params(clip_model)
         self.model_img = model.encode_image
         self.model_txt = model.encode_text
         self._gpu_preprocess = None
@@ -67,7 +67,8 @@ class ClipMapper:
         if self.enable_image:
             if "image_tensor" not in item and "image_rgb8" in item:
                 if self._gpu_preprocess is None:
-                    self._gpu_preprocess = B200Preprocess(self.model.arch.image_size, resize_mode=self._resize_mode)
+                    self._gpu_preprocess = B200Preprocess(self.model.arch.image_size, mean=self._mean, std=self._std,
+                                                          resize_mode=self._resize_mode)
                 image_embs = self.model.embed_image(self._gpu_preprocess(item["image_rgb8"]))
             else:
                 image_embs = self.model.embed_image(item["image_tensor"])

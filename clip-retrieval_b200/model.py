@@ -119,8 +119,44 @@ for _k, _a in _RN.items():
     RESNET_ARCHS[_k] = ResNetArch(*_a, quick_gelu=True)                   # bare names -> OpenAI clip.load
     RESNET_ARCHS["open_clip:" + _k] = ResNetArch(*_a, quick_gelu=False)   # QuickGELU with `-quickgelu` / `openai`
 
+
+@dataclass(frozen=True)
+class SigLIPArch:
+    """Google's SigLIP as open_clip builds it (include/b200clip.h b200_clip_create_siglip): a timm ViT image tower with
+    a latent-query attention pool and no projection (embed_dim == vision.width), and a bidirectional text tower pooled
+    at its last position with a biased projection.  LayerNorm eps 1e-6 and erf GELU throughout.  `tokenizer` names
+    the HuggingFace repository folder whose tokenizer.json the model uses."""
+    embed_dim: int
+    image_size: int
+    patch: int
+    vision: Tower
+    text: Tower
+    context_length: int = 64
+    vocab_size: int = 32000
+    tokenizer: str = "timm/ViT-B-16-SigLIP"
+    quick_gelu: bool = False
+
+
+# open_clip's SigLIP configs (pretrained tag `webli`), recalled from open_clip's model configs, not read
+# (DESIGN.md §5 (xix)).  Kept apart from ARCHS, G14_ARCHS and RESNET_ARCHS; resolve_arch reads all four.
+_SIG_B = Tower(768, 12, 12, 3072)
+_SIG_L = Tower(1024, 24, 16, 4096)
+_SIG_SO = Tower(1152, 27, 16, 4304)
+SIGLIP_ARCHS = {
+    "open_clip:ViT-B-16-SigLIP": SigLIPArch(768, 224, 16, _SIG_B, _SIG_B),
+    "open_clip:ViT-B-16-SigLIP-256": SigLIPArch(768, 256, 16, _SIG_B, _SIG_B),
+    "open_clip:ViT-B-16-SigLIP-384": SigLIPArch(768, 384, 16, _SIG_B, _SIG_B),
+    "open_clip:ViT-B-16-SigLIP-512": SigLIPArch(768, 512, 16, _SIG_B, _SIG_B),
+    "open_clip:ViT-B-16-SigLIP-i18n-256": SigLIPArch(768, 256, 16, _SIG_B, _SIG_B, vocab_size=250000,
+                                                     tokenizer="timm/ViT-B-16-SigLIP-i18n-256"),
+    "open_clip:ViT-L-16-SigLIP-256": SigLIPArch(1024, 256, 16, _SIG_L, _SIG_L),
+    "open_clip:ViT-L-16-SigLIP-384": SigLIPArch(1024, 384, 16, _SIG_L, _SIG_L),
+    "open_clip:ViT-SO400M-14-SigLIP": SigLIPArch(1152, 224, 14, _SIG_SO, _SIG_SO, context_length=16),
+    "open_clip:ViT-SO400M-14-SigLIP-384": SigLIPArch(1152, 384, 14, _SIG_SO, _SIG_SO),
+}
+
 # Every architecture a `clip_model` name can resolve to.
-KNOWN_ARCHS = {**ARCHS, **G14_ARCHS, **RESNET_ARCHS}
+KNOWN_ARCHS = {**ARCHS, **G14_ARCHS, **RESNET_ARCHS, **SIGLIP_ARCHS}
 
 # `hf_clip:<repo>` names -> (architecture key, quick_gelu): HuggingFace CLIPModel checkpoints of the same towers.
 HF_REPOS = {
@@ -181,6 +217,11 @@ def resolve_arch(clip_model):
         if pretrained == "openai":
             quick = True
         key = "open_clip:" + arch_name
+        if key in SIGLIP_ARCHS:
+            if quick or pretrained not in ("", "webli"):
+                raise ValueError("%r: SigLIP models take erf GELU and the `webli` weights only (no -quickgelu, no "
+                                 "`openai` tag)" % (clip_model,))
+            return SIGLIP_ARCHS[key], key
         if key not in KNOWN_ARCHS:
             raise ValueError("unknown clip_model %r; known: %s" % (clip_model, ", ".join(sorted(KNOWN_ARCHS))))
         return replace(KNOWN_ARCHS[key], quick_gelu=quick), key + ("-quickgelu" if quick else "")
@@ -207,6 +248,8 @@ def synthetic_state_dict(arch, seed=0):
         return torch.randn(*shape, generator=g, dtype=torch.float32) * std
 
     sd = {}
+    if isinstance(arch, SigLIPArch):
+        return _siglip_state_dict(arch, rn)
     if isinstance(arch, ResNetArch):
         _resnet_visual(sd, arch, rn, g)
 
@@ -246,6 +289,60 @@ def synthetic_state_dict(arch, seed=0):
     sd["ln_final.weight"] = 1.0 + rn(t.width, std=0.1)
     sd["ln_final.bias"] = rn(t.width, std=0.05)
     sd["text_projection"] = rn(t.width, arch.embed_dim, std=t.width ** -0.5)
+    return sd
+
+
+def _siglip_state_dict(arch, rn):
+    """SigLIP weights in open_clip's layout (visual.trunk.* from timm, text.*), with non-trivial LayerNorm affines
+    and biases."""
+    sd = {}
+
+    def ln(name, n):
+        sd[name + ".weight"] = 1.0 + rn(n, std=0.1)
+        sd[name + ".bias"] = rn(n, std=0.05)
+
+    def linear(name, n_out, n_in, std):
+        sd[name + ".weight"] = rn(n_out, n_in, std=std)
+        sd[name + ".bias"] = rn(n_out, std=0.02)
+
+    def mlp(prefix, a, b, w, h, L):
+        linear(prefix + a, h, w, (2 * w) ** -0.5)
+        linear(prefix + b, w, h, (w ** -0.5) * ((2 * L) ** -0.5))
+
+    v, t, p = arch.vision, arch.text, arch.patch
+    w, L, grid = v.width, v.layers, arch.image_size // p
+    tr = "visual.trunk."
+    linear(tr + "patch_embed.proj", w, 3 * p * p, (3 * p * p) ** -0.5)
+    sd[tr + "patch_embed.proj.weight"] = sd[tr + "patch_embed.proj.weight"].reshape(w, 3, p, p)
+    sd[tr + "pos_embed"] = rn(1, grid * grid, w, std=w ** -0.5)
+    for i in range(L):
+        b = "%sblocks.%d." % (tr, i)
+        ln(b + "norm1", w)
+        linear(b + "attn.qkv", 3 * w, w, w ** -0.5)
+        linear(b + "attn.proj", w, w, (w ** -0.5) * ((2 * L) ** -0.5))
+        ln(b + "norm2", w)
+        mlp(b, "mlp.fc1", "mlp.fc2", w, v.mlp, L)
+    ln(tr + "norm", w)
+    a = tr + "attn_pool."
+    sd[a + "latent"] = rn(1, 1, w, std=w ** -0.5)
+    linear(a + "q", w, w, w ** -0.5)
+    linear(a + "kv", 2 * w, w, w ** -0.5)
+    linear(a + "proj", w, w, w ** -0.5)
+    ln(a + "norm", w)
+    mlp(a, "mlp.fc1", "mlp.fc2", w, v.mlp, 1)
+    tw, tL = t.width, t.layers
+    sd["text.token_embedding.weight"] = rn(arch.vocab_size, tw, std=0.02)
+    sd["text.positional_embedding"] = rn(arch.context_length, tw, std=0.01)
+    for i in range(tL):
+        q = "text.transformer.resblocks.%d." % i
+        ln(q + "ln_1", tw)
+        sd[q + "attn.in_proj_weight"] = rn(3 * tw, tw, std=tw ** -0.5)
+        sd[q + "attn.in_proj_bias"] = rn(3 * tw, std=0.02)
+        linear(q + "attn.out_proj", tw, tw, (tw ** -0.5) * ((2 * tL) ** -0.5))
+        ln(q + "ln_2", tw)
+        mlp(q, "mlp.c_fc", "mlp.c_proj", tw, t.mlp, tL)
+    ln("text.ln_final", tw)
+    linear("text.text_projection", arch.embed_dim, tw, tw ** -0.5)
     return sd
 
 
@@ -341,6 +438,16 @@ class B200Clip:
         self.max_batch = int(max_batch)
         self._h = C.c_void_p()
         self._lock = threading.Lock()
+        if isinstance(arch, SigLIPArch):
+            cfg = _lib.ClipConfigC(
+                arch.embed_dim, arch.image_size, arch.patch,
+                _lib.TowerConfigC(arch.vision.width, arch.vision.layers, arch.vision.heads, arch.vision.mlp),
+                arch.context_length, arch.vocab_size,
+                _lib.TowerConfigC(arch.text.width, arch.text.layers, arch.text.heads, arch.text.mlp),
+                0, self.max_batch,
+            )
+            check(lib.b200_clip_create_siglip(C.byref(cfg), self.device_index, C.byref(self._h)), "clip_create_siglip")
+            return
         if isinstance(arch, ResNetArch):
             cfg = _lib.ClipConfigC(
                 arch.embed_dim, arch.image_size, 0, _lib.TowerConfigC(0, 0, 0, 0), arch.context_length, arch.vocab_size,
@@ -426,6 +533,9 @@ class B200Clip:
             x = x.to(torch.float32 if image else torch.int64).contiguous().numpy()
         else:
             x = np.ascontiguousarray(x, dtype=np.float32 if image else np.int64)
+        if not image and isinstance(self.arch, SigLIPArch) and (x.ndim != 2 or x.shape[1] != self.arch.context_length):
+            # the pads take part in SigLIP's attention and position T - 1 is pooled: no other width means the same
+            raise ValueError("embed_text: expected token ids [B, %d], got %r" % (self.arch.context_length, x.shape))
         B = x.shape[0]
         out = np.empty((B, self.arch.embed_dim), dtype=np_dtype)
         fn = lib.b200_clip_encode_image if image else lib.b200_clip_encode_text
@@ -491,23 +601,38 @@ def _tensor_views(sd):
 _SQUASH_TAGS = {"open_clip:ViT-H-14-378": ("dfn5b",)}
 
 
+OPENAI_MEAN = (0.48145466, 0.4578275, 0.40821073)
+OPENAI_STD = (0.26862954, 0.26130258, 0.27577711)
+# SigLIP's transform (open_clip's pretrained config for every `webli` SigLIP, as recalled: DESIGN.md §5 (xix)): squash
+# to n_px x n_px, bicubic, and normalise with mean = std = 0.5.
+SIGLIP_MEAN = SIGLIP_STD = (0.5, 0.5, 0.5)
+
+
 def preprocess_mode(clip_model):
     """"squash" or "shortest": the resize step of the transform `load_clip` returns for this name (and that
     `ClipMapper` runs on the GPU for `image_rgb8` batches)."""
+    return preprocess_params(clip_model)[0]
+
+
+def preprocess_params(clip_model):
+    """(resize mode, mean, std) of the transform `load_clip` returns for this name, and that `ClipMapper` runs on the
+    GPU for `image_rgb8` batches."""
     name = clip_model[len("synthetic:"):] if clip_model.startswith("synthetic:") else clip_model
     if name.startswith("open_clip:"):
         arch_name, _, pretrained = name.partition("/")
+        if arch_name in SIGLIP_ARCHS:
+            return "squash", SIGLIP_MEAN, SIGLIP_STD
         if arch_name.endswith("-quickgelu"):
             arch_name = arch_name[: -len("-quickgelu")]
         if pretrained in _SQUASH_TAGS.get(arch_name, ()):
-            return "squash"
-    return "shortest"
+            return "squash", OPENAI_MEAN, OPENAI_STD
+    return "shortest", OPENAI_MEAN, OPENAI_STD
 
 
-def make_preprocess(n_px, resize_mode="shortest"):
-    """torchvision Compose[Resize(n_px, BICUBIC), CenterCrop, RGB, ToTensor, Normalize(OpenAI mean/std)] —
-    the transform SURVEY.md §4 verified bit-exactly against the reference's test_tensors fixtures.  With
-    resize_mode "squash", Resize((n_px, n_px), BICUBIC) and no crop."""
+def make_preprocess(n_px, resize_mode="shortest", mean=OPENAI_MEAN, std=OPENAI_STD):
+    """torchvision Compose[Resize(n_px, BICUBIC), CenterCrop, RGB, ToTensor, Normalize(mean, std)] (OpenAI's mean /
+    std by default) — the transform SURVEY.md §4 verified bit-exactly against the reference's test_tensors fixtures.
+    With resize_mode "squash", Resize((n_px, n_px), BICUBIC) and no crop."""
     from torchvision import transforms as T
     from torchvision.transforms import InterpolationMode
 
@@ -519,7 +644,7 @@ def make_preprocess(n_px, resize_mode="shortest"):
         T.CenterCrop(n_px),
         lambda im: im.convert("RGB"),
         T.ToTensor(),
-        T.Normalize((0.48145466, 0.4578275, 0.40821073), (0.26862954, 0.26130258, 0.27577711)),
+        T.Normalize(mean, std),
     ])
 
 
@@ -623,6 +748,28 @@ def _bytes_to_unicode():
             cs.append(2 ** 8 + n)
             n += 1
     return dict(zip(bs, [chr(c) for c in cs]))
+
+
+def siglip_clean(text):
+    """open_clip's `canonicalize_text(basic_clean(text))`, the cleaning of its SigLIP tokenizers: `_` becomes a space,
+    ASCII punctuation is removed, the text is lower-cased and its whitespace collapsed."""
+    import string
+
+    text = _basic_clean(text).replace("_", " ")
+    text = text.translate(str.maketrans("", "", string.punctuation)).lower()
+    return " ".join(text.split()).strip()
+
+
+def siglip_tokenizer(arch, clip_cache_path):
+    """open_clip's HFTokenizer of a SigLIP model: `<clip_cache_path>/<arch.tokenizer>/tokenizer.json`, texts cleaned
+    by `siglip_clean`, truncated and padded (pad id 1) to the arch's context length; the `_MissingTokenizer` when the
+    file is not there."""
+    from .xlmr_clip import XLMRTokenizer
+
+    path = os.path.join(clip_cache_path, arch.tokenizer, "tokenizer.json") if clip_cache_path else None
+    if path and os.path.exists(path):
+        return XLMRTokenizer(path, pad_id=1, context_length=arch.context_length, clean=siglip_clean)
+    return _MissingTokenizer("SigLIP tokenizer (%s/tokenizer.json) not found under clip_cache_path" % arch.tokenizer)
 
 
 class _MissingTokenizer:
@@ -746,9 +893,12 @@ def load_clip(clip_model="ViT-B/32", use_jit=True, warmup_batch_size=1, clip_cac
                 "no checkpoint for %r under clip_cache_path=%r (no network here); use 'synthetic:%s' for "
                 "seeded random weights" % (clip_model, clip_cache_path, clip_model))
         model.load_state_dict(read_checkpoint(ckpt, arch))
-    preprocess = make_preprocess(arch.image_size, preprocess_mode(clip_model))
+    mode, mean, std = preprocess_params(clip_model)
+    preprocess = make_preprocess(arch.image_size, mode, mean, std)
     bpe = os.path.join(clip_cache_path, "bpe_simple_vocab_16e6.txt.gz") if clip_cache_path else None
-    if bpe and os.path.exists(bpe):
+    if isinstance(arch, SigLIPArch):
+        tokenizer = siglip_tokenizer(arch, clip_cache_path)
+    elif bpe and os.path.exists(bpe):
         tokenizer = SimpleTokenizer(bpe, arch.context_length)
     else:
         tokenizer = _MissingTokenizer("CLIP BPE vocabulary (bpe_simple_vocab_16e6.txt.gz) not found under clip_cache_path")

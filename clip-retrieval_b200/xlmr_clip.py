@@ -169,9 +169,10 @@ def synthetic_state_dict(arch, seed=0):
 class XLMRTokenizer:
     """open_clip's HFTokenizer for these models: each text cleaned by whitespace_clean(basic_clean(.)), then the
     checkpoint's `tokenizer.json` with truncation to 77 tokens (special tokens included) and padding to 77 with the
-    pad id.  texts -> LongTensor [n, 77]."""
+    pad id.  texts -> LongTensor [n, 77].  `clean` and `context_length` replace the cleaning and the 77 (SigLIP's
+    tokenizers: model.siglip_tokenizer)."""
 
-    def __init__(self, path, pad_id=1, context_length=77):
+    def __init__(self, path, pad_id=1, context_length=77, clean=None):
         try:
             from tokenizers import Tokenizer
         except ImportError as e:
@@ -179,6 +180,7 @@ class XLMRTokenizer:
         self.tok = Tokenizer.from_file(path)
         self.pad_id = int(pad_id)
         self.context_length = int(context_length)
+        self.clean = clean or (lambda t: _whitespace_clean(_basic_clean(t)))
         self.tok.enable_truncation(max_length=self.context_length)
         self.tok.enable_padding(length=self.context_length, pad_id=self.pad_id,
                                 pad_token=self.tok.id_to_token(self.pad_id) or "<pad>")
@@ -187,7 +189,7 @@ class XLMRTokenizer:
         torch = mclip._torch()
         if isinstance(texts, str):
             texts = [texts]
-        encs = self.tok.encode_batch([_whitespace_clean(_basic_clean(t)) for t in texts])
+        encs = self.tok.encode_batch([self.clean(t) for t in texts])
         return torch.tensor([e.ids for e in encs], dtype=torch.long).reshape(len(encs), self.context_length)
 
 

@@ -312,6 +312,16 @@ typedef struct b200_resnet_config {
   int32_t heads;       /* attention-pool heads: 32 w / 64 */
 } b200_resnet_config;
 int b200_clip_create_resnet(const b200_clip_config* cfg, const b200_resnet_config* rc, int device, b200_clip** out);
+/* Google's SigLIP models as open_clip builds them (ViT-B-16-SigLIP*, ViT-L-16-SigLIP-*, ViT-SO400M-14-SigLIP*): a timm
+ * ViT image tower with no class token and no ln_pre, a patch embedding with a bias, and a latent-query attention pool
+ * (one learned query, `vision.heads` heads, then proj, LayerNorm and an MLP of `vision.mlp` with a residual) whose
+ * output is the feature; a bidirectional text tower (no causal or padding mask) pooled at position context_length - 1
+ * after ln_final, with a biased Linear projection.  Every LayerNorm uses eps 1e-6, both MLPs erf GELU.  embed_dim must
+ * equal vision.width and quick_gelu must be 0.  load_weights reads open_clip's keys: visual.trunk.{patch_embed.proj,
+ * pos_embed, blocks.i.{norm1, attn.qkv, attn.proj, norm2, mlp.fc1, mlp.fc2}, norm, attn_pool.{latent, q, kv, proj,
+ * norm, mlp.fc1, mlp.fc2}} and text.{token_embedding, positional_embedding, transformer.resblocks.i.*, ln_final,
+ * text_projection}.  Every other b200_clip_* entry works on the handle unchanged. */
+int b200_clip_create_siglip(const b200_clip_config* cfg, int device, b200_clip** out);
 int b200_clip_destroy(b200_clip* m);
 /* Upload weights given as a state_dict in the open_clip/OpenAI key layout; converts to the
  * packed bf16 device layout.  Missing or mis-shaped tensors are an error. */
@@ -416,6 +426,17 @@ int b200_stem_gather_device(const float* d_pixels, int B, int S, void* d_cols, i
 int b200_avgpool_bf16_device(const void* d_in, int B, int H, int W, int C, int k, void* d_out, int device, void* stream);
 int b200_attnpool_tokens_device(const void* d_x, int B, int HW, int C, const float* d_pos, void* d_out, int device,
                                 void* stream);
+/* The two kernels of SigLIP's tower ends, for their parity tests.
+ * Latent-query attention pool: d_kv bf16 [B * T, 2w] (k | v, `heads` heads of hd = w / heads, hd a multiple of 8 up to
+ *   128), d_q fp32 [w] -> d_out bf16 [B, w], d_out[b, h hd + j] = sum_t softmax_t(q_h . k_{b,t,h} hd^-0.5) v_{b,t,h,j},
+ *   with scores, softmax and sums in fp32.
+ * Text tail: d_out [B, D] = normalise(LN_eps(x[b * T + T - 1]) @ d_proj + d_bias), d_proj bf16 [w, D], d_bias fp32
+ *   [D]; d_feat fp32 [B, D] receives the raw features; otherwise as b200_pool_ln_proj_device. */
+int b200_latent_pool_attention_device(const void* d_kv, int B, int T, int heads, int w, const float* d_q, void* d_out,
+                                      int device, void* stream);
+int b200_pool_last_ln_proj_bias_device(const void* d_x, int B, int T, int w, const float* d_gamma, const float* d_beta,
+                                       float eps, const void* d_proj, const float* d_bias, int D, float* d_feat,
+                                       void* d_out, int out_dtype, int normalize, int device, void* stream);
 /* ------------------------------------------------------------------------------------------
  * Multilingual text towers (use_mclip).  Replaces the M-CLIP text model of the query service
  * (clip_back.py:222-224,836-859: XLM-RoBERTa-Large + mean pool + LinearTransformation) and the
