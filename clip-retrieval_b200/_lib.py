@@ -59,6 +59,10 @@ class ResNetConfigC(C.Structure):
     _fields_ = [("layers", C.c_int32 * 4), ("width", C.c_int32), ("heads", C.c_int32)]
 
 
+class ConvNeXtConfigC(C.Structure):
+    _fields_ = [("depths", C.c_int32 * 4), ("dims", C.c_int32 * 4), ("head_mlp", C.c_int32), ("eps", C.c_float)]
+
+
 class TextEncoderConfigC(C.Structure):
     _fields_ = [
         ("layers", C.c_int32),
@@ -162,6 +166,7 @@ PROTOTYPES = {
     "b200_clip_create": (_i, [C.POINTER(ClipConfigC), _i, C.POINTER(_vp)]),
     "b200_clip_create_resnet": (_i, [C.POINTER(ClipConfigC), C.POINTER(ResNetConfigC), _i, C.POINTER(_vp)]),
     "b200_clip_create_siglip": (_i, [C.POINTER(ClipConfigC), _i, C.POINTER(_vp)]),
+    "b200_clip_create_convnext": (_i, [C.POINTER(ClipConfigC), C.POINTER(ConvNeXtConfigC), _i, C.POINTER(_vp)]),
     "b200_clip_destroy": (_i, [_vp]),
     "b200_clip_load_weights": (_i, [_vp, C.POINTER(TensorViewC), _i]),
     "b200_clip_encode_image_device": (_i, [_vp, _vp, _i, _vp, _i, _i, _vp]),
@@ -185,6 +190,10 @@ PROTOTYPES = {
     "b200_latent_pool_attention_device": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _i, _vp]),
     "b200_pool_last_ln_proj_bias_device": (_i, [_vp, _i, _i, _i, _vp, _vp, C.c_float, _vp, _vp, _i, _vp, _vp, _i, _i, _i,
                                                 _vp]),
+    "b200_dwconv7_ln_bf16_device": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, C.c_float, _vp, _i, _vp]),
+    "b200_ln_s2d_bf16_device": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, C.c_float, _vp, _i, _vp]),
+    "b200_convnext_head_device": (_i, [_vp, _i, _i, _i, _vp, _vp, C.c_float, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp,
+                                       _i, _i, _i, _vp]),
     "b200_index_last_hi_only_fallbacks": (_i, [_vp]),
     "b200_index_last_scan_plan": (_i, [_vp, _vp]),
     "b200_kmeans_train_f16": (_i, [_vp, _i64, _i, _i, _i, C.c_uint64, _i, _vp, _vp, _i]),

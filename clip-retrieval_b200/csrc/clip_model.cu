@@ -8,6 +8,7 @@
 // qkv, a attention output, f MLP hidden), sized for max_batch at create time so every TMA
 // descriptor is built once.
 #include "common.cuh"
+#include "convnext.cuh"
 #include "embed_kernels.cuh"
 #include "gemm.cuh"
 #include "layers.cuh"
@@ -73,6 +74,7 @@ struct b200_clip {
   bool has_text = true;       // false: an image-only handle (all-zero text tower config), no text weights or buffers
   b200::Tower vis, txt;
   b200::ResNetTower* rn = nullptr;   // the ResNet image tower (b200_clip_create_resnet) in place of vis and its front
+  b200::ConvNeXtTower* cnx = nullptr;   // the ConvNeXt image tower (b200_clip_create_convnext), likewise
   bool siglip = false;               // b200_clip_create_siglip: timm/open_clip SigLIP towers
   b200::LatentHead head;             // SigLIP's image head
   // vision front end
@@ -205,6 +207,9 @@ static int encode_image_chunk(b200_clip* m, const float* d_px, int B, void* d_ou
   if (m->rn)
     return resnet_encode(*m->rn, m->timer, CLS_GEMM, CLS_ATTN, CLS_OTHER, m->sms, d_px, B, m->feat, d_out, out_f16,
                          normalize, st);
+  if (m->cnx)
+    return convnext_encode(*m->cnx, m->timer, CLS_GEMM, CLS_OTHER, m->sms, d_px, B, m->feat, d_out, out_f16, normalize,
+                           st);
   if (m->siglip) return encode_image_chunk_siglip(m, d_px, B, d_out, out_f16, normalize, st);
   Tower& t = m->vis;
   const int g = m->grid, w = t.width, T = t.T;
@@ -462,6 +467,39 @@ int b200_clip_create_resnet(const b200_clip_config* cfg, const b200_resnet_confi
   return B200_OK;
 }
 
+// The ConvNeXt image tower (convnext.cuh) with the same text tower, staging, graphs and entries as b200_clip_create.
+int b200_clip_create_convnext(const b200_clip_config* cfg, const b200_convnext_config* nc, int device, b200_clip** out) {
+  B200_CHECK(cfg && nc && out, B200_ERR_INVALID, "clip_create_convnext: null argument");
+  const bool has_text = cfg->text.width != 0 || cfg->text.layers != 0 || cfg->text.heads != 0 || cfg->text.mlp != 0;
+  const bool no_vit = cfg->patch == 0 && cfg->vision.width == 0 && cfg->vision.layers == 0 && cfg->vision.heads == 0 &&
+                      cfg->vision.mlp == 0;
+  B200_CHECK(no_vit && cfg->max_batch >= 1 && cfg->embed_dim >= 8 && cfg->image_size >= 32 && cfg->image_size % 32 == 0 &&
+                 (!has_text || (cfg->context_length >= 1 && cfg->vocab_size >= 2)),
+             B200_ERR_INVALID, "clip_create_convnext: bad config (vision and patch must be zero, image_size a multiple of "
+             "32)");
+  int ndev = 0;
+  B200_CUDA(cudaGetDeviceCount(&ndev));
+  B200_CHECK(device >= 0 && device < ndev, B200_ERR_INVALID, "clip_create_convnext: device %d of %d", device, ndev);
+  DeviceGuard g(device);
+  b200_clip* m = new (std::nothrow) b200_clip();
+  B200_CHECK(m != nullptr, B200_ERR_OOM, "clip_create_convnext: host allocation failed");
+  m->cfg = *cfg;
+  m->device = device;
+  m->sms = sm_count(device);
+  m->has_text = has_text;
+  if (const char* e = getenv("B200_GRAPHS")) m->use_graphs = atoi(e) != 0;
+  m->cnx = new (std::nothrow) ConvNeXtTower();
+  int rc = m->cnx == nullptr ? B200_ERR_OOM : B200_OK;
+  if (rc == B200_OK) rc = convnext_create(m->allocs, m->cnx, *nc, cfg->image_size, cfg->embed_dim, cfg->max_batch);
+  if (rc == B200_OK) rc = make_text_and_staging(m);
+  if (rc != B200_OK) {
+    b200_clip_destroy(m);
+    return rc;
+  }
+  *out = m;
+  return B200_OK;
+}
+
 // SigLIP (open_clip's timm-trunk configs): the ViT handle with no class row and no ln_pre, a patch bias, the latent
 // attention-pool head, a bidirectional text tower pooled at its last position with a biased projection, and LayerNorm
 // eps 1e-6 everywhere.
@@ -531,6 +569,7 @@ int b200_clip_destroy(b200_clip* m) {
   cudaDeviceSynchronize();
   m->allocs.free_all();
   delete m->rn;
+  delete m->cnx;
   for (auto& kv : m->graphs) if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
   if (m->cap_stream) cudaStreamDestroy(m->cap_stream);
   if (m->s_copy) {
@@ -555,6 +594,7 @@ int b200_clip_load_weights(b200_clip* m, const b200_tensor_view* tensors, int n)
     return B200_OK;
   }
   if (m->rn) B200_TRY(resnet_load(ld, *m->rn));
+  else if (m->cnx) B200_TRY(convnext_load(ld, *m->cnx));
   else B200_TRY(load_vit(m, ld));
   if (m->has_text) {
     B200_TRY(ld.put_bf16("token_embedding.weight", m->tok_emb, (size_t)c.vocab_size, tw, tw));
@@ -777,6 +817,38 @@ int b200_pool_last_ln_proj_bias_device(const void* d_x, int B, int T, int w, con
   return pool_last_ln_proj_bias_norm((const __nv_bfloat16*)d_x, T, w, d_gamma, d_beta, eps,
                                      (const __nv_bfloat16*)d_proj, d_bias, D, d_feat, d_out,
                                      out_dtype == B200_OUT_F16, normalize, B, (cudaStream_t)stream);
+}
+
+int b200_dwconv7_ln_bf16_device(const void* d_x, int B, int H, int W, int C, const float* d_w49, const float* d_bias,
+                                const float* d_gamma, const float* d_beta, float eps, void* d_out, int device,
+                                void* stream) {
+  B200_CHECK(B >= 0 && (B == 0 || (d_x && d_w49 && d_bias && d_out)) && (d_gamma == nullptr || (d_beta && eps > 0.f)),
+             B200_ERR_INVALID, "dwconv7_ln: bad argument");
+  DeviceGuard g(device);
+  return dwconv7_ln((const __nv_bfloat16*)d_x, d_w49, d_bias, d_gamma, d_beta, eps, (__nv_bfloat16*)d_out, B, H, W, C,
+                    (cudaStream_t)stream);
+}
+int b200_ln_s2d_bf16_device(const void* d_x, int B, int H, int W, int C, const float* d_gamma, const float* d_beta,
+                            float eps, void* d_out, int device, void* stream) {
+  B200_CHECK(B >= 0 && eps > 0.f && (B == 0 || (d_x && d_gamma && d_beta && d_out)), B200_ERR_INVALID,
+             "ln_s2d: bad argument");
+  DeviceGuard g(device);
+  return ln_s2d((const __nv_bfloat16*)d_x, d_gamma, d_beta, eps, (__nv_bfloat16*)d_out, B, H, W, C,
+                (cudaStream_t)stream);
+}
+int b200_convnext_head_device(const void* d_x, int B, int HW, int C, const float* d_gamma, const float* d_beta, float eps,
+                              const float* d_w1T, const float* d_b1, int h, const float* d_w2T, int D, float* d_pooled,
+                              float* d_hid, float* d_feat, void* d_out, int out_dtype, int normalize, int device,
+                              void* stream) {
+  B200_CHECK(B >= 0 && HW >= 1 && C >= 1 && D >= 1 && eps > 0.f && (d_w1T == nullptr || (d_b1 && d_hid && h >= 1)) &&
+                 (B == 0 || (d_x && d_gamma && d_beta && d_w2T && d_pooled && d_feat && d_out)) &&
+                 (out_dtype == B200_OUT_F16 || out_dtype == B200_OUT_F32),
+             B200_ERR_INVALID, "convnext_head: bad argument");
+  DeviceGuard g(device);
+  const cudaStream_t st = (cudaStream_t)stream;
+  B200_TRY(mean_ln_rows((const __nv_bfloat16*)d_x, B, HW, C, d_gamma, d_beta, eps, d_pooled, st));
+  return rows_head_norm(d_pooled, C, d_w1T, d_b1, h, d_w2T, D, d_hid, d_feat, d_out, out_dtype == B200_OUT_F16,
+                        normalize, B, st);
 }
 
 int b200_clip_set_profiling(b200_clip* m, int on) {

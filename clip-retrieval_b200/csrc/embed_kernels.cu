@@ -628,6 +628,43 @@ int masked_mean_mlp_norm(const __nv_bfloat16* x, int T, int w, const int* len, c
   return B200_OK;
 }
 
+// The ConvNeXt head's first MLP layer on fp32 rows: hid[b, j] = gelu_erf(rows[b, :] . w1T[:, j] + b1[j]).
+__global__ void __launch_bounds__(256)
+rows_mlp1_bias_kernel(const float* __restrict__ rows, int w, const float* __restrict__ w1T,
+                      const float* __restrict__ b1, int h, float* __restrict__ hid) {
+  extern __shared__ float sm[];
+  float* s_row = sm;                // [w]
+  float* s_part = sm + w;           // [4][64]
+  const int b = blockIdx.y, j0 = blockIdx.x * 64;
+  for (int i = threadIdx.x; i < w; i += blockDim.x) s_row[i] = rows[(size_t)b * w + i];
+  __syncthreads();
+  const float y = split_column_dot(s_row, w, w1T, h, j0, s_part);
+  const int j = j0 + threadIdx.x;
+  if (threadIdx.x < 64 && j < h) {
+    const float v = y + b1[j];
+    hid[(size_t)b * h + j] = 0.5f * v * (1.0f + erff(v * 0.70710678118654752f));
+  }
+}
+
+int rows_head_norm(const float* rows, int w, const float* w1T, const float* b1, int h, const float* w2T, int D,
+                   float* hid, float* feat, void* out, int out_f16, int normalize, int B, cudaStream_t st) {
+  if (B == 0) return B200_OK;
+  const int k2 = w1T != nullptr ? h : w;
+  B200_CHECK((size_t)(std::max(w, k2) + 256) * sizeof(float) <= 48 * 1024, B200_ERR_UNSUPPORTED,
+             "rows_head: width %d / hidden %d too large", w, h);
+  if (w1T != nullptr) {
+    rows_mlp1_bias_kernel<<<dim3((h + 63) / 64, B), 256, (size_t)(w + 256) * sizeof(float), st>>>(rows, w, w1T, b1, h,
+                                                                                                   hid);
+    B200_LAUNCH_OK();
+  }
+  mlp2_kernel<<<dim3((D + 63) / 64, B), 256, (size_t)(k2 + 256) * sizeof(float), st>>>(w1T != nullptr ? hid : rows, k2,
+                                                                                       w2T, D, feat);
+  B200_LAUNCH_OK();
+  feat_norm_cast_kernel<<<B, 256, 0, st>>>(feat, D, out, out_f16, normalize);
+  B200_LAUNCH_OK();
+  return B200_OK;
+}
+
 int token_lengths(const int64_t* ids, int B, int T, int64_t pad_id, int* len, cudaStream_t st) {
   if (B == 0) return B200_OK;
   token_lengths_kernel<<<(B + 127) / 128, 128, 0, st>>>(ids, B, T, pad_id, len);

@@ -84,6 +84,26 @@ int masked_mean_proj_norm(const __nv_bfloat16* x, int T, int w, const int* len, 
 int masked_mean_mlp_norm(const __nv_bfloat16* x, int T, int w, const int* len, const float* w1T, int h,
                          const float* w2T, int D, float* hid, float* feat, void* out, int out_f16, int normalize, int B,
                          cudaStream_t st);
+// The ConvNeXt head's tail on fp32 rows [B, w] (the pooled, LayerNormed features): with w1T == nullptr, feat = rows @
+// w2T [w, D] (open_clip's linear head); otherwise hid = gelu_erf(rows @ w1T [w, h] + b1[h]) into hid fp32 [B, h] and
+// feat = hid @ w2T [h, D] (the MLP head).  Each layer in blocks of 64 output columns per sample, as masked_mean_mlp_norm
+// runs them; out as pool_ln_proj_norm writes it.
+int rows_head_norm(const float* rows, int w, const float* w1T, const float* b1, int h, const float* w2T, int D,
+                   float* hid, float* feat, void* out, int out_f16, int normalize, int B, cudaStream_t st);
+// ConvNeXt (dwconv.cu).  Depthwise 7x7 convolution, pad 3, fused with the block's LayerNorm: x NHWC bf16 [B, H, W, C]
+// -> out bf16 [B * H * W, C] = LN_eps(bias[c] + sum_{r,s} w49[7 r + s, c] x[h + r - 3, w + s - 3, c]) * gamma + beta,
+// the taps summed in fp32 in the order (r, s), the LayerNorm taken on the fp32 sums (never rounded to bf16 between);
+// gamma == nullptr: the convolution + bias alone.  w49 fp32 [49, C]; C a multiple of 64, at most 3072.
+int dwconv7_ln(const __nv_bfloat16* x, const float* w49, const float* bias, const float* gamma, const float* beta,
+               float eps, __nv_bfloat16* out, int B, int H, int W, int C, cudaStream_t st);
+// Downsample front: x [B, H, W, C] (H, W even, C a multiple of 8, at most 1536) -> out [B * (H/2) * (W/2), 4C] with
+// column (2 i + j) C + c = LN_eps(x[b, 2 ho + i, 2 wo + j, :])[c] * gamma[c] + beta[c].
+int ln_s2d(const __nv_bfloat16* x, const float* gamma, const float* beta, float eps, __nv_bfloat16* out, int B, int H,
+           int W, int C, cudaStream_t st);
+// Head front: pooled fp32 [B, C] = LN_eps(mean over the HW rows of sample b of x [B * HW, C]) * gamma + beta, the mean
+// an fp32 sum in ascending row order.
+int mean_ln_rows(const __nv_bfloat16* x, int B, int HW, int C, const float* gamma, const float* beta, float eps,
+                 float* pooled, cudaStream_t st);
 // len[b] = index of the first pad_id in row b of ids [B, T], T when there is none (0 for a row of padding only).
 int token_lengths(const int64_t* ids, int B, int T, int64_t pad_id, int* len, cudaStream_t st);
 // argmax(tokens, dim=-1) (first maximum) -> pool_idx[b]

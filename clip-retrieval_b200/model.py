@@ -155,8 +155,50 @@ SIGLIP_ARCHS = {
     "open_clip:ViT-SO400M-14-SigLIP-384": SigLIPArch(1152, 384, 14, _SIG_SO, _SIG_SO),
 }
 
+
+@dataclass(frozen=True)
+class ConvNeXtArch:
+    """open_clip's ConvNeXt CLIPs (include/b200clip.h b200_clip_create_convnext): timm's ConvNeXt trunk (`depths` blocks
+    per stage at widths `dims`, every LayerNorm at `eps`) under open_clip's linear or MLP (`head_mlp`) head, with the
+    standard CLIP text tower (erf GELU).  `tags` are the pretrained tags open_clip publishes for the name."""
+    embed_dim: int
+    image_size: int
+    depths: tuple
+    dims: tuple
+    head_mlp: bool
+    text: Tower
+    eps: float = 1e-6
+    tags: tuple = ()
+    context_length: int = 77
+    vocab_size: int = 49408
+    quick_gelu: bool = False
+
+
+# open_clip's ConvNeXt configs and pretrained tags, recalled from open_clip's model and pretrained configs and timm's
+# ConvNeXt, not read from any of them (DESIGN.md §5 (xx)); xxlarge's LayerNorm eps 1e-5 is timm's `norm_eps` for it.
+# Kept apart from ARCHS, G14_ARCHS, RESNET_ARCHS and SIGLIP_ARCHS; resolve_arch reads all five.
+_CNX_BASE = ((3, 3, 27, 3), (128, 256, 512, 1024))
+_CNX_LARGE = ((3, 3, 27, 3), (192, 384, 768, 1536))
+_CNX_XXL = ((3, 4, 30, 3), (384, 768, 1536, 3072))
+CONVNEXT_ARCHS = {
+    "open_clip:convnext_base": ConvNeXtArch(512, 224, *_CNX_BASE, False, Tower(512, 12, 8, 2048),
+                                            tags=("laion400m_s13b_b51k",)),
+    "open_clip:convnext_base_w": ConvNeXtArch(640, 256, *_CNX_BASE, False, Tower(640, 12, 10, 2560),
+                                              tags=("laion2b_s13b_b82k", "laion2b_s13b_b82k_augreg",
+                                                    "laion_aesthetic_s13b_b82k")),
+    "open_clip:convnext_base_w_320": ConvNeXtArch(640, 320, *_CNX_BASE, False, Tower(640, 12, 10, 2560),
+                                                  tags=("laion_aesthetic_s13b_b82k", "laion_aesthetic_s13b_b82k_augreg")),
+    "open_clip:convnext_large_d": ConvNeXtArch(768, 256, *_CNX_LARGE, True, Tower(768, 16, 12, 3072),
+                                               tags=("laion2b_s26b_b102k_augreg",)),
+    "open_clip:convnext_large_d_320": ConvNeXtArch(768, 320, *_CNX_LARGE, True, Tower(768, 16, 12, 3072),
+                                                   tags=("laion2b_s29b_b131k_ft", "laion2b_s29b_b131k_ft_soup")),
+    "open_clip:convnext_xxlarge": ConvNeXtArch(1024, 256, *_CNX_XXL, False, Tower(1024, 24, 16, 4096), eps=1e-5,
+                                               tags=("laion2b_s34b_b82k_augreg", "laion2b_s34b_b82k_augreg_rewind",
+                                                     "laion2b_s34b_b82k_augreg_soup")),
+}
+
 # Every architecture a `clip_model` name can resolve to.
-KNOWN_ARCHS = {**ARCHS, **G14_ARCHS, **RESNET_ARCHS, **SIGLIP_ARCHS}
+KNOWN_ARCHS = {**ARCHS, **G14_ARCHS, **RESNET_ARCHS, **SIGLIP_ARCHS, **CONVNEXT_ARCHS}
 
 # `hf_clip:<repo>` names -> (architecture key, quick_gelu): HuggingFace CLIPModel checkpoints of the same towers.
 HF_REPOS = {
@@ -222,6 +264,15 @@ def resolve_arch(clip_model):
                 raise ValueError("%r: SigLIP models take erf GELU and the `webli` weights only (no -quickgelu, no "
                                  "`openai` tag)" % (clip_model,))
             return SIGLIP_ARCHS[key], key
+        if key in CONVNEXT_ARCHS:
+            arch = CONVNEXT_ARCHS[key]
+            if quick:
+                raise ValueError("%r: the ConvNeXt CLIPs take erf GELU and LAION weights only (no -quickgelu, no "
+                                 "`openai` tag)" % (clip_model,))
+            if pretrained and pretrained not in arch.tags:
+                raise ValueError("%r: unknown pretrained tag; %s has %s" % (clip_model, arch_name, ", ".join(arch.tags)))
+            # the tag stays in the key: checkpoints are looked up as `<name>-<tag>.pt`
+            return arch, key + ("/" + pretrained if pretrained else "")
         if key not in KNOWN_ARCHS:
             raise ValueError("unknown clip_model %r; known: %s" % (clip_model, ", ".join(sorted(KNOWN_ARCHS))))
         return replace(KNOWN_ARCHS[key], quick_gelu=quick), key + ("-quickgelu" if quick else "")
@@ -252,6 +303,8 @@ def synthetic_state_dict(arch, seed=0):
         return _siglip_state_dict(arch, rn)
     if isinstance(arch, ResNetArch):
         _resnet_visual(sd, arch, rn, g)
+    if isinstance(arch, ConvNeXtArch):
+        _convnext_visual(sd, arch, rn, g)
 
     def tower(prefix, t):
         w, L = t.width, t.layers
@@ -271,7 +324,7 @@ def synthetic_state_dict(arch, seed=0):
             sd[p + "mlp.c_proj.bias"] = rn(w, std=0.02)
 
     t = arch.text
-    if not isinstance(arch, ResNetArch):
+    if not isinstance(arch, (ResNetArch, ConvNeXtArch)):
         v = arch.vision
         grid = arch.image_size // arch.patch
         sd["visual.conv1.weight"] = rn(v.width, 3, arch.patch, arch.patch, std=(3 * arch.patch ** 2) ** -0.5)
@@ -394,6 +447,50 @@ def _resnet_visual(sd, arch, rn, g):
     sd[a + "c_proj.bias"] = rn(arch.embed_dim, std=0.02)
 
 
+def _convnext_visual(sd, arch, rn, g):
+    """visual.trunk.* and visual.head.* of a ConvNeXtArch in open_clip's layout, with non-trivial LayerNorm affines and
+    biases and layer scales gamma uniform in [0.1, 1] (real checkpoints start them at 1e-6; near zero, every block
+    would vanish from the output and a wrong block would go unseen)."""
+    torch = _torch()
+    t = "visual.trunk."
+
+    def ln(name, n):
+        sd[name + ".weight"] = 1.0 + rn(n, std=0.1)
+        sd[name + ".bias"] = rn(n, std=0.05)
+
+    def lin(name, n_out, n_in, bias=True):
+        sd[name + ".weight"] = rn(n_out, n_in, std=n_in ** -0.5)
+        if bias:
+            sd[name + ".bias"] = rn(n_out, std=0.02)
+
+    C0 = arch.dims[0]
+    sd[t + "stem.0.weight"] = rn(C0, 3, 4, 4, std=48 ** -0.5)
+    sd[t + "stem.0.bias"] = rn(C0, std=0.02)
+    ln(t + "stem.1", C0)
+    for s, (n, C) in enumerate(zip(arch.depths, arch.dims)):
+        p = "%sstages.%d." % (t, s)
+        if s > 0:
+            Cp = arch.dims[s - 1]
+            ln(p + "downsample.0", Cp)
+            sd[p + "downsample.1.weight"] = rn(C, Cp, 2, 2, std=(4 * Cp) ** -0.5)
+            sd[p + "downsample.1.bias"] = rn(C, std=0.02)
+        for j in range(n):
+            b = "%sblocks.%d." % (p, j)
+            sd[b + "conv_dw.weight"] = rn(C, 1, 7, 7, std=49 ** -0.5)
+            sd[b + "conv_dw.bias"] = rn(C, std=0.05)
+            ln(b + "norm", C)
+            lin(b + "mlp.fc1", 4 * C, C)
+            lin(b + "mlp.fc2", C, 4 * C)
+            sd[b + "gamma"] = 0.1 + 0.9 * torch.rand(C, generator=g)
+    C3, D = arch.dims[3], arch.embed_dim
+    ln(t + "head.norm", C3)
+    if arch.head_mlp:
+        lin("visual.head.mlp.fc1", 2 * D, C3)
+        lin("visual.head.mlp.fc2", D, 2 * D, bias=False)
+    else:
+        lin("visual.head.proj", D, C3, bias=False)
+
+
 def convert_hf_state_dict(sd, arch):
     """HuggingFace CLIPModel parameter names (`hf_clip:` models) -> the OpenAI/open_clip layout."""
     torch = _torch()
@@ -447,6 +544,17 @@ class B200Clip:
                 0, self.max_batch,
             )
             check(lib.b200_clip_create_siglip(C.byref(cfg), self.device_index, C.byref(self._h)), "clip_create_siglip")
+            return
+        if isinstance(arch, ConvNeXtArch):
+            cfg = _lib.ClipConfigC(
+                arch.embed_dim, arch.image_size, 0, _lib.TowerConfigC(0, 0, 0, 0), arch.context_length, arch.vocab_size,
+                _lib.TowerConfigC(arch.text.width, arch.text.layers, arch.text.heads, arch.text.mlp),
+                1 if arch.quick_gelu else 0, self.max_batch,
+            )
+            nc = _lib.ConvNeXtConfigC((C.c_int32 * 4)(*arch.depths), (C.c_int32 * 4)(*arch.dims),
+                                      1 if arch.head_mlp else 0, arch.eps)
+            check(lib.b200_clip_create_convnext(C.byref(cfg), C.byref(nc), self.device_index, C.byref(self._h)),
+                  "clip_create_convnext")
             return
         if isinstance(arch, ResNetArch):
             cfg = _lib.ClipConfigC(

@@ -322,6 +322,26 @@ int b200_clip_create_resnet(const b200_clip_config* cfg, const b200_resnet_confi
  * norm, mlp.fc1, mlp.fc2}} and text.{token_embedding, positional_embedding, transformer.resblocks.i.*, ln_final,
  * text_projection}.  Every other b200_clip_* entry works on the handle unchanged. */
 int b200_clip_create_siglip(const b200_clip_config* cfg, int device, b200_clip** out);
+/* open_clip's ConvNeXt CLIPs (convnext_base, convnext_base_w[_320], convnext_large_d[_320], convnext_xxlarge): the image
+ * tower is timm's ConvNeXt trunk (a 4x4 stride-4 patch stem + LayerNorm, four stages of depths[s] blocks at widths
+ * dims[s], each stage s > 0 entered through LayerNorm + a 2x2 stride-2 convolution; a block is depthwise 7x7 conv ->
+ * LayerNorm -> Linear(C, 4C) -> erf GELU -> Linear(4C, C), scaled per channel by its gamma and added to its input), then
+ * the spatial mean, LayerNorm and open_clip's head: a bias-free Linear(dims[3], embed_dim) (head_mlp 0) or Linear(dims[3],
+ * 2 embed_dim) + bias -> erf GELU -> bias-free Linear(2 embed_dim, embed_dim) (head_mlp 1).  Every LayerNorm of the trunk
+ * uses eps.  `cfg` supplies the text tower (open_clip's standard CLIP text tower, top-level keys), embed_dim, image_size
+ * (a multiple of 32), quick_gelu and max_batch; its `vision` and `patch` must be zero.  dims are multiples of 64, at most
+ * 1536 for stages 0..2 and 3072 for stage 3.  load_weights reads visual.trunk.{stem.{0,1}, stages.s.downsample.{0,1}
+ * (s >= 1), stages.s.blocks.j.{conv_dw, norm, mlp.fc1, mlp.fc2, gamma}, head.norm} and visual.head.proj.weight or
+ * visual.head.mlp.{fc1.weight, fc1.bias, fc2.weight}; a missing one is B200_ERR_INVALID naming it.  Every other
+ * b200_clip_* entry works on the handle unchanged. */
+typedef struct b200_convnext_config {
+  int32_t depths[4];   /* blocks per stage */
+  int32_t dims[4];     /* width of each stage */
+  int32_t head_mlp;    /* 0: linear projection head, 1: MLP head */
+  float eps;           /* LayerNorm epsilon of the trunk (1e-6; timm's xxlarge: 1e-5) */
+} b200_convnext_config;
+int b200_clip_create_convnext(const b200_clip_config* cfg, const b200_convnext_config* ncfg, int device,
+                              b200_clip** out);
 int b200_clip_destroy(b200_clip* m);
 /* Upload weights given as a state_dict in the open_clip/OpenAI key layout; converts to the
  * packed bf16 device layout.  Missing or mis-shaped tensors are an error. */
@@ -437,6 +457,26 @@ int b200_latent_pool_attention_device(const void* d_kv, int B, int T, int heads,
 int b200_pool_last_ln_proj_bias_device(const void* d_x, int B, int T, int w, const float* d_gamma, const float* d_beta,
                                        float eps, const void* d_proj, const float* d_bias, int D, float* d_feat,
                                        void* d_out, int out_dtype, int normalize, int device, void* stream);
+/* The kernels of the ConvNeXt tower, for their parity tests.
+ * Depthwise 7x7 + LayerNorm: d_x NHWC bf16 [B, H, W, C] (C a multiple of 64, at most 3072) -> d_out bf16 [B H W, C] =
+ *   LN_eps(bias[c] + sum_{r,s} d_w49[7 r + s, c] x[h + r - 3, w + s - 3, c]) * gamma[c] + beta[c], zero padding, the
+ *   taps summed in fp32 in the order (r, s) and the LayerNorm taken on those fp32 sums; d_w49 fp32 [49, C] (conv_dw's
+ *   weight [C, 1, 7, 7] transposed); d_gamma == NULL: the convolution + bias alone (d_beta and eps unused).
+ * LayerNorm + space-to-depth: d_x [B, H, W, C] (H, W even, C a multiple of 8, at most 1536) -> d_out bf16
+ *   [B (H/2) (W/2), 4C], column (2 i + j) C + c = LN_eps(x[b, 2 ho + i, 2 wo + j, :])[c] gamma[c] + beta[c].
+ * Head: d_x bf16 [B HW, C] -> d_pooled fp32 [B, C] = LN_eps(fp32 mean of the HW rows of sample b) gamma + beta; then
+ *   with d_w1T == NULL, feat = pooled @ d_w2T fp32 [C, D]; otherwise hid = gelu_erf(pooled @ d_w1T fp32 [C, h] +
+ *   d_b1[h]) into d_hid fp32 [B, h] and feat = hid @ d_w2T fp32 [h, D]; feat into d_feat fp32 [B, D], then d_out =
+ *   feat / |feat| (normalize) as fp16 or fp32 (out_dtype). */
+int b200_dwconv7_ln_bf16_device(const void* d_x, int B, int H, int W, int C, const float* d_w49, const float* d_bias,
+                                const float* d_gamma, const float* d_beta, float eps, void* d_out, int device,
+                                void* stream);
+int b200_ln_s2d_bf16_device(const void* d_x, int B, int H, int W, int C, const float* d_gamma, const float* d_beta,
+                            float eps, void* d_out, int device, void* stream);
+int b200_convnext_head_device(const void* d_x, int B, int HW, int C, const float* d_gamma, const float* d_beta, float eps,
+                              const float* d_w1T, const float* d_b1, int h, const float* d_w2T, int D, float* d_pooled,
+                              float* d_hid, float* d_feat, void* d_out, int out_dtype, int normalize, int device,
+                              void* stream);
 /* ------------------------------------------------------------------------------------------
  * Multilingual text towers (use_mclip).  Replaces the M-CLIP text model of the query service
  * (clip_back.py:222-224,836-859: XLM-RoBERTa-Large + mean pool + LinearTransformation) and the

@@ -20,7 +20,7 @@ import sys
 import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SOURCES = ["knn_scan", "knn_ivf", "knn_ivfpq", "knn_mma", "latent_pool",
+SOURCES = ["knn_scan", "knn_ivf", "knn_ivfpq", "knn_mma", "latent_pool", "dwconv",
            "gemm", "attention", "attention_wgmma", "embed_kernels", "clip_model", "text_encoder"]
 
 
